@@ -1,4 +1,4 @@
-"""``bench.py --driver vae | vae_cl | cpc`` — BASELINE.json config 5 (VAE + CPC encoders, K = N workers, one per GPU).
+"""``bench.py --driver vae | vae_cl | cpc`` — benchmark configuration 5 (VAE + CPC encoders, K = N workers, one per GPU).
 
 Same contract as the headline arm (``bench.py:run_ours``): one engine per process, W + prime warm-up steps, EXACTLY K
 timed optimizer steps per worker bracketed by barrier + synchronize, placed so that they straddle the first

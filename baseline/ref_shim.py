@@ -1,7 +1,7 @@
 """Run the UNMODIFIED reference scripts offline and time them (SURVEY Appendix A).
 
-The reference (``baseline/_ref/src/*.py``, a verbatim copy of /root/reference made by
-``baseline/install_reference.sh``) cannot run without a network: it downloads CIFAR10 through
+The reference (``oracle/_ref/src/*.py``, a verbatim copy of the original project made by
+``oracle/install_reference.sh``) cannot run without a network: it downloads CIFAR10 through
 torchvision and has no timers.  This shim
 
 1. replaces ``torchvision.datasets.CIFAR10`` *in memory* by a synthetic dataset with the same
@@ -26,7 +26,7 @@ from typing import Dict, Optional
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_SRC = os.path.join(HERE, "_ref", "src")
+REF_SRC = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "src")
 
 
 class _StopBench(Exception):
@@ -94,7 +94,7 @@ def _use_lbfgs(src: str) -> str:
 
 def run_reference_script(script: str, consts: Dict[str, object], steps: Optional[int] = None, warmup: int = 0,
                          workdir: Optional[str] = None, on_timed_start=None, optimizer: str = "adam") -> Dict:
-    """Execute ``baseline/_ref/src/<script>``; if ``steps`` is given stop after ``warmup+steps`` optimizer steps."""
+    """Execute ``oracle/_ref/src/<script>``; if ``steps`` is given stop after ``warmup+steps`` optimizer steps."""
     path = os.path.join(REF_SRC, script)
     if not os.path.exists(path):
         raise FileNotFoundError(path)
@@ -179,7 +179,7 @@ def run_reference_bench(gpus: int, steps: int, warmup: int, driver: str = "feder
                 if driver == "cpc" else "no reference arm for driver %r" % driver}
     script = _SCRIPTS[driver]
     if not os.path.exists(os.path.join(REF_SRC, script)):
-        return {"impl": "reference", "unavailable": "baseline/_ref missing: run baseline/install_reference.sh (copies /root/reference; it has no setup.py to pip-install)"}
+        return {"impl": "reference", "unavailable": "oracle/_ref missing: run oracle/install_reference.sh /path/to/federated-pytorch-test"}
     if not torch.cuda.is_available():
         return {"impl": "reference", "unavailable": "no CUDA device"}
     per_round = max(1, -(-(50000 // gpus - 1) // 128))          # minibatches per worker per round (49 for K = 8... 391 for K = 1)
@@ -215,7 +215,7 @@ def run_reference_bench(gpus: int, steps: int, warmup: int, driver: str = "feder
                    "algo": {"federated": "fedavg", "consensus": "admm" + ("+bb" if bb else ""), "fedprox": "fedprox", "vae": "fedavg"}[driver],
                    "optimizer": optimizer, "global_batch": 128 * gpus, "K": gpus,
                    "parallelism": "reference: K=%d replicas sequential on ONE GPU (no distributed runtime)" % gpus,
-                   "script": "baseline/_ref/src/%s (unmodified; constants overridden by regex; synthetic CIFAR10 class)" % script,
+                   "script": "oracle/_ref/src/%s (unmodified; constants overridden by regex; synthetic CIFAR10 class)" % script,
                    "timed_steps": timed, "timed_optimizer_steps": [first, first + timed * gpus], "aggregations_in_window": aggs,
                    "timing": "CUDA events around optimizer steps %d..%d, observed via a wrapper on the optimizer's step()" % (first, first + timed * gpus),
                    "device_ms": res.get("device_ms"), "wall_ms": res.get("wall_ms")},

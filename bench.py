@@ -1,13 +1,23 @@
 #!/usr/bin/env python
-"""Headline benchmark (BASELINE.json): training throughput of ``federated_multi`` — ResNet18, FedAvg over
+"""Headline benchmark (configuration 2 below): training throughput of ``federated_multi`` — ResNet18, FedAvg over
 parameter blocks, one worker per GPU, batch 128 per worker, synthetic CIFAR10, random init.
 
     python bench.py --gpus N --steps K --warmup W            # N=1
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W               # N>1, one rank per GPU
     python bench.py --impl reference --gpus N ...            # the unmodified reference through an offline shim
-    python bench.py --driver consensus --bb ...              # BASELINE config 3 (adaptive ADMM); --driver fedprox
+    python bench.py --driver consensus --bb ...              # configuration 3 (adaptive ADMM); --driver fedprox
                                                              # --optimizer lbfgs (config 4); --driver vae | cpc (config 5)
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR   # also write what the last timed step computed
+
+Benchmark configurations: 1 ``no_consensus_multi`` SimpleCNN K=2 on CPU (plumbing); 2 ``federated_multi`` ResNet18
+FedAvg over parameter blocks; 3 ``consensus_multi`` ResNet18 adaptive ADMM; 4 ``fedprox_multi`` ResNet18 with LBFGSNew;
+5 ``federated_vae`` / ``federated_cpc`` (VAE and CPC encoders).  Configurations 2-5 run K = N workers, one per GPU.
+
+``--dump-outputs DIR`` (rank 0) writes, after the run, what the LAST timed step computed: the last step of the end-to-end
+window, or of the device window with --no-e2e.  That is its loss and, per local replica, a fixed seeded sample of the
+parameters and parameter gradients, as float32 ``DIR/<name>.npy``, at most 64 MB in all.  The inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 
 A *step* is one minibatch optimizer step on every worker (128*N images): zero-grad, forward, CE loss, backward,
 fused Adam on the active block, and the reference's post-step diagnostics forward; block aggregation (fused
@@ -47,10 +57,10 @@ import torch  # noqa: E402
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-STEPS_PER_ROUND = 49      # ceil(6249 / 128): the K=8 shard of the BASELINE config
+STEPS_PER_ROUND = 49      # ceil(6249 / 128): the K=8 shard of configuration 2
 PRIME_STEPS = 4           # eager warm-up + CUDA-graph capture of the step, before the W warm-up steps
 # The device window straddles the SECOND round boundary: the first aggregation of a run is warm-up like the first minibatches are
-# (first cross-GPU touch of the block's peer-mapped pages; on one 8-GPU box it cost 9 ms once, the next ones 0.7 ms — r2_scaling.md).
+# (first cross-GPU touch of the block's peer-mapped pages, which costs far more than the aggregations after it).
 TIMED_BOUNDARY = 2 * STEPS_PER_ROUND
 
 
@@ -241,8 +251,8 @@ def run_ours(args) -> dict:
     slot_ev = [torch.cuda.Event(), torch.cuda.Event()]
     pending = []
     # ONE nvidia-smi sampler for the whole run, started before the first step: its start-up (NVML attaches to every GPU of the
-    # box) stalls CUDA launches of ALL ranks for tens of ms on an 8-GPU node — inside a 50 ms window that contains a cross-rank
-    # aggregation this was measured as a 30 ms "step" (profiles/r2_scaling.md).  The windows only mark sample indices.
+    # box) stalls CUDA launches of ALL ranks, which inside a short window that contains a cross-rank aggregation would show up as
+    # one very long "step".  The windows only mark sample indices.
     smi = ClockSampler(dev.index or 0) if (topo.is_root and os.environ.get("FEDB200_BENCH_NO_SMI", "0") != "1") else None
     if smi:
         smi.start()
@@ -254,7 +264,7 @@ def run_ours(args) -> dict:
 
     def open_window(tag, ev):
         gc.collect()
-        gc.disable()      # a cyclic-GC pause (~10 ms with this heap) inside a 50 ms window is 20 % noise; re-enabled at close
+        gc.disable()      # a cyclic-GC pause inside a short window is noise of the host, not the GPU; re-enabled at close
         topo.barrier()
         torch.cuda.synchronize(dev)
         st[tag]["smi0"] = smi.mark() if smi else 0
@@ -330,6 +340,14 @@ def run_ours(args) -> dict:
 
     eng.step_hook = hook
     eng.run()
+    if args.dump_outputs and topo.is_root:
+        torch.cuda.synchronize(dev)
+        outputs = {"loss": eng.last_loss1.detach().reshape(1)}
+        for j, rep in enumerate(eng.replicas):
+            arena = rep.arenas["net"]
+            outputs["params_r%d" % j] = arena.data
+            outputs["grads_r%d" % j] = arena.grad
+        dump_outputs(args.dump_outputs, outputs)
     ms_d = _max_over_ranks(ev_d[0].elapsed_time(ev_d[1]), dev)
     images = 128 * N * K
     value = images / (ms_d / 1e3)
@@ -347,7 +365,7 @@ def run_ours(args) -> dict:
                    "timed_steps": [first_d, last_d], "aggregations_in_window": st["d"].get("aggregations"),
                    "aggregation_two_shot": bool(getattr(coll, "last_two_shot", False)),
                    "warmup_steps_before_window": first_d,
-                   "l2": "per-step working set (~1 GB of fp32 activations) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (~1 GB of fp32 activations) exceeds the 50 MB L2; no explicit flush",
                    "timing": "CUDA events on the step stream, barrier+synchronize both sides, max over ranks"},
         "clocks": st["d"].get("clocks"),
         "gpu_launches": st["d"].get("launches"),
@@ -387,6 +405,26 @@ def run_ours(args) -> dict:
     return out if topo.is_root else {}
 
 
+DUMP_BYTES = 64 << 20        # the whole dump, float32
+DUMP_SAMPLE = 1 << 22        # elements kept of a larger array: 16 MB of float32
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """``out_dir/<name>.npy`` in float32; an array longer than its share of DUMP_BYTES (at most DUMP_SAMPLE elements) is
+    replaced by the same seeded sample of its elements every run (sorted indices), so the dump stays small and comparable."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    keep = min(DUMP_SAMPLE, DUMP_BYTES // 4 // max(1, len(arrays)))
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > keep:
+            g = torch.Generator().manual_seed(1234)
+            idx = torch.randperm(flat.numel(), generator=g)[:keep].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.float().cpu().numpy())
+
+
 # ----------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -394,11 +432,11 @@ def main():
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "nccl"],
-                    help="ours | reference (unmodified reference via shim) | nccl (BASELINE 'ref-nccl': ATen model + NCCL all-reduce)")
+                    help="ours | reference (unmodified reference via shim) | nccl (ATen model + NCCL all-reduce: the baseline, not the product)")
     ap.add_argument("--driver", default="federated", choices=["federated", "consensus", "fedprox", "vae", "vae_cl", "cpc"],
                     help="which entry point is benchmarked (default: the headline federated_multi / FedAvg)")
     ap.add_argument("--algo", default=None, choices=[None, "fedavg", "admm"], help="alias: admm = --driver consensus")
-    ap.add_argument("--bb", action="store_true", help="consensus: Barzilai-Borwein adaptive rho (BASELINE config 3)")
+    ap.add_argument("--bb", action="store_true", help="consensus: Barzilai-Borwein adaptive rho (configuration 3)")
     ap.add_argument("--optimizer", default="adam", choices=["adam", "lbfgs"])
     ap.add_argument("--collective", default="auto", choices=["auto", "fused", "torch"])
     ap.add_argument("--diagnostics", default="post", choices=["post", "pre"])
@@ -406,6 +444,8 @@ def main():
     ap.add_argument("--no-fast", dest="no_fast", action="store_true")
     ap.add_argument("--no-e2e", dest="no_e2e", action="store_true")
     ap.add_argument("--no-collective-table", dest="no_collective_table", action="store_true")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss, parameters and gradients (seeded samples) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.algo == "admm":
@@ -413,6 +453,8 @@ def main():
     if args.impl == "nccl":   # the "baseline, not the product": stock ATen ops, eager, NCCL all-reduce on the flat block
         args.no_fast, args.no_graphs, args.collective = True, True, "torch"
 
+    if args.dump_outputs and (args.impl != "ours" or args.driver in ("vae", "vae_cl", "cpc")):
+        ap.error("--dump-outputs is implemented for the ResNet18 drivers of --impl ours")
     if args.impl == "reference":
         from baseline.ref_shim import run_reference_bench
 

@@ -5,8 +5,8 @@ Two extensions, both built with ``torch.utils.cpp_extension`` into
 travels with the source tree (a JIT cache under ``~/.cache`` would not):
 
 * ``fedb200_runtime`` — C++ host runtime (batch assembler), no CUDA needed;
-* ``fedb200_cuda``    — the sm_100a kernels (``csrc/*.cu``), compiled with
-  ``-gencode arch=compute_100a,code=sm_100a -lineinfo`` and nothing else: there
+* ``fedb200_cuda``    — the sm_90a kernels (``csrc/*.cu``), compiled with
+  ``-gencode arch=compute_90a,code=sm_90a -lineinfo`` and nothing else: there
   is no fallback architecture and no second backend.
 
 ``load(name)`` imports the prebuilt ``.so`` when it is newer than its sources and
@@ -26,16 +26,16 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 _BUILD = os.path.join(_HERE, "_build")
 
-CUDA_ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+CUDA_ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-lineinfo", "--use_fast_math", "-std=c++17", "--expt-relaxed-constexpr",
-              "-Xptxas", "-v", "-DFEDB200_SM100A=1"] + CUDA_ARCH_FLAGS
+              "-Xptxas", "-v"] + CUDA_ARCH_FLAGS
 CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC"]
 
 _SPECS: Dict[str, Dict] = {
     "fedb200_runtime": {"sources": ["batch_loader.cpp"], "cuda": False},
     "fedb200_cuda": {
         "sources": ["bindings.cpp", "flat_kernels.cu", "elementwise_kernels.cu", "loss_kernels.cu",
-                    "comm_kernels.cu", "gemm_tcgen05.cu", "aux_kernels.cu"],
+                    "comm_kernels.cu", "gemm_wgmma.cu", "aux_kernels.cu"],
         "cuda": True,
     },
 }
@@ -73,7 +73,7 @@ def _import_so(name: str):
 
 def build(name: str, verbose: bool = False):
     """(Re)build extension ``name`` in-tree and import it."""
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")  # silence arch autodetect; real flags are explicit
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")  # silence arch autodetect; real flags are explicit
     os.environ.setdefault("MAX_JOBS", str(min(8, os.cpu_count() or 4)))
     from torch.utils import cpp_extension
 

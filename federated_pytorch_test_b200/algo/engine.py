@@ -432,11 +432,10 @@ class Engine:
         """End of a round.  The aggregation is ONE kernel in stream order (write-back included), so the next minibatch can
         be queued right behind it; what the host wants from it (residuals, non-finite count, time-out status) is a record in
         pinned memory.  With ``deferred_rounds`` the record is read after the next minibatch has been enqueued instead of
-        draining the GPU first (measured: the step that contained the round boundary took 3.3 ms instead of 2.24 ms)."""
+        draining the GPU first, so the step that contains the round boundary does not wait for the host's read."""
         cfg = self.cfg
-        # Measured (profiles/r2_late.md §1): 1 GPU 2.308 -> 2.253 ms/step, 4 GPUs boundary step 2.5 ms in both windows; on 8 GPUs the
-        # steady-state boundary was fine (2.8 ms) but the FIRST deferred aggregation of the run cost 11 ms once and an adaptive-ADMM
-        # run was slow, with no GPU minutes left to find out why -> up to 4 ranks by default, FEDB200_DEFERRED_ROUNDS=1 forces it on.
+        # On by default up to 4 ranks only: with more ranks the first deferred aggregation of a run and adaptive-ADMM runs were not
+        # shown to gain from it.  FEDB200_DEFERRED_ROUNDS=1 forces it on.
         env = os.environ.get("FEDB200_DEFERRED_ROUNDS", "auto")
         # (only a collective with asynchronous entry points actually defers: FusedCollective; the others answer "done")
         defer = (cfg.deferred_rounds and not cfg.check_results and not cfg.be_verbose

@@ -45,7 +45,7 @@ def capture_graph(stream, body, pool=None):
 
     A CUDAGraph that is garbage (e.g. the graphs of a previous Engine, kept alive by a reference cycle) must not be
     finalised while a capture is in progress: cudaGraphExecDestroy is "not permitted when stream is capturing" and
-    invalidates the capture (measured: profiles/r2_call2).  torch.cuda.graph no longer collects by itself, so: collect
+    invalidates the capture.  torch.cuda.graph no longer collects by itself, so: collect
     first, keep the cyclic collector off during the capture."""
     import gc
 

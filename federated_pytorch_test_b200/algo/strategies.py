@@ -11,7 +11,7 @@ object driven by the block-coordinate engine:
     strat.aggregate(nadmm)            # the collective + bookkeeping -> metrics
 
 All vector work is delegated to a collective (``parallel.collective``), i.e. to
-one fused NVLink kernel per aggregation on B200.
+one fused NVLink kernel per aggregation on the GPU.
 
 Preserved reference behaviour (SURVEY §2.12): ``z`` (and ``y``) start at 0 for
 every block visit (Q6); FedProx/ADMM never write ``z`` back (Q7); ``rho`` is an
@@ -214,7 +214,7 @@ class ADMM(Strategy):
         ``a=y-yhat0, b=x-z, c=x-x0`` the quantities it needs are
         ``d11 = a.a + 2 rho a.b + rho^2 b.b``, ``d12 = a.c + rho b.c``, ``d22 = c.c``,
         so six local dots per worker + one tiny gather reproduce the sequential
-        rule without serialising the GPUs.  On B200 all of it — dots, gather through
+        rule without serialising the GPUs.  On the GPU all of it — dots, gather through
         the peer-mapped control pads, replay, ``yhat0``/``x0`` carry — is ONE kernel
         (``csrc/comm_kernels.cu: bb_update_kernel``) that leaves the new rho in
         device memory; the host only reads the log rows for the legacy print lines.

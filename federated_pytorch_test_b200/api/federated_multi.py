@@ -2,7 +2,7 @@
 
 Reference: /root/reference/src/federated_multi.py (mean over K then write-back into every
 replica, ``dual = ||z - z_new|| / N``; CE + gated elastic net; Adam 1e-3 per block visit).
-On B200 the aggregation is one fused NVLink kernel on the block slice of the replicas'
+On the GPU the aggregation is one fused NVLink kernel on the block slice of the replicas'
 parameter arenas (``csrc/comm_kernels.cu``), no NCCL on the path.
 """
 from __future__ import annotations

@@ -48,7 +48,7 @@ class CommonConfig:
     diagnostics: str = "post"       # Q17: 'post' (extra forward after the step) | 'pre'
     nan_guard: str = "raise"        # non-finite aggregation residual: 'raise' | 'warn' | 'off'
     collective: str = "auto"        # 'auto' | 'fused' | 'torch'
-    fast: bool = True               # use the hand-written sm_100a kernels on CUDA devices
+    fast: bool = True               # use the hand-written sm_90a kernels on CUDA devices
     graphs: bool = True             # CUDA-graph the per-minibatch step when possible
     distributed: bool = True        # honour torchrun env (one process per GPU); False = all K replicas here
     ckpt_dir: str = "."

@@ -1,5 +1,5 @@
 // Hand-written fp32 kernels for the small / awkward operators of the model zoo — everything that is NOT a large
-// convolution (those are on tcgen05: gemm_tcgen05.cu, wgrad_tcgen05.cuh):
+// convolution (those are on wgmma: gemm_wgmma.cu, wgrad_wgmma.cuh):
 //
 //  * gemm_f32_kernel        true-fp32 strided GEMM with bias / ELU / accumulate epilogue: nn.Linear forward, data and
 //                           weight gradients (SURVEY G5; the reference runs nn.Linear in true fp32, so this is the parity
@@ -33,7 +33,7 @@ static int aux_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -49,7 +49,7 @@ __device__ __forceinline__ float warp_sum_f(float v) {
 // BM x BN tile per CTA (64 x 64, or 32 x 32 when the 64-tiles would leave most SMs idle: the dense layers of the model zoo
 // are 128 x 16 ... 1280 x 128 outputs), 16-deep k tiles, 256 threads x (BM/16 x BN/16) outputs, true fp32 (FFMA).
 // The next k tile is fetched into registers while the current one is multiplied (one barrier per tile): these GEMMs are
-// latency bound — the first version (load, barrier, multiply, barrier) took 11-17 us for 1.5-75 MFLOP (r2_call14.log).
+// latency bound, so the load of the next tile must overlap the multiply of the current one.
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int GF_BK = 16;
 
@@ -203,7 +203,7 @@ void act_bwd_bias(const float* dout, const float* out, float* dz, float* db, lon
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// 2x2 / stride 2 max pooling, NCHW or NHWC memory (nhwc = 1: the layout the tcgen05 convolutions produce).
+// 2x2 / stride 2 max pooling, NCHW or NHWC memory (nhwc = 1: the layout the wgmma convolutions produce).
 // idx: which of the four window positions won (uint8) — the backward needs nothing else.
 // ------------------------------------------------------------------------------------------------------------------
 struct PoolGeom {
@@ -523,7 +523,7 @@ void gauss_nll_rows_bwd(const float* x, const float* mu, const float* s2, const 
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Direct convolutions for shapes the TMA / tcgen05 path cannot tile (channel counts not multiples of 4, map widths
+// Direct convolutions for shapes the TMA / wgmma path cannot tile (channel counts not multiples of 4, map widths
 // that do not divide 128): NCHW, stride 1, "valid" or zero padding, square k <= 7, weights staged in shared memory.
 //   fwd   : y = ELU?(conv(x, w) + b), optionally followed by a fused 2x2 max-pool (the pre-pool map is not stored:
 //           the backward recomputes nothing — it gets the winner index and the pooled activation)

@@ -1,4 +1,4 @@
-// Torch glue for the sm_100a kernels: tensor checks, stream selection, pybind.  All math lives in the .cu files.
+// Torch glue for the sm_90a kernels: tensor checks, stream selection, pybind.  All math lives in the .cu files.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -215,10 +215,6 @@ Tensor linear_tf32(Tensor x, Tensor w, c10::optional<Tensor> bias, bool act) {
   fb::linear_tf32(fptr(x), fptr(w), opt_ptr(bias), fptr_mut(out), M, N, K, K, K, N, act ? 1 : 0, cur_stream());
   return out;
 }
-void set_conv_trace(c10::optional<Tensor> buf) {
-  fb::set_conv_trace((buf.has_value() && buf->defined()) ? reinterpret_cast<long long*>(buf->data_ptr<int64_t>()) : nullptr);
-}
-void probe_launch(int64_t kind, int64_t grid, int64_t smem_bytes) { fb::probe_launch((int)kind, (int)grid, (int)smem_bytes, cur_stream()); }
 bool conv_supported(int64_t H_out, int64_t W_out, int64_t C_in, int64_t stride) {
   return fb::conv_geometry_supported((int)H_out, (int)W_out, (int)C_in, (int)stride);
 }
@@ -627,7 +623,7 @@ void ipc_close_handle(int64_t ptr) { cudaIpcCloseMemHandle(reinterpret_cast<void
 int64_t launch_count() { return (int64_t)fb::launch_count(); }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "federated_pytorch_test_b200: hand-written sm_100a kernels";
+  m.doc() = "federated_pytorch_test_b200: hand-written sm_90a kernels";
   m.def("launch_count", &launch_count);
   m.def("adam_prox", &adam_prox);
   m.def("bump_step", &bump_step);
@@ -650,8 +646,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("convT_pack", &convT_pack);
   m.def("linear_tf32", &linear_tf32);
   m.def("conv_supported", &conv_supported);
-  m.def("probe_launch", &probe_launch);
-  m.def("set_conv_trace", &set_conv_trace);
   m.def("conv2d_nhwc", &conv2d_nhwc);
   m.def("conv2d_nhwc_sized", &conv2d_nhwc_sized);
   m.def("conv2d_nhwc_bias_act", &conv2d_nhwc_bias_act);

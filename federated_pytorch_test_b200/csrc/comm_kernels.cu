@@ -374,7 +374,7 @@ static int comm_max_blocks(const void* kernel) {
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, COMM_THREADS, 0);
-  int m = sms * (per < 1 ? 1 : 1);                    // one CTA per SM: 148 x 512 threads saturate NVLink and HBM
+  int m = sms * (per < 1 ? 1 : 1);                    // one CTA per SM (132 on an H100 SXM) x 512 threads
   if (m > COMM_MAX_BLOCKS) m = COMM_MAX_BLOCKS;
   const int cap = env_int_c("FEDB200_COMM_BLOCKS", 0);
   if (cap > 0 && cap < m) m = cap;
@@ -398,8 +398,8 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   if (args.timeout_cycles <= 0) args.timeout_cycles = 240000000000LL;   // ~2 min at 2 GHz
   void* kargs[] = {(void*)&args};
   // Plain launch: a CTA only ever waits for the SAME-numbered CTA of its peers (never for another CTA of its own grid), so
-  // co-residency of the grid is not required; a cooperative launch costs ~5 us more per aggregation (measured,
-  // profiles/r2_collective.md).  FEDB200_COMM_COOP=1 restores it (A/B runs).
+  // co-residency of the grid is not required and a cooperative launch only adds launch cost.  FEDB200_COMM_COOP=1 restores
+  // it (A/B runs).
   static const int coop = env_int_c("FEDB200_COMM_COOP", 0);
   cudaError_t e;
   if (coop) e = cudaLaunchCooperativeKernel((void*)block_reduce_kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);

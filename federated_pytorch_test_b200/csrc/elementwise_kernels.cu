@@ -29,7 +29,7 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -80,8 +80,8 @@ void normalize_u8_nhwc(const uint8_t* in, float* out, int npix, int c_out, const
 // every loop keeps four independent 16-B loads per tensor in flight.
 //
 // Reductions end in atomicAdds on a [2C] vector that spans only a few 128-B lines, i.e. a few L2 slices: with ~600
-// blocks the ~10^5 same-line atomics, not the streaming, set the kernel time (col_stats measured 0.7 TB/s,
-// profiles/r1_run13_bn.log).  The reduction kernels therefore run at most two 512-thread blocks per SM.
+// blocks the ~10^5 same-line atomics, not the streaming, would set the kernel time.  The reduction kernels therefore run at
+// most two 512-thread blocks per SM.
 // ------------------------------------------------------------------------------------------------
 constexpr int EW_THREADS = 256;
 constexpr int RED_THREADS = 512;
@@ -145,8 +145,8 @@ static int reduce_rows_per_thread() {
 }
 static int reduce_grid(int M, int rpi) {
   // One block of four rows in flight per thread, at most two CTAs per SM.  The first version asked for >= 16 rows per thread (few
-  // blocks => few same-line atomics), which left the small tensors on 32-64 CTAs: 8.4 MB of layer4 activations in 14 us
-  // (profiles/r2_ncu_summary.md: `bn_elu_bwd_reduce_kernel<2>` grid 32, 7 % of the DRAM throughput).  FEDB200_RED_ROWS=16: old grid.
+  // blocks => few same-line atomics), which left the small tensors on 32-64 CTAs, far too few to stream them at DRAM speed.
+  // FEDB200_RED_ROWS=16: old grid.
   const int rows = reduce_rows_per_thread();
   int grid = (M + rpi * rows - 1) / (rpi * rows);
   if (grid > sm_count() * 2) grid = sm_count() * 2;
@@ -373,7 +373,7 @@ void bn_elu_bwd_reduce(const float* dout, const float* out, const float* y, cons
 
 // backward pass 2: dy = gamma*invstd*(du - sum_du/M - xhat*sum_du_xhat/M); dres = du; dgamma/dbeta from sums.
 // Rows are visited from the END of the tensor: pass 1 has just streamed dout/y/out front to back, so their tails are
-// what the 126 MB L2 still holds.
+// what the L2 (50 MB on an H100) still holds.
 template <int MODE>
 __global__ void __launch_bounds__(EW_THREADS)
 bn_elu_bwd_apply_kernel(const float* __restrict__ dout, const float* __restrict__ out, const float* __restrict__ y,
@@ -459,9 +459,9 @@ void bn_elu_bwd_apply(const float* dout, const float* out, const float* y, const
 }
 
 // ------------------------------------------------------------------------------------------------
-// EXPERIMENTAL (opt-in, FEDB200_BN_BWD_FUSED=1; written after this round's GPU budget was spent): both passes of the
+// EXPERIMENTAL (opt-in, FEDB200_BN_BWD_FUSED=1): both passes of the
 // BN(+ELU) backward in ONE cooperative kernel for the small layers (layer3 / layer4: 8 / 4 MB per tensor).  The two-pass
-// version costs a memset + 2 launches and reads every tensor twice (12 us for 4 MB, profiles/r1_run13_bn.log); here each
+// version costs a memset + 2 launches and reads every tensor twice; here each
 // thread keeps its <= MAXR rows of du and y in registers across a grid barrier, so the tensors are read once.
 // Requires gridDim.x * rows_per_iter * MAXR >= M with all blocks co-resident (cooperative launch).
 // ------------------------------------------------------------------------------------------------
@@ -575,9 +575,9 @@ void avgpool_nhwc(const float* x, float* out, int NB, int HW, int C, cudaStream_
   check_launch("avgpool_nhwc");
 }
 // ------------------------------------------------------------------------------------------------
-// EXPERIMENTAL (opt-in, FEDB200_HEAD_FUSED=1; written after this round's GPU budget was spent): classifier head
+// Fused classifier head (FEDB200_HEAD_FUSED=0 switches it off):
 // avg_pool(window) -> flatten -> Linear in ONE true-fp32 kernel per direction (SURVEY G4 + G5, simple_models.py:213-216).
-// The library path is avgpool (4 us) + a SIMT sgemm (13 us) for a 128x10x512 problem; here one block per sample pools
+// The library path is an avgpool kernel + a SIMT sgemm for a 128x10x512 problem; here one block per sample pools
 // its [HW, C] map into shared memory and eight warps produce the O <= 32 logits with FMA chains + shuffle reductions.
 // ------------------------------------------------------------------------------------------------
 constexpr int HEAD_THREADS = 256;
@@ -679,7 +679,7 @@ void weight_krsc_flip(const float* w, float* out, int C_out, int C_in, int kh, i
 // ConvTranspose2d(k = 4, stride 2, padding 1) weight [Ci, Co, 4, 4] (any strides) -> KRSC filter [4 * Co, 3, 3, Ci] of the equivalent
 // 3x3 / pad 1 convolution with phase-major output channels (ops/conv_math.py::pack_convT_s2_weight: output phase ph takes filter
 // rows 3, 1 at window positions 0, 1 and phase 1 rows 2, 0 at positions 1, 2; the other position is zero).  One launch instead
-// of a 36-way torch.stack (11 us each, 11 per VAE step: profiles/r2/r2_call14.log).
+// of a 36-way torch.stack per transposed convolution and step.
 __device__ __forceinline__ int convT_tap(int phase, int t) {
   return phase == 0 ? (t == 0 ? 3 : (t == 1 ? 1 : -1)) : (t == 0 ? -1 : (t == 1 ? 2 : 0));
 }

@@ -10,11 +10,11 @@ void count_launch(int n = 1);
 long long launch_count();
 
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------
-// A training step is ~200 short kernels (10-40 us each): launch latency + CTA ramp-up of kernel N+1 is hidden behind
+// A training step is ~200 short kernels: launch latency + CTA ramp-up of kernel N+1 is hidden behind
 // the tail of kernel N by letting N+1 become resident early.  Every kernel launched through launch_pdl() executes
 // pdl_launch_dependents() first (lets ITS successor start scheduling) and pdl_wait() before its first global-memory
 // access (blocks until the predecessor grid has completed and flushed).  Opt-in with FEDB200_PDL=1: inside the
-// CUDA-graph step the launch gaps are already hidden and the measured step time did not change.
+// CUDA-graph step the launch gaps are already hidden.
 bool pdl_enabled();
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -40,7 +40,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 #endif
 
-// ---- tcgen05 implicit GEMM (gemm_tcgen05.cu) -------------------------------------------------------
+// ---- wgmma implicit GEMM (gemm_wgmma.cu) -----------------------------------------------------------
 int pick_block_n(int M, int N);
 void linear_tf32(const float* x, const float* w, const float* bias, float* out, int M, int N, int K, int ldx, int ldw,
                  int ldo, int act, cudaStream_t stream);
@@ -64,13 +64,11 @@ bool conv_multidil_supported(int H_out, int W_out, int C_in, int stride, int bra
 void conv2d_nhwc_multidil_tf32(const float* x, const float* w, const float* bias, int act, float* y, int NB, int H, int W, int C_in,
                                int C_out, int branches, int kh, int kw, int stride, const int* dils, const int* pads, int H_out,
                                int W_out, cudaStream_t stream);
-// weight gradient on tcgen05 (MN-major operands, split over the pixel range, red.add into dw)
+// weight gradient on wgmma (operands gathered K-major into shared memory, split over the pixel range, red.add into dw)
 bool conv_wgrad_supported(int C_x, int C_out, int stride, int W_out, int H_out);
 void conv_wgrad_tf32(const float* x, const float* dy, float* dw, int NB, int H, int W, int C_x, int C_w, int C_out, int kh,
                      int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream);
 
-void set_conv_trace(long long* buf);   // [16] clock64 stamps of CTA 0 of the next persistent conv launches (nullptr = off)
-void probe_launch(int kind, int grid, int smem_bytes, cudaStream_t stream);   // launch-floor probes (tools/)
 
 // ---- flat-vector kernels (flat_kernels.cu) ---------------------------------------------------------
 void adam_prox(float* x, const float* g, float* m, float* v, const int* step_dev, int n, float lr, float b1, float b2,
@@ -157,7 +155,7 @@ constexpr int COMM_MAX_K = 64;       // contributions (workers) per aggregation
 constexpr int COMM_MAX_LOCAL = 16;   // replicas hosted by one process
 constexpr int COMM_MAX_WORLD = 16;   // processes meeting through peer memory
 constexpr int COMM_THREADS = 512;
-constexpr int COMM_MAX_BLOCKS = 160; // CTAs per aggregation kernel (one per SM on a B200: 148)
+constexpr int COMM_MAX_BLOCKS = 160; // CTAs per aggregation kernel (one per SM: 132 on an H100 SXM)
 
 // Control pad (uint32 words; one pad per rank, mapped into every peer).  Flags hold the epoch of the aggregation that
 // last signalled them (monotonic, compared with >=), so nothing is ever reset.

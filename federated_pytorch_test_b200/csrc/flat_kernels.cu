@@ -26,7 +26,7 @@ bool pdl_enabled() {
   static int v = -1;
   if (v < 0) {
     const char* e = std::getenv("FEDB200_PDL");
-    v = (e != nullptr && std::atoi(e) != 0) ? 1 : 0;   // opt-in: measured neutral inside the captured step (2.93 vs 2.90 ms)
+    v = (e != nullptr && std::atoi(e) != 0) ? 1 : 0;   // opt-in: inside a captured step the launch gaps are already hidden
   }
   return v == 1;
 }
@@ -43,7 +43,7 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

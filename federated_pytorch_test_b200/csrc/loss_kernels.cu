@@ -89,7 +89,7 @@ void vae_loss_fwd(const float* recon, const float* x, int n, const float* mu, co
                   cudaStream_t s) {
   cudaMemsetAsync(out, 0, sizeof(float), s);
   int grid = (n + 1023) / 1024;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > 132 * 4) grid = 132 * 4;
   if (grid < 1) grid = 1;
   vae_fwd_kernel<<<grid, 256, 0, s>>>(recon, x, n, mu, logvar, nl, out);
   check_launch("vae_loss_fwd");
@@ -109,7 +109,7 @@ vae_bwd_kernel(const float* __restrict__ recon, const float* __restrict__ x, int
 void vae_loss_bwd(const float* recon, const float* x, int n, const float* mu, const float* logvar, int nl,
                   const float* gout, float* drecon, float* dmu, float* dlogvar, cudaStream_t s) {
   int grid = (n + 1023) / 1024;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > 132 * 4) grid = 132 * 4;
   if (grid < 1) grid = 1;
   vae_bwd_kernel<<<grid, 256, 0, s>>>(recon, x, n, mu, logvar, nl, gout, drecon, dmu, dlogvar);
   check_launch("vae_loss_bwd");

@@ -104,7 +104,7 @@ def normalize_batch(u8_nhwc: torch.Tensor, mean, std, channels_last: bool = Fals
     """uint8 NHWC -> float32 NCHW-shaped tensor ``(x/255 - mean)/std``.
 
     With ``channels_last=True`` the result keeps NHWC memory (a permuted view),
-    which is what the sm_100a conv path consumes; on CUDA this is one kernel.
+    which is what the sm_90a conv path consumes; on CUDA this is one kernel.
     """
     if u8_nhwc.is_cuda:
         from ..ops import functional as FX

@@ -5,7 +5,7 @@ Behavioural spec: /root/reference/src/simple_models.py:436-514
 
 The five dilated stem convolutions read the same input and their outputs are
 concatenated on the channel axis: :func:`ops.functional.dilated_stem` runs them
-as one tcgen05 launch that writes the concatenated tensor (SURVEY G6).
+as one wgmma launch that writes the concatenated tensor (SURVEY G6).
 """
 from __future__ import annotations
 

@@ -6,8 +6,8 @@ registration order, attribute names (``conv1/bn1/layer1..4/linear``,
 indices, message sizes (SURVEY §2.2) and checkpoints carry over.
 
 What is different: every ``conv -> BatchNorm(train) -> (+residual) -> ELU``
-group goes through ONE call, :func:`ops.functional.conv_bn_act`, which on a
-B200 runs the hand-written sm_100a path (tcgen05 implicit-GEMM conv whose
+group goes through ONE call, :func:`ops.functional.conv_bn_act`, which on
+an H100 runs the hand-written sm_90a path (wgmma implicit-GEMM conv whose
 epilogue emits the BN batch statistics, then one fused normalise+residual+ELU
 pass; NHWC activations) and otherwise falls back to the ATen composition with
 identical semantics.

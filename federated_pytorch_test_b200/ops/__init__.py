@@ -1,4 +1,4 @@
-"""Operators: ``functional`` (dispatch + ATen oracle) and ``cuda_ops`` (sm_100a kernels)."""
+"""Operators: ``functional`` (dispatch + ATen oracle) and ``cuda_ops`` (sm_90a kernels)."""
 from . import functional
 
 __all__ = ["functional"]

@@ -9,9 +9,9 @@ four phases together are one 2x2 convolution with ``4*Ci`` output channels whose
 (zeros where a phase has no tap):   row phase 0 <- filter row 1 at dr=0;  row phase 1 <- filter row 2 at dr=0 and
 filter row 0 at dr=1 (same for columns).  The result ``[N, Ho, Wo, 2, 2, Ci]`` is interleaved into ``[N, 2Ho, 2Wo, Ci]``.
 
-Why: the strided data gradients were the slowest library kernels left in the step (cuDNN ``strided_dgrad``: 104 us for
-layer2.0.conv1 alone, profiles/r1_run19_step_kernels.txt) while the same FLOPs run in ~10 us on our implicit-GEMM
-kernel; 7/16 of the packed filter is zero padding, which is cheaper than four launches.
+Why: a strided data gradient as a library call (cuDNN ``strided_dgrad``) is a slow kernel, while one stride-1 implicit
+GEMM over the phase-packed filter keeps the tensor cores busy; 7/16 of the packed filter is zero padding, which is cheaper
+than four launches.
 
 Everything here is plain PyTorch (runs on CPU for the tests); the convolution itself is injected.
 """
@@ -118,7 +118,7 @@ def conv3x3_oracle(x_nhwc: torch.Tensor, w_krsc: torch.Tensor) -> torch.Tensor:
 # the SAME input with the same k x k / stride, their own dilation d_b / padding p_b and their own output channels, followed by a
 # channel concatenation, as ONE implicit GEMM:
 #     y[n, ho, wo, (b, co)] = sum_{r, s, ci} x[n, ho*stride + r*d_b - p_b, wo*stride + s*d_b - p_b, ci] * W_b[co, r, s, ci]
-# The kernel (csrc/igemm_persist_tcgen05.cuh, IgemmParams::ms_*) enumerates "filter rows" R = (b, r) of a merged filter
+# The kernel (csrc/igemm_wgmma.cuh, IgemmParams::ms_*) enumerates "filter rows" R = (b, r) of a merged filter
 # Wm[(b', co), (b, r), s, ci] = W_b[co, r, s, ci] if b' == b else 0 (block diagonal), and row R reads the input through branch
 # R // k's dilation and padding.  Everything below is plain PyTorch: the packing used by the GPU path and an oracle that gathers
 # the taps exactly in the kernel's order.
@@ -187,7 +187,7 @@ def tap_packed_gemm_oracle(x_nhwc: torch.Tensor, w_krsc: torch.Tensor, stride: i
 
 
 # ------------------------------------------------------------------------------------------------
-# Shuffle store (csrc/gemm_tcgen05.cu: conv2d_nhwc_shuffle_tf32): the phase-packed stride-1 convolution of `dgrad_s2` does not write
+# Shuffle store (csrc/gemm_wgmma.cu: conv2d_nhwc_shuffle_tf32): the phase-packed stride-1 convolution of `dgrad_s2` does not write
 # [N, Ho, Wo, (ph, pw, ci)] and shuffle it afterwards; each 32-row x 32-column epilogue chunk (32 consecutive output pixels of the
 # packed convolution = 32 / Wo whole rows, 32 consecutive packed channels = one phase, channels ci0 .. ci0+31) is ONE bulk tensor
 # store through a 5-D tensor map over the result viewed as {ci, pw, wo, ph, n*Ho + ho} with box {32, 1, Wo, 1, 32 / Wo} at

@@ -1,4 +1,4 @@
-"""Python face of the sm_100a extension (``csrc/``): thin wrappers and the
+"""Python face of the sm_90a extension (``csrc/``): thin wrappers and the
 ``torch.autograd.Function``s that wire the kernels into autograd.
 
 Activation layout on this path: NHWC memory.  Tensors keep their logical NCHW
@@ -7,10 +7,10 @@ fall-backs used for the few ops that have no hand-written kernel yet) sees
 ordinary tensors, while the kernels receive the underlying [N,H,W,C] buffer.
 
 Kernel inventory (SURVEY §2.10 ids):
-  G1  conv2d_nhwc          tcgen05 implicit GEMM (TMA 4-D boxes -> smem -> UMMA.tf32 -> TMEM), BN stats in epilogue
+  G1  conv2d_nhwc          wgmma implicit GEMM (TMA 4-D boxes -> smem -> wgmma tf32 -> registers), BN stats in epilogue
   G2/3 bn_elu_fwd/bwd      BatchNorm(train) + residual + ELU fused, two-pass backward
   G4  avgpool / pool_linear
-  G5  linear_tf32          tcgen05 GEMM with bias+ELU epilogue
+  G5  linear_tf32          wgmma GEMM with bias+ELU epilogue
   G9  cross_entropy        fused log-softmax/NLL fwd, softmax-minus-onehot bwd
   G10 vae_loss             single fused reduction fwd, elementwise bwd
   G14-16 flat ops          adam_prox, penalty, L-BFGS algebra (see flatops.py)
@@ -294,7 +294,7 @@ def _s2_dgrad(e, dy: torch.Tensor, wk: torch.Tensor, trainable: bool, persistent
 
 
 # ----------------------------------------------------------------------------
-# weight gradient on tcgen05 (csrc/wgrad_tcgen05.cuh): MN-major operands straight from the NHWC activations,
+# weight gradient on wgmma (csrc/wgrad_wgmma.cuh): MN-major operands straight from the NHWC activations,
 # split over the pixel range, partial sums red.add-ed into dW
 # ----------------------------------------------------------------------------
 WGRAD = os.environ.get("FEDB200_WGRAD", "1") != "0"
@@ -414,10 +414,9 @@ class _ConvBnAct(torch.autograd.Function):
 
 # ----------------------------------------------------------------------------
 # Identity-shortcut blocks: the gradient that reaches the block input is dgrad(conv1) + d(residual).  Autograd adds
-# the two with a separate elementwise kernel (11 `add` launches, 85 us per step, profiles/r1_run19_*).  Routing the
+# the two with a separate elementwise kernel (one `add` launch per identity block and step).  Routing the
 # block input through the conv1 Function as a second, pass-through output hands BOTH gradients to one backward call,
-# which lets the data-gradient convolution accumulate straight into the residual gradient (read-modify-write epilogue
-# in the weight-stationary kernel, bulk reduce-add in the persistent kernel).  Opt-in: FEDB200_SKIP_FUSED=1.
+# which lets the data-gradient convolution accumulate straight into the residual gradient (bulk reduce-add epilogue).  Opt-in: FEDB200_SKIP_FUSED=1.
 # ----------------------------------------------------------------------------
 SKIP_FUSED = os.environ.get("FEDB200_SKIP_FUSED", "0") == "1"
 
@@ -488,12 +487,12 @@ def conv_bn_act_skip(x, conv: nn.Conv2d, bn: nn.BatchNorm2d):
 
 # ----------------------------------------------------------------------------
 # conv + bias (+ ELU) of the VAE / CPC networks (SURVEY G6, G7, G8) — forward AND backward on hand-written kernels:
-#   forward   implicit GEMM on tcgen05 with bias + ELU in the epilogue (transposed convs: 3x3 conv with 4*C_out phase
+#   forward   implicit GEMM on wgmma with bias + ELU in the epilogue (transposed convs: 3x3 conv with 4*C_out phase
 #             channels + pixel shuffle, ops/conv_math.py)
 #   dz, db    one pass: dout * ELU'(z) recomputed from the saved output + per-channel sums   (act_bwd_bias kernel)
 #   dx        stride-2 4x4: the transposed-conv kernel path with the same weights; stride 1: rotated filter;
 #             transposed conv: the forward stride-2 conv kernel
-#   dw        tcgen05 weight-gradient kernel (wgrad_tcgen05.cuh); for transposed convs with the roles of x and dz swapped
+#   dw        wgmma weight-gradient kernel (wgrad_wgmma.cuh); for transposed convs with the roles of x and dz swapped
 # FEDB200_CONV_ACT=0 restores the ATen / cuDNN composition (A/B runs).
 # ----------------------------------------------------------------------------
 CONV_ACT = os.environ.get("FEDB200_CONV_ACT", "1") != "0"
@@ -616,10 +615,10 @@ def dilated_stem_supported(x: torch.Tensor, convs) -> bool:
 
 
 class _DilatedStem(torch.autograd.Function):
-    """``cat([ELU?(conv_b(x)) for b], 1)`` as ONE tcgen05 implicit GEMM: the filter rows of the launch are (branch, row) pairs,
+    """``cat([ELU?(conv_b(x)) for b], 1)`` as ONE wgmma implicit GEMM: the filter rows of the launch are (branch, row) pairs,
     every branch reads the input through its own dilation / padding (IgemmParams::ms_*), the block-diagonal weight matrix sends
     branch b to its own output channels, bias + ELU in the epilogue, one bulk tensor store per chunk of the concatenated tensor.
-    Backward: one bias+ELU' pass over the concatenated gradient, one tcgen05 weight-gradient launch per branch."""
+    Backward: one bias+ELU' pass over the concatenated gradient, one wgmma weight-gradient launch per branch."""
 
     @staticmethod
     def forward(ctx, x, cfg, *params):
@@ -751,8 +750,8 @@ def conv1x1_linear(x: torch.Tensor, conv: nn.Conv2d, act: bool) -> torch.Tensor:
 
 def unfold_conv_supported(x: torch.Tensor, conv: nn.Module) -> bool:
     """Stride-1 convolutions on tiny maps with many channels (the 2x2 convolutions of the CPC context network on its 3x3 / 4x4
-    latent grid, SURVEY G8): im2col rows [N * Ho * Wo, Ci * k * k] x the dense-layer GEMM kernel with the bias + ELU epilogue.
-    Measured before (direct-convolution kernel, `profiles/r2/r2_call14.log`): 254 us forward / 420 us data gradient for a 75 MFLOP layer."""
+    latent grid, SURVEY G8): im2col rows [N * Ho * Wo, Ci * k * k] x the dense-layer GEMM kernel with the bias + ELU epilogue,
+    which keeps far more threads busy than a direct convolution over a 3x3 / 4x4 map."""
     if not (CONV_ACT and LINEAR_F32) or not isinstance(conv, nn.Conv2d) or isinstance(conv, nn.ConvTranspose2d):
         return False
     if x.dim() != 4 or x.dtype != torch.float32 or conv.groups != 1 or conv.padding_mode != "zeros" or isinstance(conv.padding, str):
@@ -768,7 +767,7 @@ def unfold_conv(x: torch.Tensor, conv: nn.Conv2d, act: bool) -> torch.Tensor:
     N, C, H, W = x.shape
     kh, kw = conv.kernel_size
     Ho, Wo = H + 2 * conv.padding[0] - kh + 1, W + 2 * conv.padding[1] - kw + 1
-    # im2col as ONE strided copy (F.unfold launches an im2col kernel per sample: 1024 launches per two CPC steps, r2_call15.log)
+    # im2col as ONE strided copy (F.unfold launches an im2col kernel per sample)
     xp = F.pad(x, (conv.padding[1], conv.padding[1], conv.padding[0], conv.padding[0])) if (conv.padding[0] or conv.padding[1]) else x
     rows = xp.unfold(2, kh, 1).unfold(3, kw, 1).permute(0, 2, 3, 1, 4, 5).reshape(N * Ho * Wo, C * kh * kw)
     out = _LinearAct.apply(rows, conv.weight.reshape(conv.out_channels, C * kh * kw), conv.bias, bool(act))
@@ -806,7 +805,7 @@ class _AvgPoolNHWC(torch.autograd.Function):
         return dx.permute(0, 3, 1, 2)
 
 
-HEAD_FUSED = os.environ.get("FEDB200_HEAD_FUSED", "1") != "0"   # confirmed on a B200 (profiles/r2_*): default on
+HEAD_FUSED = os.environ.get("FEDB200_HEAD_FUSED", "1") != "0"   # default on
 
 
 def _dense_wgrad(dz: torch.Tensor, x: torch.Tensor, wparam) -> Optional[torch.Tensor]:
@@ -859,7 +858,7 @@ def pool_linear(x, linear: nn.Linear, window: int) -> torch.Tensor:
 # ----------------------------------------------------------------------------
 # dense layers (SURVEY G5).  Default: hand-written TRUE-fp32 kernels (the reference's nn.Linear precision, any shape:
 # 128x10x512 classifier, 400->120->84->10 of Net, the VAE / VAE-CL heads) with bias + ELU in the GEMM epilogue;
-# FEDB200_TF32_LINEAR=1 routes 16-byte aligned layers to the tcgen05 GEMM (TF32 products) instead.
+# FEDB200_TF32_LINEAR=1 routes 16-byte aligned layers to the wgmma GEMM (TF32 products) instead.
 # ----------------------------------------------------------------------------
 LINEAR_F32 = os.environ.get("FEDB200_LINEAR_F32", "1") != "0"
 

@@ -1,6 +1,6 @@
 """Level-1 algebra on flat parameter vectors (SURVEY G14-G16, G20).
 
-Every routine has the sm_100a implementation in ``csrc/flat_kernels.cu``
+Every routine has the sm_90a implementation in ``csrc/flat_kernels.cu``
 (reached through :mod:`.cuda_ops` for CUDA tensors) and the ATen composition
 below, which is also the oracle the kernels are tested against.
 

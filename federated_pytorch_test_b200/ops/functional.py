@@ -2,9 +2,9 @@
 
 Each function has exactly two implementations:
 
-* the sm_100a path in :mod:`..ops.cuda_ops` (hand-written kernels from
+* the sm_90a path in :mod:`..ops.cuda_ops` (hand-written kernels from
   ``csrc/``), selected when the tensors live on a CUDA device and the fast
-  path is enabled (default on a B200);
+  path is enabled (default on an H100);
 * the ATen composition below, used on CPU (tests, plumbing runs) and as the
   numerical oracle for the kernels.
 
@@ -86,7 +86,7 @@ def pool_linear(x: torch.Tensor, linear: nn.Linear, window: int = 4) -> torch.Te
 
 def conv_act(x: torch.Tensor, conv: nn.Module, act: bool = True) -> torch.Tensor:
     """``ELU?(conv(x))`` for the bias-carrying convs / transposed convs of the VAE and CPC nets
-    (/root/reference/src/simple_models.py:249-265, :441-451, :478-481, :503-504).  On B200: tcgen05 implicit GEMM with bias +
+    (/root/reference/src/simple_models.py:249-265, :441-451, :478-481, :503-504).  On the GPU: wgmma implicit GEMM with bias +
     ELU in the epilogue and hand-written backward kernels (cuda_ops._ConvAct); 1x1 convs on odd-sized latent grids run
     on the dense-layer GEMM kernels, other small convs on the direct-convolution kernel."""
     if _use_fast(x):
@@ -106,7 +106,7 @@ def conv_act(x: torch.Tensor, conv: nn.Module, act: bool = True) -> torch.Tensor
 
 def dilated_stem(x: torch.Tensor, convs, act: bool = True) -> torch.Tensor:
     """``cat([ELU?(conv(x)) for conv in convs], 1)`` for convolutions that differ only in dilation / padding — the five-branch
-    stem of the CPC encoder (/root/reference/src/simple_models.py:455-460).  On B200 ONE tcgen05 launch reads the input once per
+    stem of the CPC encoder (/root/reference/src/simple_models.py:455-460).  On the GPU ONE wgmma launch reads the input once per
     tap and writes the concatenated tensor (cuda_ops._DilatedStem); elsewhere branch by branch."""
     if _use_fast(x):
         from . import cuda_ops
@@ -119,7 +119,7 @@ def dilated_stem(x: torch.Tensor, convs, act: bool = True) -> torch.Tensor:
 def conv_act_pool(x: torch.Tensor, conv: nn.Conv2d, act: bool = True, pool: bool = False) -> torch.Tensor:
     """``max_pool2d?(ELU?(conv(x)), 2, 2)`` — one stage of Net / Net1 / Net2 (/root/reference/src/simple_models.py:19-21,
     :60-66, :103-110).  Net / Net1 (3..64 channels, 5x5 / 3x3 "valid" convs on 28/10-wide maps): ONE direct-convolution
-    kernel with bias, ELU and the pooling fused; Net2 (padded 3x3, 64..512 channels): tcgen05 conv + NHWC max-pool kernel."""
+    kernel with bias, ELU and the pooling fused; Net2 (padded 3x3, 64..512 channels): wgmma conv + NHWC max-pool kernel."""
     if _use_fast(x):
         from . import cuda_ops
 
@@ -151,8 +151,8 @@ def global_avg_pool(x: torch.Tensor) -> torch.Tensor:
 
 
 def linear_act(x: torch.Tensor, linear: nn.Linear, act: bool = True) -> torch.Tensor:
-    """``ELU?(x @ W^T + b)``; on B200 one hand-written GEMM kernel with the bias + ELU epilogue (true fp32 by default —
-    the reference's nn.Linear precision; FEDB200_TF32_LINEAR=1: tcgen05) and hand-written backward kernels."""
+    """``ELU?(x @ W^T + b)``; on the GPU one hand-written GEMM kernel with the bias + ELU epilogue (true fp32 by default —
+    the reference's nn.Linear precision; FEDB200_TF32_LINEAR=1: wgmma) and hand-written backward kernels."""
     if _use_fast(x):
         from . import cuda_ops
 

@@ -4,7 +4,7 @@ The reference evaluates the VAE-CL costs with Python loops over the batch
 (/root/reference/src/federated_vae_cl.py:101-140: ~5 000 tiny kernels per step)
 and InfoNCE with a P^2 loop of ``torch.dot`` (federated_cpc.py:161-178).  The
 same quantities are computed here as a few batched tensor expressions — and, on
-B200, as single fused kernels (``csrc/loss_kernels.cu``) behind
+the GPU, as single fused kernels (``csrc/loss_kernels.cu``) behind
 ``torch.autograd.Function``s.  The ``*_reference`` variants are literal
 transcriptions of the math with loops, kept as test oracles.
 """
@@ -66,7 +66,7 @@ def vae_cl_costs(ekhat, mu_xi, sig2_xi, mu_b, sig2_b, mu_th, sig2_th, x) -> Tupl
     mu_th, sig2_th = _stack(mu_th, Kc), _stack(sig2_th, Kc)   # [Kc,B,3,32,32]
     mu_xi, sig2_xi = _stack(mu_xi, Kc), _stack(sig2_xi, Kc)   # [Kc,B,L]
     mu_b, sig2_b = _stack(mu_b, Kc), _stack(sig2_b, Kc)
-    # c1: E_q(k)[ -log p(x|theta) ]  (weighted Gaussian NLL).  On B200 the [Kc, B, 3072] -> [Kc, B] reduction (the only
+    # c1: E_q(k)[ -log p(x|theta) ]  (weighted Gaussian NLL).  On the GPU the [Kc, B, 3072] -> [Kc, B] reduction (the only
     # large tensors of this loss: 2 x 15.7 MB at Kc = 10, B = 128) is ONE kernel forward and one backward (SURVEY G11).
     if x.is_cuda and FX.fast_path_enabled() and x.dtype == torch.float32:
         from . import cuda_ops

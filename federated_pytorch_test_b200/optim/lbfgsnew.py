@@ -17,7 +17,7 @@ Implementation is new and flat-vector based:
   ``torch.cat``s, lbfgsnew.py:81-121);
 * curvature pairs live in two ``[history, n]`` ring buffers; the two-loop
   recursion, the pair update and the Welford update go through
-  :mod:`..ops.flatops`, which on a B200 are fused sm_100a kernels with
+  :mod:`..ops.flatops`, which on an H100 are fused sm_90a kernels with
   device-resident scalars (SURVEY G16) and otherwise ATen;
 * every host decision of one inner iteration reads its scalars in one batch.
 

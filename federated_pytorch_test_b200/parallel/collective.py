@@ -16,7 +16,7 @@ parameter arenas).  :class:`TorchCollective` implements them with ATen (+ a
 ``torch.distributed`` all-reduce across processes: Gloo on CPU, NCCL on GPUs) —
 this is the *baseline* and the test oracle.  :class:`FusedCollective`
 (``parallel/fused.py``) implements the same interface with the hand-written
-sm_100a kernels that reduce straight out of peer memory over NVLink.
+sm_90a kernels that reduce straight out of peer memory over NVLink.
 """
 from __future__ import annotations
 
@@ -171,7 +171,7 @@ class TorchCollective:
 
 
 def make_collective(topo: Topology, kind: str = "auto"):
-    """``kind``: 'torch' (baseline), 'fused' (sm_100a kernels; error if unavailable), 'auto'."""
+    """``kind``: 'torch' (baseline), 'fused' (sm_90a kernels; error if unavailable), 'auto'."""
     if kind == "torch":
         return TorchCollective(topo)
     want_fused = kind == "fused" or (kind == "auto" and topo.device.type == "cuda")

@@ -1,4 +1,4 @@
-"""``FusedCollective`` — the block collectives as ONE sm_100a kernel each, reducing
+"""``FusedCollective`` — the block collectives as ONE sm_90a kernel each, reducing
 straight out of peer memory over NVLink (``csrc/comm_kernels.cu``).  No NCCL on this path.
 
 Reference loops being replaced (Python loops over a dict of K modules): FedAvg mean + write-back + dual residual
@@ -155,8 +155,8 @@ class FusedCollective(TorchCollective):
         self.ctrl = self.heap.alloc(_PAD_WORDS, dtype=torch.int32)
         self.ctrl_ptrs = list(self.heap.locate(self.ctrl)[0]["peer_ptrs"])
         self._aux: Dict[Tuple[int, str], torch.Tensor] = {}
-        # in-switch reduction pays from 4 peers on; between 2 GPUs the P2P variant of the same kernel is faster (nothing to reduce
-        # in the switch: 58.5 vs 77.3 us at 18.9 MB, profiles/r2_collective.md).  FEDB200_MULTIMEM=0|1 forces either.
+        # in-switch reduction pays from 4 peers on; between 2 GPUs there is nothing to reduce in the switch and the P2P variant of
+        # the same kernel is used.  FEDB200_MULTIMEM=0|1 forces either.
         mm = os.environ.get("FEDB200_MULTIMEM", "auto")
         self.default_multimem = (topo.world_size > 2) if mm == "auto" else (mm != "0")
         self.use_multimem = self.default_multimem
@@ -169,8 +169,8 @@ class FusedCollective(TorchCollective):
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
-        cross-rank handshake happen here, at engine construction, not inside the first training round (measured: the
-        first launch costs ~10 ms).  Collective: every rank calls it at the same point."""
+        cross-rank handshake happen here, at engine construction, not inside the first training round (the first launch
+        is far slower than the ones after it).  Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
         self._warm = True

@@ -9,8 +9,7 @@ aggregation are launched on W streams and meet at their barriers while co-reside
 (``max_blocks``) so that all of them fit on the chip at once, and the barrier timeout is short, so a scheduling
 accident surfaces as ``CollectiveTimeout`` instead of a hang.
 
-Used by ``tests/test_gpu_loopback.py`` (single-GPU box: the driver's ``pytest -m gpu`` run) and by
-``tools/bench_collective.py --loopback``.
+Used by ``tests/test_gpu_loopback.py``, which runs the fused collectives on a single GPU.
 """
 from __future__ import annotations
 

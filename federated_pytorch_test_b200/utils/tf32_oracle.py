@@ -1,9 +1,9 @@
 """A float64 oracle for networks whose convolutions run on the TF32 tensor cores.
 
-``tcgen05.mma.kind::tf32`` reads fp32 operands and uses their upper 19 bits (sign, 8 exponent, 10 mantissa bits); products
+The tensor core's tf32 MMA reads fp32 operands and uses their upper 19 bits (sign, 8 exponent, 10 mantissa bits); products
 are exact and accumulated in fp32.  Comparing such a network with a plain fp64 oracle mixes two things: the 2^-11 operand
 rounding itself and — in networks with max-pooling — the pool winners that this rounding flips, each of which moves a
-gradient term (a few per cent of a conv weight gradient in Net2, tools/diag_net2_tf32.py).  This oracle reproduces the
+gradient term (a few per cent of a conv weight gradient in Net2).  This oracle reproduces the
 operand rounding in all three products of a convolution (forward, data gradient, weight gradient) and evaluates
 everything else in float64, so that a kernel bug (wrong tap, wrong layout, missing term) still shows up at 1e-2..1
 while the expected TF32 behaviour cancels.

@@ -30,7 +30,7 @@ def test_cli_overrides():
     assert c.use_resnet is False and c.Nloop == 2
 
 
-def test_legacy_checkpoint_interop(tmp_path, ref_models):
+def test_legacy_checkpoint_interop(tmp_path, golden):
     net = models.Net()
     FlatArena(net)
     opt = torch.optim.Adam(net.parameters())
@@ -38,14 +38,16 @@ def test_legacy_checkpoint_interop(tmp_path, ref_models):
     assert os.path.basename(path) == "s3.model"
     blob = torch.load(path, weights_only=False)
     assert sorted(blob) == ["epoch", "model_state_dict", "optimizer_state_dict", "running_loss"]
-    ref = ref_models.Net()
-    ref.load_state_dict(blob["model_state_dict"])          # the reference can read our file
-    x = torch.randn(2, 3, 32, 32)
-    torch.testing.assert_close(ref(x), net(x))
-    torch.save({"model_state_dict": ref_models.Net().state_dict(), "epoch": 0, "optimizer_state_dict": {}, "running_loss": 0.0},
+    layout = golden["net_state_layout"]                     # the original Net's state-dict keys and shapes
+    assert [(k, tuple(v.shape)) for k, v in blob["model_state_dict"].items()] == layout   # the original can read our file
+    g = torch.Generator().manual_seed(3)
+    theirs = {k: torch.randn(shape, generator=g) for k, shape in layout}
+    torch.save({"model_state_dict": theirs, "epoch": 0, "optimizer_state_dict": {}, "running_loss": 0.0},
                ckpt.worker_path(str(tmp_path), 4))
     ckpt.load_worker(str(tmp_path), 4, net, "cpu")          # and we can read the reference's
     assert net._flat_arena.check_views() and net.training
+    for k, v in net.state_dict().items():                   # and we can read the original's
+        torch.testing.assert_close(v, theirs[k])
 
 
 def test_log_formats_golden():

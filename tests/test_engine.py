@@ -1,4 +1,4 @@
-"""End-to-end engine tests on CPU: driver smoke runs (BASELINE.json config 1), parity of one
+"""End-to-end engine tests on CPU: driver smoke runs (benchmark configuration 1, bench.py), parity of one
 block visit against a literal reference-style loop, multi-process (gloo) == single-process."""
 import os
 import sys
@@ -22,7 +22,7 @@ def _run(mod, **kw):
 
 
 def test_no_consensus_simplecnn_k2_cpu():
-    """BASELINE.json config 1: no_consensus_multi SimpleCNN K=2 on CPU."""
+    """Benchmark configuration 1 (bench.py): no_consensus_multi SimpleCNN K=2 on CPU."""
     eng, lines = _run(no_consensus_multi, K=2, Nepoch=2, max_minibatches=4, check_results=True, use_cuda=False)
     assert lines[0] == "Epoch 0" and lines[-1] == "Finished Training"
     assert sum(l.startswith("Accuracy of the network") for l in lines) == 4
@@ -106,27 +106,27 @@ def test_vae_vaecl_cpc_drivers(tmp_path):
 
 
 # ----------------------------------------------------------------------------------------------
-def test_block_visit_matches_reference_style_loop(ref_utils, ref_models):
-    """One ADMM block visit: BlockAdam + closed-form penalty on arena slices  ==  the reference recipe
-    (torch.optim.Adam + autograd through torch.cat, get/put_trainable_values) on the same batches."""
-    from federated_pytorch_test_b200.algo.engine import Engine, EngineConfig, Replica, Task, Visit
-    from federated_pytorch_test_b200.algo.strategies import ADMM
-    from federated_pytorch_test_b200.parallel import Topology, TorchCollective
-    from federated_pytorch_test_b200.utils import init_weights
+BV_K, BV_B, BV_STEPS, BV_ROUNDS, BV_RHO, BV_CI, BV_LAM1, BV_LAM2 = 2, 16, 3, 2, 0.1, 4, 1e-4, 1e-4
 
-    K, B, steps, rounds, rho, ci = 2, 16, 3, 2, 0.1, 4
+
+def _block_visit_data():
     g = torch.Generator().manual_seed(0)
-    data = {k: [(torch.randn(B, 3, 32, 32, generator=g), torch.randint(0, 10, (B,), generator=g)) for _ in range(steps)] for k in range(K)}
-    lam1, lam2 = 1e-4, 1e-4
+    return {k: [(torch.randn(BV_B, 3, 32, 32, generator=g), torch.randint(0, 10, (BV_B,), generator=g)) for _ in range(BV_STEPS)]
+            for k in range(BV_K)}
 
-    # ---- reference-style ----
+
+def reference_style_block_visit(rm, ru):
+    """The original recipe (torch.optim.Adam + autograd through torch.cat, get/put_trainable_values) with the original
+    models / utilities ``rm`` / ``ru``: the (primal, dual) trace and the final block values.  Run by oracle/make_golden.py."""
+    K, steps, rounds, rho, ci, lam1, lam2 = BV_K, BV_STEPS, BV_ROUNDS, BV_RHO, BV_CI, BV_LAM1, BV_LAM2
+    data = _block_visit_data()
     nets = {}
     for k in range(K):
-        nets[k] = ref_models.Net()
+        nets[k] = rm.Net()
         torch.manual_seed(0)
-        nets[k].apply(ref_utils.init_weights)
-        ref_utils.unfreeze_one_block(nets[k], ci)
-    N = ref_utils.get_trainable_values(nets[0]).numel()
+        nets[k].apply(ru.init_weights)
+        ru.unfreeze_one_block(nets[k], ci)
+    N = ru.get_trainable_values(nets[0]).numel()
     z = torch.zeros(N)
     ys = {k: torch.zeros(N) for k in range(K)}
     opts = {k: torch.optim.Adam(filter(lambda p: p.requires_grad, nets[k].parameters()), lr=1e-3) for k in range(K)}
@@ -141,7 +141,7 @@ def test_block_visit_matches_reference_style_loop(ref_utils, ref_models):
                 loss = loss + lam1 * torch.norm(vec, 1) + lam2 * torch.norm(vec, 2) ** 2   # block 4 of Net is gated on
                 loss.backward()
                 opts[k].step()
-        xs = {k: ref_utils.get_trainable_values(nets[k]) for k in range(K)}
+        xs = {k: ru.get_trainable_values(nets[k]) for k in range(K)}
         znew = sum(ys[k] + rho * xs[k] for k in range(K)) / (K * rho)
         dual = float(torch.norm(z - znew)) / N
         z = znew
@@ -151,6 +151,21 @@ def test_block_visit_matches_reference_style_loop(ref_utils, ref_models):
             primal += float(torch.norm(yd))
             ys[k].add_(yd)
         ref_trace.append((primal / N, dual))
+    return {"trace": ref_trace, "final": [ru.get_trainable_values(nets[k]).detach().clone() for k in range(K)]}
+
+
+def test_block_visit_matches_reference_style_loop(golden):
+    """One ADMM block visit: BlockAdam + closed-form penalty on arena slices  ==  the original recipe on the same
+    batches (its stored trace and final values)."""
+    from federated_pytorch_test_b200.algo.engine import Engine, EngineConfig, Replica, Task, Visit
+    from federated_pytorch_test_b200.algo.strategies import ADMM
+    from federated_pytorch_test_b200.parallel import Topology, TorchCollective
+    from federated_pytorch_test_b200.utils import init_weights
+
+    K, rounds, rho, ci, lam1, lam2 = BV_K, BV_ROUNDS, BV_RHO, BV_CI, BV_LAM1, BV_LAM2
+    data = _block_visit_data()
+    ref = golden["block_visit"]
+    ref_trace = ref["trace"]
 
     # ---- engine ----
     class FixedTask(Task):
@@ -185,7 +200,7 @@ def test_block_visit_matches_reference_style_loop(ref_utils, ref_models):
     lo, hi = models.Net().train_order_block_ids()[ci]
     for k in range(K):
         mine = eng.replicas[k].arenas["net"].compact(lo, hi)
-        torch.testing.assert_close(mine, ref_utils.get_trainable_values(nets[k]), rtol=1e-3, atol=1e-5)
+        torch.testing.assert_close(mine, ref["final"][k], rtol=1e-3, atol=1e-5)
 
 
 # ----------------------------------------------------------------------------------------------

@@ -218,7 +218,7 @@ def test_net_fast_path_matches_fp64_oracle(name):
     """Net / Net1 run entirely in true fp32 on the fast path (direct convolutions with ELU + max-pool fused, fp32 dense kernels).
     The input seed is fixed: a max-pool winner that is a near-tie at fp32 resolution may be resolved differently by an fp64
     oracle, which moves one term of a conv weight gradient (~1 % of an entry) — a property of the comparison, not of the kernels
-    (tools/diag_net_seeds.py; the layer-level tests above pin the kernels at 1e-4)."""
+    (the layer-level tests above pin the kernels at 1e-4)."""
     torch.manual_seed(1000)
     x = torch.randn(32, 3, 32, 32, device=DEV)
     y = torch.randint(0, 10, (32,), device=DEV)
@@ -231,8 +231,8 @@ def _l2_err(u, v):
 
 def test_net2_fast_path_vs_fp64_oracles():
     """Net2's convolutions run on the TF32 tensor cores.  A plain fp64 oracle disagrees with that by MORE than TF32's 2^-11:
-    the operand rounding flips ~0.02 % of the 2x2 max-pool winners (measured per stage: 92 / 68 / 42 / 11 windows at batch 32,
-    tools/diag_net2_tf32.py, profiles/r2/r2_call14.log) and every flip moves one term of the upstream gradients, which shows up
+    the operand rounding flips a small fraction of the 2x2 max-pool winners and every flip moves one term of the upstream
+    gradients, which shows up
     as 2-6 % relative L2 error in the conv weight gradients while everything downstream of the last pool (conv4.bias, fc*) agrees
     to 5e-4.  An oracle that rounds the conv operands to TF32 (round-to-nearest) removes 2/3 of that.  (ATen / cuDNN on this
     image does not take a plain-TF32 path for these shapes — its error against fp64 is 1e-4 — so it is no yardstick either.)

@@ -1,4 +1,4 @@
-"""Every entry point end to end on the GPU through the fast path (fused collectives, sm_100a kernels, CUDA graphs
+"""Every entry point end to end on the GPU through the fast path (fused collectives, sm_90a kernels, CUDA graphs
 where applicable).  Small configurations; the point is coverage of the CUDA code paths of all seven drivers."""
 import os
 
@@ -48,7 +48,7 @@ def test_consensus_admm_bb_resnet_fused():
 
 
 def test_fedprox_lbfgs_resnet():
-    """BASELINE.json config 4 (fedprox_multi + LBFGSNew) in miniature."""
+    """Benchmark configuration 4 (fedprox_multi + LBFGSNew, bench.py) in miniature."""
     eng, lines = _run(fedprox_multi, K=2, Nloop=1, Nadmm=1, max_minibatches=1, check_results=False, model="ResNet9",
                       default_batch=32, optimizer="lbfgs", graphs=False)
     assert len([l for l in lines if l.startswith("block=[")]) == 8

@@ -1,10 +1,10 @@
 """GPU checks of code paths that started as opt-in switches in round 1.
 
-Now DEFAULT (confirmed on B200, round 2: kernel tests, the three VAE / CPC drivers, bench): conv + bias + ELU of the VAE /
+Now DEFAULT (kernel tests, the three VAE / CPC drivers, bench): conv + bias + ELU of the VAE /
 CPC networks and the transposed-conv decomposition, forward AND backward on hand-written kernels (``FEDB200_CONV_ACT``);
 the fused classifier head (``FEDB200_HEAD_FUSED``).  These tests run in every ``-m gpu`` session.
 
-Still opt-in (measured neutral or slower inside the captured step, profiles/r2_switches.md): ``FEDB200_BN_BWD_FUSED=1``,
+Still opt-in: ``FEDB200_BN_BWD_FUSED=1``,
 ``FEDB200_SKIP_FUSED=1``; their tests run only when the switch is set:
 
     FEDB200_SKIP_FUSED=1 python -m pytest tests/test_gpu_experimental.py -m gpu -q -k "identity_block or accumulating"

@@ -1,5 +1,5 @@
-"""Numerics of every hand-written sm_100a kernel against a plain PyTorch fp32 reference of the same op.
-Run on the B200 box: ``python -m pytest tests -m gpu``."""
+"""Numerics of every hand-written sm_90a kernel against a plain PyTorch fp32 reference of the same op.
+Run on an H100: ``python -m pytest tests -m gpu``."""
 import math
 
 import pytest
@@ -37,7 +37,7 @@ def rel_err(a, b):
 def test_extension_is_native_and_loaded():
     e = cuda_ops.ext()
     assert e.__file__.endswith(".so") and "federated_pytorch_test_b200/_build" in e.__file__
-    assert torch.cuda.get_device_capability(0)[0] == 10, "these kernels are sm_100a only"
+    assert torch.cuda.get_device_capability(0) == (9, 0), "these kernels are sm_90a only"
 
 
 # ------------------------------------------------------------------------------------------ flat ops
@@ -310,8 +310,8 @@ def test_resnet18_fast_path_matches_aten_and_respects_freezing():
         lb = F.cross_entropy(b(x), y)
         lb.backward()
         FX.set_fast_path(True)
-        # error budget measured on a B200 (tools/measure_resnet_err.py, profiles/r2/r2_call5.log): whole-network gradients of
-        # the tf32 fast path vs an fp64 oracle 1.0e-3 ... 2.7e-3 (cuDNN with TF32 on: the same 1.0e-3 ... 2.8e-3), loss 5e-5
+        # error budget: whole-network gradients of the tf32 fast path vs an fp64 oracle are ~1e-3 ... 3e-3, like cuDNN with
+        # TF32 on; the loss agrees to ~5e-5
         assert float(la) == pytest.approx(float(lb), rel=1e-3)
         for (n, pa), (_, pb) in zip(a.named_parameters(), b.named_parameters()):
             assert (pa.grad is None) == (pb.grad is None), n
@@ -419,27 +419,40 @@ def test_host_resident_loader_matches_device_resident():
 
 # ------------------------------------------------------------------------------------------ conv kernel variants
 VARIANT_ENVS = [
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1"),                       # generic single-CTA kernel
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_KPS="1"),      # one k-block per pipeline stage
+    # Switches of the Blackwell kernels that have no Hopper counterpart (KPS, MT, CLUSTER, 2CTA, HALO, WS) select nothing
+    # here: those sets run the default wgmma kernel on the same shapes.
+    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1"),                       # one K slice: statistics fused in the epilogue
+    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_KPS="1"),
     dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_PERSIST="0"),  # one tile per CTA (non-persistent)
     dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="2", FEDB200_BLOCK_N="64"), # persistent, several tiles per CTA, split-K
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_MT="2"),       # 256-row CTA tiles (two accumulators share B)
+    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_MT="2"),
     dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_MT="1"),
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="2", FEDB200_MT="2", FEDB200_BLOCK_N="256"),  # single TMEM stage
+    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="2", FEDB200_MT="2", FEDB200_BLOCK_N="256"),  # 256: widest tile (128)
     dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_MT="2", FEDB200_BLOCK_N="64"),
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="4"),                       # split-K with red.global.add
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_CLUSTER="4"),  # weight-tile TMA multicast
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_2CTA="1"),     # cta_group::2 pairs
-    dict(FEDB200_WS="0", FEDB200_HALO="2"),                                           # halo tile, one box for 9 taps
-    dict(FEDB200_WS="1"),                                                             # weight-stationary persistent
+    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="4"),                       # split-K with bulk reduce-adds
+    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_CLUSTER="4"),
+    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_2CTA="1"),
+    dict(FEDB200_WS="0", FEDB200_HALO="2"),
+    dict(FEDB200_WS="1"),
+    # choices of the wgmma kernel
+    dict(),                                                                           # defaults
+    dict(FEDB200_SPLITK="8", FEDB200_BLOCK_N="32"),
+    dict(FEDB200_SPLITK="1", FEDB200_BLOCK_N="32"),                                   # 64 x 32 wgmma tiles
+    dict(FEDB200_SPLITK="2", FEDB200_BLOCK_N="128"),
+    dict(FEDB200_SPLITK="2", FEDB200_PERSIST="0"),
+    dict(FEDB200_SPLITK="1", FEDB200_TMA_STORE="0"),                                  # direct stores from the accumulator fragments
+    dict(FEDB200_SPLITK="2", FEDB200_TMA_STORE="0"),                                  # split-K through atomics
+    dict(FEDB200_TAP_PACK="0"),                                                       # one tap per k-block at C_in = 4
+    dict(FEDB200_TAP_PACK="0", FEDB200_BLOCK_N="32"),
 ]
 
 
-@pytest.mark.parametrize("env", VARIANT_ENVS, ids=lambda e: ",".join("%s=%s" % (k[8:], v) for k, v in e.items()))
+@pytest.mark.parametrize("env", VARIANT_ENVS, ids=lambda e: ",".join("%s=%s" % (k[8:], v) for k, v in e.items()) or "defaults")
 @pytest.mark.parametrize("B,H,Ci,Co", [(5, 32, 64, 64), (3, 32, 4, 64), (6, 16, 128, 128), (16, 8, 256, 256), (20, 32, 64, 64)])
 def test_conv_kernel_variants(monkeypatch, env, B, H, Ci, Co):
     import os
-    for k in ("FEDB200_WS", "FEDB200_HALO", "FEDB200_SPLITK", "FEDB200_CLUSTER", "FEDB200_2CTA", "FEDB200_BLOCK_N", "FEDB200_KPS", "FEDB200_PERSIST", "FEDB200_MT"):
+    for k in ("FEDB200_WS", "FEDB200_HALO", "FEDB200_SPLITK", "FEDB200_CLUSTER", "FEDB200_2CTA", "FEDB200_BLOCK_N", "FEDB200_KPS",
+              "FEDB200_PERSIST", "FEDB200_MT", "FEDB200_TMA_STORE", "FEDB200_TAP_PACK"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)

@@ -1,5 +1,5 @@
 """Multi-GPU: the fused NVLink collectives across processes (one rank per GPU) against NCCL all-reduce.
-Needs >= 2 GPUs (``gpurun --gpus 2``); skipped otherwise."""
+Needs >= 2 GPUs; skipped otherwise."""
 import os
 
 import pytest

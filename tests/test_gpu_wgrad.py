@@ -1,7 +1,7 @@
-"""Weight gradient on tcgen05 (csrc/wgrad_tcgen05.cuh: MN-major operands, pixel-range split, red.add epilogue) against
+"""Weight gradient on wgmma (csrc/wgrad_wgmma.cuh: operands gathered K-major, pixel-range split, red.add epilogue) against
 an fp64 PyTorch oracle — every ResNet18 site, the VAE / CPC sites (4x4 stride 2, dilated, channel counts that are not
 multiples of 32), odd geometries (3x3 latent grid, batch not a multiple of the pixel box) and the in-place
-accumulation into a gradient buffer.  Reference sites: /root/reference/src/simple_models.py:137-147,191,249-265,441-451."""
+accumulation into a gradient buffer.  Sites: the ResNet18, VAE and CPC convolutions of the original models."""
 import pytest
 import torch
 

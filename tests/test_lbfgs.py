@@ -1,4 +1,4 @@
-"""LBFGSNew against the reference implementation (SURVEY §2.5, §4)."""
+"""LBFGSNew against the original implementation (SURVEY §2.5, §4): its stored trajectories (tests/golden)."""
 import warnings
 
 import pytest
@@ -34,12 +34,12 @@ def _rosenbrock(cls):
 def test_rosenbrock_golden():
     x, calls, iters, evals = _rosenbrock(LBFGSNew)
     torch.testing.assert_close(x, torch.tensor([1.0, 1.0]), atol=1e-5, rtol=0)
-    assert (calls, iters) == (655, 31)  # BASELINE.md §2
+    assert (calls, iters) == (655, 31)  # the original LBFGSNew on this problem
 
 
-def test_rosenbrock_identical_to_reference(ref_lbfgs):
-    a, b = _rosenbrock(ref_lbfgs.LBFGSNew), _rosenbrock(LBFGSNew)
-    assert torch.equal(a[0], b[0]) and a[1:] == b[1:]
+def test_rosenbrock_identical_to_reference(golden):
+    a, b = golden["lbfgs"]["rosenbrock"], _rosenbrock(LBFGSNew)
+    assert torch.equal(a[0], b[0]) and tuple(a[1:]) == tuple(b[1:])
 
 
 def _stochastic(cls, arena=False, steps=5):
@@ -70,19 +70,19 @@ def _stochastic(cls, arena=False, steps=5):
     return log, vec, opt
 
 
-def test_stochastic_identical_to_reference(ref_lbfgs):
-    a, b = _stochastic(ref_lbfgs.LBFGSNew), _stochastic(LBFGSNew)
-    assert [x[1:] for x in a[0]] == [x[1:] for x in b[0]]          # forward/backward counts per step
-    assert torch.equal(a[1], b[1])                                 # bit-identical iterates
-    ka = sorted(a[2].state_dict()["state"][0].keys())
-    kb = sorted(b[2].state_dict()["state"][0].keys())
-    assert ka == kb
+def test_stochastic_identical_to_reference(golden):
+    a, b = golden["lbfgs"], _stochastic(LBFGSNew)
+    assert [tuple(x) for x in a["stochastic_counts"]] == [x[1:] for x in b[0]]   # forward/backward counts per step
+    # the whole iterate: bit-identical on the CPU the golden data was recorded on; on another CPU the float rounding of its
+    # convolution kernels (~1e-7) is all that may differ
+    torch.testing.assert_close(b[1], a["stochastic_vec"], rtol=1e-5, atol=1e-7)
+    assert a["state_keys"] == sorted(b[2].state_dict()["state"][0].keys())
 
 
-def test_stochastic_on_arena_close_to_reference(ref_lbfgs):
-    a, c = _stochastic(ref_lbfgs.LBFGSNew), _stochastic(LBFGSNew, arena=True)
-    assert [x[1:] for x in a[0]] == [x[1:] for x in c[0]]
-    torch.testing.assert_close(a[1], c[1], rtol=1e-4, atol=1e-5)
+def test_stochastic_on_arena_close_to_reference(golden):
+    a, c = golden["lbfgs"], _stochastic(LBFGSNew, arena=True)
+    assert [tuple(x) for x in a["stochastic_counts"]] == [x[1:] for x in c[0]]
+    torch.testing.assert_close(c[1], a["stochastic_vec"], rtol=1e-4, atol=1e-5)
     assert c[2]._v().fused
 
 

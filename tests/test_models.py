@@ -1,4 +1,5 @@
-"""Model zoo: shapes, parameter/block inventory (SURVEY §2.2) and forward parity with the reference."""
+"""Model zoo: shapes, parameter/block inventory (SURVEY §2.2) and forward parity with the original models (stored
+outputs of the original code on the same seeded weights and inputs: tests/golden, oracle/make_golden.py)."""
 import pytest
 import torch
 
@@ -48,66 +49,67 @@ PAIRS = [("Net", lambda m: m.Net(), (4, 3, 32, 32)), ("Net1", lambda m: m.Net1()
 
 
 @pytest.mark.parametrize("name,make,shape", PAIRS)
-def test_forward_matches_reference(ref_models, name, make, shape):
-    """Same state_dict keys, and identical outputs when given the reference's weights."""
+def test_forward_matches_reference(golden, fill, name, make, shape):
+    """Same state_dict keys, and the original's outputs for the same weights and input, in train mode (BatchNorm on batch
+    statistics) and in eval mode (running statistics)."""
     FX.set_fast_path(False)
-    torch.manual_seed(0)
-    ref = make(ref_models)
-    mine = make(models)
-    assert list(ref.state_dict().keys()) == list(mine.state_dict().keys())
-    mine.load_state_dict(ref.state_dict())
-    x = torch.randn(*shape)
-    torch.testing.assert_close(mine(x), ref(x), rtol=1e-5, atol=1e-5)
+    ref = golden["forward"][name]
+    mine = fill(make(models))
+    assert list(mine.state_dict().keys()) == ref["keys"]
+    x = torch.randn(*shape, generator=torch.Generator().manual_seed(1))
+    with torch.no_grad():
+        torch.testing.assert_close(mine.train()(x), ref["y_train"], rtol=1e-5, atol=1e-5)
+        fill(mine)
+        torch.testing.assert_close(mine.eval()(x), ref["y"], rtol=1e-5, atol=1e-5)
 
 
-def test_encoder_predictor_match_reference(ref_models):
-    torch.manual_seed(0)
-    ref, mine = ref_models.EncoderCNN(64), models.EncoderCNN(64)
-    mine.load_state_dict(ref.state_dict())
-    x = torch.randn(6, 8, 32, 32)
-    torch.testing.assert_close(mine(x), ref(x), rtol=1e-5, atol=1e-5)
-    rp, mp = ref_models.PredictorCNN(64, 8), models.PredictorCNN(64, 8)
-    mp.load_state_dict(rp.state_dict())
-    a, b = torch.randn(2, 64, 3, 3), torch.randn(2, 64, 3, 3)
-    for u, v in zip(mp(a, b), rp(a, b)):
-        torch.testing.assert_close(u, v)
+def test_encoder_predictor_match_reference(golden, fill):
+    ref = golden["encoder_predictor"]
+    with torch.no_grad():
+        mine = fill(models.EncoderCNN(64)).eval()
+        x = torch.randn(6, 8, 32, 32, generator=torch.Generator().manual_seed(2))
+        torch.testing.assert_close(mine(x), ref["enc"], rtol=1e-5, atol=1e-5)
+        mp = fill(models.PredictorCNN(64, 8)).eval()
+        a = torch.randn(2, 64, 3, 3, generator=torch.Generator().manual_seed(3))
+        b = torch.randn(2, 64, 3, 3, generator=torch.Generator().manual_seed(4))
+        for u, v in zip(mp(a, b), ref["pred"]):
+            torch.testing.assert_close(u, v)
 
 
-def test_vae_deterministic_parts_match_reference(ref_models):
-    torch.manual_seed(0)
-    ref, mine = ref_models.AutoEncoderCNN(), models.AutoEncoderCNN()
-    mine.load_state_dict(ref.state_dict())
-    x = torch.rand(3, 3, 32, 32)
-    for u, v in zip(mine.encode(x), ref.encode(x)):
-        torch.testing.assert_close(u, v, rtol=1e-5, atol=1e-6)
-    z = torch.randn(3, 10)
-    torch.testing.assert_close(mine.decode(z), ref.decode(z), rtol=1e-5, atol=1e-6)
+def test_vae_deterministic_parts_match_reference(golden, fill):
+    ref = golden["vae"]
+    with torch.no_grad():
+        mine = fill(models.AutoEncoderCNN()).eval()
+        x = torch.rand(3, 3, 32, 32, generator=torch.Generator().manual_seed(5))
+        for u, v in zip(mine.encode(x), ref["encode"]):
+            torch.testing.assert_close(u, v, rtol=1e-5, atol=1e-6)
+        z = torch.randn(3, 10, generator=torch.Generator().manual_seed(6))
+        torch.testing.assert_close(mine.decode(z), ref["decode"], rtol=1e-5, atol=1e-6)
 
 
-def test_vae_cl_batched_equals_loop(ref_models):
-    torch.manual_seed(0)
-    ref = ref_models.AutoEncoderCNNCL(K=4, L=8)
-    a = models.AutoEncoderCNNCL(K=4, L=8, batched_clusters=True)
-    b = models.AutoEncoderCNNCL(K=4, L=8, batched_clusters=False)
-    a.load_state_dict(ref.state_dict())
-    b.load_state_dict(ref.state_dict())
+def test_vae_cl_batched_equals_loop(golden, fill):
+    ref = golden["vae_cl"]
+    a = fill(models.AutoEncoderCNNCL(K=4, L=8, batched_clusters=True)).eval()
+    b = models.AutoEncoderCNNCL(K=4, L=8, batched_clusters=False).eval()
+    b.load_state_dict(a.state_dict())
     a.force_disable_repr()
     b.force_disable_repr()
-    x = torch.rand(5, 3, 32, 32)
-    torch.testing.assert_close(a.encodeclus(x), ref.encodeclus(x), rtol=1e-5, atol=1e-6)
-    oa, ob = a(x), b(x)
-    torch.testing.assert_close(oa[0], ob[0])
-    for da, db in zip(oa[1:], ob[1:]):
-        for k in range(4):
-            torch.testing.assert_close(da[k], db[k], rtol=1e-5, atol=1e-6)
-    # deterministic heads against the reference, cluster by cluster
-    ek = torch.zeros(5, 4)
-    ek[:, 2] = 1
-    for u, v in zip(a.encode(x, ek), ref.encode(x, ek)):
-        torch.testing.assert_close(u, v, rtol=1e-5, atol=1e-6)
-    z = torch.randn(5, 8)
-    for u, v in zip(a.decode(ek, z), ref.decode(ek, z)):
-        torch.testing.assert_close(u, v, rtol=1e-5, atol=1e-6)
+    x = torch.rand(5, 3, 32, 32, generator=torch.Generator().manual_seed(8))
+    with torch.no_grad():
+        torch.testing.assert_close(a.encodeclus(x), ref["encodeclus"], rtol=1e-5, atol=1e-6)
+        oa, ob = a(x), b(x)
+        torch.testing.assert_close(oa[0], ob[0])
+        for da, db in zip(oa[1:], ob[1:]):
+            for k in range(4):
+                torch.testing.assert_close(da[k], db[k], rtol=1e-5, atol=1e-6)
+        # deterministic heads against the original, cluster by cluster
+        ek = torch.zeros(5, 4)
+        ek[:, 2] = 1
+        for u, v in zip(a.encode(x, ek), ref["encode"]):
+            torch.testing.assert_close(u, v, rtol=1e-5, atol=1e-6)
+        z = torch.randn(5, 8, generator=torch.Generator().manual_seed(9))
+        for u, v in zip(a.decode(ek, z), ref["decode"]):
+            torch.testing.assert_close(u, v, rtol=1e-5, atol=1e-6)
 
 
 def test_disable_repr_quirk_preserved():
