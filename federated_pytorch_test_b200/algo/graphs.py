@@ -67,7 +67,8 @@ class GraphedEval:
     """Evaluation forward of one replica at one batch shape as a CUDA graph (SURVEY G21, X6): the reference evaluates all K
     models on 10 000 test images after EVERY aggregation round (79 batches x K x 360 rounds for ResNet18,
     /root/reference/src/federated_multi.py:108-121) with ~70 eager launches per batch.  Captured here: forward (train-mode
-    BatchNorm statistics included, Q4) + the fused argmax / compare / count kernel; the counter lives on the device."""
+    BatchNorm statistics included, Q4, or eval-mode BatchNorm with ``eval_bn='running'``: the network's mode at capture time is
+    baked in, so callers key graphs by it) + the fused argmax / compare / count kernel; the counter lives on the device."""
 
     WARMUP = 2
 

@@ -72,6 +72,8 @@ class ClassifierTask(Task):
         self.cfg, self.topo = cfg, topo
         self.lambda1, self.lambda2 = lambda1, lambda2
         self.whole_model = whole_model  # no_consensus: all parameters trainable, no block schedule
+        if cfg.eval_bn not in ("batch", "running"):
+            raise ValueError("eval_bn must be 'batch' or 'running', got %r" % (cfg.eval_bn,))
         name = cfg.model or ("ResNet18" if cfg.use_resnet else "Net")
         self.model_name = name
         self.factory = _MODEL_FACTORIES[name]
@@ -168,36 +170,45 @@ class ClassifierTask(Task):
     def evaluate(self, reps: List[Replica], engine: Engine) -> List[float]:
         """Test-set accuracy of every local replica (verification_error_check, federated_multi.py:108-121).
 
-        Networks stay in training mode as in the reference (Q4): BatchNorm uses batch
-        statistics and keeps updating its running statistics on test data.  Runs
+        By default networks stay in training mode as in the reference (Q4): BatchNorm
+        uses batch statistics and keeps updating its running statistics on test data.
+        With ``eval_bn='running'`` each network is evaluated in eval mode (running
+        statistics, left unchanged) and put back into training mode afterwards.  Runs
         under ``no_grad`` (no numerical effect).  Counting stays on the device; one
         read per replica.
         """
         fused = self.topo.device.type == "cuda" and FX.fast_path_enabled()
         graphed = fused and bool(getattr(self.cfg, "graphs", False))
+        running = self.cfg.eval_bn == "running"
         counters = []
         for rep in reps:
             net = rep.nets["net"]
             counter = self._eval_counters.setdefault(rep.ck, torch.zeros(2, dtype=torch.int64, device=rep.device))
             counter.zero_()                                                      # [#correct, #seen], stays on the device
-            for x, y in self.test_loader(rep.ck):
-                if graphed:
-                    from ..algo.graphs import GraphedEval
+            if running:
+                net.eval()
+            try:
+                for x, y in self.test_loader(rep.ck):
+                    if graphed:
+                        from ..algo.graphs import GraphedEval
 
-                    key = (rep.ck, tuple(x.shape))
-                    ge = self._eval_graphs.get(key)
-                    if ge is None:
-                        ge = self._eval_graphs[key] = GraphedEval(net, (x, y), counter, rep.device)
-                    ge.run((x, y))                                               # forward + argmax/compare/count: one graph launch
-                    continue
-                logits = net(x)
-                if fused:
-                    from ..ops import cuda_ops
+                        key = (rep.ck, tuple(x.shape), net.training)             # a graph bakes in the BatchNorm mode
+                        ge = self._eval_graphs.get(key)
+                        if ge is None:
+                            ge = self._eval_graphs[key] = GraphedEval(net, (x, y), counter, rep.device)
+                        ge.run((x, y))                                           # forward + argmax/compare/count: one graph launch
+                        continue
+                    logits = net(x)
+                    if fused:
+                        from ..ops import cuda_ops
 
-                    cuda_ops.argmax_count(logits, y, counter)                    # argmax + compare + count: one kernel (G21)
-                else:
-                    counter[0] += (logits.argmax(dim=1) == y).sum()
-                    counter[1] += y.shape[0]
+                        cuda_ops.argmax_count(logits, y, counter)                # argmax + compare + count: one kernel (G21)
+                    else:
+                        counter[0] += (logits.argmax(dim=1) == y).sum()
+                        counter[1] += y.shape[0]
+            finally:
+                if running:
+                    net.train()
             counters.append(counter)
         accs = []
         for rep, counter in zip(reps, counters):                                 # ONE read per replica, after all forwards are queued

@@ -46,6 +46,8 @@ class CommonConfig:
     fix_shard_off_by_one: bool = False   # Q1
     intended_elastic_net_gate: bool = False  # Q2: regularise whenever the block holds dense-layer weights
     diagnostics: str = "post"       # Q17: 'post' (extra forward after the step) | 'pre'
+    eval_bn: str = "batch"          # Q4: 'batch' (reference: train-mode BN at evaluation, running stats updated by test data) | 'running' (net.eval())
+                                    # classifier drivers only: the VAE, VAE-CL and CPC networks have no BatchNorm and do not evaluate
     nan_guard: str = "raise"        # non-finite aggregation residual: 'raise' | 'warn' | 'off'
     collective: str = "auto"        # 'auto' | 'fused' | 'torch'
     fast: bool = True               # use the hand-written sm_90a kernels on CUDA devices

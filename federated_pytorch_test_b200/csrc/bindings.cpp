@@ -108,19 +108,27 @@ void col_stats(Tensor y, Tensor stats) {
   fb::col_stats(fptr(y), fptr_mut(stats), (int)(y.numel() / C), C, cur_stream());
 }
 // y, out: [M, C] views of NHWC tensors.  Returns (out, save_mean, save_invstd).
-std::vector<Tensor> bn_elu_fwd(Tensor y, Tensor stats, Tensor gamma, Tensor beta, c10::optional<Tensor> residual,
+// use_running: eval-mode BatchNorm on the running statistics (left unchanged); stats may be None and (out, None, None) is returned.
+std::vector<Tensor> bn_elu_fwd(Tensor y, c10::optional<Tensor> stats, Tensor gamma, Tensor beta, c10::optional<Tensor> residual,
                                c10::optional<Tensor> running_mean, c10::optional<Tensor> running_var, double eps,
-                               double momentum, bool act, bool self_clean) {
+                               double momentum, bool act, bool self_clean, bool use_running) {
   CHECK_F32_CUDA(y); CHECK_CONTIG(y);
   c10::cuda::CUDAGuard guard(y.device());
   const int C = (int)y.size(-1);
   const int M = (int)(y.numel() / C);
   auto out = torch::empty_like(y);
-  auto sm = torch::empty({C}, y.options()), si = torch::empty({C}, y.options());
   float* rm = (running_mean.has_value() && running_mean->defined()) ? running_mean->data_ptr<float>() : nullptr;
   float* rv = (running_var.has_value() && running_var->defined()) ? running_var->data_ptr<float>() : nullptr;
-  TORCH_CHECK(stats.numel() >= 2 * C + (self_clean ? 1 : 0), "stats buffer too small");
-  fb::bn_elu_fwd(fptr(y), fptr_mut(stats), fptr(gamma), fptr(beta), opt_ptr(residual), fptr_mut(out), rm, rv, fptr_mut(sm),
+  if (use_running) {
+    TORCH_CHECK(rm != nullptr && rv != nullptr, "bn_elu_fwd: use_running needs running_mean and running_var");
+    fb::bn_elu_fwd(fptr(y), nullptr, fptr(gamma), fptr(beta), opt_ptr(residual), fptr_mut(out), rm, rv, nullptr, nullptr, M, C,
+                   (float)eps, 0.f, act ? 1 : 0, 0, cur_stream(), 1);
+    return {out, Tensor(), Tensor()};
+  }
+  TORCH_CHECK(stats.has_value() && stats->defined(), "bn_elu_fwd: stats required");
+  auto sm = torch::empty({C}, y.options()), si = torch::empty({C}, y.options());
+  TORCH_CHECK(stats->numel() >= 2 * C + (self_clean ? 1 : 0), "stats buffer too small");
+  fb::bn_elu_fwd(fptr(y), stats->data_ptr<float>(), fptr(gamma), fptr(beta), opt_ptr(residual), fptr_mut(out), rm, rv, fptr_mut(sm),
                  fptr_mut(si), M, C, (float)eps, (float)momentum, act ? 1 : 0, self_clean ? 1 : 0, cur_stream());
   return {out, sm, si};
 }
@@ -333,6 +341,36 @@ Tensor conv2d_nhwc_bias_act(Tensor x, Tensor w, c10::optional<Tensor> bias, bool
   auto y = torch::empty({NB, Ho, Wo, Co}, x.options());
   fb::conv2d_nhwc_bias_act_tf32(fptr(x), fptr(w), opt_ptr(bias), act ? 1 : 0, fptr_mut(y), NB, H, W, Ci, Co, kh, kw, (int)stride,
                                 (int)pad, (int)dil, Ho, Wo, cur_stream());
+  return y;
+}
+
+// conv + eval-mode BatchNorm (running statistics) (+ residual) (+ ELU): inference of the ResNet groups.  x [N,H,W,Ci],
+// w [Co,kh,kw,Ci], residual [N,Ho,Wo,Co] or None; returns y [N,Ho,Wo,Co].  The running statistics are only read.
+Tensor conv2d_nhwc_bn_eval(Tensor x, Tensor w, Tensor gamma, Tensor beta, Tensor running_mean, Tensor running_var, double eps,
+                           c10::optional<Tensor> residual, bool act, int64_t stride, int64_t pad) {
+  CHECK_F32_CUDA(x); CHECK_F32_CUDA(w); CHECK_CONTIG(x); CHECK_CONTIG(w);
+  TORCH_CHECK(x.dim() == 4 && w.dim() == 4 && x.size(3) == w.size(3), "conv2d_nhwc_bn_eval: x [N,H,W,Ci], w [Co,kh,kw,Ci]");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int NB = (int)x.size(0), H = (int)x.size(1), W = (int)x.size(2), Ci = (int)x.size(3);
+  const int Co = (int)w.size(0), kh = (int)w.size(1), kw = (int)w.size(2);
+  const int Ho = (H + 2 * (int)pad - (kh - 1) - 1) / (int)stride + 1;
+  const int Wo = (W + 2 * (int)pad - (kw - 1) - 1) / (int)stride + 1;
+  TORCH_CHECK(Ho > 0 && Wo > 0, "conv2d_nhwc_bn_eval: empty output");
+  for (const Tensor* t : {&gamma, &beta, &running_mean, &running_var}) {
+    CHECK_F32_CUDA((*t));
+    TORCH_CHECK(t->numel() == Co && t->is_contiguous(), "conv2d_nhwc_bn_eval: BatchNorm parameters and statistics must be [Co]");
+  }
+  const float* res = nullptr;
+  if (residual.has_value() && residual->defined()) {
+    CHECK_F32_CUDA((*residual)); CHECK_CONTIG((*residual));
+    TORCH_CHECK(residual->dim() == 4 && residual->size(0) == NB && residual->size(1) == Ho && residual->size(2) == Wo &&
+                residual->size(3) == Co, "conv2d_nhwc_bn_eval: residual must be [N,Ho,Wo,Co]");
+    res = residual->data_ptr<float>();
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(res) & 15) == 0, "conv2d_nhwc_bn_eval: residual must be 16-byte aligned");
+  }
+  auto y = torch::empty({NB, Ho, Wo, Co}, x.options());
+  fb::conv2d_nhwc_bn_eval_tf32(fptr(x), fptr(w), fptr(gamma), fptr(beta), fptr(running_mean), fptr(running_var), (float)eps, res,
+                               act ? 1 : 0, fptr_mut(y), NB, H, W, Ci, Co, kh, kw, (int)stride, (int)pad, 1, Ho, Wo, cur_stream());
   return y;
 }
 
@@ -638,7 +676,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("col_stats", &col_stats);
   m.def("head_fwd", &head_fwd);
   m.def("head_bwd", &head_bwd);
-  m.def("bn_elu_fwd", &bn_elu_fwd);
+  m.def("bn_elu_fwd", &bn_elu_fwd, py::arg("y"), py::arg("stats"), py::arg("gamma"), py::arg("beta"), py::arg("residual"),
+        py::arg("running_mean"), py::arg("running_var"), py::arg("eps"), py::arg("momentum"), py::arg("act"),
+        py::arg("self_clean"), py::arg("use_running") = false);
   m.def("bn_elu_bwd", &bn_elu_bwd);
   m.def("avgpool_nhwc", &avgpool_nhwc);
   m.def("avgpool_nhwc_bwd", &avgpool_nhwc_bwd);
@@ -649,6 +689,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv2d_nhwc", &conv2d_nhwc);
   m.def("conv2d_nhwc_sized", &conv2d_nhwc_sized);
   m.def("conv2d_nhwc_bias_act", &conv2d_nhwc_bias_act);
+  m.def("conv2d_nhwc_bn_eval", &conv2d_nhwc_bn_eval);
   m.def("conv2d_nhwc_accumulate", &conv2d_nhwc_accumulate);
   m.def("conv2d_nhwc_shuffle", &conv2d_nhwc_shuffle);
   m.def("conv_shuffle_supported", &conv_shuffle_supported);

@@ -3,7 +3,9 @@
 //  * normalize_u8_nhwc : uint8 NHWC pixels -> (x/255-mean)/std as NHWC (optionally padded to 4 channels) or NCHW
 //  * col_stats        : per-channel sum / sum of squares (only for layers whose conv did not emit them)
 //  * bn_elu_fwd        : BatchNorm(batch stats from the conv epilogue) + residual + ELU in ONE pass; block 0 also
-//                        updates the running statistics and stores mean/invstd for the backward pass
+//                        updates the running statistics and stores mean/invstd for the backward pass.  Running-statistics
+//                        mode (eval-mode BatchNorm after a split-K convolution): normalises with running_mean / running_var,
+//                        writes nothing else; y may then be `out` itself (every element is read once, by the thread that writes it)
 //  * bn_elu_bwd_reduce / bn_elu_bwd_apply : the two passes of the fused ELU'+BN backward
 //  * avgpool_nhwc (+bwd), weight_krsc_flip (dgrad weights: swap Cin/Cout, rotate taps by 180 degrees)
 #include "fedb200.h"
@@ -189,6 +191,8 @@ void col_stats(const float* y, float* stats, int M, int C, cudaStream_t s) {
   check_launch("col_stats");
 }
 
+// RUNNING: eval-mode BatchNorm on the running statistics (its own instantiation: the training launches keep their code)
+template <bool RUNNING>
 __global__ void __launch_bounds__(EW_THREADS)
 bn_elu_fwd_kernel(const float* __restrict__ y, float* __restrict__ stats, const float* __restrict__ gamma,
                   const float* __restrict__ beta, const float* __restrict__ residual, float* __restrict__ out,
@@ -199,7 +203,22 @@ bn_elu_fwd_kernel(const float* __restrict__ y, float* __restrict__ stats, const 
   const RowLayout L = row_layout(C, EW_THREADS);
   const bool active = L.r0 < L.rpi;
   float sc[4] = {0, 0, 0, 0}, sh[4] = {0, 0, 0, 0};
-  if (active) {
+  if constexpr (RUNNING) {
+    if (active) {
+      // eval-mode BatchNorm: the running statistics as they are (read only), nothing saved for a backward pass
+      const float4 m = reinterpret_cast<const float4*>(running_mean)[L.cq];
+      const float4 v = reinterpret_cast<const float4*>(running_var)[L.cq];
+      const float4 g = reinterpret_cast<const float4*>(gamma)[L.cq];
+      const float4 b = reinterpret_cast<const float4*>(beta)[L.cq];
+      const float mm[4] = {m.x, m.y, m.z, m.w}, vv[4] = {v.x, v.y, v.z, v.w};
+      const float gg[4] = {g.x, g.y, g.z, g.w}, bb[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        sc[j] = gg[j] * rsqrtf(vv[j] + eps);
+        sh[j] = fmaf(-mm[j], sc[j], bb[j]);
+      }
+    }
+  } else if (active) {
     const float invM = 1.f / float(M);
     const float4 s1 = reinterpret_cast<const float4*>(stats)[L.cq];
     const float4 s2 = reinterpret_cast<const float4*>(stats + C)[L.cq];
@@ -227,7 +246,7 @@ bn_elu_fwd_kernel(const float* __restrict__ y, float* __restrict__ stats, const 
       }
     }
   }
-  if (self_clean) {
+  if (!RUNNING && self_clean) {
     // Every thread of this block has consumed the statistics.  The last block to say so zeroes the accumulators (and
     // the counter behind them) for the next convolution that uses this buffer: no memset launch per layer.
     __syncthreads();
@@ -267,12 +286,14 @@ bn_elu_fwd_kernel(const float* __restrict__ y, float* __restrict__ stats, const 
 }
 void bn_elu_fwd(const float* y, float* stats, const float* gamma, const float* beta, const float* residual,
                 float* out, float* running_mean, float* running_var, float* save_mean, float* save_invstd, int M, int C,
-                float eps, float momentum, int act, int self_clean, cudaStream_t s) {
+                float eps, float momentum, int act, int self_clean, cudaStream_t s, int use_running) {
   if ((C & 3) || C > 4 * EW_THREADS) throw std::runtime_error("fedb200: bn_elu_fwd needs C % 4 == 0 and C <= 1024");
+  if (use_running && (running_mean == nullptr || running_var == nullptr))
+    throw std::runtime_error("fedb200: bn_elu_fwd: the running-statistics mode needs running_mean and running_var");
   const int rpi = EW_THREADS / (C >> 2);
-  launch_pdl(bn_elu_fwd_kernel, dim3(stream_grid(M, rpi)), dim3(EW_THREADS), 0, s, y, stats, gamma, beta, residual, out, running_mean,
-                                                                running_var, save_mean, save_invstd, M, C, eps, momentum,
-                                                                act, self_clean);
+  launch_pdl(use_running ? bn_elu_fwd_kernel<true> : bn_elu_fwd_kernel<false>, dim3(stream_grid(M, rpi)), dim3(EW_THREADS), 0, s, y,
+             stats, gamma, beta, residual, out, running_mean, running_var, save_mean, save_invstd, M, C, eps, momentum, act,
+             self_clean);
   check_launch("bn_elu_fwd");
 }
 

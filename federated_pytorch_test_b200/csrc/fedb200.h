@@ -54,6 +54,12 @@ void conv2d_nhwc_accumulate_tf32(const float* x, const float* w, float* y, int N
 void conv2d_nhwc_bias_act_tf32(const float* x, const float* w, const float* bias, int act, float* y, int NB, int H, int W,
                                int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
                                cudaStream_t stream);
+// y = act(BN_eval(conv(x, w)) + residual) with BatchNorm on its running statistics (inference); residual: [NB*H_out*W_out, C_out]
+// or nullptr.  One launch without split-K, else the split-K convolution + an in-place bn_elu_fwd (running-statistics mode).
+void conv2d_nhwc_bn_eval_tf32(const float* x, const float* w, const float* gamma, const float* beta, const float* mean,
+                              const float* var, float eps, const float* residual, int act, float* y, int NB, int H, int W,
+                              int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
+                              cudaStream_t stream);
 
 // phase-packed stride-1 conv stored straight into the pixel-shuffled [N, 2Ho, 2Wo, C4/4] result (stride-2 dgrad, transposed conv)
 bool conv_shuffle_supported(int H_out, int W_out, int C_in, int Ci_out);
@@ -93,9 +99,11 @@ void normalize_u8_nhwc(const uint8_t* in, float* out, int npix, int c_out, const
                        int to_nchw, int H, int W, cudaStream_t s);
 void col_stats(const float* y, float* stats, int M, int C, cudaStream_t s);
 // stats: [2C] sums (+ one uint counter behind them when self_clean: the kernel zeroes the buffer after the last read)
+// use_running: eval-mode BatchNorm on running_mean / running_var (read only); stats, save_mean / save_invstd, momentum and
+// self_clean are unused, and out may equal y
 void bn_elu_fwd(const float* y, float* stats, const float* gamma, const float* beta, const float* residual,
                 float* out, float* running_mean, float* running_var, float* save_mean, float* save_invstd, int M, int C,
-                float eps, float momentum, int act, int self_clean, cudaStream_t s);
+                float eps, float momentum, int act, int self_clean, cudaStream_t s, int use_running = 0);
 // out == nullptr (allowed when the layer had no residual input): ELU' is recomputed from y, gamma, beta
 void bn_elu_bwd_reduce(const float* dout, const float* out, const float* y, const float* mean, const float* invstd,
                        const float* gamma, const float* beta, float* sums, int M, int C, int act, int sums_clean, cudaStream_t s);

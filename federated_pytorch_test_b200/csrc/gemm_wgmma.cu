@@ -111,10 +111,10 @@ static int num_sms() {
 
 static const CUtensorMap* g_out_map_override = nullptr;     // set (and cleared) by conv2d_nhwc_shuffle_tf32 around its dispatch
 
-template <int BN, int ST>
+template <int BN, int ST, bool EVAL_BN>
 static void launch(const CUtensorMap& ta, const CUtensorMap& tb, IgemmParams p, cudaStream_t stream) {
   using S = IgemmSmem<BN, ST>;
-  auto kernel = igemm_wgmma_kernel<BN, ST>;
+  auto kernel = igemm_wgmma_kernel<BN, ST, EVAL_BN>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
@@ -137,12 +137,17 @@ static void launch(const CUtensorMap& ta, const CUtensorMap& tb, IgemmParams p, 
 }
 
 // Stages: as many k-blocks in flight as fit next to the epilogue buffers (~192 KB of the 227 KB a block may use).
-static void dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const IgemmParams& p, cudaStream_t s) {
+template <bool EVAL_BN>
+static void dispatch_tile(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const IgemmParams& p, cudaStream_t s) {
   switch (bn) {
-    case 32: launch<32, 8>(ta, tb, p, s); break;
-    case 64: launch<64, 8>(ta, tb, p, s); break;
-    default: launch<128, 6>(ta, tb, p, s); break;
+    case 32: launch<32, 8, EVAL_BN>(ta, tb, p, s); break;
+    case 64: launch<64, 8, EVAL_BN>(ta, tb, p, s); break;
+    default: launch<128, 6, EVAL_BN>(ta, tb, p, s); break;
   }
+}
+static void dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const IgemmParams& p, cudaStream_t s) {
+  if (p.bn_gamma != nullptr) dispatch_tile<true>(bn, ta, tb, p, s);
+  else dispatch_tile<false>(bn, ta, tb, p, s);
 }
 
 // The widest N tile that N allows (fewer passes over the activations), up to 128 columns: a 64 x 128 fp32 accumulator
@@ -197,11 +202,22 @@ bool conv_geometry_supported(int H_out, int W_out, int C_in, int stride) {
   return true;
 }
 
+// Eval-mode BatchNorm of conv2d_nhwc_bn_eval_tf32: running statistics, affine parameters and an optional residual.
+struct BnEvalArgs {
+  const float* gamma;
+  const float* beta;
+  const float* mean;
+  const float* var;
+  float eps;
+  const float* residual;
+};
+
 // Generic implicit-GEMM convolution.  bias / act (ELU) are applied in the epilogue (VAE / CPC convolutions, SURVEY G6;
-// no BatchNorm statistics and no split-K in that case).
+// no BatchNorm statistics and no split-K in that case).  With `eval_bn` the epilogue applies eval-mode BatchNorm + residual + act
+// when the convolution runs as one K slice; otherwise bn_elu_fwd does it in place after the split-K convolution.
 static void conv2d_generic(const float* x, const float* w, float* y, float* stats, const float* bias, int act, int NB, int H,
                            int W, int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
-                           cudaStream_t stream, int accumulate = 0);
+                           cudaStream_t stream, int accumulate = 0, const BnEvalArgs* eval_bn = nullptr);
 
 void conv2d_nhwc_tf32(const float* x, const float* w, float* y, float* stats, int NB, int H, int W, int C_in, int C_out,
                       int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream) {
@@ -221,6 +237,16 @@ void conv2d_nhwc_accumulate_tf32(const float* x, const float* w, float* y, int N
   conv2d_generic(x, w, y, nullptr, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 1);
 }
 
+// y = act(BN_eval(conv(x, w)) + residual): inference with BatchNorm on its running statistics.  One launch when the
+// convolution needs no split-K; otherwise the split-K convolution into y, then one in-place bn_elu_fwd pass.
+void conv2d_nhwc_bn_eval_tf32(const float* x, const float* w, const float* gamma, const float* beta, const float* mean,
+                              const float* var, float eps, const float* residual, int act, float* y, int NB, int H, int W,
+                              int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
+                              cudaStream_t stream) {
+  const BnEvalArgs args{gamma, beta, mean, var, eps, residual};
+  conv2d_generic(x, w, y, nullptr, nullptr, act, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 0, &args);
+}
+
 // Tap packing (IgemmParams::cw): with C_in <= 16 a 32-wide k-block holds 4 (C_in <= 8) or 2 taps instead of one tap padded with
 // zeros.  FEDB200_TAP_PACK=0 switches it off (A/B runs).
 static int pick_tap_pack(int C_in) {
@@ -230,7 +256,7 @@ static int pick_tap_pack(int C_in) {
 
 static void conv2d_generic(const float* x, const float* w, float* y, float* stats, const float* bias, int act, int NB, int H,
                            int W, int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
-                           cudaStream_t stream, int accumulate) {
+                           cudaStream_t stream, int accumulate, const BnEvalArgs* eval_bn) {
   if (!conv_geometry_supported(H_out, W_out, C_in, stride))
     throw std::runtime_error("fedb200: conv geometry not supported by the wgmma path");
   const int rows = 128 / W_out;
@@ -256,7 +282,7 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
   p.out = y; p.ldo = C_out; p.bias = bias; p.act = act; p.stats = stats;
   p.k_splits = 1; p.kb_per_split = p.num_k_blocks;
   p.accumulate = accumulate;
-  if (bias == nullptr && act == 0) {   // bias / activation must see the complete sum
+  if (bias == nullptr && (act == 0 || eval_bn != nullptr)) {   // bias / activation must see the complete sum
     const int splits = pick_k_splits(M, C_out, bn, p.num_k_blocks);
     if (splits > 1) {
       p.kb_per_split = (p.num_k_blocks + splits - 1) / splits;
@@ -265,8 +291,20 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
       if (!accumulate) cudaMemsetAsync(y, 0, size_t(M) * C_out * sizeof(float), stream);
     }
   }
+  if (eval_bn != nullptr) {
+    if ((C_out & 3) != 0) throw std::runtime_error("fedb200: eval-mode BatchNorm epilogue needs C_out % 4 == 0");
+    if (p.k_splits > 1) {
+      p.act = 0;                       // the nonlinear part runs on the complete sums, after the reduction
+    } else {
+      p.bn_gamma = eval_bn->gamma; p.bn_beta = eval_bn->beta; p.bn_mean = eval_bn->mean; p.bn_var = eval_bn->var;
+      p.bn_eps = eval_bn->eps; p.residual = eval_bn->residual; p.ldr = C_out;
+    }
+  }
   dispatch(bn, ta, tb, p, stream);
   if (p.k_splits > 1 && stats != nullptr) col_stats(y, stats, M, C_out, stream);
+  if (p.k_splits > 1 && eval_bn != nullptr)   // running-statistics mode, in place
+    bn_elu_fwd(y, nullptr, eval_bn->gamma, eval_bn->beta, eval_bn->residual, y, const_cast<float*>(eval_bn->mean),
+               const_cast<float*>(eval_bn->var), nullptr, nullptr, M, C_out, eval_bn->eps, 0.f, act, 0, stream, 1);
 }
 
 // ------------------------------------------------------------------------------------------------

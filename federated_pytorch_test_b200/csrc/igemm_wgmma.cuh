@@ -15,7 +15,8 @@
 //                   then the fused epilogue:
 //   * bias + ELU (dense layers, VAE / CPC convolutions), or
 //   * per-channel sum / sum-of-squares of the tile (BatchNorm batch statistics, reduced across the CTA in shared
-//     memory, one atomicAdd per channel per tile);
+//     memory, one atomicAdd per channel per tile), or
+//   * eval-mode BatchNorm from the running statistics + residual + ELU (inference: conv + BN + add + ELU in one launch);
 //   * output through a 128B-swizzled staging tile and bulk tensor stores (reduce-adds for split-K / accumulation), or
 //     direct stores when the row pitch is not 16-byte aligned.
 #pragma once
@@ -61,6 +62,16 @@ struct IgemmParams {
   int shuffle_ci;        // > 0: the N columns are (ph, pw, ci) phase-packed channels of a stride-2 data gradient /
                          // transposed conv; each 32 x 32 chunk is stored to out[n, 2 ho + ph, 2 wo + pw, ci0 .. ci0 + 31] through a
                          // 5-D tensor map (no separate pixel-shuffle pass).  shuffle_ci = channels of the shuffled output.
+  // eval-mode BatchNorm (k_splits == 1, stats == nullptr): column c -> v * s_c + t_c with s_c = gamma_c / sqrt(var_c + eps),
+  // t_c = beta_c - mean_c * s_c (per tile in shared memory), then + residual, then act.  bn_gamma == nullptr: off (the host
+  // launches the EVAL_BN instantiation of the kernel exactly when it is set).
+  const float* bn_gamma;
+  const float* bn_beta;
+  const float* bn_mean;
+  const float* bn_var;
+  float bn_eps;
+  const float* residual; // [M, ldr] (NHWC, like the output) or nullptr; ldr even, 8-byte aligned
+  int ldr;
 };
 
 template <int BLOCK_N, int STAGES>
@@ -69,7 +80,7 @@ struct IgemmSmem {
   static constexpr int B_BYTES = BLOCK_N * IG_BLOCK_K * 4;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;         // one k-block: [A | B]
   static constexpr int STAGING_BYTES = 2 * 64 * 32 * 4;         // per consumer warpgroup: two 32 x 32 output boxes
-  static constexpr int STATS_BYTES = 2 * BLOCK_N * 4;           // column partials (sum, sumsq) of the current tile
+  static constexpr int STATS_BYTES = 2 * BLOCK_N * 4;           // column partials (sum, sumsq) or eval-BN (scale, shift) of the tile
   static constexpr int BAR_BYTES = 2 * STAGES * 8;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + STAGING_BYTES + STATS_BYTES + BAR_BYTES + 1024;  // + align slack
 };
@@ -94,7 +105,9 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
 }
 
-template <int BLOCK_N, int STAGES>
+// EVAL_BN: the eval-mode BatchNorm (+ residual) epilogue (IgemmParams::bn_*) is compiled in; a separate instantiation, so the
+// training and GEMM launches keep the plain epilogue's code and register budget.
+template <int BLOCK_N, int STAGES, bool EVAL_BN>
 __global__ void __launch_bounds__(IG_THREADS, 1)
 igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                    const __grid_constant__ CUtensorMap tmap_c, const IgemmParams p) {
@@ -224,6 +237,21 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   uint32_t ph = 0;
   for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
     const TileCoord c = decode_tile(p, t, BLOCK_N);
+    if constexpr (EVAL_BN) {
+      // eval-mode BatchNorm: the tile's per-column scale / shift, once per tile, in the (otherwise unused) statistics area
+      named_bar_sync(3, 256);                    // the previous tile's epilogue has read them
+      for (int cc = threadIdx.x - 128; cc < BLOCK_N; cc += 256) {
+        const int col = c.n0 + cc;
+        float sc = 0.f, sh = 0.f;
+        if (col < p.N) {
+          sc = __ldg(p.bn_gamma + col) * rsqrtf(__ldg(p.bn_var + col) + p.bn_eps);
+          sh = fmaf(-__ldg(p.bn_mean + col), sc, __ldg(p.bn_beta + col));
+        }
+        colsum[cc] = sc;
+        colsum[BLOCK_N + cc] = sh;
+      }
+      named_bar_sync(3, 256);
+    }
     // ---- main loop: one k-block per stage, the previous stage is released once its MMAs have retired
     int prev = -1;
     for (int i = 0; i < c.kb_count; ++i) {
@@ -250,6 +278,15 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     const bool ok_a = row_a < p.M, ok_b = row_b < p.M;
 #pragma unroll
     for (int i = 0; i < NACC / 4; ++i) {
+      // residual pair (col, col + 1) of rows a and b: one 8-byte load each (N is even on this path)
+      float2 ra = make_float2(0.f, 0.f), rb = ra;
+      if constexpr (EVAL_BN) {
+        if (p.residual != nullptr && c.n0 + 8 * i + col_in < p.N) {
+          const float* r0 = p.residual + c.n0 + 8 * i + col_in;
+          if (ok_a) ra = __ldg(reinterpret_cast<const float2*>(r0 + size_t(row_a) * p.ldr));
+          if (ok_b) rb = __ldg(reinterpret_cast<const float2*>(r0 + size_t(row_b) * p.ldr));
+        }
+      }
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int col = c.n0 + 8 * i + col_in + e;
@@ -258,6 +295,11 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           const float b = __ldg(p.bias + col);
           va += b;
           vb += b;
+        }
+        if constexpr (EVAL_BN) {
+          const float sc = colsum[8 * i + col_in + e], sh = colsum[BLOCK_N + 8 * i + col_in + e];
+          va = fmaf(va, sc, sh) + (e ? ra.y : ra.x);
+          vb = fmaf(vb, sc, sh) + (e ? rb.y : rb.x);
         }
         if (p.act) { va = elu1(va); vb = elu1(vb); }
         acc[4 * i + e] = ok_a ? va : 0.f;         // rows past M are clipped by the store and must not reach the statistics

@@ -9,6 +9,7 @@ ordinary tensors, while the kernels receive the underlying [N,H,W,C] buffer.
 Kernel inventory (SURVEY §2.10 ids):
   G1  conv2d_nhwc          wgmma implicit GEMM (TMA 4-D boxes -> smem -> wgmma tf32 -> registers), BN stats in epilogue
   G2/3 bn_elu_fwd/bwd      BatchNorm(train) + residual + ELU fused, two-pass backward
+       conv2d_nhwc_bn_eval  conv + BatchNorm(eval, running statistics) + residual + ELU in the conv epilogue (inference)
   G4  avgpool / pool_linear
   G5  linear_tf32          wgmma GEMM with bias+ELU epilogue
   G9  cross_entropy        fused log-softmax/NLL fwd, softmax-minus-onehot bwd
@@ -140,14 +141,14 @@ def _krsc(w: torch.Tensor) -> torch.Tensor:
     return p if p.is_contiguous() else p.contiguous()
 
 
-def conv_bn_act_supported(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d) -> bool:
+def _conv_bn_geometry_supported(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d) -> bool:
     if not (isinstance(conv, nn.Conv2d) and isinstance(bn, nn.BatchNorm2d)):
         return False
     if conv.bias is not None or conv.groups != 1 or conv.padding_mode != "zeros":
         return False
     if conv.stride[0] != conv.stride[1] or conv.padding[0] != conv.padding[1] or conv.dilation != (1, 1):
         return False
-    if x.dtype != torch.float32 or x.dim() != 4 or not bn.training or not bn.track_running_stats or bn.momentum is None:
+    if x.dtype != torch.float32 or x.dim() != 4:
         return False
     kh, kw = conv.kernel_size
     s, p = conv.stride[0], conv.padding[0]
@@ -157,6 +158,42 @@ def conv_bn_act_supported(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d) 
     if cin < 0 or conv.out_channels % 4 != 0:
         return False
     return bool(ext().conv_supported(Ho, Wo, cin, s))
+
+
+def conv_bn_act_supported(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d) -> bool:
+    if not isinstance(bn, nn.BatchNorm2d) or not bn.training or not bn.track_running_stats or bn.momentum is None:
+        return False
+    return _conv_bn_geometry_supported(x, conv, bn)
+
+
+def conv_bn_act_eval_supported(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d,
+                               residual: Optional[torch.Tensor] = None) -> bool:
+    """Eval-mode BatchNorm (running statistics) when no gradient is needed: the inference path of ``conv_bn_act_eval``.
+    With a gradient to compute the ATen composition runs instead (eval-mode training has no kernels)."""
+    if not isinstance(bn, nn.BatchNorm2d) or bn.training or not bn.track_running_stats or bn.running_mean is None \
+            or bn.weight is None or bn.bias is None:
+        return False
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, conv.weight, bn.weight, bn.bias, residual)):
+        return False
+    if residual is not None and (residual.shape[1] != conv.out_channels or residual.dtype != torch.float32):
+        return False
+    return _conv_bn_geometry_supported(x, conv, bn)
+
+
+def conv_bn_act_eval(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d, residual: Optional[torch.Tensor] = None,
+                     act: bool = True) -> torch.Tensor:
+    """``ELU?(BN_eval(conv(x)) (+ residual))`` on the running statistics, which stay untouched: one wgmma launch with
+    BatchNorm, residual and ELU in the epilogue (or the split-K convolution + one elementwise pass).  Not differentiable;
+    touches no cached statistics or filter buffers of the training path."""
+    xn = _nhwc(x)
+    wk = _krsc(conv.weight)
+    if xn.shape[3] == 3:  # stem: pad 3 -> 4 channels so that the pixel pitch is 16 B (TMA requirement)
+        xn = F.pad(xn, (0, 1))
+        wk = F.pad(wk, (0, 1))
+    res = _nhwc(residual) if residual is not None else None
+    out = ext().conv2d_nhwc_bn_eval(xn, wk, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, res, bool(act),
+                                    conv.stride[0], conv.padding[0])
+    return out.permute(0, 3, 1, 2)
 
 
 _FLIP_CACHE = {}

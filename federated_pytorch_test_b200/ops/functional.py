@@ -46,11 +46,15 @@ def conv_bn_act(
 
     Semantics follow /root/reference/src/simple_models.py:149-154: batch
     statistics are used (and running statistics updated) whenever the module
-    is in training mode, which in the reference is *always* (SURVEY Q4).
+    is in training mode, which in the reference is *always* (SURVEY Q4).  In
+    eval mode (``bn.eval()``) the running statistics normalise and stay
+    unchanged; without a gradient to compute that runs as one kernel.
     """
     if _use_fast(x):
         from . import cuda_ops
 
+        if cuda_ops.conv_bn_act_eval_supported(x, conv, bn, residual):
+            return cuda_ops.conv_bn_act_eval(x, conv, bn, residual, act)
         if cuda_ops.conv_bn_act_supported(x, conv, bn):
             return cuda_ops.conv_bn_act(x, conv, bn, residual, act)
     y = F.conv2d(x, conv.weight, conv.bias, conv.stride, conv.padding, conv.dilation, conv.groups)
