@@ -17,7 +17,7 @@ import torch.nn as nn
 from .. import models
 from ..algo.engine import Engine, EngineConfig, Replica, Task, Visit
 from ..config import CommonConfig
-from ..data.cifar import CifarData, ShardLoader, shard_ranges, worker_norm
+from ..data.cifar import CifarData, ShardLoader, augment_key, shard_ranges, worker_norm
 from ..ops import functional as FX
 from ..ops import losses
 from ..parallel.collective import make_collective
@@ -129,7 +129,8 @@ class ClassifierTask(Task):
             mean, std = worker_norm(ck, self.cfg.biased_input)
             ld = ShardLoader(self.data.train_images, self.data.train_labels, self.shards[ck], self.cfg.default_batch,
                              self.topo.device, mean, std, shuffle=True, seed=self.cfg.seed + 1000 * ck,
-                             channels_last=self.channels_last)
+                             channels_last=self.channels_last, augment=self.cfg.augment,
+                             aug_key=augment_key(self.cfg.seed, ck))
             self._loaders[ck] = ld
         return ld
 

@@ -28,6 +28,8 @@ class VAETask(common.ClassifierTask):
     label_mode = "reference"
 
     def __init__(self, cfg, topo):
+        if cfg.augment:     # the loader would crop and flip the VAE's reconstruction targets too
+            raise ValueError("augment is supported by the classifier drivers only, not by %s" % type(self).__name__)
         cfg_model = cfg.model
         cfg.model = "Net"  # placeholder for the base-class probe; replaced below
         super().__init__(cfg, topo)

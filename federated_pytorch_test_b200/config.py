@@ -48,6 +48,7 @@ class CommonConfig:
     diagnostics: str = "post"       # Q17: 'post' (extra forward after the step) | 'pre'
     eval_bn: str = "batch"          # Q4: 'batch' (reference: train-mode BN at evaluation, running stats updated by test data) | 'running' (net.eval())
                                     # classifier drivers only: the VAE, VAE-CL and CPC networks have no BatchNorm and do not evaluate
+    augment: bool = False           # random 4-pixel-padded crop + horizontal flip of training batches (classifier drivers only)
     nan_guard: str = "raise"        # non-finite aggregation residual: 'raise' | 'warn' | 'off'
     collective: str = "auto"        # 'auto' | 'fused' | 'torch'
     fast: bool = True               # use the hand-written sm_90a kernels on CUDA devices

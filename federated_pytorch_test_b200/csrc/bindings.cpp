@@ -101,6 +101,33 @@ Tensor normalize_u8(Tensor u8, std::vector<double> mean, std::vector<double> std
   fb::normalize_u8_nhwc(u8.data_ptr<uint8_t>(), fptr_mut(out), (int)(N * H * W), (int)c_out, m3, s3, to_nchw ? 1 : 0, (int)H, (int)W, cur_stream());
   return out;
 }
+// key: the 64-bit augmentation key, bit pattern passed as int64.  rows: optional int64 indices into u8 (every index must be
+// a valid row); without them u8 holds the batch itself.
+Tensor augment_normalize_u8(Tensor u8, c10::optional<Tensor> rows, int64_t key, int64_t counter, std::vector<double> mean,
+                            std::vector<double> stdv, bool to_nchw) {
+  TORCH_CHECK(u8.is_cuda() && u8.scalar_type() == torch::kUInt8 && u8.dim() == 4 && u8.size(3) == 3 && u8.is_contiguous(),
+              "augment_normalize_u8 expects a contiguous CUDA uint8 [N,H,W,3] tensor");
+  TORCH_CHECK(counter >= 0, "augment_normalize_u8: negative counter");
+  c10::cuda::CUDAGuard guard(u8.device());
+  int64_t N = u8.size(0);
+  const int64_t H = u8.size(1), W = u8.size(2);
+  const int64_t* rp = nullptr;
+  if (rows.has_value() && rows->defined()) {
+    TORCH_CHECK(rows->is_cuda() && rows->device() == u8.device() && rows->scalar_type() == torch::kInt64 && rows->dim() == 1 &&
+                    rows->is_contiguous(),
+                "augment_normalize_u8: rows must be a contiguous int64 vector on the images' device");
+    N = rows->numel();
+    rp = rows->data_ptr<int64_t>();
+  }
+  TORCH_CHECK(N * H * W < (int64_t(1) << 31), "augment_normalize_u8: batch too large");
+  float m3[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s3[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
+  auto opts = torch::TensorOptions().dtype(torch::kFloat32).device(u8.device());
+  Tensor out = to_nchw ? torch::empty({N, 3, H, W}, opts) : torch::empty({N, H, W, 3}, opts);
+  if (N == 0) return out;
+  fb::augment_normalize_u8(u8.data_ptr<uint8_t>(), rp, fptr_mut(out), (int)N, (int)H, (int)W, (uint64_t)key, (uint64_t)counter,
+                           m3, s3, to_nchw ? 1 : 0, cur_stream());
+  return out;
+}
 void col_stats(Tensor y, Tensor stats) {
   CHECK_F32_CUDA(y); CHECK_CONTIG(y);
   c10::cuda::CUDAGuard guard(y.device());
@@ -673,6 +700,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("multi_dot", &multi_dot);
   m.def("lbfgs_two_loop", &lbfgs_two_loop);
   m.def("normalize_u8", &normalize_u8);
+  m.def("augment_normalize_u8", &augment_normalize_u8, py::arg("u8"), py::arg("rows"), py::arg("key"), py::arg("counter"),
+        py::arg("mean"), py::arg("std"), py::arg("to_nchw"));
   m.def("col_stats", &col_stats);
   m.def("head_fwd", &head_fwd);
   m.def("head_bwd", &head_bwd);

@@ -1,6 +1,7 @@
 // Memory-bound fused elementwise kernels of the ResNet path (SURVEY G2-G4, G22): all NHWC fp32,
 // 128-bit accesses along the channel axis, per-channel parameters staged in shared memory.
 //  * normalize_u8_nhwc : uint8 NHWC pixels -> (x/255-mean)/std as NHWC (optionally padded to 4 channels) or NCHW
+//  * augment_normalize_u8 : the same with the batch gather, a random padded crop and a random horizontal flip fused in
 //  * col_stats        : per-channel sum / sum of squares (only for layers whose conv did not emit them)
 //  * bn_elu_fwd        : BatchNorm(batch stats from the conv epilogue) + residual + ELU in ONE pass; block 0 also
 //                        updates the running statistics and stores mean/invstd for the backward pass.  Running-statistics
@@ -73,6 +74,68 @@ void normalize_u8_nhwc(const uint8_t* in, float* out, int npix, int c_out, const
   normalize_u8_kernel<<<grid, 256, 0, s>>>(in, out, npix, c_out, mean3[0], mean3[1], mean3[2], std3[0], std3[1],
                                            std3[2], to_nchw, H * W);
   check_launch("normalize_u8");
+}
+
+// ------------------------------------------------------------------------------------------------
+// Training augmentation fused into the input stage: gather (optional) + RandomCrop(padding=4) + RandomHorizontalFlip +
+// normalisation + layout change, one thread per output pixel.  Sample n of the batch draws from
+// z = splitmix64_finaliser(key + (counter + n + 1) * 0x9E3779B97F4A7C15) and dx = (z[31:0] * 9) >> 32,
+// dy = (z[62:32] * 9) >> 31, flip = z[63]; data/cifar.py (augment_draws) documents the draw and evaluates it on the CPU.
+// Out-of-range source pixels are 0 before normalisation; the arithmetic is normalize_u8_kernel's, so a crop at (4, 4)
+// without a flip reproduces it bit for bit.
+__device__ __forceinline__ uint64_t splitmix64_finaliser(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+__global__ void __launch_bounds__(256)
+augment_normalize_u8_kernel(const uint8_t* __restrict__ in, const int64_t* __restrict__ rows, float* __restrict__ out,
+                            int npix, uint64_t key, uint64_t counter, float m0, float m1, float m2, float s0, float s1,
+                            float s2, int to_nchw, int H, int W) {
+  constexpr int PAD = 4;
+  const float sc[3] = {1.f / (255.f * s0), 1.f / (255.f * s1), 1.f / (255.f * s2)};
+  const float sh[3] = {-m0 / s0, -m1 / s1, -m2 / s2};
+  const int HW = H * W;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
+    const int n = p / HW, r = p - n * HW, h = r / W, w = r - h * W;
+    const uint64_t z = splitmix64_finaliser(key + (counter + uint64_t(n) + 1ull) * 0x9E3779B97F4A7C15ull);
+    const int dx = int(((z & 0xFFFFFFFFull) * 9ull) >> 32);
+    const int dy = int((((z >> 32) & 0x7FFFFFFFull) * 9ull) >> 31);
+    const int sy = h + dy - PAD;
+    const int sx = ((z >> 63) ? W - 1 - w : w) + dx - PAD;
+    uint8_t c0 = 0, c1 = 0, c2 = 0;
+    if (unsigned(sy) < unsigned(H) && unsigned(sx) < unsigned(W)) {
+      const int64_t row = rows != nullptr ? rows[n] : int64_t(n);
+      const uint8_t* px = in + ((size_t(row) * H + sy) * W + sx) * 3;
+      c0 = px[0];
+      c1 = px[1];
+      c2 = px[2];
+    }
+    const float v0 = fmaf(float(c0), sc[0], sh[0]);
+    const float v1 = fmaf(float(c1), sc[1], sh[1]);
+    const float v2 = fmaf(float(c2), sc[2], sh[2]);
+    if (to_nchw) {
+      float* o = out + size_t(n) * 3 * HW + r;
+      o[0] = v0;
+      o[HW] = v1;
+      o[2 * HW] = v2;
+    } else {
+      float* o = out + size_t(p) * 3;
+      o[0] = v0;
+      o[1] = v1;
+      o[2] = v2;
+    }
+  }
+}
+void augment_normalize_u8(const uint8_t* in, const int64_t* rows, float* out, int n, int H, int W, uint64_t key,
+                          uint64_t counter, const float* mean3, const float* std3, int to_nchw, cudaStream_t s) {
+  const int npix = n * H * W;
+  int grid = (npix + 255) / 256;
+  if (grid > sm_count() * 16) grid = sm_count() * 16;
+  augment_normalize_u8_kernel<<<grid, 256, 0, s>>>(in, rows, out, npix, key, counter, mean3[0], mean3[1], mean3[2],
+                                                   std3[0], std3[1], std3[2], to_nchw, H, W);
+  check_launch("augment_normalize_u8");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -97,6 +97,11 @@ size_t lbfgs_two_loop_work_floats(int k);
 // ---- elementwise / normalisation (elementwise_kernels.cu) ------------------------------------------
 void normalize_u8_nhwc(const uint8_t* in, float* out, int npix, int c_out, const float* mean3, const float* std3,
                        int to_nchw, int H, int W, cudaStream_t s);
+// n samples of training augmentation (random 4-pixel-padded crop + horizontal flip) + normalisation, NCHW or NHWC (3
+// channels) out.  rows: int64 indices of the samples in `in` (device-resident dataset), or nullptr when `in` already holds
+// the n samples.  Sample i draws from (key, counter + i); the draw is documented in data/cifar.py (augment_draws).
+void augment_normalize_u8(const uint8_t* in, const int64_t* rows, float* out, int n, int H, int W, uint64_t key,
+                          uint64_t counter, const float* mean3, const float* std3, int to_nchw, cudaStream_t s);
 void col_stats(const float* y, float* stats, int M, int C, cudaStream_t s);
 // stats: [2C] sums (+ one uint counter behind them when self_clean: the kernel zeroes the buffer after the last read)
 // use_running: eval-mode BatchNorm on running_mean / running_var (read only); stats, save_mean / save_invstd, momentum and

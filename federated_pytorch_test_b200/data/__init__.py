@@ -1,6 +1,7 @@
-"""Data: synthetic CIFAR10 / LOFAR sources, reference shard math, loaders."""
-from .cifar import CifarData, ShardLoader, make_synthetic_cifar, normalize_batch, shard_ranges, worker_norm
+"""Data: synthetic CIFAR10 / LOFAR sources, reference shard math, loaders, training augmentation."""
+from .cifar import (CifarData, ShardLoader, augment_batch, augment_draws, augment_key, augment_u8, make_synthetic_cifar,
+                    normalize_batch, shard_ranges, worker_norm)
 from .lofar import LofarSource, get_data_minibatch
 
 __all__ = ["CifarData", "ShardLoader", "make_synthetic_cifar", "normalize_batch", "shard_ranges", "worker_norm",
-           "LofarSource", "get_data_minibatch"]
+           "augment_batch", "augment_draws", "augment_key", "augment_u8", "LofarSource", "get_data_minibatch"]

@@ -17,6 +17,15 @@ What this module does instead (SURVEY G22, §7.1 ``data/``):
   ``ToTensor``/``Normalize`` per PIL image on the CPU;
 * identical shard arithmetic (including the off-by-one, switchable) and
   identical per-worker normalisation constants.
+
+Training augmentation (opt-in, ``--augment``; the reference has none) is torchvision's ``RandomCrop(32, padding=4)``
+followed by ``RandomHorizontalFlip(0.5)`` on the raw uint8 image, before normalisation, so padded pixels come out as
+``-mean/std``.  On the CUDA fast path it is fused into the input kernel
+(:func:`ops.cuda_ops.augment_normalize_u8`: gather + crop + flip + normalisation + layout, one launch per batch);
+:func:`augment_batch` is the ATen composition used on the CPU and with ``fast=False``.  The random draws are
+counter-based, not a ``torch.Generator``: sample ``i`` of a batch takes :func:`augment_draws` ``(key, counter + i)``, where
+``key`` is fixed per worker (:func:`augment_key`) and ``counter`` is the number of samples its loader has handed out.
+So augmentation does not touch the shuffle generator, and a batch does not depend on the process topology.
 """
 from __future__ import annotations
 
@@ -121,6 +130,69 @@ def normalize_batch(u8_nhwc: torch.Tensor, mean, std, channels_last: bool = Fals
 
 
 # ----------------------------------------------------------------------------
+# training augmentation: random padded crop + horizontal flip, counter-based draws
+# ----------------------------------------------------------------------------
+AUG_PAD = 4
+_MASK64 = (1 << 64) - 1
+_GOLDEN_GAMMA = 0x9E3779B97F4A7C15
+
+
+def _splitmix64_finaliser(z: np.ndarray) -> np.ndarray:
+    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return z ^ (z >> np.uint64(31))
+
+
+def augment_key(seed: int, ck: int) -> int:
+    """64-bit augmentation key of worker ``ck`` in a run seeded with ``seed``."""
+    z = np.array([((int(seed) & 0xFFFFFFFF) << 32) | (int(ck) & 0xFFFFFFFF)], dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        return int(_splitmix64_finaliser(z)[0])
+
+
+def augment_draws(key: int, counter: int, n: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Crop offsets and flip bits of samples ``counter .. counter + n - 1`` of a loader with key ``key``.
+
+    Sample ``c`` takes the 64-bit word ``z = F(key + (c + 1) * 0x9E3779B97F4A7C15 mod 2**64)``, i.e. output ``c`` of a
+    splitmix64 generator seeded with ``key``, where ``F`` is the splitmix64 finaliser::
+
+        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  z = z ^ (z >> 31)
+
+    and maps its bits to ``dx = (z[31:0] * 9) >> 32``, ``dy = (z[62:32] * 9) >> 31`` (both in ``[0, 8]``) and
+    ``flip = z[63]``.  The augmented image is ``out[h][w] = img[h + dy - 4][w' + dx - 4]`` with ``w' = W - 1 - w`` when
+    flipped and ``w`` otherwise; pixels outside the image are 0.  The CUDA kernel evaluates the same function bit for
+    bit.  Returns ``dx``, ``dy`` (int64) and ``flip`` (bool), each of length ``n``.
+    """
+    c = np.arange(n, dtype=np.uint64) + np.uint64((int(counter) + 1) & _MASK64)
+    with np.errstate(over="ignore"):
+        z = _splitmix64_finaliser(np.uint64(int(key) & _MASK64) + c * np.uint64(_GOLDEN_GAMMA))
+    dx = ((z & np.uint64(0xFFFFFFFF)) * np.uint64(9)) >> np.uint64(32)
+    dy = (((z >> np.uint64(32)) & np.uint64(0x7FFFFFFF)) * np.uint64(9)) >> np.uint64(31)
+    flip = (z >> np.uint64(63)) != 0
+    return (torch.from_numpy(dx.astype(np.int64)), torch.from_numpy(dy.astype(np.int64)),
+            torch.from_numpy(flip.astype(np.bool_)))
+
+
+def augment_u8(u8_nhwc: torch.Tensor, key: int, counter: int) -> torch.Tensor:
+    """The augmented uint8 NHWC batch (zero padding, gather, flip) of :func:`augment_draws`, on ``u8_nhwc``'s device."""
+    n, H, W, _ = u8_nhwc.shape
+    dev = u8_nhwc.device
+    dx, dy, flip = (t.to(dev) for t in augment_draws(key, counter, n))
+    padded = torch.nn.functional.pad(u8_nhwc, (0, 0, AUG_PAD, AUG_PAD, AUG_PAD, AUG_PAD))   # [n, H+8, W+8, C], zeros
+    hs = torch.arange(H, device=dev)
+    ws = torch.arange(W, device=dev)
+    rows = hs.view(1, H) + dy.view(n, 1)                                                     # h + dy in padded coordinates
+    cols = torch.where(flip.view(n, 1), (W - 1 - ws).view(1, W), ws.view(1, W)) + dx.view(n, 1)
+    return padded[torch.arange(n, device=dev).view(n, 1, 1), rows.view(n, H, 1), cols.view(n, 1, W)]
+
+
+def augment_batch(u8_nhwc: torch.Tensor, mean, std, channels_last: bool, key: int, counter: int) -> torch.Tensor:
+    """Augmented, normalised training batch: :func:`augment_u8` then :func:`normalize_batch` (the ATen composition the
+    fused kernel is checked against)."""
+    return normalize_batch(augment_u8(u8_nhwc, key, counter), mean, std, channels_last)
+
+
+# ----------------------------------------------------------------------------
 @dataclass
 class CifarData:
     """The four arrays every driver needs."""
@@ -162,11 +234,14 @@ class ShardLoader:
     ``images``/``labels`` may live on the compute device (HBM-resident dataset)
     or in pinned host memory; in the latter case each batch is gathered by the
     native batch assembler and copied H2D asynchronously, double buffered.
+
+    ``augment=True`` crops and flips every sample at random (see the module docstring) with draws keyed by ``aug_key``;
+    ``aug_counter`` counts the samples handed out so far and advances by the batch size with every yielded batch.
     """
 
     def __init__(self, images: torch.Tensor, labels: torch.Tensor, indices: Sequence[int], batch_size: int,
                  device: torch.device, mean, std, shuffle: bool = True, seed: int = 0,
-                 channels_last: bool = False, with_labels: bool = True):
+                 channels_last: bool = False, with_labels: bool = True, augment: bool = False, aug_key: int = 0):
         self.images, self.labels = images, labels
         self.index = torch.as_tensor(list(indices) if not isinstance(indices, torch.Tensor) else indices, dtype=torch.int64)
         self.batch_size = int(batch_size)
@@ -176,6 +251,9 @@ class ShardLoader:
         self.gen = torch.Generator().manual_seed(seed)
         self.channels_last = channels_last
         self.with_labels = with_labels
+        self.augment = bool(augment)
+        self.aug_key = int(aug_key) & _MASK64
+        self.aug_counter = 0
         self.prefetch_order = True     # see _device_order(); a loader abandoned mid-epoch simply never prefetches
         self._next_order = None
         self.host_resident = not images.is_cuda and self.device.type == "cuda"
@@ -223,7 +301,10 @@ class ShardLoader:
                 self._next_order = None
                 self._next_order = self._device_order()
             idx = dev_order[b * self.batch_size:(b + 1) * self.batch_size]
-            x = normalize_batch(self.images.index_select(0, idx), self.mean, self.std, self.channels_last)
+            if self.augment:
+                x = self._augmented(self.images, idx)
+            else:
+                x = normalize_batch(self.images.index_select(0, idx), self.mean, self.std, self.channels_last)
             y = self.labels.index_select(0, idx)
             if x.device != self.device:
                 x, y = x.to(self.device), y.to(self.device)
@@ -234,5 +315,23 @@ class ShardLoader:
         asm.start_epoch(order)
         for b in range(nb):
             u8, lab = asm.next_batch_to(self.device)  # pinned staging -> async H2D on the copy stream
-            x = normalize_batch(u8, self.mean, self.std, self.channels_last)
+            if self.augment:
+                x = self._augmented(u8, None)
+            else:
+                x = normalize_batch(u8, self.mean, self.std, self.channels_last)
             yield x, lab
+
+    def _augmented(self, images: torch.Tensor, idx: Optional[torch.Tensor]) -> torch.Tensor:
+        """Augmented, normalised batch of ``images[idx]`` (``images`` itself when ``idx`` is None); advances the counter."""
+        counter = self.aug_counter
+        self.aug_counter += images.shape[0] if idx is None else idx.numel()
+        if images.is_cuda:
+            from ..ops import functional as FX
+
+            if FX.fast_path_enabled():
+                from ..ops import cuda_ops
+
+                return cuda_ops.augment_normalize_u8(images, idx, self.aug_key, counter, self.mean, self.std,
+                                                     self.channels_last)   # gather + crop + flip + normalise: one launch
+        u8 = images if idx is None else images.index_select(0, idx)
+        return augment_batch(u8, self.mean, self.std, self.channels_last, self.aug_key, counter)

@@ -16,6 +16,7 @@ Kernel inventory (SURVEY §2.10 ids):
   G10 vae_loss             single fused reduction fwd, elementwise bwd
   G14-16 flat ops          adam_prox, penalty, L-BFGS algebra (see flatops.py)
   G22 normalize_u8         uint8 NHWC -> normalised float, layout change fused
+      augment_normalize_u8 the same with batch gather + random padded crop + horizontal flip fused (training augmentation)
 
 Reference call sites these replace (library calls in the reference): conv + BatchNorm + ELU + residual
 ``src/simple_models.py:137-153`` / ``:191-216``, ``avg_pool2d`` + ``linear`` ``:213-216``, cross-entropy
@@ -125,6 +126,21 @@ def normalize_u8(u8_nhwc: torch.Tensor, mean, std, channels_last: bool) -> torch
         out = ext().normalize_u8(u8, list(mean), list(std), 3, False)   # [N,H,W,3]
         return out.permute(0, 3, 1, 2)
     return ext().normalize_u8(u8, list(mean), list(std), 3, True)
+
+
+def augment_normalize_u8(images_u8: torch.Tensor, rows: Optional[torch.Tensor], key: int, counter: int, mean, std,
+                         channels_last: bool) -> torch.Tensor:
+    """Training batch in one launch: ``images_u8[rows]`` (or ``images_u8`` itself when ``rows`` is None), each sample
+    randomly cropped from its 4-pixel zero-padded image and randomly flipped, then normalised as :func:`normalize_u8`.
+    Sample ``i`` draws from ``(key, counter + i)`` as ``data.cifar.augment_draws`` documents."""
+    u8 = images_u8.contiguous()
+    k = int(key) & 0xFFFFFFFFFFFFFFFF
+    k = k - (1 << 64) if k >= (1 << 63) else k                           # the key's bit pattern as an int64
+    if rows is not None:
+        rows = rows.to(torch.int64).contiguous()
+    if channels_last:
+        return ext().augment_normalize_u8(u8, rows, k, int(counter), list(mean), list(std), False).permute(0, 3, 1, 2)
+    return ext().augment_normalize_u8(u8, rows, k, int(counter), list(mean), list(std), True)
 
 
 # ----------------------------------------------------------------------------

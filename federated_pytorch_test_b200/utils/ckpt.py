@@ -80,7 +80,8 @@ def save_resume(path: str, engine, position: Dict) -> str:
     """True resume record (SURVEY §5.4), written by the engine after every aggregation round when
     ``EngineConfig.resume_path`` is set: schedule position ``(nloop, visit, round)`` = where to RE-ENTER, consensus
     state of the open block visit (z, y_k, rho table, BB vectors), per-replica weights + BatchNorm buffers, the
-    optimizers' flat state (Adam moments + step / L-BFGS history, direction, Welford statistics), loader RNG streams,
+    optimizers' flat state (Adam moments + step / L-BFGS history, direction, Welford statistics), loader RNG streams and
+    augmentation counters,
     global RNG states and the run counters.  Written atomically (tmp + rename); one file per rank."""
     strat_state = {}
     for k, v in engine.strategy.state().items():
@@ -97,7 +98,8 @@ def save_resume(path: str, engine, position: Dict) -> str:
     for ck, ld in getattr(engine.task, "_loaders", {}).items():
         if hasattr(ld, "gen"):
             nxt = getattr(ld, "_next_order", None)        # the next epoch's permutation may already have been drawn (prefetch)
-            loaders[ck] = {"gen": ld.gen.get_state(), "next_order": None if nxt is None else nxt.detach().cpu().clone()}
+            loaders[ck] = {"gen": ld.gen.get_state(), "next_order": None if nxt is None else nxt.detach().cpu().clone(),
+                           "aug_counter": int(getattr(ld, "aug_counter", 0))}
     rec = {
         "position": dict(position),
         "strategy": engine.strategy.name,
@@ -145,6 +147,7 @@ def load_resume(path: str, engine) -> Dict:
             ld.gen.set_state(state["gen"])
             nxt = state.get("next_order")
             ld._next_order = None if nxt is None else nxt.to(ld.images.device)
+            ld.aug_counter = int(state.get("aug_counter", 0))      # augmentation draws continue where the record left off
     cnt = rec.get("counters") or {}
     engine.images_seen = int(cnt.get("images_seen", 0))
     engine.steps_done = int(cnt.get("steps_done", 0))
