@@ -112,6 +112,95 @@ class FedAvg(Strategy):
         self.z.copy_(st["z"].to(self.z.device))
 
 
+class FedOpt(FedAvg):
+    """FedAvg with a server optimizer (FedAvgM, Hsu et al. 2019; FedAdagrad / FedAdam / FedYogi, Reddi et al. 2021,
+    Algorithm 2 without bias correction).  The round's mean change ``d = mean_k x_k - z`` is a pseudo-gradient:
+
+    * avgm:     ``m <- beta m + d``;                                          ``z <- z + lr m``
+    * adagrad:  ``m <- beta1 m + (1 - beta1) d``;  ``v <- v + d^2``;          ``z <- z + lr m / (sqrt(v) + tau)``
+    * adam:     same ``m``;  ``v <- beta2 v + (1 - beta2) d^2``;              same ``z``
+    * yogi:     same ``m``;  ``v <- v - (1 - beta2) d^2 sign(v - d^2)``;      same ``z``
+
+    and the new ``z`` is written into every replica, as FedAvg does.  ``z`` is the server model: the mean of the replicas
+    at the start of a block visit (one extra aggregation launch per visit).  ``m`` / ``v`` belong to a block and persist
+    across its visits for the whole run (``m = 0``, ``v = tau^2`` at its first visit); on the fused collective they are
+    slices of symmetric arenas, so two-shot ranks broadcast their slice of both into every rank and every rank ends each
+    round with the same ``z``, ``m`` and ``v``."""
+
+    name = "fedopt"
+
+    def __init__(self, collective, topo, kind: str = "adam", lr: float = 0.0, momentum: float = 0.9, beta1: float = 0.9,
+                 beta2: float = 0.99, tau: float = 1e-3):
+        from ..config import check_server_opt
+        from ..parallel.collective import FEDOPT_KINDS
+
+        super().__init__(collective, topo)
+        if kind not in FEDOPT_KINDS:
+            raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
+        check_server_opt(kind, lr, momentum, beta1, beta2, tau)
+        self.kind = kind
+        self.adaptive = kind != "avgm"
+        self.lr = float(lr) or (1e-2 if self.adaptive else 1.0)
+        self.beta1 = float(beta1 if self.adaptive else momentum)
+        self.beta2, self.tau = float(beta2), float(tau)
+        self.m: Optional[torch.Tensor] = None
+        self.v: Optional[torch.Tensor] = None
+        self.ms: Dict[int, torch.Tensor] = {}              # block index -> server state slice, for the whole run
+        self.vs: Dict[int, torch.Tensor] = {}
+        self._restored: Dict[int, tuple] = {}              # state of blocks read from a resume record, installed at their visit
+        if hasattr(collective, "warm_fedopt"):
+            collective.warm_fedopt = True
+
+    def begin_block(self, ci: int, N: int, xs: List[torch.Tensor]) -> None:
+        super().begin_block(ci, N, xs)
+        if ci not in self.ms:
+            self.ms[ci] = self.coll.zeros_like_block(xs[0], "srv_m")
+            if self.adaptive:
+                self.vs[ci] = self.coll.zeros_like_block(xs[0], "srv_v").fill_(self.tau * self.tau)
+            if ci in self._restored:
+                self._install(ci, *self._restored.pop(ci))
+        self.m, self.v = self.ms[ci], self.vs.get(ci)
+        self.coll.fedavg_(xs, self.z, write_back=False)          # the server model: the replicas' mean, no write-back
+
+    def _hyper(self):
+        return self.kind, self.lr, self.beta1, self.beta2, self.tau
+
+    def aggregate(self, nadmm: int) -> Dict[str, float]:
+        dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper())
+        return {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}
+
+    def aggregate_begin(self, nadmm: int):
+        if getattr(self.coll, "supports_async", False):
+            self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper())
+            return ("pending", self.N)
+        return ("done", self.aggregate(nadmm))
+
+    def state(self) -> Dict[str, object]:
+        """``z`` and the state of every block visited so far in the run, including blocks restored from a resume record
+        that this process has not visited yet (their state is still the recorded one)."""
+        ms = {ci: m for ci, (m, _) in self._restored.items()}
+        vs = {ci: v for ci, (_, v) in self._restored.items() if v is not None}
+        ms.update(self.ms)
+        vs.update(self.vs)
+        return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs}
+
+    def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
+        self.ms[ci].copy_(m.to(self.ms[ci].device))
+        if self.adaptive:
+            self.vs[ci].copy_(v.to(self.vs[ci].device))
+
+    def load_state(self, st: Dict[str, object]) -> None:
+        if st.get("server_opt") != self.kind:
+            raise ValueError("resume record holds server optimizer %r, this run uses %r" % (st.get("server_opt"), self.kind))
+        self.z.copy_(st["z"].to(self.z.device))
+        vs = st.get("v") or {}
+        for ci, m in (st.get("m") or {}).items():
+            if ci in self.ms:
+                self._install(ci, m, vs.get(ci))
+            else:                                                 # buffers are made at the block's next visit
+                self._restored[ci] = (m, vs.get(ci))
+
+
 class FedProx(Strategy):
     name = "fedprox"
 

@@ -69,10 +69,38 @@ class NoConsensusConfig(CommonConfig):
     Nadmm: int = 1
 
 
+SERVER_OPTS = ("none", "avgm", "adagrad", "adam", "yogi")
+
+
+def check_server_opt(server_opt: str, server_lr: float, server_momentum: float, server_beta1: float, server_beta2: float,
+                     server_tau: float) -> None:
+    """Raise ``ValueError`` unless the server-optimizer settings of :class:`FederatedConfig` are valid."""
+    if server_opt not in SERVER_OPTS:
+        raise ValueError("server_opt must be one of %s, got %r" % (", ".join(SERVER_OPTS), server_opt))
+    if not server_lr >= 0.0:
+        raise ValueError("server_lr must be >= 0, got %r" % (server_lr,))
+    for name, val in (("server_momentum", server_momentum), ("server_beta1", server_beta1), ("server_beta2", server_beta2)):
+        if not 0.0 <= val < 1.0:
+            raise ValueError("%s must lie in [0, 1), got %r" % (name, val))
+    if not server_tau > 0.0:
+        raise ValueError("server_tau must be > 0, got %r" % (server_tau,))
+
+
 @dataclass
 class FederatedConfig(CommonConfig):
     lambda1: float = 0.0001
     lambda2: float = 0.0001
+    # server optimizer on the round's mean change (FedAvgM, FedAdagrad, FedAdam, FedYogi); 'none' = plain FedAvg
+    server_opt: str = "none"        # 'none' | 'avgm' | 'adagrad' | 'adam' | 'yogi'
+    server_lr: float = 0.0          # 0 = the variant's default: 1.0 for avgm, 1e-2 for adagrad / adam / yogi
+    server_momentum: float = 0.9    # avgm
+    server_beta1: float = 0.9       # adagrad / adam / yogi
+    server_beta2: float = 0.99      # adam / yogi
+    server_tau: float = 1e-3        # adaptivity floor: z += lr m / (sqrt(v) + tau); v starts at tau^2
+
+    def __post_init__(self):
+        check_server_opt(self.server_opt, self.server_lr, self.server_momentum, self.server_beta1, self.server_beta2,
+                         self.server_tau)
 
 
 @dataclass

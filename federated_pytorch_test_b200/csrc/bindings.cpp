@@ -628,6 +628,58 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
   fb::block_reduce_launch(a, cur_stream());
 }
 
+// FedAvg with a server optimizer (FedOpt instantiation of the aggregation kernel): opt = FEDOPT_AVGM .. FEDOPT_YOGI, m / v
+// the server state slices (v unused by avgm), mw / vw and mc_m / mc_v their two-shot broadcast targets.
+void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, double tau, Tensor m, c10::optional<Tensor> v,
+                         std::vector<int64_t> x_ptrs, std::vector<int64_t> local_idx, Tensor z, int64_t n, Tensor out,
+                         Tensor scratch, std::vector<int64_t> ctrl_ptrs, Tensor sync, int64_t world, int64_t rank,
+                         int64_t mc_x, int64_t mc_m, int64_t mc_v, std::vector<int64_t> xw_ptrs,
+                         std::vector<int64_t> mw_ptrs, std::vector<int64_t> vw_ptrs, bool two_shot, int64_t max_blocks,
+                         double timeout_s) {
+  TORCH_CHECK(opt >= fb::FEDOPT_AVGM && opt <= fb::FEDOPT_YOGI, "block_reduce_fedopt: unknown server optimizer ", opt);
+  const bool adaptive = opt != fb::FEDOPT_AVGM;
+  CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch); CHECK_F32_CUDA(m); CHECK_CONTIG(m);
+  TORCH_CHECK(out.numel() >= fb::COMM_OUT_FLOATS && scratch.numel() >= fb::COMM_SCRATCH_FLOATS, "out / scratch too small");
+  TORCH_CHECK(z.numel() == n && m.numel() == n, "block_reduce_fedopt: z and m must have the block's length");
+  if (adaptive) {
+    TORCH_CHECK(v.has_value() && v->defined(), "block_reduce_fedopt: adaptive server optimizers need v");
+    CHECK_F32_CUDA((*v)); CHECK_CONTIG((*v));
+    TORCH_CHECK(v->numel() == n, "block_reduce_fedopt: v must have the block's length");
+  }
+  c10::cuda::CUDAGuard guard(z.device());
+  fb::CommArgs a{};
+  a.mode = 0; a.K = (int)x_ptrs.size(); a.n_local = (int)local_idx.size(); a.world = (int)world; a.rank = (int)rank;
+  a.n = (int)n; a.two_shot = two_shot ? 1 : 0; a.max_blocks = (int)max_blocks;
+  TORCH_CHECK(a.K <= fb::COMM_MAX_K && a.n_local <= fb::COMM_MAX_LOCAL && a.world <= fb::COMM_MAX_WORLD,
+              "block_reduce_fedopt: limits exceeded");
+  for (int k = 0; k < a.K; ++k) a.x[k] = reinterpret_cast<const float*>(x_ptrs[k]);
+  for (int j = 0; j < a.n_local; ++j) a.xl[j] = reinterpret_cast<float*>(x_ptrs[local_idx[j]]);
+  for (int p = 0; p < a.world; ++p) {
+    a.xw[p] = p < (int)xw_ptrs.size() ? reinterpret_cast<float*>(xw_ptrs[p]) : nullptr;
+    a.mw[p] = p < (int)mw_ptrs.size() ? reinterpret_cast<float*>(mw_ptrs[p]) : nullptr;
+    a.vw[p] = p < (int)vw_ptrs.size() ? reinterpret_cast<float*>(vw_ptrs[p]) : nullptr;
+  }
+  if (a.two_shot) {
+    TORCH_CHECK(mc_x != 0 || (int)xw_ptrs.size() == a.world, "two-shot FedOpt needs broadcast targets for the weights");
+    TORCH_CHECK(mc_m != 0 || (int)mw_ptrs.size() == a.world, "two-shot FedOpt needs peer-mapped m");
+    TORCH_CHECK(!adaptive || mc_v != 0 || (int)vw_ptrs.size() == a.world, "two-shot FedOpt needs peer-mapped v");
+  }
+  a.mc_x = reinterpret_cast<float*>(mc_x);
+  a.mc_m = reinterpret_cast<float*>(mc_m);
+  a.mc_v = reinterpret_cast<float*>(mc_v);
+  a.z = z.data_ptr<float>();
+  a.out = out.data_ptr<float>();
+  a.scratch = scratch.data_ptr<float>();
+  fill_ctrl(a.ctrl, ctrl_ptrs, a.world);
+  a.sync = reinterpret_cast<uint32_t*>(sync.data_ptr<int>());
+  a.timeout_cycles = (long long)(timeout_s * 1.9e9);
+  a.opt = (int)opt;
+  a.lr = (float)lr; a.beta1 = (float)beta1; a.beta2 = (float)beta2; a.tau = (float)tau;
+  a.m = m.data_ptr<float>();
+  a.v = adaptive ? v->data_ptr<float>() : nullptr;
+  fb::block_reduce_launch(a, cur_stream());
+}
+
 // Barzilai-Borwein update (consensus_multi.py:242-278) as one kernel; see BBArgs.
 void bb_update(std::vector<Tensor> xs, std::vector<Tensor> ys, std::vector<Tensor> yhat0s, std::vector<Tensor> x0s, Tensor z,
                std::vector<int64_t> workers, int64_t K, Tensor rho_dev, Tensor log, Tensor scratch, Tensor out,
@@ -749,6 +801,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("smallconv_dgrad", &smallconv_dgrad);
   m.def("smallconv_wgrad", &smallconv_wgrad);
   m.def("block_reduce", &block_reduce);
+  m.def("block_reduce_fedopt", &block_reduce_fedopt);
   m.def("bb_update", &bb_update);
   m.def("ipc_get_handle", &ipc_get_handle);
   m.def("ipc_open_handle", &ipc_open_handle);

@@ -24,6 +24,8 @@
 // rank (threads 0..world-1 signal / poll one peer each): there is no grid-wide barrier in the kernel.
 //
 // mode: 0 = FedAvg (z = sum x / K, write-back), 1 = FedProx (no write-back), 2 = ADMM (z = sum(y + rho x)/(K rho)).
+// A second instantiation (FEDOPT) runs FedAvg with a server optimizer (FedAvgM / FedAdagrad / FedAdam / FedYogi) between
+// the reduction and the write-back.
 // Reference sites: /root/reference/src/federated_multi.py:203-217, fedprox_multi.py:211-232, consensus_multi.py:242-299.
 #include "fedb200.h"
 
@@ -149,6 +151,36 @@ __device__ __forceinline__ float4 gather_v4(const CommArgs& a, size_t off, float
   return acc;
 }
 
+// Server optimizer step on one element (Reddi et al. 2021, Algorithm 2, no bias correction; FedAvgM: Hsu et al. 2019).
+// d = mean - z is the round's pseudo-gradient; m and v are updated in place; returns the new server model.
+__device__ __forceinline__ float fedopt_step(const CommArgs& a, float z, float mean, float& m, float& v) {
+  const float d = mean - z;
+  if (a.opt == FEDOPT_AVGM) {                       // z + lr m, evaluated as mean + (lr m - d): exactly FedAvg's mean when
+    m = fmaf(a.beta1, m, d);                        // beta = 0 and lr = 1
+    return mean + fmaf(a.lr, m, -d);
+  }
+  m = fmaf(a.beta1, m, (1.f - a.beta1) * d);
+  const float d2 = d * d;
+  if (a.opt == FEDOPT_ADAGRAD) {
+    v += d2;
+  } else if (a.opt == FEDOPT_ADAM) {
+    v = fmaf(a.beta2, v, (1.f - a.beta2) * d2);
+  } else {                                          // yogi: v - (1 - beta2) d^2 sign(v - d^2)
+    const float s = v > d2 ? 1.f : (v < d2 ? -1.f : 0.f);
+    v = fmaf(-(1.f - a.beta2) * d2, s, v);
+  }
+  return fmaf(a.lr, m / (sqrtf(v) + a.tau), z);
+}
+__device__ __forceinline__ float4 fedopt_step_v4(const CommArgs& a, float4 z, float4 mean, float4& m, float4& v) {
+  return make_float4(fedopt_step(a, z.x, mean.x, m.x, v.x), fedopt_step(a, z.y, mean.y, m.y, v.y),
+                     fedopt_step(a, z.z, mean.z, m.z, v.z), fedopt_step(a, z.w, mean.w, m.w, v.w));
+}
+
+// FEDOPT = false: FedAvg / FedProx / ADMM (a.mode).  FEDOPT = true: FedAvg (mode 0) whose new model is a server optimizer
+// step from z instead of the plain mean.  Pass 1 forms the step from the reduced mean, z and the state m (and v): one-shot
+// stores z, m, v locally; two-shot rank r broadcasts slice r of the new weights, of m and of v into every rank, so every rank
+// ends the round with the same z, m and v.  Pass 2 is FedAvg's.
+template <bool FEDOPT>
 __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const CommArgs a) {
   __shared__ float sm[32];
   __shared__ int s_abort;
@@ -189,6 +221,31 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
         const size_t off = u == 0 ? off0 : off1;
         const float4 acc = accs[u];
         const float4 zn = make_float4(acc.x * inv_scale, acc.y * inv_scale, acc.z * inv_scale, acc.w * inv_scale);
+        if constexpr (FEDOPT) {
+          const bool adaptive = a.opt != FEDOPT_AVGM;
+          const float4 zo = *reinterpret_cast<const float4*>(a.z + off);
+          float4 mv = *reinterpret_cast<const float4*>(a.m + off);
+          float4 vv = adaptive ? *reinterpret_cast<const float4*>(a.v + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 zs = fedopt_step_v4(a, zo, zn, mv, vv);
+          if (!a.two_shot) {
+            const float dx = zo.x - zs.x, dy = zo.y - zs.y, dz = zo.z - zs.z, dw = zo.w - zs.w;
+            dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
+            if (!(isfinite(zs.x) && isfinite(zs.y) && isfinite(zs.z) && isfinite(zs.w))) bad += 1.f;
+            *reinterpret_cast<float4*>(a.z + off) = zs;
+            *reinterpret_cast<float4*>(a.m + off) = mv;
+            if (adaptive) *reinterpret_cast<float4*>(a.v + off) = vv;
+          } else {                                 // weights, m and v of slice r into every rank (dual + NaN check: pass 2)
+            if (a.mc_x != nullptr) multimem_st_v4(a.mc_x + off, zs);
+            else for (int p = 0; p < a.world; ++p) st_sys_v4(a.xw[p] + off, zs);
+            if (a.mc_m != nullptr) multimem_st_v4(a.mc_m + off, mv);
+            else for (int p = 0; p < a.world; ++p) st_sys_v4(a.mw[p] + off, mv);
+            if (adaptive) {
+              if (a.mc_v != nullptr) multimem_st_v4(a.mc_v + off, vv);
+              else for (int p = 0; p < a.world; ++p) st_sys_v4(a.vw[p] + off, vv);
+            }
+          }
+          continue;
+        }
         if (!(a.two_shot && a.mode == 0)) {       // two-shot FedAvg takes both from the finished weights in pass 2
           const float4 zo = *reinterpret_cast<const float4*>(a.z + off);
           const float dx = zo.x - zn.x, dy = zo.y - zn.y, dz = zo.z - zn.z, dw = zo.w - zn.w;
@@ -221,7 +278,13 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
         acc += a.mode == 2 ? fmaf(rho, xv, ld_sys_f32(a.y[k] + i)) : xv;
       }
     }
-    const float zn = acc * inv_scale;
+    float zn = acc * inv_scale;
+    if constexpr (FEDOPT) {                        // every rank steps its own copy of the tail
+      float mv = a.m[i], vv = a.opt != FEDOPT_AVGM ? a.v[i] : 0.f;
+      zn = fedopt_step(a, a.z[i], zn, mv, vv);
+      a.m[i] = mv;
+      if (a.opt != FEDOPT_AVGM) a.v[i] = vv;
+    }
     const float d = a.z[i] - zn;
     if (!a.two_shot || a.mode == 0 || a.rank == 0) dual = fmaf(d, d, dual);     // two-shot FedProx/ADMM: the dual parts are summed over ranks
     if (!isfinite(zn)) bad += 1.f;
@@ -387,9 +450,14 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
     throw std::runtime_error("fedb200: block_reduce: too many contributions / replicas / ranks");
   if (args.two_shot && (args.world <= 1 || args.n_local != 1 || args.K != args.world))
     throw std::runtime_error("fedb200: two-shot aggregation needs one replica per rank");
-  static int max_blocks = 0;
-  if (max_blocks == 0) max_blocks = comm_max_blocks((const void*)block_reduce_kernel);
-  int cap = max_blocks;
+  if (args.opt != FEDOPT_NONE &&
+      (args.opt > FEDOPT_YOGI || args.mode != 0 || args.m == nullptr || (args.opt != FEDOPT_AVGM && args.v == nullptr)))
+    throw std::runtime_error("fedb200: block_reduce: server optimizer needs mode 0 and its state vectors");
+  const void* kernel = args.opt != FEDOPT_NONE ? (const void*)block_reduce_kernel<true> : (const void*)block_reduce_kernel<false>;
+  static int max_blocks[2] = {0, 0};
+  int& mb = max_blocks[args.opt != FEDOPT_NONE];
+  if (mb == 0) mb = comm_max_blocks(kernel);
+  int cap = mb;
   if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;
   const int n4 = args.n >> 2;
   const int work4 = args.two_shot ? (n4 + args.world - 1) / args.world : n4;
@@ -402,8 +470,8 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   // it (A/B runs).
   static const int coop = env_int_c("FEDB200_COMM_COOP", 0);
   cudaError_t e;
-  if (coop) e = cudaLaunchCooperativeKernel((void*)block_reduce_kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
-  else e = cudaLaunchKernel((void*)block_reduce_kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
+  if (coop) e = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
+  else e = cudaLaunchKernel(kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
   if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: block_reduce launch: ") + cudaGetErrorString(e));
   count_launch();
 }

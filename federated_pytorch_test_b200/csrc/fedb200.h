@@ -210,7 +210,18 @@ struct CommArgs {
   uint32_t* ctrl[COMM_MAX_WORLD];    // control pads of every rank (peer-mapped), COMM_PAD_WORDS words each
   uint32_t* sync;                    // local: [0] = epoch of the last completed collective
   long long timeout_cycles;          // per barrier; a timeout sets out[OUT_STATUS] = 100 + missing rank and lets the kernel end
+  // ---- server optimizer (FedOpt instantiation only; mode must be 0): d = mean - z is a pseudo-gradient, the step replaces
+  // the plain mean as the new model.  m / v persist across rounds in device memory.
+  int opt;                           // FEDOPT_NONE selects the FedAvg / FedProx / ADMM kernel
+  float lr, beta1, beta2, tau;       // avgm: beta1 is the momentum
+  float* m;                          // local server state slices: momentum / first moment, second moment (adaptive only)
+  float* v;
+  float* mw[COMM_MAX_WORLD];         // two-shot: rank p's m / v slice (broadcast targets over P2P)
+  float* vw[COMM_MAX_WORLD];
+  float* mc_m;                       // multicast addresses of the m / v slices (multimem.st) or nullptr
+  float* mc_v;
 };
+constexpr int FEDOPT_NONE = 0, FEDOPT_AVGM = 1, FEDOPT_ADAGRAD = 2, FEDOPT_ADAM = 3, FEDOPT_YOGI = 4;
 void block_reduce_launch(const CommArgs& args, cudaStream_t s);
 
 // Barzilai-Borwein / spectral penalty update of consensus ADMM as ONE kernel (SURVEY G20, X4): six dots per worker

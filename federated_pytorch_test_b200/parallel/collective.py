@@ -4,7 +4,8 @@ Logical collectives of the reference (SURVEY §2.9; Python loops over a dict on
 one device):
 
 * X1 FedAvg  ``z' = sum_k x_k / K``; ``dual = ||z - z'||``; write ``z'`` into every replica
-  (/root/reference/src/federated_multi.py:204-217)
+  (/root/reference/src/federated_multi.py:204-217); with a server optimizer (``fedopt_``) ``z'`` is its step from ``z``
+  along ``mean_k x_k - z`` instead of the plain mean
 * X2 FedProx ``z' = mean``; ``dual``; ``primal = sum_k ||rho (x_k - z')||``; no write-back
   (fedprox_multi.py:211-232)
 * X3 ADMM    ``z' = sum_k (y_k + rho x_k) / (K rho)``; ``dual``; ``y_k += rho (x_k - z')``;
@@ -26,6 +27,9 @@ import torch
 import torch.distributed as dist
 
 from .topology import Topology
+
+# server optimizers of FedAvg (Hsu et al. 2019; Reddi et al. 2021), in the order of the kernel's codes 1..4
+FEDOPT_KINDS = ("avgm", "adagrad", "adam", "yogi")
 
 
 class TorchCollective:
@@ -88,6 +92,36 @@ class TorchCollective:
         if write_back:
             for x in xs:
                 x.copy_(znew)
+        return dual_sq
+
+    @torch.no_grad()
+    def fedopt_(self, xs: List[torch.Tensor], z: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], kind: str,
+                lr: float, beta1: float, beta2: float, tau: float) -> torch.Tensor:
+        """FedAvg with a server optimizer, in place: ``d = mean_k x_k - z`` is the pseudo-gradient of server optimizer
+        ``kind`` (one of :data:`FEDOPT_KINDS`; ``beta1`` is the momentum of 'avgm'), whose state ``m`` (and ``v``, unused
+        by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``."""
+        mean = self.sum_blocks(xs).div_(self.topo.K)
+        d = mean - z
+        if kind == "avgm":
+            m.mul_(beta1).add_(d)
+            znew = mean + (lr * m - d)          # = z + lr m; exactly the mean when beta = 0 and lr = 1 (FedAvg)
+        else:
+            m.mul_(beta1).add_(d, alpha=1.0 - beta1)
+            d2 = d * d
+            if kind == "adagrad":
+                v.add_(d2)
+            elif kind == "adam":
+                v.mul_(beta2).add_(d2, alpha=1.0 - beta2)
+            elif kind == "yogi":
+                v.sub_((1.0 - beta2) * d2 * torch.sign(v - d2))
+            else:
+                raise ValueError("unknown server optimizer %r" % (kind,))
+            znew = z + lr * m / (v.sqrt() + tau)
+        diff = z - znew
+        dual_sq = torch.dot(diff, diff)
+        z.copy_(znew)
+        for x in xs:
+            x.copy_(znew)
         return dual_sq
 
     @torch.no_grad()

@@ -36,7 +36,7 @@ import torch
 import torch.distributed as dist
 
 from ..ops import cuda_ops
-from .collective import TorchCollective
+from .collective import FEDOPT_KINDS, TorchCollective
 from .topology import Topology
 
 _MAX_LOCAL = 16
@@ -166,11 +166,13 @@ class FusedCollective(TorchCollective):
         self.last_nonfinite = 0.0
         self.last_two_shot = False
         self.last_rho = float("nan")
+        self.warm_fedopt = False          # set by the FedOpt strategy: warm the server-optimizer instantiation too
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
         cross-rank handshake happen here, at engine construction, not inside the first training round (the first launch
-        is far slower than the ones after it).  Collective: every rank calls it at the same point."""
+        is far slower than the ones after it).  The server-optimizer kernel is warmed only when ``warm_fedopt`` is set.
+        Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
         self._warm = True
@@ -179,12 +181,16 @@ class FusedCollective(TorchCollective):
         ys = [self.zeros_like_block(x, "y") for x in xs]
         z = self.zeros_like_block(xs[0], "z")
         rho = torch.full((1,), 0.5, dtype=torch.float32, device=self.topo.device)
+        if self.warm_fedopt:
+            m, v = self.zeros_like_block(xs[0], "srv_m"), self.zeros_like_block(xs[0], "srv_v")
         keep = self.two_shot_mode
         for mode_2shot in ("0", "1"):
             self.two_shot_mode = mode_2shot
             self._launch(0, xs, None, z, 0.0)
             self._launch(1, xs, None, z, 0.5)
             self._launch(2, xs, ys, z, 0.5, rho)
+            if self.warm_fedopt:
+                self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3)
         self.two_shot_mode = keep
         x0 = [torch.zeros_like(x) for x in xs]
         yh = [torch.zeros_like(x) for x in xs]
@@ -262,6 +268,31 @@ class FusedCollective(TorchCollective):
         self.launches += 1
         self.last_two_shot = bool(two)
 
+    def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float) -> None:
+        """FedAvg with a server optimizer: mode 0 of the kernel's FedOpt instantiation.  Two-shot, rank r broadcasts slice r
+        of the new weights, of ``m`` and of ``v`` into every rank, so ``m`` / ``v`` must be symmetric slices then
+        (:meth:`zeros_like_block`)."""
+        n = xs[0].numel()
+        adaptive = kind != "avgm"
+        if any(t.numel() != n for t in xs) or z.numel() != n or m.numel() != n or (adaptive and v.numel() != n):
+            raise ValueError("block slices must have equal length")
+        W = self.topo.world_size
+        xp, local_idx, mcx = self._tables(xs)
+        two = self._want_two_shot(0, xs, z, n) and self.heap.contains(m) and (not adaptive or self.heap.contains(v))
+        mcm = mcv = 0
+        xw, mw, vw = [], [], []
+        if two:
+            xw = [xp[r] for r in range(W)]
+            mw, _, mcm = self._tables([m])
+            if adaptive:
+                vw, _, mcv = self._tables([v])
+        self.ext.block_reduce_fedopt(FEDOPT_KINDS.index(kind) + 1, float(lr), float(beta1), float(beta2), float(tau), m,
+                                     v if adaptive else None, xp, local_idx, z, n, self.out, self.scratch, self.ctrl_ptrs,
+                                     self.sync, W, self.topo.rank, mcx, mcm, mcv, xw, mw, vw, bool(two), self.max_blocks,
+                                     self.timeout_s)
+        self.launches += 1
+        self.last_two_shot = bool(two)
+
     supports_async = True
 
     def _record_async(self) -> None:
@@ -275,6 +306,10 @@ class FusedCollective(TorchCollective):
 
     def launch_fedavg_(self, xs, z, write_back: bool = True) -> None:
         self._launch(0 if write_back else 1, xs, None, z, 0.0)
+        self._record_async()
+
+    def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float) -> None:
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau)
         self._record_async()
 
     def launch_fedprox_(self, xs, z, rho: float) -> None:
@@ -304,6 +339,11 @@ class FusedCollective(TorchCollective):
     @torch.no_grad()
     def fedavg_(self, xs, z, write_back: bool = True):
         self._launch(0 if write_back else 1, xs, None, z, 0.0)
+        return self.read_record()[OUT_DUAL_SQ]
+
+    @torch.no_grad()
+    def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float):
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()

@@ -89,6 +89,8 @@ def save_resume(path: str, engine, position: Dict) -> str:
             strat_state[k] = v.detach().cpu().clone()
         elif isinstance(v, list):
             strat_state[k] = [t.detach().cpu().clone() for t in v]
+        elif isinstance(v, dict):                  # per-block state, e.g. a server optimizer's moments by block index
+            strat_state[k] = {i: t.detach().cpu().clone() for i, t in v.items()}
         else:
             strat_state[k] = v
     opts = {}
