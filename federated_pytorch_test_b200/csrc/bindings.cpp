@@ -253,8 +253,13 @@ Tensor linear_tf32(Tensor x, Tensor w, c10::optional<Tensor> bias, bool act) {
 bool conv_supported(int64_t H_out, int64_t W_out, int64_t C_in, int64_t stride) {
   return fb::conv_geometry_supported((int)H_out, (int)W_out, (int)C_in, (int)stride);
 }
+// Tile orientation the convolution picks by itself for this output shape (fb::CONV_ORIENT_ROW / _PIXEL)
+int64_t conv_orientation(int64_t NB, int64_t H_out, int64_t W_out, int64_t C_out, int64_t stride) {
+  return fb::pick_conv_orientation((int)NB, (int)H_out, (int)W_out, (int)C_out, (int)stride);
+}
 // x: [N,H,W,Ci] contiguous; w: [Co,kh,kw,Ci] contiguous.  Returns y [N,Ho,Wo,Co]; stats (2*Co) accumulated if given.
-Tensor conv2d_nhwc(Tensor x, Tensor w, c10::optional<Tensor> stats, int64_t stride, int64_t pad, int64_t dil) {
+// orient: -1 = chosen from the shape, 0 = row-major tiles, 1 = pixel-major tiles (C_out 64 / 128).
+Tensor conv2d_nhwc(Tensor x, Tensor w, c10::optional<Tensor> stats, int64_t stride, int64_t pad, int64_t dil, int64_t orient) {
   CHECK_F32_CUDA(x); CHECK_F32_CUDA(w); CHECK_CONTIG(x); CHECK_CONTIG(w);
   TORCH_CHECK(x.dim() == 4 && w.dim() == 4 && x.size(3) == w.size(3), "conv2d_nhwc: x [N,H,W,Ci], w [Co,kh,kw,Ci]");
   c10::cuda::CUDAGuard guard(x.device());
@@ -264,7 +269,8 @@ Tensor conv2d_nhwc(Tensor x, Tensor w, c10::optional<Tensor> stats, int64_t stri
   const int Wo = (W + 2 * (int)pad - (int)dil * (kw - 1) - 1) / (int)stride + 1;
   auto y = torch::empty({NB, Ho, Wo, Co}, x.options());
   float* st = (stats.has_value() && stats->defined()) ? stats->data_ptr<float>() : nullptr;
-  fb::conv2d_nhwc_tf32(fptr(x), fptr(w), fptr_mut(y), st, NB, H, W, Ci, Co, kh, kw, (int)stride, (int)pad, (int)dil, Ho, Wo, cur_stream());
+  fb::conv2d_nhwc_tf32(fptr(x), fptr(w), fptr_mut(y), st, NB, H, W, Ci, Co, kh, kw, (int)stride, (int)pad, (int)dil, Ho, Wo, cur_stream(),
+                       (int)orient);
   return y;
 }
 
@@ -340,7 +346,7 @@ Tensor conv2d_nhwc_multidil(Tensor x, Tensor w, c10::optional<Tensor> bias, bool
 }
 
 // y += conv(x, w), in place (experimental)
-Tensor conv2d_nhwc_accumulate(Tensor x, Tensor w, Tensor y, int64_t stride, int64_t pad, int64_t dil) {
+Tensor conv2d_nhwc_accumulate(Tensor x, Tensor w, Tensor y, int64_t stride, int64_t pad, int64_t dil, int64_t orient) {
   CHECK_F32_CUDA(x); CHECK_F32_CUDA(w); CHECK_F32_CUDA(y); CHECK_CONTIG(x); CHECK_CONTIG(w); CHECK_CONTIG(y);
   TORCH_CHECK(x.dim() == 4 && w.dim() == 4 && y.dim() == 4 && x.size(3) == w.size(3), "conv2d_nhwc_accumulate: x [N,H,W,Ci], w [Co,kh,kw,Ci]");
   c10::cuda::CUDAGuard guard(x.device());
@@ -350,7 +356,7 @@ Tensor conv2d_nhwc_accumulate(Tensor x, Tensor w, Tensor y, int64_t stride, int6
   const int Wo = (W + 2 * (int)pad - (int)dil * (kw - 1) - 1) / (int)stride + 1;
   TORCH_CHECK(y.size(0) == NB && y.size(1) == Ho && y.size(2) == Wo && y.size(3) == Co, "conv2d_nhwc_accumulate: y must be [N,Ho,Wo,Co]");
   fb::conv2d_nhwc_accumulate_tf32(fptr(x), fptr(w), fptr_mut(y), NB, H, W, Ci, Co, kh, kw, (int)stride, (int)pad, (int)dil, Ho, Wo,
-                                  cur_stream());
+                                  cur_stream(), (int)orient);
   return y;
 }
 
@@ -767,11 +773,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("convT_pack", &convT_pack);
   m.def("linear_tf32", &linear_tf32);
   m.def("conv_supported", &conv_supported);
-  m.def("conv2d_nhwc", &conv2d_nhwc);
+  m.def("conv_orientation", &conv_orientation);
+  m.def("conv2d_nhwc", &conv2d_nhwc, py::arg("x"), py::arg("w"), py::arg("stats"), py::arg("stride"), py::arg("pad"), py::arg("dil"),
+        py::arg("orient") = -1);
   m.def("conv2d_nhwc_sized", &conv2d_nhwc_sized);
   m.def("conv2d_nhwc_bias_act", &conv2d_nhwc_bias_act);
   m.def("conv2d_nhwc_bn_eval", &conv2d_nhwc_bn_eval);
-  m.def("conv2d_nhwc_accumulate", &conv2d_nhwc_accumulate);
+  m.def("conv2d_nhwc_accumulate", &conv2d_nhwc_accumulate, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("stride"), py::arg("pad"),
+        py::arg("dil"), py::arg("orient") = -1);
   m.def("conv2d_nhwc_shuffle", &conv2d_nhwc_shuffle);
   m.def("conv_shuffle_supported", &conv_shuffle_supported);
   m.def("conv2d_nhwc_multidil", &conv2d_nhwc_multidil);

@@ -45,11 +45,18 @@ int pick_block_n(int M, int N);
 void linear_tf32(const float* x, const float* w, const float* bias, float* out, int M, int N, int K, int ldx, int ldw,
                  int ldo, int act, cudaStream_t stream);
 bool conv_geometry_supported(int H_out, int W_out, int C_in, int stride);
+// Tile orientation of the convolution kernel: ROW = 128 pixels x BLOCK_N channels (igemm_wgmma_kernel), PIXEL = 64 / 128
+// channels x 256 pixels (igemm_wgmma_pix_kernel, C_out 64 or 128); AUTO = the choice of pick_conv_orientation.
+enum { CONV_ORIENT_AUTO = -1, CONV_ORIENT_ROW = 0, CONV_ORIENT_PIXEL = 1 };
+// The orientation conv2d_nhwc_tf32 / conv2d_nhwc_accumulate_tf32 use by themselves for this shape (stride-1/2, no split-K).
+int pick_conv_orientation(int NB, int H_out, int W_out, int C_out, int stride);
 void conv2d_nhwc_tf32(const float* x, const float* w, float* y, float* stats, int NB, int H, int W, int C_in, int C_out,
-                      int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream);
+                      int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream,
+                      int orient = CONV_ORIENT_AUTO);
 // y += conv(x, w) (experimental: residual-gradient accumulation fused into the data-gradient convolution)
 void conv2d_nhwc_accumulate_tf32(const float* x, const float* w, float* y, int NB, int H, int W, int C_in, int C_out, int kh,
-                                 int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream);
+                                 int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream,
+                                 int orient = CONV_ORIENT_AUTO);
 // same kernel with bias + optional ELU in the epilogue (no statistics, no split-K): VAE / CPC convolutions
 void conv2d_nhwc_bias_act_tf32(const float* x, const float* w, const float* bias, int act, float* y, int NB, int H, int W,
                                int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,

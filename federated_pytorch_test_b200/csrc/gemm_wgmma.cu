@@ -150,6 +150,29 @@ static void dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const
   else dispatch_tile<false>(bn, ta, tb, p, s);
 }
 
+// Pixel-major kernel (C_out = 64 / 128): 4 stages of [256 pixels | C_out weight rows] x 32 channels next to 32 KB of staging.
+template <int CO>
+static void launch_pix(const CUtensorMap& ta, const CUtensorMap& tb, IgemmParams p, cudaStream_t stream) {
+  constexpr int ST = 4;
+  using S = PixSmem<CO, ST>;
+  auto kernel = igemm_wgmma_pix_kernel<CO, ST>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
+    if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: cudaFuncSetAttribute(igemm_pix): ") + cudaGetErrorString(e));
+    configured = true;
+  }
+  p.m_tiles = (p.M + PX_BLOCK_M - 1) / PX_BLOCK_M;
+  p.n_tiles = 1;
+  p.total_tiles = p.m_tiles;
+  p.tma_store = 1;
+  const CUtensorMap tc = make_tmap_out(p.out, p.M, p.N, p.ldo, 32);
+  const int grid = std::min(p.total_tiles, num_sms());
+  cudaError_t e = launch_pdl(kernel, dim3(grid), dim3(IG_THREADS), S::TOTAL, stream, ta, tb, tc, p);
+  if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: igemm_pix launch: ") + cudaGetErrorString(e));
+  count_launch();
+}
+
 // The widest N tile that N allows (fewer passes over the activations), up to 128 columns: a 64 x 128 fp32 accumulator
 // is 64 registers per thread of a consumer warpgroup.  FEDB200_BLOCK_N overrides for experiments.
 int pick_block_n(int M, int N) {
@@ -202,6 +225,24 @@ bool conv_geometry_supported(int H_out, int W_out, int C_in, int stride) {
   return true;
 }
 
+// The 256-pixel activation box of the pixel-major kernel: whole output rows, and whole images or rows of one image.
+static bool pix_geometry_supported(int H_out, int W_out, int stride) {
+  if (W_out > PX_BLOCK_M || (PX_BLOCK_M % W_out) != 0) return false;
+  const int rows = PX_BLOCK_M / W_out;
+  if (rows <= H_out ? (H_out % rows) != 0 : (rows % H_out) != 0) return false;
+  return (rows <= H_out ? rows : H_out) * stride <= 256;
+}
+
+// Pixel-major tiles for C_out 64 / 128 when the 256-pixel tiles alone come close to one per SM (the 128-pixel tiles of
+// the other orientation would balance a short grid better); FEDB200_BLOCK_N experiments keep the row-major kernel.
+int pick_conv_orientation(int NB, int H_out, int W_out, int C_out, int stride) {
+  if (env_int("FEDB200_BLOCK_N", 0) != 0) return CONV_ORIENT_ROW;
+  if (C_out != 64 && C_out != 128) return CONV_ORIENT_ROW;
+  if (!pix_geometry_supported(H_out, W_out, stride)) return CONV_ORIENT_ROW;
+  const long long tiles = (static_cast<long long>(NB) * H_out * W_out + PX_BLOCK_M - 1) / PX_BLOCK_M;
+  return tiles >= num_sms() - num_sms() / 8 ? CONV_ORIENT_PIXEL : CONV_ORIENT_ROW;
+}
+
 // Eval-mode BatchNorm of conv2d_nhwc_bn_eval_tf32: running statistics, affine parameters and an optional residual.
 struct BnEvalArgs {
   const float* gamma;
@@ -217,11 +258,14 @@ struct BnEvalArgs {
 // when the convolution runs as one K slice; otherwise bn_elu_fwd does it in place after the split-K convolution.
 static void conv2d_generic(const float* x, const float* w, float* y, float* stats, const float* bias, int act, int NB, int H,
                            int W, int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
-                           cudaStream_t stream, int accumulate = 0, const BnEvalArgs* eval_bn = nullptr);
+                           cudaStream_t stream, int accumulate = 0, const BnEvalArgs* eval_bn = nullptr,
+                           int orient = CONV_ORIENT_ROW);
 
 void conv2d_nhwc_tf32(const float* x, const float* w, float* y, float* stats, int NB, int H, int W, int C_in, int C_out,
-                      int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream) {
-  conv2d_generic(x, w, y, stats, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream);
+                      int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream, int orient) {
+  if (orient == CONV_ORIENT_AUTO) orient = pick_conv_orientation(NB, H_out, W_out, C_out, stride);
+  conv2d_generic(x, w, y, stats, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 0, nullptr,
+                 orient);
 }
 
 void conv2d_nhwc_bias_act_tf32(const float* x, const float* w, const float* bias, int act, float* y, int NB, int H, int W,
@@ -233,8 +277,10 @@ void conv2d_nhwc_bias_act_tf32(const float* x, const float* w, const float* bias
 // y += conv(x, w): the residual-gradient accumulation of an identity-shortcut block fused into the data-gradient
 // convolution (experimental, FEDB200_SKIP_FUSED=1): bulk tensor reduce-add epilogue.
 void conv2d_nhwc_accumulate_tf32(const float* x, const float* w, float* y, int NB, int H, int W, int C_in, int C_out, int kh,
-                                 int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream) {
-  conv2d_generic(x, w, y, nullptr, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 1);
+                                 int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream, int orient) {
+  if (orient == CONV_ORIENT_AUTO) orient = pick_conv_orientation(NB, H_out, W_out, C_out, stride);
+  conv2d_generic(x, w, y, nullptr, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 1, nullptr,
+                 orient);
 }
 
 // y = act(BN_eval(conv(x, w)) + residual): inference with BatchNorm on its running statistics.  One launch when the
@@ -256,14 +302,20 @@ static int pick_tap_pack(int C_in) {
 
 static void conv2d_generic(const float* x, const float* w, float* y, float* stats, const float* bias, int act, int NB, int H,
                            int W, int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
-                           cudaStream_t stream, int accumulate, const BnEvalArgs* eval_bn) {
+                           cudaStream_t stream, int accumulate, const BnEvalArgs* eval_bn, int orient) {
   if (!conv_geometry_supported(H_out, W_out, C_in, stride))
     throw std::runtime_error("fedb200: conv geometry not supported by the wgmma path");
-  const int rows = 128 / W_out;
+  const bool pix = orient == CONV_ORIENT_PIXEL;
+  if (pix && ((C_out != 64 && C_out != 128) || bias != nullptr || act != 0 || eval_bn != nullptr ||
+              !pix_geometry_supported(H_out, W_out, stride) || (reinterpret_cast<uintptr_t>(y) & 15) != 0))
+    throw std::runtime_error("fedb200: pixel-major convolution needs C_out 64 / 128, a plain, statistics or accumulate epilogue, "
+                             "whole-row 256-pixel tiles and a 16-byte aligned output");
+  const int tile_m = pix ? PX_BLOCK_M : IG_BLOCK_M;
+  const int rows = tile_m / W_out;
   const int boxH = rows <= H_out ? rows : H_out;
   const int boxN = rows <= H_out ? 1 : rows / H_out;
   const int M = NB * H_out * W_out;
-  const int bn = pick_block_n(M, C_out);
+  const int bn = pix ? C_out : pick_block_n(M, C_out);
   const int cw = pick_tap_pack(C_in);
   CUtensorMap ta = make_tmap_nhwc(x, NB, H, W, C_in, boxN, boxH, W_out, stride, cw);
   CUtensorMap tb = make_tmap_2d(w, C_out, uint64_t(kh) * kw * C_in, uint64_t(kh) * kw * C_in, bn, cw);
@@ -282,6 +334,11 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
   p.out = y; p.ldo = C_out; p.bias = bias; p.act = act; p.stats = stats;
   p.k_splits = 1; p.kb_per_split = p.num_k_blocks;
   p.accumulate = accumulate;
+  if (pix) {
+    if (C_out == 64) launch_pix<64>(ta, tb, p, stream);
+    else launch_pix<128>(ta, tb, p, stream);
+    return;
+  }
   if (bias == nullptr && (act == 0 || eval_bn != nullptr)) {   // bias / activation must see the complete sum
     const int splits = pick_k_splits(M, C_out, bn, p.num_k_blocks);
     if (splits > 1) {

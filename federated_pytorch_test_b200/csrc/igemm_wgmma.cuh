@@ -88,13 +88,13 @@ struct IgemmSmem {
 struct TileCoord {
   int m0, n0, kb_begin, kb_count;
 };
-__device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int t, int block_n) {
+__device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int t, int block_m, int block_n) {
   const int n_idx = t % p.n_tiles;
   const int rest = t / p.n_tiles;
   const int m_idx = rest % p.m_tiles;
   const int z = rest / p.m_tiles;
   TileCoord c;
-  c.m0 = m_idx * IG_BLOCK_M;
+  c.m0 = m_idx * block_m;
   c.n0 = n_idx * block_n;
   c.kb_begin = z * p.kb_per_split;
   c.kb_count = min(p.kb_per_split, p.num_k_blocks - c.kb_begin);
@@ -103,6 +103,76 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int t, in
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+
+// TMA producer (one thread): walks this CTA's tiles and streams their k-blocks through the STAGES-deep ring, each stage
+// [A: TILE_M operand rows (pixels or GEMM rows) x 32 | B: BLOCK_N weight rows x 32], full / empty mbarrier protocol.
+template <int TILE_M, int BLOCK_N, int STAGES, int A_BYTES, int STAGE_BYTES>
+__device__ __forceinline__ void igemm_produce(const IgemmParams& p, uint8_t* tiles, uint64_t* full_bar, uint64_t* empty_bar,
+                                              const CUtensorMap* tmap_a, const CUtensorMap* tmap_b) {
+  int s = 0;
+  uint32_t ph = 0;
+  const int cwp = (p.cw == 8 || p.cw == 16) ? p.cw : 0;        // tap packing
+  const int tpk = cwp ? IG_BLOCK_K / cwp : 1;
+  const int img_oob = p.is_conv ? p.M / p.HW_out + 1 : 0;        // first image index past the tensor: the TMA unit zero-fills
+  const int col_oob = p.taps_total * p.b_cols_per_tap + IG_BLOCK_K;   // first weight column past the filter (+ a box)
+  // tap -> offset inside the (padded) input window
+  auto tap_offset = [&](int rr_, int sx_, int& cw_, int& ch_) {
+    cw_ = sx_ * p.dil - p.pad;
+    ch_ = rr_ * p.dil;
+    if (p.ms_kh > 0) {                                          // multi-dilation: rows are (branch, row) pairs
+      const int br = rr_ / p.ms_kh, rr = rr_ - br * p.ms_kh;
+      const int d = int((p.ms_dil >> (8 * br)) & 0xffull), pd = int((p.ms_pad >> (8 * br)) & 0xffull);
+      cw_ = sx_ * d - pd;
+      ch_ = rr * d - pd;
+    }
+  };
+  for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+    const TileCoord c = decode_tile(p, t, TILE_M, BLOCK_N);
+    int img = 0, h0 = 0;
+    if (p.is_conv) {                    // past the end: image index >= NB, the TMA unit zero-fills
+      img = c.m0 / p.HW_out;
+      h0 = ((c.m0 - img * p.HW_out) / p.W_out) * p.stride - p.pad;
+    }
+    int tap = c.kb_begin / p.cblocks;
+    int cb = c.kb_begin - tap * p.cblocks;
+    int r = tap / p.taps_w, sx = tap - r * p.taps_w;
+    for (int kb = c.kb_begin; kb < c.kb_begin + c.kb_count; ++kb) {
+      mbar_wait(&empty_bar[s], ph ^ 1);
+      uint8_t* a_dst = tiles + s * STAGE_BYTES;
+      uint8_t* b_dst = a_dst + A_BYTES;
+      mbar_arrive_expect_tx(&full_bar[s], uint32_t(STAGE_BYTES));
+      if (cwp) {
+        // tpk taps per k-block, each a [TILE_M rows x cwp channels] sub-tile of A and a [BLOCK_N x cwp] sub-tile of B
+        const int sub_a = TILE_M * cwp * 4, sub_b = BLOCK_N * cwp * 4;
+        for (int jt = 0; jt < tpk; ++jt) {
+          const int tp = kb * tpk + jt;
+          const bool real = tp < p.taps_total;
+          int cw = 0, ch = 0;
+          if (real) tap_offset(tp / p.taps_w, tp % p.taps_w, cw, ch);
+          // a tap past the filter: image index out of range -> zeros
+          tma_load_4d(a_dst + jt * sub_a, tmap_a, &full_bar[s], 0, cw, h0 + ch, real ? img : img_oob);
+          tma_load_2d(b_dst + jt * sub_b, tmap_b, &full_bar[s], real ? tp * p.b_cols_per_tap : col_oob, c.n0);
+        }
+      } else {
+        int cw, ch;
+        tap_offset(r, sx, cw, ch);
+        if (p.is_conv)
+          tma_load_4d(a_dst, tmap_a, &full_bar[s], cb * IG_BLOCK_K, cw, h0 + ch, img);
+        else
+          tma_load_2d(a_dst, tmap_a, &full_bar[s], kb * IG_BLOCK_K, c.m0);
+        tma_load_2d(b_dst, tmap_b, &full_bar[s], (r * p.taps_w + sx) * p.b_cols_per_tap + cb * IG_BLOCK_K, c.n0);
+        if (++cb == p.cblocks) {
+          cb = 0;
+          if (++sx == p.taps_w) { sx = 0; ++r; }
+        }
+      }
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+  }
 }
 
 // EVAL_BN: the eval-mode BatchNorm (+ residual) epilogue (IgemmParams::bn_*) is compiled in; a separate instantiation, so the
@@ -145,68 +215,8 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 
   if (wg == 0) {
     // ===================== TMA producer =====================
-    if (threadIdx.x == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      const int cwp = (p.cw == 8 || p.cw == 16) ? p.cw : 0;        // tap packing
-      const int tpk = cwp ? IG_BLOCK_K / cwp : 1;
-      const int img_oob = p.is_conv ? p.M / p.HW_out + 1 : 0;        // first image index past the tensor: the TMA unit zero-fills
-      const int col_oob = p.taps_total * p.b_cols_per_tap + IG_BLOCK_K;   // first weight column past the filter (+ a box)
-      // tap -> offset inside the (padded) input window
-      auto tap_offset = [&](int rr_, int sx_, int& cw_, int& ch_) {
-        cw_ = sx_ * p.dil - p.pad;
-        ch_ = rr_ * p.dil;
-        if (p.ms_kh > 0) {                                          // multi-dilation: rows are (branch, row) pairs
-          const int br = rr_ / p.ms_kh, rr = rr_ - br * p.ms_kh;
-          const int d = int((p.ms_dil >> (8 * br)) & 0xffull), pd = int((p.ms_pad >> (8 * br)) & 0xffull);
-          cw_ = sx_ * d - pd;
-          ch_ = rr * d - pd;
-        }
-      };
-      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
-        const TileCoord c = decode_tile(p, t, BLOCK_N);
-        int img = 0, h0 = 0;
-        if (p.is_conv) {                    // past the end: image index >= NB, the TMA unit zero-fills
-          img = c.m0 / p.HW_out;
-          h0 = ((c.m0 - img * p.HW_out) / p.W_out) * p.stride - p.pad;
-        }
-        int tap = c.kb_begin / p.cblocks;
-        int cb = c.kb_begin - tap * p.cblocks;
-        int r = tap / p.taps_w, sx = tap - r * p.taps_w;
-        for (int kb = c.kb_begin; kb < c.kb_begin + c.kb_count; ++kb) {
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* a_dst = tiles + s * S::STAGE_BYTES;
-          uint8_t* b_dst = a_dst + S::A_BYTES;
-          mbar_arrive_expect_tx(&full_bar[s], uint32_t(S::STAGE_BYTES));
-          if (cwp) {
-            // tpk taps per k-block, each a [128 rows x cwp channels] sub-tile of A and a [BLOCK_N x cwp] sub-tile of B
-            const int sub_a = IG_BLOCK_M * cwp * 4, sub_b = BLOCK_N * cwp * 4;
-            for (int jt = 0; jt < tpk; ++jt) {
-              const int tp = kb * tpk + jt;
-              const bool real = tp < p.taps_total;
-              int cw = 0, ch = 0;
-              if (real) tap_offset(tp / p.taps_w, tp % p.taps_w, cw, ch);
-              // a tap past the filter: image index out of range -> zeros
-              tma_load_4d(a_dst + jt * sub_a, &tmap_a, &full_bar[s], 0, cw, h0 + ch, real ? img : img_oob);
-              tma_load_2d(b_dst + jt * sub_b, &tmap_b, &full_bar[s], real ? tp * p.b_cols_per_tap : col_oob, c.n0);
-            }
-          } else {
-            int cw, ch;
-            tap_offset(r, sx, cw, ch);
-            if (p.is_conv)
-              tma_load_4d(a_dst, &tmap_a, &full_bar[s], cb * IG_BLOCK_K, cw, h0 + ch, img);
-            else
-              tma_load_2d(a_dst, &tmap_a, &full_bar[s], kb * IG_BLOCK_K, c.m0);
-            tma_load_2d(b_dst, &tmap_b, &full_bar[s], (r * p.taps_w + sx) * p.b_cols_per_tap + cb * IG_BLOCK_K, c.n0);
-            if (++cb == p.cblocks) {
-              cb = 0;
-              if (++sx == p.taps_w) { sx = 0; ++r; }
-            }
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-      }
-    }
+    if (threadIdx.x == 0)
+      igemm_produce<IG_BLOCK_M, BLOCK_N, STAGES, S::A_BYTES, S::STAGE_BYTES>(p, tiles, full_bar, empty_bar, &tmap_a, &tmap_b);
     return;
   }
 
@@ -236,7 +246,7 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   int s = 0;
   uint32_t ph = 0;
   for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
-    const TileCoord c = decode_tile(p, t, BLOCK_N);
+    const TileCoord c = decode_tile(p, t, IG_BLOCK_M, BLOCK_N);
     if constexpr (EVAL_BN) {
       // eval-mode BatchNorm: the tile's per-column scale / shift, once per tile, in the (otherwise unused) statistics area
       named_bar_sync(3, 256);                    // the previous tile's epilogue has read them
@@ -397,6 +407,200 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     }
   }
   if (p.tma_store && tid == 0) tma_store_wait_read();   // shared memory must outlive the last bulk store's read
+}
+
+// ================================================================================================================
+// Pixel-major convolution for C_out = 64 / 128: output channels on the wgmma M side, 256 output pixels on the N side.
+// wgmma.m64n256k8 reads its 64-row weight operand and the 256-pixel activation operand from shared memory at
+// 1/64 + 1/16 B per multiply-accumulate (against 4/N + 1/16 for the 128-pixel x N-channel tile above), and a stage of
+// 64 or 128 weight rows + 256 pixels costs the TMA fill less shared-memory bandwidth per MAC as well.
+// Same producer, ring protocol, tap packing and tile walk as igemm_wgmma_kernel; the stage is [pixels (A) | weights (B)].
+//   C_out = 64  (ping-pong): each consumer warpgroup owns every other tile (64 ch x 256 px); one warpgroup's main loop
+//               runs while the other one's epilogue does (the ring hands the stages out in tile order).
+//   C_out = 128 (cooperative): warpgroup g computes channels [64 g, 64 g + 64) of every tile.
+// Epilogues: plain store, BatchNorm sum / sum of squares (IgemmParams::stats), or reduce-add (IgemmParams::accumulate).
+// The [channel][pixel] fragment is transposed through 128B-swizzled 32 x 32 staging boxes into NHWC bulk tensor stores.
+// Requires k_splits == 1, no bias / activation / eval-mode BatchNorm, and a 16-byte aligned output with ldo == C_out.
+// ================================================================================================================
+constexpr int PX_BLOCK_M = 256;     // output pixels per tile
+
+template <int CO, int STAGES>
+struct PixSmem {
+  static constexpr int A_BYTES = PX_BLOCK_M * IG_BLOCK_K * 4;   // 32 KB of pixels
+  static constexpr int B_BYTES = CO * IG_BLOCK_K * 4;           // 8 / 16 KB of weights
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGING_BYTES = 2 * 2 * 2 * 32 * 32 * 4; // per consumer warpgroup: two buffers of two 32 x 32 boxes
+  static constexpr int BAR_BYTES = 2 * STAGES * 8;
+  static constexpr int TOTAL = STAGES * STAGE_BYTES + STAGING_BYTES + BAR_BYTES + 1024;  // + align slack
+};
+
+template <int CO, int STAGES>
+__global__ void __launch_bounds__(IG_THREADS, 1)
+igemm_wgmma_pix_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_c, const IgemmParams p) {
+  using S = PixSmem<CO, STAGES>;
+  static_assert(CO == 64 || CO == 128, "pixel-major tiles serve 64 or 128 output channels");
+  static_assert(S::TOTAL <= 227 * 1024, "shared memory budget");
+  static_assert(S::STAGE_BYTES % 1024 == 0, "stages must keep the 1024-byte swizzle alignment");
+  constexpr bool PINGPONG = CO == 64;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* tiles = smem;
+  float* staging = reinterpret_cast<float*>(smem + STAGES * S::STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES + S::STAGING_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
+
+  const int wg = threadIdx.x >> 7;
+  const int tid = threadIdx.x & 127;
+
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_c);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], PINGPONG ? 1 : 2);   // the tile's warpgroup / both warpgroups release a stage
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0)
+      igemm_produce<PX_BLOCK_M, CO, STAGES, S::A_BYTES, S::STAGE_BYTES>(p, tiles, full_bar, empty_bar, &tmap_a, &tmap_b);
+    return;
+  }
+  setmaxnreg_inc<232>();
+
+  const int g = wg - 1;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int ch_wg = PINGPONG ? 0 : 64 * g;                       // first output channel of this warpgroup
+  const uint32_t cwq = (p.cw == 8 || p.cw == 16) ? uint32_t(p.cw) : uint32_t(IG_BLOCK_K);
+  const uint32_t mma_per_sub = cwq / IG_MMA_K;
+  // wgmma A = the weight rows of this warpgroup's channels, wgmma B = the 256 pixel rows
+  const uint64_t adesc0 = make_kmajor_desc(smem_u32(tiles) + uint32_t(S::A_BYTES) + uint32_t(ch_wg) * cwq * 4u, cwq * 4u);
+  const uint64_t bdesc0 = make_kmajor_desc(smem_u32(tiles), cwq * 4u);
+  uint32_t a_off[IG_BLOCK_K / IG_MMA_K], b_off[IG_BLOCK_K / IG_MMA_K];
+#pragma unroll
+  for (int k = 0; k < IG_BLOCK_K / IG_MMA_K; ++k) {
+    const uint32_t sub = uint32_t(k) / mma_per_sub, in = uint32_t(k) - sub * mma_per_sub;
+    a_off[k] = (sub * uint32_t(CO) * cwq * 4u + in * 32u) >> 4;
+    b_off[k] = (sub * uint32_t(PX_BLOCK_M) * cwq * 4u + in * 32u) >> 4;
+  }
+  float* stg = staging + g * 4096;            // [2 buffers][2 boxes][32 pixels][32 channels], chunk index XOR (pixel & 7)
+  const uint32_t wg_bar = 1 + uint32_t(g);
+  const int ch_lo = 16 * warp + (lane >> 2);  // channel (within the warpgroup's 64) of d[4i], d[4i+1]; d[4i+2..3]: + 8
+  const int px_in = 2 * (lane & 3);           // pixel of d[4i] within its 8-pixel block
+
+  float acc[128];
+  const int step = PINGPONG ? 2 : 1;
+  for (int j = PINGPONG ? g : 0, t = blockIdx.x + j * gridDim.x; t < p.total_tiles; j += step, t += step * gridDim.x) {
+    const TileCoord c = decode_tile(p, t, PX_BLOCK_M, CO);
+    // ring position of this tile's first k-block: every tile has num_k_blocks of them (no split-K)
+    const uint32_t pos = uint32_t(j) * uint32_t(c.kb_count);
+    int s = int(pos % STAGES);
+    uint32_t ph = (pos / STAGES) & 1u;
+    // Ping-pong: the main loops take turns (named barrier 3 + g: "warpgroup g may start").  A full-barrier parity wait
+    // only tells the last two fills of a stage apart, so a warpgroup may wait on its k-blocks only once every k-block
+    // before them has been waited on, i.e. once the other warpgroup's main loop has passed its last wait.
+    if (PINGPONG && j > 0) named_bar_sync(3 + uint32_t(g), 256);
+    int prev = -1;
+    for (int i = 0; i < c.kb_count; ++i) {
+      mbar_wait(&full_bar[s], ph);
+      const uint64_t so = uint64_t(uint32_t(s) * uint32_t(S::STAGE_BYTES >> 4));
+      wgmma_fence();
+      wgmma_fence_acc(acc);
+#pragma unroll
+      for (int k = 0; k < IG_BLOCK_K / IG_MMA_K; ++k)
+        wgmma_tf32_n256(acc, adesc0 + so + a_off[k], bdesc0 + so + b_off[k], (i > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_fence_acc(acc);
+      wgmma_wait<1>();
+      if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+      prev = s;
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+    // hand the turn to the other warpgroup if it has a next tile (every arrival meets exactly one wait)
+    if (PINGPONG && t + gridDim.x < p.total_tiles) named_bar_arrive(4 - uint32_t(g), 256);
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+
+    // ---- epilogue.  Pixels past M (last tile of an odd batch) must not reach the statistics; the store clips them.
+    if (c.m0 + PX_BLOCK_M > p.M) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (c.m0 + 8 * i + px_in + e >= p.M) { acc[4 * i + e] = 0.f; acc[4 * i + 2 + e] = 0.f; }
+    }
+    if (p.stats != nullptr) {
+      // a row of the fragment is one channel: sum inside the thread, then over the 4 lanes of the quad
+      float s1a = 0.f, s2a = 0.f, s1b = 0.f, s2b = 0.f;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float va = acc[4 * i + e], vb = acc[4 * i + 2 + e];
+          s1a += va; s2a = fmaf(va, va, s2a);
+          s1b += vb; s2b = fmaf(vb, vb, s2b);
+        }
+      }
+#pragma unroll
+      for (int o = 1; o < 4; o <<= 1) {
+        s1a += __shfl_xor_sync(0xffffffffu, s1a, o);
+        s2a += __shfl_xor_sync(0xffffffffu, s2a, o);
+        s1b += __shfl_xor_sync(0xffffffffu, s1b, o);
+        s2b += __shfl_xor_sync(0xffffffffu, s2b, o);
+      }
+      if ((lane & 3) == 0) {
+        const int ca = ch_wg + ch_lo;
+        atomicAdd(p.stats + ca, s1a);
+        atomicAdd(p.stats + p.N + ca, s2a);
+        atomicAdd(p.stats + ca + 8, s1b);
+        atomicAdd(p.stats + p.N + ca + 8, s2b);
+      }
+    }
+    // 8 chunks of 32 pixels x 64 channels, double-buffered: a buffer is rewritten once the stores of two chunks ago have read it
+#pragma unroll
+    for (int q = 0; q < PX_BLOCK_M / 32; ++q) {
+      float* buf = stg + (q & 1) * 2048;
+      if (tid == 0) tma_store_wait_read_n<1>();
+      named_bar_sync(wg_bar, 128);
+#pragma unroll
+      for (int ii = 0; ii < 4; ++ii) {
+        const int i = 4 * q + ii;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int ch = ch_lo + 8 * h;                   // 0..63
+          const int cc = ch & 31;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int px = 8 * ii + px_in + e;            // 0..31: the staging row
+            buf[(ch >> 5) * 1024 + px * 32 + (((uint32_t(cc) >> 2) ^ uint32_t(px & 7)) << 2) + (cc & 3)] = acc[4 * i + 2 * h + e];
+          }
+        }
+      }
+      fence_proxy_async();
+      named_bar_sync(wg_bar, 128);
+      if (tid == 0) {
+        const int row0 = c.m0 + 32 * q;
+        if (row0 < p.M) {
+#pragma unroll
+          for (int b = 0; b < 2; ++b) {
+            if (p.accumulate) tma_reduce_add_2d(&tmap_c, buf + b * 1024, ch_wg + 32 * b, row0);
+            else tma_store_2d(&tmap_c, buf + b * 1024, ch_wg + 32 * b, row0);
+          }
+        }
+        tma_store_commit();
+      }
+    }
+  }
+  if (tid == 0) tma_store_wait_read();   // shared memory must outlive the last bulk store's read
 }
 
 }  // namespace fedb200
