@@ -188,6 +188,7 @@ class Engine:
         self._adam_cache: Dict = {}
         self.stop_requested = False
         self.step_hook: Optional[Callable[["Engine"], None]] = None
+        self.attack: Optional[Callable[["Engine"], None]] = None   # simulated Byzantine workers, before every aggregation
         self.last_loss1: Optional[torch.Tensor] = None
         self.graph_replays = 0
         self._pending_round = None
@@ -440,6 +441,8 @@ class Engine:
         # (only a collective with asynchronous entry points actually defers: FusedCollective; the others answer "done")
         defer = (cfg.deferred_rounds and not cfg.check_results and not cfg.be_verbose
                  and not cfg.resume_path and env != "0" and (env == "1" or self.topo.world_size <= 4))
+        if self.attack is not None:
+            self.attack(self)
         with nvtx_range("fedb200:aggregate"), self.timers.phase("aggregate"):
             token = self.strategy.aggregate_begin(nadmm) if defer else ("done", self.strategy.aggregate(nadmm))
         self._pending_round = (token, visit, nloop, nadmm, epoch, N)

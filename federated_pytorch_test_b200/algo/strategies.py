@@ -90,16 +90,37 @@ class NoConsensus(Strategy):
 
 
 class FedAvg(Strategy):
+    """FedAvg: ``z <-`` the mean of the K replicas, written back into every replica.  ``aggregator`` 'median' or
+    'trimmed_mean' (Yin et al. 2018) replaces the mean by a coordinate-wise order statistic over the K replicas that a
+    minority of diverging or malicious workers cannot move arbitrarily far (``trimmed_mean`` drops
+    ``floor(trim_fraction K)`` values at each end); the round is otherwise the same."""
+
     name = "fedavg"
     write_back = True
 
+    def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1):
+        from ..config import check_aggregator, trim_count
+
+        super().__init__(collective, topo)
+        check_aggregator(aggregator, trim_fraction, topo.K)
+        self.aggregator = aggregator
+        self.trim_b = trim_count(trim_fraction, topo.K) if aggregator == "trimmed_mean" else 0
+        if aggregator != "mean" and hasattr(collective, "warm_robust"):
+            collective.warm_robust = True
+
     def aggregate(self, nadmm: int) -> Dict[str, float]:
-        dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True)
+        if self.aggregator == "mean":
+            dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True)
+        else:
+            dual_sq = self.coll.robust_(self.xs, self.z, self.aggregator, self.trim_b)
         return {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
-            self.coll.launch_fedavg_(self.xs, self.z, True)
+            if self.aggregator == "mean":
+                self.coll.launch_fedavg_(self.xs, self.z, True)
+            else:
+                self.coll.launch_robust_(self.xs, self.z, self.aggregator, self.trim_b)
             return ("pending", self.N)
         return ("done", self.aggregate(nadmm))
 
@@ -108,7 +129,20 @@ class FedAvg(Strategy):
             return token[1]
         return {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]}
 
+    def _robust_state(self) -> Dict[str, object]:
+        return {} if self.aggregator == "mean" else {"aggregator": self.aggregator, "trim_b": self.trim_b}
+
+    def _check_robust_state(self, st: Dict[str, object]) -> None:
+        got = (st.get("aggregator", "mean"), int(st.get("trim_b", 0)))
+        if got != (self.aggregator, self.trim_b):
+            raise ValueError("resume record holds aggregator %r (trim_b %d), this run uses %r (trim_b %d)"
+                             % (got + (self.aggregator, self.trim_b)))
+
+    def state(self) -> Dict[str, object]:
+        return {"z": self.z, **self._robust_state()}
+
     def load_state(self, st: Dict[str, object]) -> None:
+        self._check_robust_state(st)
         self.z.copy_(st["z"].to(self.z.device))
 
 
@@ -125,16 +159,17 @@ class FedOpt(FedAvg):
     at the start of a block visit (one extra aggregation launch per visit).  ``m`` / ``v`` belong to a block and persist
     across its visits for the whole run (``m = 0``, ``v = tau^2`` at its first visit); on the fused collective they are
     slices of symmetric arenas, so two-shot ranks broadcast their slice of both into every rank and every rank ends each
-    round with the same ``z``, ``m`` and ``v``."""
+    round with the same ``z``, ``m`` and ``v``.  With a robust ``aggregator`` its aggregate replaces the mean in ``d``
+    (e.g. robust FedAdam); the server model at the start of a visit stays the mean (the replicas are equal then)."""
 
     name = "fedopt"
 
     def __init__(self, collective, topo, kind: str = "adam", lr: float = 0.0, momentum: float = 0.9, beta1: float = 0.9,
-                 beta2: float = 0.99, tau: float = 1e-3):
+                 beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1):
         from ..config import check_server_opt
         from ..parallel.collective import FEDOPT_KINDS
 
-        super().__init__(collective, topo)
+        super().__init__(collective, topo, aggregator, trim_fraction)
         if kind not in FEDOPT_KINDS:
             raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
         check_server_opt(kind, lr, momentum, beta1, beta2, tau)
@@ -165,13 +200,16 @@ class FedOpt(FedAvg):
     def _hyper(self):
         return self.kind, self.lr, self.beta1, self.beta2, self.tau
 
+    def _agg_kw(self) -> Dict[str, object]:
+        return {} if self.aggregator == "mean" else {"agg": self.aggregator, "trim_b": self.trim_b}
+
     def aggregate(self, nadmm: int) -> Dict[str, float]:
-        dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper())
+        dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw())
         return {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
-            self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper())
+            self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw())
             return ("pending", self.N)
         return ("done", self.aggregate(nadmm))
 
@@ -182,7 +220,7 @@ class FedOpt(FedAvg):
         vs = {ci: v for ci, (_, v) in self._restored.items() if v is not None}
         ms.update(self.ms)
         vs.update(self.vs)
-        return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs}
+        return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state()}
 
     def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
         self.ms[ci].copy_(m.to(self.ms[ci].device))
@@ -192,6 +230,7 @@ class FedOpt(FedAvg):
     def load_state(self, st: Dict[str, object]) -> None:
         if st.get("server_opt") != self.kind:
             raise ValueError("resume record holds server optimizer %r, this run uses %r" % (st.get("server_opt"), self.kind))
+        self._check_robust_state(st)
         self.z.copy_(st["z"].to(self.z.device))
         vs = st.get("v") or {}
         for ci, m in (st.get("m") or {}).items():

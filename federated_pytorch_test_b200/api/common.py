@@ -227,9 +227,10 @@ def save_legacy(cfg: CommonConfig, engine: Engine, model_key: str = "net") -> No
 
 
 def run_engine(cfg: CommonConfig, task: Task, topo: Topology, coll, strategy, ecfg: Optional[EngineConfig] = None,
-               log: Callable[[str], None] = print) -> Engine:
+               log: Callable[[str], None] = print, attack: Optional[Callable[[Engine], None]] = None) -> Engine:
     metrics = MetricsLog(cfg.metrics_path or None)
     engine = Engine(task, topo, strategy, coll, ecfg or engine_config(cfg), log=log, metrics=metrics)
+    engine.attack = attack
     if cfg.resume:
         ckpt.load_resume(cfg.resume, engine)
     engine.run()

@@ -7,9 +7,14 @@ parameter arenas (``csrc/comm_kernels.cu``), no NCCL on the path.
 
 ``--server_opt avgm|adagrad|adam|yogi`` replaces the plain mean by a server optimizer step (``FedOpt``), fused into
 the same kernel; the default ``none`` is the reference's FedAvg.
+
+``--aggregator median|trimmed_mean`` (``--trim_fraction``) replaces the mean of the K replicas by a coordinate-wise order
+statistic (Byzantine-robust aggregation), with or without a server optimizer; ``--byzantine b --attack
+signflip|gaussian|nan --attack_scale s`` turns the last b workers into simulated attackers (``algo/byzantine.py``).
 """
 from __future__ import annotations
 
+from ..algo.byzantine import ByzantineAttack
 from ..algo.strategies import FedAvg, FedOpt
 from ..config import FederatedConfig, parse_config
 from . import common
@@ -18,16 +23,24 @@ Config = FederatedConfig
 
 
 def make_strategy(cfg: Config, coll, topo):
+    robust = {} if cfg.aggregator == "mean" else dict(aggregator=cfg.aggregator, trim_fraction=cfg.trim_fraction)
     if cfg.server_opt == "none":
-        return FedAvg(coll, topo)
+        return FedAvg(coll, topo, **robust)
     return FedOpt(coll, topo, cfg.server_opt, cfg.server_lr, cfg.server_momentum, cfg.server_beta1, cfg.server_beta2,
-                  cfg.server_tau)
+                  cfg.server_tau, **robust)
+
+
+def make_attack(cfg: Config):
+    """The simulated Byzantine workers of the run, or None (``byzantine = 0``)."""
+    if cfg.byzantine == 0:
+        return None
+    return ByzantineAttack(cfg.K, cfg.byzantine, cfg.attack, cfg.attack_scale, cfg.seed)
 
 
 def run(cfg: Config, log=print):
     topo, coll = common.setup_runtime(cfg)
     task = common.ClassifierTask(cfg, topo, cfg.lambda1, cfg.lambda2)
-    engine = common.run_engine(cfg, task, topo, coll, make_strategy(cfg, coll, topo), None, log)
+    engine = common.run_engine(cfg, task, topo, coll, make_strategy(cfg, coll, topo), None, log, attack=make_attack(cfg))
     common.save_legacy(cfg, engine)
     return engine
 

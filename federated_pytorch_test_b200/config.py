@@ -86,6 +86,39 @@ def check_server_opt(server_opt: str, server_lr: float, server_momentum: float, 
         raise ValueError("server_tau must be > 0, got %r" % (server_tau,))
 
 
+AGGREGATORS = ("mean", "median", "trimmed_mean")
+ROBUST_MAX_K = 16                   # the robust rules sort the K values of a coordinate in registers
+ATTACKS = ("signflip", "gaussian", "nan")
+
+
+def trim_count(trim_fraction: float, K: int) -> int:
+    """Values dropped at each end by the trimmed mean: ``floor(trim_fraction * K)`` (``scipy.stats.trim_mean``)."""
+    return int(trim_fraction * K)
+
+
+def check_aggregator(aggregator: str, trim_fraction: float, K: int) -> None:
+    """Raise ``ValueError`` unless the aggregation rule of :class:`FederatedConfig` is valid for ``K`` workers."""
+    if aggregator not in AGGREGATORS:
+        raise ValueError("aggregator must be one of %s, got %r" % (", ".join(AGGREGATORS), aggregator))
+    if not 0.0 <= trim_fraction < 0.5:
+        raise ValueError("trim_fraction must lie in [0, 0.5), got %r" % (trim_fraction,))
+    if aggregator != "mean" and K > ROBUST_MAX_K:
+        raise ValueError("aggregator %r supports at most %d workers, got K = %d" % (aggregator, ROBUST_MAX_K, K))
+    if aggregator == "trimmed_mean" and trim_count(trim_fraction, K) == 0:
+        raise ValueError("trim_fraction %r trims nothing at K = %d (floor(trim_fraction * K) = 0): the trimmed mean would "
+                         "be the mean" % (trim_fraction, K))
+
+
+def check_byzantine(byzantine: int, attack: str, attack_scale: float, K: int) -> None:
+    """Raise ``ValueError`` unless the simulated-attacker settings of :class:`FederatedConfig` are valid."""
+    if not 0 <= byzantine < K:
+        raise ValueError("byzantine must lie in [0, K) = [0, %d), got %r" % (K, byzantine))
+    if attack not in ATTACKS:
+        raise ValueError("attack must be one of %s, got %r" % (", ".join(ATTACKS), attack))
+    if not attack_scale > 0.0:
+        raise ValueError("attack_scale must be > 0, got %r" % (attack_scale,))
+
+
 @dataclass
 class FederatedConfig(CommonConfig):
     lambda1: float = 0.0001
@@ -97,10 +130,19 @@ class FederatedConfig(CommonConfig):
     server_beta1: float = 0.9       # adagrad / adam / yogi
     server_beta2: float = 0.99      # adam / yogi
     server_tau: float = 1e-3        # adaptivity floor: z += lr m / (sqrt(v) + tau); v starts at tau^2
+    # Byzantine-robust aggregation: coordinate-wise order statistic over the K workers instead of their mean
+    aggregator: str = "mean"        # 'mean' | 'median' | 'trimmed_mean'
+    trim_fraction: float = 0.1      # trimmed_mean: drop floor(trim_fraction * K) values at each end
+    # simulated Byzantine workers K - byzantine .. K - 1 (worker 0 stays honest), applied before every aggregation
+    byzantine: int = 0
+    attack: str = "signflip"        # 'signflip': x <- z - s (x - z) | 'gaussian': x <- z + s N(0, 1) | 'nan': x <- NaN
+    attack_scale: float = 4.0       # s
 
     def __post_init__(self):
         check_server_opt(self.server_opt, self.server_lr, self.server_momentum, self.server_beta1, self.server_beta2,
                          self.server_tau)
+        check_aggregator(self.aggregator, self.trim_fraction, self.K)
+        check_byzantine(self.byzantine, self.attack, self.attack_scale, self.K)
 
 
 @dataclass

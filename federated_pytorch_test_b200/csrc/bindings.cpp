@@ -587,6 +587,7 @@ void smallconv_wgrad(Tensor dz, Tensor x, Tensor dw, c10::optional<Tensor> db, i
 
 // ---------------------------------------------------------------------------------------------- collectives
 // Pointers are passed as integers: local tensors' data_ptr() or peer-mapped addresses from symmetric memory.
+// agg = AGG_MEAN / AGG_MEDIAN / AGG_TRIMMED picks the aggregation rule (trim_b: values dropped at each end, trimmed mean).
 static void fill_ctrl(uint32_t** dst, const std::vector<int64_t>& ctrl_ptrs, int world) {
   for (int p = 0; p < world && p < (int)ctrl_ptrs.size(); ++p) dst[p] = reinterpret_cast<uint32_t*>(ctrl_ptrs[p]);
 }
@@ -594,7 +595,7 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
                   Tensor z, int64_t n, double rho, c10::optional<Tensor> rho_dev, Tensor out, Tensor scratch,
                   std::vector<int64_t> ctrl_ptrs, Tensor sync, int64_t world, int64_t rank, int64_t mc_x, int64_t mc_y,
                   int64_t mc_z, std::vector<int64_t> xw_ptrs, std::vector<int64_t> zw_ptrs, bool two_shot,
-                  int64_t max_blocks, double timeout_s) {
+                  int64_t max_blocks, double timeout_s, int64_t agg, int64_t trim_b) {
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch);
   TORCH_CHECK(out.numel() >= fb::COMM_OUT_FLOATS && scratch.numel() >= fb::COMM_SCRATCH_FLOATS, "out / scratch too small");
   c10::cuda::CUDAGuard guard(z.device());
@@ -631,6 +632,7 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
   fill_ctrl(a.ctrl, ctrl_ptrs, a.world);
   a.sync = reinterpret_cast<uint32_t*>(sync.data_ptr<int>());
   a.timeout_cycles = (long long)(timeout_s * 1.9e9);
+  a.agg = (int)agg; a.trim_b = (int)trim_b;
   fb::block_reduce_launch(a, cur_stream());
 }
 
@@ -641,7 +643,7 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
                          Tensor scratch, std::vector<int64_t> ctrl_ptrs, Tensor sync, int64_t world, int64_t rank,
                          int64_t mc_x, int64_t mc_m, int64_t mc_v, std::vector<int64_t> xw_ptrs,
                          std::vector<int64_t> mw_ptrs, std::vector<int64_t> vw_ptrs, bool two_shot, int64_t max_blocks,
-                         double timeout_s) {
+                         double timeout_s, int64_t agg, int64_t trim_b) {
   TORCH_CHECK(opt >= fb::FEDOPT_AVGM && opt <= fb::FEDOPT_YOGI, "block_reduce_fedopt: unknown server optimizer ", opt);
   const bool adaptive = opt != fb::FEDOPT_AVGM;
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch); CHECK_F32_CUDA(m); CHECK_CONTIG(m);
@@ -683,6 +685,7 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
   a.lr = (float)lr; a.beta1 = (float)beta1; a.beta2 = (float)beta2; a.tau = (float)tau;
   a.m = m.data_ptr<float>();
   a.v = adaptive ? v->data_ptr<float>() : nullptr;
+  a.agg = (int)agg; a.trim_b = (int)trim_b;
   fb::block_reduce_launch(a, cur_stream());
 }
 

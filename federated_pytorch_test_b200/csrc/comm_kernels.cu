@@ -176,11 +176,97 @@ __device__ __forceinline__ float4 fedopt_step_v4(const CommArgs& a, float4 z, fl
                      fedopt_step(a, z.z, mean.z, m.z, v.z), fedopt_step(a, z.w, mean.w, m.w, v.w));
 }
 
+// ---- robust aggregation: coordinate-wise median / trimmed mean (Yin et al. 2018) --------------------------------------
+// Batcher's odd-even merge sort network on P = 4 / 8 / 16 values, as a compile-time comparator list (5 / 19 / 63
+// compare-exchanges).  The loops below unroll completely, so every index is a constant and the values stay in registers.
+template <int P>
+struct OddEvenMergeNet {
+  int n = 0;
+  int lo[P * P] = {};
+  int hi[P * P] = {};
+  constexpr OddEvenMergeNet() {
+    for (int p = 1; p < P; p <<= 1)
+      for (int k = p; k >= 1; k >>= 1)
+        for (int j = k % p; j + k < P; j += 2 * k)
+          for (int i = 0; i < k && i + j + k < P; ++i)
+            if ((i + j) / (2 * p) == (i + j + k) / (2 * p)) {
+              lo[n] = i + j;
+              hi[n] = i + j + k;
+              ++n;
+            }
+  }
+};
+
+// NaN orders as +inf, +-inf keep their sign: NaN / Inf in at most trim_b workers (median: fewer than half) cannot reach
+// the aggregate.
+__device__ __forceinline__ float robust_canon(float x) { return isnan(x) ? __int_as_float(0x7f800000) : x; }
+
+// Sorts v[0..P) (the K inputs, padded with +inf) and returns the rule's aggregate.  median: the middle value for odd K,
+// (lo + hi) * 0.5 of the two middle values for even K (np.median).  trimmed mean: the sum of the sorted values
+// trim_b .. K - trim_b - 1 in ascending order, divided (correctly rounded) by K - 2 trim_b (scipy.stats.trim_mean); only
+// the kept values are summed, so an extreme value cannot cancel against the rest.
+template <int P>
+__device__ __forceinline__ float robust_select(const CommArgs& a, float (&v)[P]) {
+  constexpr OddEvenMergeNet<P> net{};
+#pragma unroll
+  for (int c = 0; c < net.n; ++c) {
+    const float x = v[net.lo[c]], y = v[net.hi[c]];
+    v[net.lo[c]] = fminf(x, y);
+    v[net.hi[c]] = fmaxf(x, y);
+  }
+  if (a.agg == AGG_MEDIAN) {
+    const int ilo = (a.K - 1) >> 1, ihi = a.K >> 1;
+    float lo = 0.f, hi = 0.f;
+#pragma unroll
+    for (int j = 0; j < P; ++j) {
+      if (j == ilo) lo = v[j];
+      if (j == ihi) hi = v[j];
+    }
+    return (a.K & 1) ? hi : (lo + hi) * 0.5f;
+  }
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < P; ++j)
+    if (j >= a.trim_b && j < a.K - a.trim_b) s += v[j];
+  return __fdiv_rn(s, float(a.K - 2 * a.trim_b));
+}
+
+// the rule's aggregate over all K workers at float4 index `off`: K peer loads (never the multicast address), then one
+// sort per lane
+template <int P>
+__device__ __forceinline__ float4 robust_gather_v4(const CommArgs& a, size_t off) {
+  float vx[P], vy[P], vz[P], vw[P];
+  const float inf = __int_as_float(0x7f800000);
+#pragma unroll
+  for (int k = 0; k < P; ++k) {
+    float4 xv = make_float4(inf, inf, inf, inf);
+    if (k < a.K) xv = ld_sys_v4(a.x[k] + off);
+    vx[k] = robust_canon(xv.x); vy[k] = robust_canon(xv.y); vz[k] = robust_canon(xv.z); vw[k] = robust_canon(xv.w);
+  }
+  return make_float4(robust_select<P>(a, vx), robust_select<P>(a, vy), robust_select<P>(a, vz), robust_select<P>(a, vw));
+}
+template <int P>
+__device__ __forceinline__ float robust_gather_f32(const CommArgs& a, int i) {
+  float v[P];
+#pragma unroll
+  for (int k = 0; k < P; ++k) v[k] = k < a.K ? robust_canon(ld_sys_f32(a.x[k] + i)) : __int_as_float(0x7f800000);
+  return robust_select<P>(a, v);
+}
+
+// AGG_PAD = 0: the mean (sum; scaled by the caller).  AGG_PAD = 4 / 8 / 16: the robust rule on K <= AGG_PAD inputs.
+template <int AGG_PAD>
+__device__ __forceinline__ float4 reduce_v4(const CommArgs& a, size_t off, float rho, bool use_mc) {
+  if constexpr (AGG_PAD == 0) return gather_v4(a, off, rho, use_mc);
+  else return robust_gather_v4<AGG_PAD>(a, off);
+}
+
 // FEDOPT = false: FedAvg / FedProx / ADMM (a.mode).  FEDOPT = true: FedAvg (mode 0) whose new model is a server optimizer
 // step from z instead of the plain mean.  Pass 1 forms the step from the reduced mean, z and the state m (and v): one-shot
 // stores z, m, v locally; two-shot rank r broadcasts slice r of the new weights, of m and of v into every rank, so every rank
 // ends the round with the same z, m and v.  Pass 2 is FedAvg's.
-template <bool FEDOPT>
+// AGG_PAD > 0: the robust instantiations (modes 0 / 1): pass 1 takes the median / trimmed mean of the K workers instead of
+// their mean (with FEDOPT, as the server optimizer's aggregate); everything else is shared with the mean.
+template <bool FEDOPT, int AGG_PAD>
 __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const CommArgs a) {
   __shared__ float sm[32];
   __shared__ int s_abort;
@@ -189,7 +275,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   __syncthreads();
   const uint32_t epoch = a.sync[0] + 1;
   const float rho = a.rho_dev != nullptr ? __ldg(a.rho_dev) : a.rho;
-  const float inv_scale = a.mode == 2 ? 1.f / (float(a.K) * rho) : 1.f / float(a.K);
+  const float inv_scale = AGG_PAD > 0 ? 1.f : a.mode == 2 ? 1.f / (float(a.K) * rho) : 1.f / float(a.K);
   const int n4 = a.n >> 2;
   const int nslices = a.two_shot ? a.world : 1;
   const int chunk4 = a.two_shot ? (n4 + a.world - 1) / a.world : n4;
@@ -213,8 +299,8 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       const bool has1 = i1 < hi;
       const size_t off0 = 4 * size_t(i), off1 = 4 * size_t(has1 ? i1 : i);
       float4 accs[2];
-      accs[0] = gather_v4(a, off0, rho, use_mc);
-      accs[1] = has1 ? gather_v4(a, off1, rho, use_mc) : accs[0];
+      accs[0] = reduce_v4<AGG_PAD>(a, off0, rho, use_mc);
+      accs[1] = has1 ? reduce_v4<AGG_PAD>(a, off1, rho, use_mc) : accs[0];
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
         if (u == 1 && !has1) break;
@@ -269,7 +355,9 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   if (blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
     const int i = tail0 + threadIdx.x;
     float acc = 0.f;
-    if (use_mc) {
+    if constexpr (AGG_PAD > 0) {
+      acc = robust_gather_f32<AGG_PAD>(a, i);
+    } else if (use_mc) {
       acc = multimem_ld_reduce_f32(a.mc_x + i);
       if (a.mode == 2) acc = fmaf(rho, acc, multimem_ld_reduce_f32(a.mc_y + i));
     } else {
@@ -453,9 +541,26 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   if (args.opt != FEDOPT_NONE &&
       (args.opt > FEDOPT_YOGI || args.mode != 0 || args.m == nullptr || (args.opt != FEDOPT_AVGM && args.v == nullptr)))
     throw std::runtime_error("fedb200: block_reduce: server optimizer needs mode 0 and its state vectors");
-  const void* kernel = args.opt != FEDOPT_NONE ? (const void*)block_reduce_kernel<true> : (const void*)block_reduce_kernel<false>;
-  static int max_blocks[2] = {0, 0};
-  int& mb = max_blocks[args.opt != FEDOPT_NONE];
+  if (args.agg != AGG_MEAN) {
+    if (args.agg != AGG_MEDIAN && args.agg != AGG_TRIMMED)
+      throw std::runtime_error("fedb200: block_reduce: unknown aggregation rule");
+    if (args.K > COMM_MAX_K_ROBUST)
+      throw std::runtime_error("fedb200: block_reduce: robust aggregation supports at most 16 workers");
+    if (args.mode == 2) throw std::runtime_error("fedb200: block_reduce: robust aggregation needs mode 0 or 1");
+    if (args.agg == AGG_TRIMMED && (args.trim_b < 0 || 2 * args.trim_b >= args.K))
+      throw std::runtime_error("fedb200: block_reduce: trimmed mean needs 0 <= 2 trim_b < K");
+  }
+  const bool fo = args.opt != FEDOPT_NONE;
+  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers]
+  const void* kernels[2][4] = {
+      {(const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
+       (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>},
+      {(const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
+       (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>}};
+  const int pad = args.agg == AGG_MEAN ? 0 : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
+  const void* kernel = kernels[fo][pad];
+  static int max_blocks[2][4] = {};
+  int& mb = max_blocks[fo][pad];
   if (mb == 0) mb = comm_max_blocks(kernel);
   int cap = mb;
   if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;

@@ -227,8 +227,15 @@ struct CommArgs {
   float* vw[COMM_MAX_WORLD];
   float* mc_m;                       // multicast addresses of the m / v slices (multimem.st) or nullptr
   float* mc_v;
+  // ---- robust aggregation (modes 0 / 1, with or without a server optimizer): a per-coordinate order statistic over the
+  // K workers replaces the mean.  Computed in registers, so K <= COMM_MAX_K_ROBUST; peers are read over P2P even when a
+  // multicast object is bound (no in-switch order statistics).
+  int agg;                           // AGG_MEAN selects the instantiations above
+  int trim_b;                        // AGG_TRIMMED: values dropped at each end (0 <= 2 trim_b < K)
 };
 constexpr int FEDOPT_NONE = 0, FEDOPT_AVGM = 1, FEDOPT_ADAGRAD = 2, FEDOPT_ADAM = 3, FEDOPT_YOGI = 4;
+constexpr int AGG_MEAN = 0, AGG_MEDIAN = 1, AGG_TRIMMED = 2;
+constexpr int COMM_MAX_K_ROBUST = 16;
 void block_reduce_launch(const CommArgs& args, cudaStream_t s);
 
 // Barzilai-Borwein / spectral penalty update of consensus ADMM as ONE kernel (SURVEY G20, X4): six dots per worker

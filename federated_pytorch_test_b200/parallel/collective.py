@@ -5,7 +5,8 @@ one device):
 
 * X1 FedAvg  ``z' = sum_k x_k / K``; ``dual = ||z - z'||``; write ``z'`` into every replica
   (/root/reference/src/federated_multi.py:204-217); with a server optimizer (``fedopt_``) ``z'`` is its step from ``z``
-  along ``mean_k x_k - z`` instead of the plain mean
+  along ``mean_k x_k - z`` instead of the plain mean; with a robust rule (``robust_``) ``z'`` is the coordinate-wise
+  median or trimmed mean of the K workers instead of their mean
 * X2 FedProx ``z' = mean``; ``dual``; ``primal = sum_k ||rho (x_k - z')||``; no write-back
   (fedprox_multi.py:211-232)
 * X3 ADMM    ``z' = sum_k (y_k + rho x_k) / (K rho)``; ``dual``; ``y_k += rho (x_k - z')``;
@@ -30,6 +31,16 @@ from .topology import Topology
 
 # server optimizers of FedAvg (Hsu et al. 2019; Reddi et al. 2021), in the order of the kernel's codes 1..4
 FEDOPT_KINDS = ("avgm", "adagrad", "adam", "yogi")
+# Byzantine-robust aggregation rules (Yin et al. 2018), in the order of the kernel's codes 1..2 (0 is the mean)
+ROBUST_AGGS = ("median", "trimmed_mean")
+
+
+def check_robust(K: int, agg: str, trim_b: int) -> None:
+    """Raise ``ValueError`` unless ``agg`` is a robust rule that can run over ``K`` workers with ``trim_b``."""
+    if agg not in ROBUST_AGGS:
+        raise ValueError("robust aggregation rule must be one of %s, got %r" % (", ".join(ROBUST_AGGS), agg))
+    if agg == "trimmed_mean" and not 0 <= 2 * trim_b < K:
+        raise ValueError("trimmed mean needs 0 <= 2 trim_b < K, got trim_b = %r at K = %d" % (trim_b, K))
 
 
 class TorchCollective:
@@ -78,6 +89,40 @@ class TorchCollective:
             full[ck] = local_rows[i]
         return self._allreduce(full)
 
+    def gather_blocks(self, xs: Sequence[torch.Tensor]) -> torch.Tensor:
+        """``[K, n]``: the block slices of ALL K workers, row ``ck`` = worker ``ck`` (local replica ``j`` of rank ``r`` is
+        worker ``r + j * world``)."""
+        local = torch.stack(list(xs))
+        W = self.topo.world_size
+        if not self.topo.is_distributed:
+            parts = [local]
+        else:
+            parts = [torch.empty_like(local) for _ in range(W)]
+            dist.all_gather(parts, local, group=self.topo.group)
+        full = torch.empty((self.topo.K,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
+        for r, part in enumerate(parts):
+            for j in range(part.shape[0]):
+                full[r + j * W] = part[j]
+        return full
+
+    def robust_aggregate(self, xs: Sequence[torch.Tensor], agg: str, trim_b: int) -> torch.Tensor:
+        """Coordinate-wise order statistic over all K workers (fresh tensor).  NaN orders as +inf, +-inf keep their sign.
+        'median': the middle value for odd K, ``(lo + hi) * 0.5`` of the two middle values for even K (``np.median``).
+        'trimmed_mean': drop ``trim_b`` values at each end and average the rest, summed in ascending order
+        (``scipy.stats.trim_mean``)."""
+        K = self.topo.K
+        check_robust(K, agg, trim_b)
+        full = self.gather_blocks(xs)
+        full = torch.where(torch.isnan(full), torch.full_like(full, float("inf")), full)
+        srt = torch.sort(full, dim=0).values
+        if agg == "median":
+            hi = srt[K // 2]
+            return hi.clone() if K % 2 else (srt[K // 2 - 1] + hi) * 0.5
+        acc = srt[trim_b].clone()
+        for j in range(trim_b + 1, K - trim_b):
+            acc.add_(srt[j])
+        return acc.div_(K - 2 * trim_b)
+
     def barrier(self) -> None:
         self.topo.barrier()
 
@@ -95,12 +140,30 @@ class TorchCollective:
         return dual_sq
 
     @torch.no_grad()
+    def robust_(self, xs: List[torch.Tensor], z: torch.Tensor, agg: str, trim_b: int = 0,
+                write_back: bool = True) -> torch.Tensor:
+        """:meth:`fedavg_` with a robust rule (:meth:`robust_aggregate`) in place of the mean: ``z <-`` the aggregate,
+        optionally ``x_k <- z``; returns ``||z_old - z_new||^2`` (0-dim)."""
+        znew = self.robust_aggregate(xs, agg, trim_b)
+        diff = z - znew
+        dual_sq = torch.dot(diff, diff)
+        z.copy_(znew)
+        if write_back:
+            for x in xs:
+                x.copy_(znew)
+        return dual_sq
+
+    @torch.no_grad()
     def fedopt_(self, xs: List[torch.Tensor], z: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], kind: str,
-                lr: float, beta1: float, beta2: float, tau: float) -> torch.Tensor:
+                lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean", trim_b: int = 0) -> torch.Tensor:
         """FedAvg with a server optimizer, in place: ``d = mean_k x_k - z`` is the pseudo-gradient of server optimizer
         ``kind`` (one of :data:`FEDOPT_KINDS`; ``beta1`` is the momentum of 'avgm'), whose state ``m`` (and ``v``, unused
-        by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``."""
-        mean = self.sum_blocks(xs).div_(self.topo.K)
+        by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``.
+        With a robust rule ``agg`` (one of :data:`ROBUST_AGGS`) its aggregate replaces the mean in ``d``."""
+        if agg == "mean":
+            mean = self.sum_blocks(xs).div_(self.topo.K)
+        else:
+            mean = self.robust_aggregate(xs, agg, trim_b)
         d = mean - z
         if kind == "avgm":
             m.mul_(beta1).add_(d)

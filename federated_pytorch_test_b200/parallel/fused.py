@@ -26,6 +26,10 @@ memory, so an aggregation round is host-free and CUDA-graph capturable: one coop
 Small blocks are reduced ONE-SHOT (every rank pulls the whole vector: ``multimem.ld_reduce`` in the
 switch, or K P2P loads); blocks of 256 KB and more TWO-SHOT: rank r reduces slice r and broadcasts
 it with ``multimem.st`` (or P2P stores) into every rank's weights / consensus vector.
+
+The robust rules (coordinate-wise median / trimmed mean) run in separate instantiations of the same kernel: every
+coordinate's K values are loaded over P2P (there is no in-switch order statistic; the two-shot broadcast may still use
+``multimem.st``) and sorted in registers, so K <= 16.
 """
 from __future__ import annotations
 
@@ -36,7 +40,7 @@ import torch
 import torch.distributed as dist
 
 from ..ops import cuda_ops
-from .collective import FEDOPT_KINDS, TorchCollective
+from .collective import FEDOPT_KINDS, ROBUST_AGGS, TorchCollective, check_robust
 from .topology import Topology
 
 _MAX_LOCAL = 16
@@ -167,11 +171,13 @@ class FusedCollective(TorchCollective):
         self.last_two_shot = False
         self.last_rho = float("nan")
         self.warm_fedopt = False          # set by the FedOpt strategy: warm the server-optimizer instantiation too
+        self.warm_robust = False          # set by robust strategies: warm the robust instantiation(s) for this K too
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
         cross-rank handshake happen here, at engine construction, not inside the first training round (the first launch
-        is far slower than the ones after it).  The server-optimizer kernel is warmed only when ``warm_fedopt`` is set.
+        is far slower than the ones after it).  The server-optimizer kernel is warmed only when ``warm_fedopt`` is set, the
+        robust kernels (of this K; with the server optimizer if both are set) only when ``warm_robust`` is set.
         Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
@@ -191,6 +197,10 @@ class FusedCollective(TorchCollective):
             self._launch(2, xs, ys, z, 0.5, rho)
             if self.warm_fedopt:
                 self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3)
+            if self.warm_robust:
+                self._launch(0, xs, None, z, 0.0, agg="median")
+                if self.warm_fedopt:
+                    self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, agg="median")
         self.two_shot_mode = keep
         x0 = [torch.zeros_like(x) for x in xs]
         yh = [torch.zeros_like(x) for x in xs]
@@ -242,7 +252,18 @@ class FusedCollective(TorchCollective):
             return False
         return self.two_shot_mode == "1" or n * 4 >= TWO_SHOT_MIN_BYTES
 
-    def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None) -> None:
+    def _agg_code(self, agg: str, trim_b: int) -> int:
+        """Kernel code of aggregation rule ``agg`` (0 = the mean); raises ``ValueError`` for a rule the kernel cannot run."""
+        if agg == "mean":
+            return 0
+        check_robust(self.topo.K, agg, trim_b)
+        if self.topo.K > 16:
+            raise ValueError("robust aggregation supports at most 16 workers, got K = %d" % self.topo.K)
+        return ROBUST_AGGS.index(agg) + 1
+
+    def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None, agg: str = "mean", trim_b: int = 0) -> None:
+        """Modes 0 / 1 take a robust rule ``agg`` (:data:`ROBUST_AGGS`) in place of the mean."""
+        code = self._agg_code(agg, trim_b)
         n = xs[0].numel()
         if any(t.numel() != n for t in xs) or z.numel() != n:
             raise ValueError("block slices must have equal length")
@@ -264,14 +285,16 @@ class FusedCollective(TorchCollective):
                     mcz = za["mc_ptr"] + zoff
         self.ext.block_reduce(mode, xp, yp, local_idx, z, n, float(rho), rho_dev, self.out, self.scratch, self.ctrl_ptrs,
                               self.sync, W, self.topo.rank, mcx, mcy, mcz, xw, zw, bool(two), self.max_blocks,
-                              self.timeout_s)
+                              self.timeout_s, code, int(trim_b))
         self.launches += 1
         self.last_two_shot = bool(two)
 
-    def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float) -> None:
+    def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
+                       trim_b: int = 0) -> None:
         """FedAvg with a server optimizer: mode 0 of the kernel's FedOpt instantiation.  Two-shot, rank r broadcasts slice r
         of the new weights, of ``m`` and of ``v`` into every rank, so ``m`` / ``v`` must be symmetric slices then
-        (:meth:`zeros_like_block`)."""
+        (:meth:`zeros_like_block`).  A robust rule ``agg`` replaces the mean as the aggregate the step is taken towards."""
+        code = self._agg_code(agg, trim_b)
         n = xs[0].numel()
         adaptive = kind != "avgm"
         if any(t.numel() != n for t in xs) or z.numel() != n or m.numel() != n or (adaptive and v.numel() != n):
@@ -289,7 +312,7 @@ class FusedCollective(TorchCollective):
         self.ext.block_reduce_fedopt(FEDOPT_KINDS.index(kind) + 1, float(lr), float(beta1), float(beta2), float(tau), m,
                                      v if adaptive else None, xp, local_idx, z, n, self.out, self.scratch, self.ctrl_ptrs,
                                      self.sync, W, self.topo.rank, mcx, mcm, mcv, xw, mw, vw, bool(two), self.max_blocks,
-                                     self.timeout_s)
+                                     self.timeout_s, code, int(trim_b))
         self.launches += 1
         self.last_two_shot = bool(two)
 
@@ -308,8 +331,13 @@ class FusedCollective(TorchCollective):
         self._launch(0 if write_back else 1, xs, None, z, 0.0)
         self._record_async()
 
-    def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float) -> None:
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau)
+    def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
+                       trim_b: int = 0) -> None:
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b)
+        self._record_async()
+
+    def launch_robust_(self, xs, z, agg: str, trim_b: int = 0, write_back: bool = True) -> None:
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, agg=agg, trim_b=trim_b)
         self._record_async()
 
     def launch_fedprox_(self, xs, z, rho: float) -> None:
@@ -342,8 +370,14 @@ class FusedCollective(TorchCollective):
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
-    def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float):
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau)
+    def robust_(self, xs, z, agg: str, trim_b: int = 0, write_back: bool = True):
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, agg=agg, trim_b=trim_b)
+        return self.read_record()[OUT_DUAL_SQ]
+
+    @torch.no_grad()
+    def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
+                trim_b: int = 0):
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
