@@ -310,6 +310,8 @@ class Engine:
         xs = [rep.block(visit) for rep in self.replicas]
         arena0 = self.replicas[0].arenas[visit.model]
         N = arena0.count(visit.lo, visit.hi)
+        if getattr(strat, "dp", False):            # DP noise goes to parameters only, not to the arena's alignment padding
+            strat.set_param_layout(visit.ci, arena0.chunk_counts(visit.lo, visit.hi))
         strat.begin_block(visit.ci, N, xs)
         self.optimizers = [self._make_optimizer(rep, visit) for rep in self.replicas]
         first_round = 0

@@ -93,32 +93,94 @@ class FedAvg(Strategy):
     """FedAvg: ``z <-`` the mean of the K replicas, written back into every replica.  ``aggregator`` 'median' or
     'trimmed_mean' (Yin et al. 2018) replaces the mean by a coordinate-wise order statistic over the K replicas that a
     minority of diverging or malicious workers cannot move arbitrarily far (``trimmed_mean`` drops
-    ``floor(trim_fraction K)`` values at each end); the round is otherwise the same."""
+    ``floor(trim_fraction K)`` values at each end); the round is otherwise the same.
+
+    ``dp_clip > 0`` makes it DP-FedAvg (client-level differential privacy, McMahan et al. 2018; ``algo/privacy.py``).
+    With ``z`` the server model the round started from, every worker's update ``x_k - z`` is clipped to
+    ``C = dp_clip sqrt(N)`` (a worker within the bound is not written at all), and ``z <- mean_k x_k + (sigma C / K) xi``
+    with ``sigma = dp_noise`` and ``xi`` the counter-based draw of DP round ``t`` (``t`` counts the DP rounds of the run and
+    lives in device memory).  Each round is two launches on the fused collective (clip, aggregate).  ``z`` starts each
+    block visit as the server model, i.e. the replicas' common value, instead of 0 (Q6), so the ``dual`` of the first round
+    of a visit differs from plain FedAvg.  The round metrics gain ``dp_clipped`` (workers clipped), ``dp_update_norm``
+    (mean pre-clip update norm over the K workers), ``dp_clip_norm`` (``C``) and ``dp_epsilon`` (spent so far at
+    ``dp_delta``)."""
 
     name = "fedavg"
     write_back = True
 
-    def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1):
-        from ..config import check_aggregator, trim_count
+    def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1, dp_clip: float = 0.0,
+                 dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0):
+        from ..config import check_aggregator, check_dp, trim_count
 
         super().__init__(collective, topo)
         check_aggregator(aggregator, trim_fraction, topo.K)
+        check_dp(dp_clip, dp_noise, dp_delta, aggregator)
         self.aggregator = aggregator
         self.trim_b = trim_count(trim_fraction, topo.K) if aggregator == "trimmed_mean" else 0
         if aggregator != "mean" and hasattr(collective, "warm_robust"):
             collective.warm_robust = True
+        self.dp = dp_clip > 0.0
+        self.dp_clip, self.dp_noise, self.dp_delta = float(dp_clip), float(dp_noise), float(dp_delta)
+        self.dp_rounds = 0                     # host mirror of the device round counter dp_t
+        if self.dp:
+            from .privacy import noise_key
+
+            self.dp_key = noise_key(seed)
+            self.dp_t = torch.zeros(1, dtype=torch.int64, device=topo.device)
+            self.dp_layouts: Dict[int, torch.Tensor] = {}     # block index -> parameter layout (DPRound.valid)
+            if hasattr(collective, "warm_dp"):
+                collective.warm_dp = True
+
+    def begin_block(self, ci: int, N: int, xs: List[torch.Tensor]) -> None:
+        super().begin_block(ci, N, xs)
+        if self.dp:                            # the server model: the replicas are equal here, so a local copy suffices
+            self.z.copy_(xs[0])
+
+    # -- DP -------------------------------------------------------------------------------------------------------
+    def set_param_layout(self, ci: int, chunk_counts: List[int]) -> None:
+        """The parameter layout of block ``ci`` (``FlatArena.chunk_counts``): the noise skips the alignment padding.
+        Without it every float of the block slice is noised."""
+        if ci not in self.dp_layouts:
+            self.dp_layouts[ci] = torch.tensor(chunk_counts, dtype=torch.uint8, device=self.topo.device)
+
+    def dp_bound(self) -> float:
+        """``C`` of the current block."""
+        return self.dp_clip * math.sqrt(self.N)
+
+    def _dp_kw(self) -> Dict[str, object]:
+        """Clip the local replicas (first launch of a DP round) and return the noise argument of the aggregation."""
+        if not self.dp:
+            return {}
+        from ..parallel.collective import DPRound
+
+        C = self.dp_bound()
+        self.coll.dp_clip_(self.xs, self.z, C)
+        self.dp_rounds += 1
+        return {"dp": DPRound(self.dp_noise * C / self.topo.K, self.dp_key, self.dp_t, self.dp_layouts.get(self.ci))}
+
+    def dp_epsilon(self, rounds: Optional[int] = None) -> float:
+        from .privacy import gaussian_epsilon
+
+        return gaussian_epsilon(self.dp_noise, self.dp_rounds if rounds is None else rounds, self.dp_delta)
+
+    def _with_dp(self, metrics: Dict[str, float]) -> Dict[str, float]:
+        if self.dp:
+            clipped, norms = self.coll.last_dp
+            metrics.update(dp_clipped=float(clipped), dp_update_norm=float(norms) / self.topo.K,
+                           dp_clip_norm=self.dp_bound(), dp_epsilon=self.dp_epsilon())
+        return metrics
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         if self.aggregator == "mean":
-            dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True)
+            dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw())
         else:
             dual_sq = self.coll.robust_(self.xs, self.z, self.aggregator, self.trim_b)
-        return {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}
+        return self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             if self.aggregator == "mean":
-                self.coll.launch_fedavg_(self.xs, self.z, True)
+                self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw())
             else:
                 self.coll.launch_robust_(self.xs, self.z, self.aggregator, self.trim_b)
             return ("pending", self.N)
@@ -127,7 +189,7 @@ class FedAvg(Strategy):
     def aggregate_end(self, token) -> Dict[str, float]:
         if token[0] == "done":
             return token[1]
-        return {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]}
+        return self._with_dp({"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]})
 
     def _robust_state(self) -> Dict[str, object]:
         return {} if self.aggregator == "mean" else {"aggregator": self.aggregator, "trim_b": self.trim_b}
@@ -138,11 +200,27 @@ class FedAvg(Strategy):
             raise ValueError("resume record holds aggregator %r (trim_b %d), this run uses %r (trim_b %d)"
                              % (got + (self.aggregator, self.trim_b)))
 
+    def _dp_state(self) -> Dict[str, object]:
+        if not self.dp:
+            return {}
+        return {"dp": (self.dp_clip, self.dp_noise, self.dp_delta, self.dp_key), "dp_t": self.dp_rounds}
+
+    def _check_dp_state(self, st: Dict[str, object]) -> None:
+        got = tuple(st["dp"]) if st.get("dp") is not None else None
+        want = self._dp_state().get("dp")
+        if got != want:
+            raise ValueError("resume record holds DP settings (dp_clip, dp_noise, dp_delta, key) %r, this run uses %r"
+                             % (got, want))
+        if self.dp:
+            self.dp_rounds = int(st["dp_t"])
+            self.dp_t.fill_(self.dp_rounds)
+
     def state(self) -> Dict[str, object]:
-        return {"z": self.z, **self._robust_state()}
+        return {"z": self.z, **self._robust_state(), **self._dp_state()}
 
     def load_state(self, st: Dict[str, object]) -> None:
         self._check_robust_state(st)
+        self._check_dp_state(st)
         self.z.copy_(st["z"].to(self.z.device))
 
 
@@ -160,16 +238,19 @@ class FedOpt(FedAvg):
     across its visits for the whole run (``m = 0``, ``v = tau^2`` at its first visit); on the fused collective they are
     slices of symmetric arenas, so two-shot ranks broadcast their slice of both into every rank and every rank ends each
     round with the same ``z``, ``m`` and ``v``.  With a robust ``aggregator`` its aggregate replaces the mean in ``d``
-    (e.g. robust FedAdam); the server model at the start of a visit stays the mean (the replicas are equal then)."""
+    (e.g. robust FedAdam); the server model at the start of a visit stays the mean (the replicas are equal then).  With DP
+    (``dp_clip > 0``) the noised mean of the clipped workers replaces the mean in ``d`` (DP-FedAdam etc.: post-processing),
+    and the server model at the start of a visit is the replicas' common value, copied locally (no launch)."""
 
     name = "fedopt"
 
     def __init__(self, collective, topo, kind: str = "adam", lr: float = 0.0, momentum: float = 0.9, beta1: float = 0.9,
-                 beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1):
+                 beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1,
+                 dp_clip: float = 0.0, dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0):
         from ..config import check_server_opt
         from ..parallel.collective import FEDOPT_KINDS
 
-        super().__init__(collective, topo, aggregator, trim_fraction)
+        super().__init__(collective, topo, aggregator, trim_fraction, dp_clip, dp_noise, dp_delta, seed)
         if kind not in FEDOPT_KINDS:
             raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
         check_server_opt(kind, lr, momentum, beta1, beta2, tau)
@@ -195,7 +276,8 @@ class FedOpt(FedAvg):
             if ci in self._restored:
                 self._install(ci, *self._restored.pop(ci))
         self.m, self.v = self.ms[ci], self.vs.get(ci)
-        self.coll.fedavg_(xs, self.z, write_back=False)          # the server model: the replicas' mean, no write-back
+        if not self.dp:                                           # (DP: FedAvg.begin_block copied the replicas' value)
+            self.coll.fedavg_(xs, self.z, write_back=False)      # the server model: the replicas' mean, no write-back
 
     def _hyper(self):
         return self.kind, self.lr, self.beta1, self.beta2, self.tau
@@ -204,12 +286,12 @@ class FedOpt(FedAvg):
         return {} if self.aggregator == "mean" else {"agg": self.aggregator, "trim_b": self.trim_b}
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
-        dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw())
-        return {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}
+        dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw())
+        return self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
-            self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw())
+            self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw())
             return ("pending", self.N)
         return ("done", self.aggregate(nadmm))
 
@@ -220,7 +302,7 @@ class FedOpt(FedAvg):
         vs = {ci: v for ci, (_, v) in self._restored.items() if v is not None}
         ms.update(self.ms)
         vs.update(self.vs)
-        return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state()}
+        return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state(), **self._dp_state()}
 
     def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
         self.ms[ci].copy_(m.to(self.ms[ci].device))
@@ -231,6 +313,7 @@ class FedOpt(FedAvg):
         if st.get("server_opt") != self.kind:
             raise ValueError("resume record holds server optimizer %r, this run uses %r" % (st.get("server_opt"), self.kind))
         self._check_robust_state(st)
+        self._check_dp_state(st)
         self.z.copy_(st["z"].to(self.z.device))
         vs = st.get("v") or {}
         for ci, m in (st.get("m") or {}).items():

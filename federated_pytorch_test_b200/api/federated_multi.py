@@ -11,10 +11,15 @@ the same kernel; the default ``none`` is the reference's FedAvg.
 ``--aggregator median|trimmed_mean`` (``--trim_fraction``) replaces the mean of the K replicas by a coordinate-wise order
 statistic (Byzantine-robust aggregation), with or without a server optimizer; ``--byzantine b --attack
 signflip|gaussian|nan --attack_scale s`` turns the last b workers into simulated attackers (``algo/byzantine.py``).
+
+``--dp_clip c --dp_noise sigma --dp_delta delta`` makes the mean DP-FedAvg (client-level differential privacy, with or
+without a server optimizer): every worker's block update is clipped to ``c sqrt(N)`` and Gaussian noise is added to the
+mean (``algo/privacy.py``).  The root logs ``dp: ...`` lines with the planned and the spent epsilon.
 """
 from __future__ import annotations
 
 from ..algo.byzantine import ByzantineAttack
+from ..algo.privacy import dp_line
 from ..algo.strategies import FedAvg, FedOpt
 from ..config import FederatedConfig, parse_config
 from . import common
@@ -24,6 +29,8 @@ Config = FederatedConfig
 
 def make_strategy(cfg: Config, coll, topo):
     robust = {} if cfg.aggregator == "mean" else dict(aggregator=cfg.aggregator, trim_fraction=cfg.trim_fraction)
+    if cfg.dp_clip > 0.0:
+        robust.update(dp_clip=cfg.dp_clip, dp_noise=cfg.dp_noise, dp_delta=cfg.dp_delta, seed=cfg.seed)
     if cfg.server_opt == "none":
         return FedAvg(coll, topo, **robust)
     return FedOpt(coll, topo, cfg.server_opt, cfg.server_lr, cfg.server_momentum, cfg.server_beta1, cfg.server_beta2,
@@ -40,7 +47,14 @@ def make_attack(cfg: Config):
 def run(cfg: Config, log=print):
     topo, coll = common.setup_runtime(cfg)
     task = common.ClassifierTask(cfg, topo, cfg.lambda1, cfg.lambda2)
-    engine = common.run_engine(cfg, task, topo, coll, make_strategy(cfg, coll, topo), None, log, attack=make_attack(cfg))
+    strategy = make_strategy(cfg, coll, topo)
+    dp_log = strategy.dp and topo.is_root
+    if dp_log:
+        planned = cfg.Nloop * len(list(task.visits(0))) * cfg.Nadmm * cfg.Nepoch
+        log(dp_line(cfg.dp_noise, cfg.dp_clip, cfg.dp_delta, planned, planned=True))
+    engine = common.run_engine(cfg, task, topo, coll, strategy, None, log, attack=make_attack(cfg))
+    if dp_log:
+        log(dp_line(cfg.dp_noise, cfg.dp_clip, cfg.dp_delta, strategy.dp_rounds, planned=False))
     common.save_legacy(cfg, engine)
     return engine
 

@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import argparse
 import dataclasses
+import math
 from dataclasses import dataclass, field
 from typing import Optional, Sequence, Type, TypeVar
 
@@ -119,6 +120,19 @@ def check_byzantine(byzantine: int, attack: str, attack_scale: float, K: int) ->
         raise ValueError("attack_scale must be > 0, got %r" % (attack_scale,))
 
 
+def check_dp(dp_clip: float, dp_noise: float, dp_delta: float, aggregator: str) -> None:
+    """Raise ``ValueError`` unless the differential-privacy settings of :class:`FederatedConfig` are valid."""
+    if not (math.isfinite(dp_clip) and dp_clip >= 0.0):
+        raise ValueError("dp_clip must be finite and >= 0 (0 = off), got %r" % (dp_clip,))
+    if not dp_noise >= 0.0:
+        raise ValueError("dp_noise must be >= 0, got %r" % (dp_noise,))
+    if not 0.0 < dp_delta < 1.0:
+        raise ValueError("dp_delta must lie in (0, 1), got %r" % (dp_delta,))
+    if dp_clip > 0.0 and aggregator != "mean":
+        raise ValueError("dp_clip needs aggregator 'mean' (robust rules have a different sensitivity), got aggregator %r"
+                         % (aggregator,))
+
+
 @dataclass
 class FederatedConfig(CommonConfig):
     lambda1: float = 0.0001
@@ -137,12 +151,18 @@ class FederatedConfig(CommonConfig):
     byzantine: int = 0
     attack: str = "signflip"        # 'signflip': x <- z - s (x - z) | 'gaussian': x <- z + s N(0, 1) | 'nan': x <- NaN
     attack_scale: float = 4.0       # s
+    # client-level differential privacy (DP-FedAvg): clip every worker's block update to C = dp_clip * sqrt(N), add
+    # N(0, (dp_noise C / K)^2) noise to the mean (algo/privacy.py)
+    dp_clip: float = 0.0            # 0 = off
+    dp_noise: float = 1.0           # noise multiplier sigma (0 = clipping only)
+    dp_delta: float = 1e-5          # delta at which epsilon is reported
 
     def __post_init__(self):
         check_server_opt(self.server_opt, self.server_lr, self.server_momentum, self.server_beta1, self.server_beta2,
                          self.server_tau)
         check_aggregator(self.aggregator, self.trim_fraction, self.K)
         check_byzantine(self.byzantine, self.attack, self.attack_scale, self.K)
+        check_dp(self.dp_clip, self.dp_noise, self.dp_delta, self.aggregator)
 
 
 @dataclass

@@ -588,6 +588,27 @@ void smallconv_wgrad(Tensor dz, Tensor x, Tensor dw, c10::optional<Tensor> db, i
 // ---------------------------------------------------------------------------------------------- collectives
 // Pointers are passed as integers: local tensors' data_ptr() or peer-mapped addresses from symmetric memory.
 // agg = AGG_MEAN / AGG_MEDIAN / AGG_TRIMMED picks the aggregation rule (trim_b: values dropped at each end, trimmed mean).
+// DP rounds (dp_t given): noise std of the mean, key of the noise stream, the device round counter (int64), the stats
+// record of the dp_clip launch that precedes the aggregation and, optionally, the block's parameter layout (dp_valid).
+static void set_dp(fb::CommArgs& a, double dp_std, int64_t dp_key, const c10::optional<Tensor>& dp_t,
+                   const c10::optional<Tensor>& dp_stats, const c10::optional<Tensor>& dp_valid) {
+  if (!dp_t.has_value() || !dp_t->defined()) return;
+  TORCH_CHECK(dp_t->is_cuda() && dp_t->scalar_type() == at::kLong && dp_t->numel() >= 1, "DP round counter: int64 CUDA tensor");
+  TORCH_CHECK(dp_stats.has_value() && dp_stats->defined() && dp_stats->numel() >= fb::DP_STATS_FLOATS,
+              "DP rounds need the dp_clip stats record");
+  CHECK_F32_CUDA((*dp_stats));
+  a.dp = 1;
+  a.dp_std = (float)dp_std;
+  a.dp_key = (unsigned long long)dp_key;
+  a.dp_t = reinterpret_cast<long long*>(dp_t->data_ptr<int64_t>());
+  a.dp_stats = dp_stats->data_ptr<float>() + fb::DP_NORM;
+  if (dp_valid.has_value() && dp_valid->defined()) {
+    TORCH_CHECK(dp_valid->is_cuda() && dp_valid->scalar_type() == at::kByte && dp_valid->is_contiguous() &&
+                    dp_valid->numel() >= (a.n + fb::DP_CHUNK - 1) / fb::DP_CHUNK,
+                "DP parameter layout: uint8 CUDA tensor with one count per 32-float chunk of the block");
+    a.dp_valid = dp_valid->data_ptr<uint8_t>();
+  }
+}
 static void fill_ctrl(uint32_t** dst, const std::vector<int64_t>& ctrl_ptrs, int world) {
   for (int p = 0; p < world && p < (int)ctrl_ptrs.size(); ++p) dst[p] = reinterpret_cast<uint32_t*>(ctrl_ptrs[p]);
 }
@@ -595,7 +616,8 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
                   Tensor z, int64_t n, double rho, c10::optional<Tensor> rho_dev, Tensor out, Tensor scratch,
                   std::vector<int64_t> ctrl_ptrs, Tensor sync, int64_t world, int64_t rank, int64_t mc_x, int64_t mc_y,
                   int64_t mc_z, std::vector<int64_t> xw_ptrs, std::vector<int64_t> zw_ptrs, bool two_shot,
-                  int64_t max_blocks, double timeout_s, int64_t agg, int64_t trim_b) {
+                  int64_t max_blocks, double timeout_s, int64_t agg, int64_t trim_b, double dp_std, int64_t dp_key,
+                  c10::optional<Tensor> dp_t, c10::optional<Tensor> dp_stats, c10::optional<Tensor> dp_valid) {
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch);
   TORCH_CHECK(out.numel() >= fb::COMM_OUT_FLOATS && scratch.numel() >= fb::COMM_SCRATCH_FLOATS, "out / scratch too small");
   c10::cuda::CUDAGuard guard(z.device());
@@ -633,6 +655,7 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
   a.sync = reinterpret_cast<uint32_t*>(sync.data_ptr<int>());
   a.timeout_cycles = (long long)(timeout_s * 1.9e9);
   a.agg = (int)agg; a.trim_b = (int)trim_b;
+  set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
   fb::block_reduce_launch(a, cur_stream());
 }
 
@@ -643,7 +666,9 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
                          Tensor scratch, std::vector<int64_t> ctrl_ptrs, Tensor sync, int64_t world, int64_t rank,
                          int64_t mc_x, int64_t mc_m, int64_t mc_v, std::vector<int64_t> xw_ptrs,
                          std::vector<int64_t> mw_ptrs, std::vector<int64_t> vw_ptrs, bool two_shot, int64_t max_blocks,
-                         double timeout_s, int64_t agg, int64_t trim_b) {
+                         double timeout_s, int64_t agg, int64_t trim_b, double dp_std, int64_t dp_key,
+                         c10::optional<Tensor> dp_t, c10::optional<Tensor> dp_stats,
+                         c10::optional<Tensor> dp_valid) {
   TORCH_CHECK(opt >= fb::FEDOPT_AVGM && opt <= fb::FEDOPT_YOGI, "block_reduce_fedopt: unknown server optimizer ", opt);
   const bool adaptive = opt != fb::FEDOPT_AVGM;
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch); CHECK_F32_CUDA(m); CHECK_CONTIG(m);
@@ -686,7 +711,26 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
   a.m = m.data_ptr<float>();
   a.v = adaptive ? v->data_ptr<float>() : nullptr;
   a.agg = (int)agg; a.trim_b = (int)trim_b;
+  set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
   fb::block_reduce_launch(a, cur_stream());
+}
+
+// DP-FedAvg update clipping of the local replicas xs against the server model z, bound C; see DPClipArgs.
+void dp_clip(std::vector<Tensor> xs, Tensor z, double bound, Tensor stats, int64_t max_blocks) {
+  TORCH_CHECK(!xs.empty() && xs.size() <= (size_t)fb::COMM_MAX_LOCAL, "dp_clip: bad replica count");
+  CHECK_F32_CUDA(z); CHECK_CONTIG(z); CHECK_F32_CUDA(stats);
+  TORCH_CHECK(stats.numel() >= fb::DP_STATS_FLOATS, "dp_clip: stats too small");
+  c10::cuda::CUDAGuard guard(z.device());
+  fb::DPClipArgs a{};
+  a.n = (int)z.numel(); a.n_local = (int)xs.size(); a.max_blocks = (int)max_blocks; a.bound = (float)bound;
+  for (int j = 0; j < a.n_local; ++j) {
+    CHECK_F32_CUDA(xs[j]); CHECK_CONTIG(xs[j]);
+    TORCH_CHECK(xs[j].numel() == a.n, "dp_clip: block slices must have z's length");
+    a.x[j] = fptr_mut(xs[j]);
+  }
+  a.z = fptr(z);
+  a.stats = fptr_mut(stats);
+  fb::dp_clip_launch(a, cur_stream());
 }
 
 // Barzilai-Borwein update (consensus_multi.py:242-278) as one kernel; see BBArgs.
@@ -814,6 +858,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("smallconv_wgrad", &smallconv_wgrad);
   m.def("block_reduce", &block_reduce);
   m.def("block_reduce_fedopt", &block_reduce_fedopt);
+  m.def("dp_clip", &dp_clip);
   m.def("bb_update", &bb_update);
   m.def("ipc_get_handle", &ipc_get_handle);
   m.def("ipc_open_handle", &ipc_open_handle);

@@ -25,7 +25,8 @@
 //
 // mode: 0 = FedAvg (z = sum x / K, write-back), 1 = FedProx (no write-back), 2 = ADMM (z = sum(y + rho x)/(K rho)).
 // A second instantiation (FEDOPT) runs FedAvg with a server optimizer (FedAvgM / FedAdagrad / FedAdam / FedYogi) between
-// the reduction and the write-back.
+// the reduction and the write-back.  DP instantiations add DP-FedAvg's Gaussian noise to the mean, after dp_clip_kernel
+// (end of file) has clipped the workers' updates.
 // Reference sites: /root/reference/src/federated_multi.py:203-217, fedprox_multi.py:211-232, consensus_multi.py:242-299.
 #include "fedb200.h"
 
@@ -260,13 +261,63 @@ __device__ __forceinline__ float4 reduce_v4(const CommArgs& a, size_t off, float
   else return robust_gather_v4<AGG_PAD>(a, off);
 }
 
+// ---- DP-FedAvg noise: counter-based standard normals (Box-Muller on splitmix64 words) ----------------------------------
+// Coordinates 2p and 2p + 1 of DP round t share the word w = F(F(key + (t + 1) G) + (p + 1) G), arithmetic mod 2^64, with
+// F the splitmix64 finaliser and G = 0x9E3779B97F4A7C15.  u1 = (w[63:40] + 1) 2^-24 in (0, 1], u2 = w[23:0] 2^-24 in
+// [0, 1), r = sqrt(-2 ln u1):  xi_2p = r cos(2 pi u2),  xi_2p+1 = r sin(2 pi u2).  algo/privacy.py (dp_noise) is the
+// float64 numpy oracle.  The draw depends on (key, t, i) only: every rank, one-shot or two-shot, adds the same noise.
+constexpr uint64_t DP_GAMMA = 0x9E3779B97F4A7C15ull;
+__device__ __forceinline__ uint64_t dp_mix(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+__device__ __forceinline__ float2 dp_normal_pair(uint64_t round_key, uint64_t p) {
+  const uint64_t w = dp_mix(round_key + (p + 1ull) * DP_GAMMA);
+  // in double precision: the extension is built with --use_fast_math, whose single-precision log / sincos intrinsics
+  // are off by ~1e-4 in the tails; rounded once to float, xi is within an ulp of the float64 oracle
+  const double u1 = double((w >> 40) + 1ull) * 5.9604644775390625e-8;      // exact: 24-bit integers times 2^-24
+  const double u2 = double(w & 0xFFFFFFull) * 5.9604644775390625e-8;
+  const double r = sqrt(-2.0 * log(u1));
+  double s, c;
+  sincospi(2.0 * u2, &s, &c);
+  return make_float2(float(r * c), float(r * s));
+}
+// DP: the mean plus dp_std * xi at float4 index `off` (a multiple of 4: coordinate pairs off / 2 and off / 2 + 1) or at
+// coordinate i, in the round t = *dp_t the kernel was launched for (the last CTA advances it only after every CTA is done).
+// Alignment padding (dp_valid) gets no noise.  (The kernel calls these through `DP ? noised : mean`, which keeps the other
+// instantiations' code exactly as it was.)
+__device__ __forceinline__ uint64_t dp_round_key(const CommArgs& a) {
+  return dp_mix(a.dp_key + uint64_t(*a.dp_t + 1) * DP_GAMMA);
+}
+// noise std of coordinate i: dp_std for a parameter, 0 for padding
+__device__ __forceinline__ float dp_std_at(const CommArgs& a, size_t i) {
+  if (a.dp_valid == nullptr) return a.dp_std;
+  return int(i % DP_CHUNK) < int(a.dp_valid[i / DP_CHUNK]) ? a.dp_std : 0.f;
+}
+template <bool DP>
+__device__ __forceinline__ float4 dp_noised_v4(const CommArgs& a, size_t off, float4 mean) {
+  const uint64_t key = dp_round_key(a);
+  const float2 g0 = dp_normal_pair(key, off >> 1), g1 = dp_normal_pair(key, (off >> 1) + 1);
+  return make_float4(fmaf(dp_std_at(a, off), g0.x, mean.x), fmaf(dp_std_at(a, off + 1), g0.y, mean.y),
+                     fmaf(dp_std_at(a, off + 2), g1.x, mean.z), fmaf(dp_std_at(a, off + 3), g1.y, mean.w));
+}
+template <bool DP>
+__device__ __forceinline__ float dp_noised_f32(const CommArgs& a, int i, float mean) {
+  const float2 g = dp_normal_pair(dp_round_key(a), uint64_t(i >> 1));
+  return fmaf(dp_std_at(a, size_t(i)), (i & 1) ? g.y : g.x, mean);
+}
+
 // FEDOPT = false: FedAvg / FedProx / ADMM (a.mode).  FEDOPT = true: FedAvg (mode 0) whose new model is a server optimizer
 // step from z instead of the plain mean.  Pass 1 forms the step from the reduced mean, z and the state m (and v): one-shot
 // stores z, m, v locally; two-shot rank r broadcasts slice r of the new weights, of m and of v into every rank, so every rank
 // ends the round with the same z, m and v.  Pass 2 is FedAvg's.
 // AGG_PAD > 0: the robust instantiations (modes 0 / 1): pass 1 takes the median / trimmed mean of the K workers instead of
 // their mean (with FEDOPT, as the server optimizer's aggregate); everything else is shared with the mean.
-template <bool FEDOPT, int AGG_PAD>
+// DP: the DP-FedAvg instantiations (mode 0, the mean, AGG_PAD = 0): pass 1 adds dp_std * xi to the mean before the optional
+// server step (one-shot, two-shot and the scalar tail alike); phase C exchanges the clip statistics of dp_clip_kernel
+// across ranks, and the last CTA advances the round counter dp_t.
+template <bool FEDOPT, int AGG_PAD, bool DP = false>
 __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const CommArgs a) {
   __shared__ float sm[32];
   __shared__ int s_abort;
@@ -306,7 +357,9 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
         if (u == 1 && !has1) break;
         const size_t off = u == 0 ? off0 : off1;
         const float4 acc = accs[u];
-        const float4 zn = make_float4(acc.x * inv_scale, acc.y * inv_scale, acc.z * inv_scale, acc.w * inv_scale);
+        const float4 zn = DP ? dp_noised_v4<DP>(a, off, make_float4(acc.x * inv_scale, acc.y * inv_scale, acc.z * inv_scale,
+                                                                     acc.w * inv_scale))
+                             : make_float4(acc.x * inv_scale, acc.y * inv_scale, acc.z * inv_scale, acc.w * inv_scale);
         if constexpr (FEDOPT) {
           const bool adaptive = a.opt != FEDOPT_AVGM;
           const float4 zo = *reinterpret_cast<const float4*>(a.z + off);
@@ -366,7 +419,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
         acc += a.mode == 2 ? fmaf(rho, xv, ld_sys_f32(a.y[k] + i)) : xv;
       }
     }
-    float zn = acc * inv_scale;
+    float zn = DP ? dp_noised_f32<DP>(a, i, acc * inv_scale) : acc * inv_scale;
     if constexpr (FEDOPT) {                        // every rank steps its own copy of the tail
       float mv = a.m[i], vv = a.opt != FEDOPT_AVGM ? a.v[i] : 0.f;
       zn = fedopt_step(a, a.z[i], zn, mv, vv);
@@ -503,6 +556,50 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       nonfinite = a.two_shot ? b : nonfinite;
     }
   }
+  // DP (mode 0): the clip statistics of dp_clip_kernel, summed over the local replicas and then over the ranks in rank
+  // order, so every rank reports the same values
+  if constexpr (DP) {
+    __shared__ float s_dp[2];
+    if (threadIdx.x == 0) {
+      float clipped = 0.f, norms = 0.f;
+      for (int j = 0; j < a.n_local; ++j) {
+        norms += a.dp_stats[j];
+        clipped += a.dp_stats[COMM_MAX_LOCAL + j];
+      }
+      s_dp[0] = clipped;
+      s_dp[1] = norms;
+    }
+    __syncthreads();
+    if (a.world > 1) {
+      if (threadIdx.x < a.world) {
+        float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_DP_PAYLOAD) + 2 * a.rank;
+        st_sys_f32(pay + 0, s_dp[0]);
+        st_sys_f32(pay + 1, s_dp[1]);
+        __threadfence_system();
+        st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_C + a.rank, epoch);
+        if (s_abort == 0 && !wait_flag(a.ctrl[a.rank] + PAD_FLAG_C + threadIdx.x, epoch, a.timeout_cycles)) {
+          a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
+          atomicExch(&s_abort, 1);
+        }
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_DP_PAYLOAD);
+        float c = 0.f, s = 0.f;
+        for (int r = 0; r < a.world; ++r) {
+          c += ld_sys_f32(pay + 2 * r + 0);
+          s += ld_sys_f32(pay + 2 * r + 1);
+        }
+        s_dp[0] = c;
+        s_dp[1] = s;
+      }
+    }
+    if (threadIdx.x == 0) {
+      a.out[OUT_DP_CLIPPED] = s_dp[0];
+      a.out[OUT_DP_NORM_SUM] = s_dp[1];
+      *a.dp_t += 1;                                // every CTA has read t: the next round (or graph replay) draws t + 1
+    }
+  }
   if (threadIdx.x == 0) {
     a.out[OUT_DUAL_SQ] = dual_sq;
     a.out[OUT_PRIMAL] = primal;
@@ -550,16 +647,20 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
     if (args.agg == AGG_TRIMMED && (args.trim_b < 0 || 2 * args.trim_b >= args.K))
       throw std::runtime_error("fedb200: block_reduce: trimmed mean needs 0 <= 2 trim_b < K");
   }
+  if (args.dp && (args.agg != AGG_MEAN || args.mode != 0 || args.dp_t == nullptr || args.dp_stats == nullptr))
+    throw std::runtime_error("fedb200: block_reduce: DP needs mode 0, the mean, a round counter and clip statistics");
   const bool fo = args.opt != FEDOPT_NONE;
-  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers]
-  const void* kernels[2][4] = {
+  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean]
+  const void* kernels[2][5] = {
       {(const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
-       (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>},
+       (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>,
+       (const void*)block_reduce_kernel<false, 0, true>},
       {(const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
-       (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>}};
-  const int pad = args.agg == AGG_MEAN ? 0 : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
+       (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>,
+       (const void*)block_reduce_kernel<true, 0, true>}};
+  const int pad = args.dp ? 4 : args.agg == AGG_MEAN ? 0 : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
   const void* kernel = kernels[fo][pad];
-  static int max_blocks[2][4] = {};
+  static int max_blocks[2][5] = {};
   int& mb = max_blocks[fo][pad];
   if (mb == 0) mb = comm_max_blocks(kernel);
   int cap = mb;
@@ -578,6 +679,118 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   if (coop) e = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
   else e = cudaLaunchKernel(kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
   if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: block_reduce launch: ") + cudaGetErrorString(e));
+  count_launch();
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// DP-FedAvg update clipping (McMahan et al. 2018) — see DPClipArgs in fedb200.h
+// ------------------------------------------------------------------------------------------------------------------
+// Pass 1 reads z and every local replica once (4 n (n_local + 1) bytes); each CTA stores its partial sums of squares, and
+// after grid.sync() every CTA adds the partials in CTA order, so the norms are deterministic and equal in every CTA.
+// Squares are summed in double: no finite float32 update can overflow it, so a non-finite norm means a non-finite input.
+// Pass 2 rewrites only the replicas over the bound: x <- z + s (x - z), s = C / ||x - z||, in double (an update near the
+// float range cannot overflow x - z).  A non-finite norm is never clipped, so NaN / Inf reach the aggregation kernel (and
+// its non-finite count) untouched.
+__device__ __forceinline__ double warp_add_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ double block_add_d(double v, double* sm) {
+  v = warp_add_d(v);
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double r = 0.0;
+  if (threadIdx.x < 32) {
+    r = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : 0.0;
+    r = warp_add_d(r);
+  }
+  __syncthreads();
+  return r;  // valid in thread 0
+}
+__global__ void __launch_bounds__(COMM_THREADS, 1) dp_clip_kernel(const DPClipArgs a) {
+  cg::grid_group grid = cg::this_grid();
+  __shared__ double sm[32];
+  __shared__ double s_scale[COMM_MAX_LOCAL];
+  double* part = reinterpret_cast<double*>(a.stats + DP_PART);     // [COMM_MAX_LOCAL][COMM_MAX_BLOCKS]
+  const int n4 = a.n >> 2;
+  const int tid = blockIdx.x * blockDim.x + threadIdx.x;
+  const int nth = gridDim.x * blockDim.x;
+  double acc[COMM_MAX_LOCAL];
+#pragma unroll
+  for (int j = 0; j < COMM_MAX_LOCAL; ++j) acc[j] = 0.0;
+  for (int i = tid; i < n4; i += nth) {
+    const float4 zv = reinterpret_cast<const float4*>(a.z)[i];
+#pragma unroll
+    for (int j = 0; j < COMM_MAX_LOCAL; ++j) {
+      if (j < a.n_local) {
+        const float4 xv = reinterpret_cast<const float4*>(a.x[j])[i];
+        const double dx = double(xv.x) - zv.x, dy = double(xv.y) - zv.y, dz = double(xv.z) - zv.z,
+                     dw = double(xv.w) - zv.w;
+        acc[j] = fma(dx, dx, fma(dy, dy, fma(dz, dz, fma(dw, dw, acc[j]))));
+      }
+    }
+  }
+  for (int i = (n4 << 2) + tid; i < a.n; i += nth) {
+    const float zv = a.z[i];
+#pragma unroll
+    for (int j = 0; j < COMM_MAX_LOCAL; ++j) {
+      if (j < a.n_local) {
+        const double d = double(a.x[j][i]) - zv;
+        acc[j] = fma(d, d, acc[j]);
+      }
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < COMM_MAX_LOCAL; ++j) {
+    if (j < a.n_local) {                           // uniform across the CTA: the barriers inside block_add_d are safe
+      const double v = block_add_d(acc[j], sm);
+      if (threadIdx.x == 0) part[j * COMM_MAX_BLOCKS + blockIdx.x] = v;
+    }
+  }
+  __threadfence();
+  grid.sync();
+
+  if (threadIdx.x < a.n_local) {
+    const int j = threadIdx.x;
+    double s = 0.0;
+    for (int b = 0; b < int(gridDim.x); ++b) s += __ldcg(part + j * COMM_MAX_BLOCKS + b);
+    const double norm = sqrt(s);
+    const bool clip = isfinite(norm) && norm > double(a.bound);
+    s_scale[j] = clip ? double(a.bound) / norm : 0.0;
+    if (blockIdx.x == 0) {
+      a.stats[DP_NORM + j] = float(norm);
+      a.stats[DP_CLIPPED + j] = clip ? 1.f : 0.f;
+    }
+  }
+  __syncthreads();
+  for (int j = 0; j < a.n_local; ++j) {
+    const double s = s_scale[j];
+    if (s == 0.0) continue;                        // within the bound (or non-finite): not written at all
+    float* x = a.x[j];
+    for (int i = tid; i < n4; i += nth) {
+      const float4 zv = reinterpret_cast<const float4*>(a.z)[i];
+      float4 xv = reinterpret_cast<const float4*>(x)[i];
+      xv = make_float4(float(fma(s, double(xv.x) - zv.x, zv.x)), float(fma(s, double(xv.y) - zv.y, zv.y)),
+                       float(fma(s, double(xv.z) - zv.z, zv.z)), float(fma(s, double(xv.w) - zv.w, zv.w)));
+      reinterpret_cast<float4*>(x)[i] = xv;
+    }
+    for (int i = (n4 << 2) + tid; i < a.n; i += nth) x[i] = float(fma(s, double(x[i]) - a.z[i], double(a.z[i])));
+  }
+}
+
+void dp_clip_launch(const DPClipArgs& args, cudaStream_t s) {
+  if (args.n_local < 1 || args.n_local > COMM_MAX_LOCAL || args.n < 1)
+    throw std::runtime_error("fedb200: dp_clip: bad replica count or block length");
+  static int max_blocks = 0;
+  if (max_blocks == 0) max_blocks = comm_max_blocks((const void*)dp_clip_kernel);
+  int cap = max_blocks;
+  if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;
+  const int want = ((args.n >> 2) + COMM_THREADS - 1) / COMM_THREADS;
+  const int grid = want < 1 ? 1 : (want > cap ? cap : want);
+  void* kargs[] = {(void*)&args};
+  cudaError_t e = cudaLaunchCooperativeKernel((void*)dp_clip_kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
+  if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: dp_clip launch: ") + cudaGetErrorString(e));
   count_launch();
 }
 

@@ -185,12 +185,15 @@ constexpr int PAD_FLAG_C = PAD_FLAG_B + COMM_MAX_BLOCKS * COMM_MAX_WORLD;     //
 constexpr int PAD_FLAG_D = PAD_FLAG_C + COMM_MAX_WORLD;                       // [COMM_MAX_WORLD]  Barzilai-Borwein rows posted
 constexpr int PAD_PAYLOAD = PAD_FLAG_D + COMM_MAX_WORLD;                      // [COMM_MAX_WORLD][4] floats: dual^2 part, primal part, #non-finite
 constexpr int PAD_BBROWS = PAD_PAYLOAD + 4 * COMM_MAX_WORLD;                  // [COMM_MAX_K][8] floats: six dots per worker
+constexpr int PAD_DP_PAYLOAD = PAD_BBROWS + 8 * COMM_MAX_K;                   // [COMM_MAX_WORLD][2] floats: #clipped, sum of norms
 constexpr int COMM_PAD_WORDS = 8192;
-static_assert(PAD_BBROWS + 8 * COMM_MAX_K <= COMM_PAD_WORDS, "control pad too small");
+static_assert(PAD_DP_PAYLOAD + 2 * COMM_MAX_WORLD <= COMM_PAD_WORDS, "control pad too small");
 
-// out record of an aggregation (floats): what the host reads back, once per round
+// out record of an aggregation (floats): what the host reads back, once per round.  DP rounds add the number of clipped
+// workers and the sum of their pre-clip update norms, over all K.
 constexpr int OUT_DUAL_SQ = 0, OUT_PRIMAL = 1, OUT_NONFINITE = 2, OUT_STATUS = 3, OUT_RHO = 4, OUT_EPOCH = 5, OUT_TWO_SHOT = 6;
-constexpr int COMM_OUT_FLOATS = 8;
+constexpr int OUT_DP_CLIPPED = 8, OUT_DP_NORM_SUM = 9;
+constexpr int COMM_OUT_FLOATS = 12;
 // device scratch (floats): [0] dual^2, [1] #non-finite, [2] ticket (as uint), [4 + j] per-replica primal^2; self-cleaning
 constexpr int COMM_SCRATCH_FLOATS = 4 + COMM_MAX_LOCAL;
 
@@ -232,11 +235,41 @@ struct CommArgs {
   // multicast object is bound (no in-switch order statistics).
   int agg;                           // AGG_MEAN selects the instantiations above
   int trim_b;                        // AGG_TRIMMED: values dropped at each end (0 <= 2 trim_b < K)
+  // ---- client-level differential privacy (DP-FedAvg, McMahan et al. 2018; mode 0 with the mean, with or without a server
+  // optimizer): the replicas were clipped by dp_clip_kernel; the Gaussian noise dp_std * xi(key, t, i) is added to the mean.
+  int dp;                            // 0 selects the instantiations above
+  float dp_std;                      // noise std of the mean: sigma C / K
+  unsigned long long dp_key;         // key of the run's noise stream
+  long long* dp_t;                   // device: index t of this DP round over the run; the last CTA increments it
+  const float* dp_stats;             // dp_clip_kernel's [DP_NORM ..) record: per-replica norms, then clipped flags
+  // per DP_CHUNK-float chunk of the slice, how many of its leading floats are parameters (the rest is the arena's
+  // alignment padding, which gets no noise and stays zero); nullptr: every float is a parameter
+  const unsigned char* dp_valid;
 };
+constexpr int DP_CHUNK = 32;
 constexpr int FEDOPT_NONE = 0, FEDOPT_AVGM = 1, FEDOPT_ADAGRAD = 2, FEDOPT_ADAM = 3, FEDOPT_YOGI = 4;
 constexpr int AGG_MEAN = 0, AGG_MEDIAN = 1, AGG_TRIMMED = 2;
 constexpr int COMM_MAX_K_ROBUST = 16;
 void block_reduce_launch(const CommArgs& args, cudaStream_t s);
+
+// DP-FedAvg update clipping on the local replicas, as ONE cooperative kernel touching no peer memory: ||x_j - z|| per
+// replica, grid.sync(), then x_j <- z + (C / ||x_j - z||) (x_j - z) for the replicas over the bound C only (the others are
+// not written).  Norms and clipped flags go to the stats record, which the DP aggregation kernel that follows reads.
+struct DPClipArgs {
+  int n, n_local, max_blocks;
+  float bound;                       // C
+  float* x[COMM_MAX_LOCAL];          // this process' replicas
+  const float* z;                    // the server model the round started from
+  float* stats;                      // [DP_STATS_FLOATS]
+};
+// stats record (floats): per-CTA partial sums of squares as doubles [COMM_MAX_LOCAL][COMM_MAX_BLOCKS] (2 floats each),
+// then per replica the pre-clip norm [COMM_MAX_LOCAL] and the clipped flag (0 / 1) [COMM_MAX_LOCAL].  Every launch
+// overwrites what it reads: no cleaning.
+constexpr int DP_PART = 0;
+constexpr int DP_NORM = 2 * COMM_MAX_LOCAL * COMM_MAX_BLOCKS;
+constexpr int DP_CLIPPED = DP_NORM + COMM_MAX_LOCAL;
+constexpr int DP_STATS_FLOATS = DP_CLIPPED + COMM_MAX_LOCAL;
+void dp_clip_launch(const DPClipArgs& args, cudaStream_t s);
 
 // Barzilai-Borwein / spectral penalty update of consensus ADMM as ONE kernel (SURVEY G20, X4): six dots per worker
 // straight from (x, y, yhat0, x0, z), rows exchanged through the control pads, the reference's sequential

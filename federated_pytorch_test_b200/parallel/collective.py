@@ -6,7 +6,8 @@ one device):
 * X1 FedAvg  ``z' = sum_k x_k / K``; ``dual = ||z - z'||``; write ``z'`` into every replica
   (/root/reference/src/federated_multi.py:204-217); with a server optimizer (``fedopt_``) ``z'`` is its step from ``z``
   along ``mean_k x_k - z`` instead of the plain mean; with a robust rule (``robust_``) ``z'`` is the coordinate-wise
-  median or trimmed mean of the K workers instead of their mean
+  median or trimmed mean of the K workers instead of their mean; with DP (``dp_clip_`` first, then ``dp=`` on
+  ``fedavg_`` / ``fedopt_``) the workers' updates are clipped and Gaussian noise is added to the mean (DP-FedAvg)
 * X2 FedProx ``z' = mean``; ``dual``; ``primal = sum_k ||rho (x_k - z')||``; no write-back
   (fedprox_multi.py:211-232)
 * X3 ADMM    ``z' = sum_k (y_k + rho x_k) / (K rho)``; ``dual``; ``y_k += rho (x_k - z')``;
@@ -22,6 +23,7 @@ sm_90a kernels that reduce straight out of peer memory over NVLink.
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence, Tuple
 
 import torch
@@ -43,6 +45,26 @@ def check_robust(K: int, agg: str, trim_b: int) -> None:
         raise ValueError("trimmed mean needs 0 <= 2 trim_b < K, got trim_b = %r at K = %d" % (trim_b, K))
 
 
+@dataclass
+class DPRound:
+    """The noise of one DP-FedAvg round: ``std * xi(key, t, i)`` is added to the mean (``algo/privacy.py: dp_noise``).
+    ``t`` is a one-element int64 tensor on the block's device: the round index over the run, advanced by the round.
+    ``valid`` (uint8, on the block's device; None = every float is a parameter) holds, per 32-float chunk of the block,
+    how many of its leading floats are parameters: the arena's alignment padding gets no noise and stays zero."""
+
+    std: float
+    key: int
+    t: torch.Tensor
+    valid: Optional[torch.Tensor] = None
+
+    def mask(self, n: int) -> Optional[torch.Tensor]:
+        """Boolean mask of the parameter coordinates of an ``n``-float block (None: all of them)."""
+        if self.valid is None:
+            return None
+        i = torch.arange(n, device=self.valid.device)
+        return (i % 32) < self.valid.long()[i // 32]
+
+
 class TorchCollective:
     """ATen + torch.distributed implementation (baseline / oracle / CPU)."""
 
@@ -52,6 +74,7 @@ class TorchCollective:
     def __init__(self, topo: Topology):
         self.topo = topo
         self.launches = 0  # number of framework-owned kernels launched (0 here: library path)
+        self.last_dp = (0.0, 0.0)   # DP rounds: (#clipped workers, sum of their pre-clip update norms) over all K
 
     # -- arena hooks ------------------------------------------------------
     def arena_allocator(self) -> Optional[Callable]:
@@ -128,9 +151,44 @@ class TorchCollective:
 
     # -- operators --------------------------------------------------------
     @torch.no_grad()
-    def fedavg_(self, xs: List[torch.Tensor], z: torch.Tensor, write_back: bool = True) -> torch.Tensor:
-        """In place: ``z <- mean_k x_k``, optionally ``x_k <- z``; returns ``||z_old - z_new||^2`` (0-dim)."""
+    def dp_clip_(self, xs: List[torch.Tensor], z: torch.Tensor, bound: float) -> None:
+        """DP-FedAvg update clipping, in place: every local ``x_k`` with ``||x_k - z|| > bound`` becomes
+        ``z + (bound / ||x_k - z||) (x_k - z)``; the others are not written (nor are non-finite norms).  The number of
+        clipped workers and the sum of the pre-clip norms over all K go to :attr:`last_dp`."""
+        stats = torch.zeros(2, dtype=torch.float64, device=z.device)
+        z64 = z.double()
+        for x in xs:                                  # in double: no finite float32 update overflows the norm
+            d = x.double() - z64
+            norm = torch.linalg.vector_norm(d)
+            stats[1] += norm
+            if bool(torch.isfinite(norm)) and bool(norm > bound):
+                stats[0] += 1.0
+                x.copy_(z64 + (bound / norm) * d)
+        c, s = self.sum_scalars(stats).tolist()
+        self.last_dp = (c, s)
+
+    @staticmethod
+    def _add_dp_noise_(mean: torch.Tensor, dp: DPRound) -> None:
+        """``mean += std * xi(key, t)`` (the same draw on every rank), then ``t += 1``."""
+        from ..algo.privacy import dp_noise
+
+        t = int(dp.t.item())
+        if dp.std != 0.0:
+            xi = torch.from_numpy(dp_noise(dp.key, t, mean.numel())).to(device=mean.device, dtype=mean.dtype)
+            mask = dp.mask(mean.numel())
+            if mask is not None:
+                xi.mul_(mask)
+            mean.add_(xi.mul_(dp.std))
+        dp.t.add_(1)
+
+    @torch.no_grad()
+    def fedavg_(self, xs: List[torch.Tensor], z: torch.Tensor, write_back: bool = True,
+                dp: Optional[DPRound] = None) -> torch.Tensor:
+        """In place: ``z <- mean_k x_k``, optionally ``x_k <- z``; returns ``||z_old - z_new||^2`` (0-dim).  With ``dp``
+        the mean is noised (:class:`DPRound`; clip the replicas with :meth:`dp_clip_` first)."""
         znew = self.sum_blocks(xs).div_(self.topo.K)
+        if dp is not None:
+            self._add_dp_noise_(znew, dp)
         diff = z - znew
         dual_sq = torch.dot(diff, diff)
         z.copy_(znew)
@@ -155,13 +213,17 @@ class TorchCollective:
 
     @torch.no_grad()
     def fedopt_(self, xs: List[torch.Tensor], z: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], kind: str,
-                lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean", trim_b: int = 0) -> torch.Tensor:
+                lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean", trim_b: int = 0,
+                dp: Optional[DPRound] = None) -> torch.Tensor:
         """FedAvg with a server optimizer, in place: ``d = mean_k x_k - z`` is the pseudo-gradient of server optimizer
         ``kind`` (one of :data:`FEDOPT_KINDS`; ``beta1`` is the momentum of 'avgm'), whose state ``m`` (and ``v``, unused
         by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``.
-        With a robust rule ``agg`` (one of :data:`ROBUST_AGGS`) its aggregate replaces the mean in ``d``."""
+        With a robust rule ``agg`` (one of :data:`ROBUST_AGGS`) its aggregate replaces the mean in ``d``; with ``dp`` the
+        noised mean does (DP-FedOpt: post-processing)."""
         if agg == "mean":
             mean = self.sum_blocks(xs).div_(self.topo.K)
+            if dp is not None:
+                self._add_dp_noise_(mean, dp)
         else:
             mean = self.robust_aggregate(xs, agg, trim_b)
         d = mean - z

@@ -30,6 +30,11 @@ it with ``multimem.st`` (or P2P stores) into every rank's weights / consensus ve
 The robust rules (coordinate-wise median / trimmed mean) run in separate instantiations of the same kernel: every
 coordinate's K values are loaded over P2P (there is no in-switch order statistic; the two-shot broadcast may still use
 ``multimem.st``) and sorted in registers, so K <= 16.
+
+DP-FedAvg (client-level differential privacy) is two launches per round, in stream order and host-free: a cooperative
+clip kernel on each rank's own replicas (no peer memory), then DP instantiations of the aggregation kernel, which add
+the counter-based Gaussian noise to the mean and advance the device-resident round counter, so a graph-captured round
+draws fresh noise on every replay.
 """
 from __future__ import annotations
 
@@ -40,15 +45,18 @@ import torch
 import torch.distributed as dist
 
 from ..ops import cuda_ops
-from .collective import FEDOPT_KINDS, ROBUST_AGGS, TorchCollective, check_robust
+from .collective import FEDOPT_KINDS, ROBUST_AGGS, DPRound, TorchCollective, check_robust
 from .topology import Topology
 
 _MAX_LOCAL = 16
-_OUT_FLOATS = 8
+_OUT_FLOATS = 12
 _SCRATCH_FLOATS = 4 + _MAX_LOCAL
+_MAX_BLOCKS = 160                                         # csrc/fedb200.h: COMM_MAX_BLOCKS
+_DP_STATS_FLOATS = 2 * _MAX_LOCAL * _MAX_BLOCKS + 2 * _MAX_LOCAL      # DP_STATS_FLOATS: double partials, norms, flags
 _BB_SCRATCH_FLOATS = 8 * _MAX_LOCAL + 8 + _MAX_LOCAL
 _PAD_WORDS = 8192
 OUT_DUAL_SQ, OUT_PRIMAL, OUT_NONFINITE, OUT_STATUS, OUT_RHO, OUT_EPOCH, OUT_TWO_SHOT = range(7)
+OUT_DP_CLIPPED, OUT_DP_NORM_SUM = 8, 9
 
 TWO_SHOT_MIN_BYTES = int(os.environ.get("FEDB200_TWO_SHOT_BYTES", str(256 * 1024)))
 TWO_SHOT_MODE = os.environ.get("FEDB200_TWO_SHOT", "auto")          # 'auto' | '0' (never) | '1' (whenever legal)
@@ -151,6 +159,7 @@ class FusedCollective(TorchCollective):
         self.out = torch.zeros(_OUT_FLOATS, dtype=torch.float32, device=dev)
         self.scratch = torch.zeros(_SCRATCH_FLOATS, dtype=torch.float32, device=dev)
         self.bb_scratch = torch.zeros(_BB_SCRATCH_FLOATS, dtype=torch.float32, device=dev)
+        self.dp_stats = torch.zeros(_DP_STATS_FLOATS, dtype=torch.float32, device=dev)
         self.bb_log = torch.zeros(8 * max(topo.K, 1), dtype=torch.float32, device=dev)
         self.sync = torch.zeros(4, dtype=torch.int32, device=dev)
         self._host_out = torch.zeros(self.out.numel(), dtype=torch.float32).pin_memory()
@@ -172,12 +181,14 @@ class FusedCollective(TorchCollective):
         self.last_rho = float("nan")
         self.warm_fedopt = False          # set by the FedOpt strategy: warm the server-optimizer instantiation too
         self.warm_robust = False          # set by robust strategies: warm the robust instantiation(s) for this K too
+        self.warm_dp = False              # set by DP strategies: warm the clip kernel and the DP instantiation(s) too
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
         cross-rank handshake happen here, at engine construction, not inside the first training round (the first launch
         is far slower than the ones after it).  The server-optimizer kernel is warmed only when ``warm_fedopt`` is set, the
-        robust kernels (of this K; with the server optimizer if both are set) only when ``warm_robust`` is set.
+        robust kernels (of this K; with the server optimizer if both are set) only when ``warm_robust`` is set, the DP
+        kernels (likewise) only when ``warm_dp`` is set.
         Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
@@ -201,6 +212,12 @@ class FusedCollective(TorchCollective):
                 self._launch(0, xs, None, z, 0.0, agg="median")
                 if self.warm_fedopt:
                     self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, agg="median")
+            if self.warm_dp:
+                dp = DPRound(1e-3, 0, torch.zeros(1, dtype=torch.int64, device=self.topo.device))
+                self.dp_clip_(xs, z, 1.0)
+                self._launch(0, xs, None, z, 0.0, dp=dp)
+                if self.warm_fedopt:
+                    self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, dp=dp)
         self.two_shot_mode = keep
         x0 = [torch.zeros_like(x) for x in xs]
         yh = [torch.zeros_like(x) for x in xs]
@@ -261,8 +278,20 @@ class FusedCollective(TorchCollective):
             raise ValueError("robust aggregation supports at most 16 workers, got K = %d" % self.topo.K)
         return ROBUST_AGGS.index(agg) + 1
 
-    def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None, agg: str = "mean", trim_b: int = 0) -> None:
-        """Modes 0 / 1 take a robust rule ``agg`` (:data:`ROBUST_AGGS`) in place of the mean."""
+    def _dp_args(self, dp: Optional[DPRound]):
+        """The DP arguments of the aggregation bindings: noise std, key (as a signed 64-bit int), counter, clip stats,
+        parameter layout."""
+        if dp is None:
+            return 0.0, 0, None, None, None
+        key = int(dp.key) & ((1 << 64) - 1)
+        return float(dp.std), key - (1 << 64) if key >= 1 << 63 else key, dp.t, self.dp_stats, dp.valid
+
+    def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None, agg: str = "mean", trim_b: int = 0,
+                dp: Optional[DPRound] = None) -> None:
+        """Modes 0 / 1 take a robust rule ``agg`` (:data:`ROBUST_AGGS`) in place of the mean; mode 0 with the mean takes
+        the noise of a DP round (``dp``; after :meth:`dp_clip_`)."""
+        if dp is not None and (mode != 0 or agg != "mean"):
+            raise ValueError("DP aggregation needs FedAvg with the mean")
         code = self._agg_code(agg, trim_b)
         n = xs[0].numel()
         if any(t.numel() != n for t in xs) or z.numel() != n:
@@ -285,16 +314,19 @@ class FusedCollective(TorchCollective):
                     mcz = za["mc_ptr"] + zoff
         self.ext.block_reduce(mode, xp, yp, local_idx, z, n, float(rho), rho_dev, self.out, self.scratch, self.ctrl_ptrs,
                               self.sync, W, self.topo.rank, mcx, mcy, mcz, xw, zw, bool(two), self.max_blocks,
-                              self.timeout_s, code, int(trim_b))
+                              self.timeout_s, code, int(trim_b), *self._dp_args(dp))
         self.launches += 1
         self.last_two_shot = bool(two)
 
     def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                       trim_b: int = 0) -> None:
+                       trim_b: int = 0, dp: Optional[DPRound] = None) -> None:
         """FedAvg with a server optimizer: mode 0 of the kernel's FedOpt instantiation.  Two-shot, rank r broadcasts slice r
         of the new weights, of ``m`` and of ``v`` into every rank, so ``m`` / ``v`` must be symmetric slices then
-        (:meth:`zeros_like_block`).  A robust rule ``agg`` replaces the mean as the aggregate the step is taken towards."""
+        (:meth:`zeros_like_block`).  A robust rule ``agg`` replaces the mean as the aggregate the step is taken towards; a
+        DP round (``dp``, mean only) noises the mean first."""
         code = self._agg_code(agg, trim_b)
+        if dp is not None and agg != "mean":
+            raise ValueError("DP aggregation needs the mean")
         n = xs[0].numel()
         adaptive = kind != "avgm"
         if any(t.numel() != n for t in xs) or z.numel() != n or m.numel() != n or (adaptive and v.numel() != n):
@@ -312,7 +344,7 @@ class FusedCollective(TorchCollective):
         self.ext.block_reduce_fedopt(FEDOPT_KINDS.index(kind) + 1, float(lr), float(beta1), float(beta2), float(tau), m,
                                      v if adaptive else None, xp, local_idx, z, n, self.out, self.scratch, self.ctrl_ptrs,
                                      self.sync, W, self.topo.rank, mcx, mcm, mcv, xw, mw, vw, bool(two), self.max_blocks,
-                                     self.timeout_s, code, int(trim_b))
+                                     self.timeout_s, code, int(trim_b), *self._dp_args(dp))
         self.launches += 1
         self.last_two_shot = bool(two)
 
@@ -327,14 +359,25 @@ class FusedCollective(TorchCollective):
             self._out_event.record()
             self._out_pending = True
 
-    def launch_fedavg_(self, xs, z, write_back: bool = True) -> None:
-        self._launch(0 if write_back else 1, xs, None, z, 0.0)
+    def launch_fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None) -> None:
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp)
         self._record_async()
 
     def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                       trim_b: int = 0) -> None:
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b)
+                       trim_b: int = 0, dp: Optional[DPRound] = None) -> None:
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp)
         self._record_async()
+
+    @torch.no_grad()
+    def dp_clip_(self, xs, z, bound: float) -> None:
+        """DP-FedAvg update clipping of the local replicas (one cooperative launch, no peer memory, no host work).  Its
+        statistics reach :attr:`last_dp` through the record of the DP aggregation that must follow."""
+        if any(t.numel() != z.numel() for t in xs):
+            raise ValueError("block slices must have equal length")
+        self.ext.dp_clip(list(xs), z, float(bound), self.dp_stats, self.max_blocks)
+        self.launches += 1
+
+    launch_dp_clip_ = dp_clip_
 
     def launch_robust_(self, xs, z, agg: str, trim_b: int = 0, write_back: bool = True) -> None:
         self._launch(0 if write_back else 1, xs, None, z, 0.0, agg=agg, trim_b=trim_b)
@@ -361,12 +404,13 @@ class FusedCollective(TorchCollective):
                                     % (self.topo.rank, self.timeout_s, int(vals[OUT_STATUS]) - 100, int(vals[OUT_EPOCH])))
         self.last_nonfinite = vals[OUT_NONFINITE]
         self.last_rho = vals[OUT_RHO]
+        self.last_dp = (vals[OUT_DP_CLIPPED], vals[OUT_DP_NORM_SUM])
         return vals
 
     # -- operators ----------------------------------------------------------------------
     @torch.no_grad()
-    def fedavg_(self, xs, z, write_back: bool = True):
-        self._launch(0 if write_back else 1, xs, None, z, 0.0)
+    def fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None):
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
@@ -376,8 +420,8 @@ class FusedCollective(TorchCollective):
 
     @torch.no_grad()
     def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                trim_b: int = 0):
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b)
+                trim_b: int = 0, dp: Optional[DPRound] = None):
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()

@@ -109,6 +109,19 @@ class FlatArena:
         a, b = self.span(lo, hi)
         return self.data[a:b]
 
+    def chunk_counts(self, lo: int, hi: int, chunk: int = 32) -> List[int]:
+        """Per ``chunk``-float chunk of :meth:`block` ``(lo, hi)``, how many of its leading floats are parameters (the
+        rest is alignment padding).  Needs ``align`` to be a multiple of ``chunk``, so no chunk spans two parameters."""
+        if self.align % chunk:
+            raise ValueError("chunk_counts needs align (%d) to be a multiple of %d" % (self.align, chunk))
+        a, b = self.span(lo, hi)
+        counts = [0] * (-(-(b - a) // chunk))
+        for i in range(lo, hi + 1):
+            rel = self.offsets[i] - a
+            for c in range(rel // chunk, -(-(rel + self.numels[i]) // chunk)):
+                counts[c] = min(chunk, rel + self.numels[i] - c * chunk)
+        return counts
+
     def block_grad(self, lo: int, hi: int) -> torch.Tensor:
         a, b = self.span(lo, hi)
         return self.grad[a:b]
