@@ -42,6 +42,7 @@ from ..optim.lbfgsnew import LBFGSNew
 from ..parallel.topology import Topology
 from ..utils.flat import FlatArena
 from ..utils.metrics import MetricsLog, PhaseTimers, nvtx_range
+from .compress import payload_bytes
 from .strategies import Penalty, Strategy
 
 
@@ -494,8 +495,10 @@ class Engine:
         if agg_ms:
             out["aggregate_us"] = 1e3 * agg_ms / max(out.get("aggregate_count", 1), 1)
             W = max(self.topo.world_size, 1)
-            if W > 1:
-                out["bus_GBs"] = 2.0 * (W - 1) / W * 4.0 * N / (out["aggregate_us"] * 1e-6) / 1e9
+            if W > 1:                          # compressed rounds move their payload instead of 4 bytes per coordinate
+                bits = getattr(self.strategy, "q_bits", 0)
+                nbytes = payload_bytes(N, bits) if bits else 4.0 * N
+                out["bus_GBs"] = 2.0 * (W - 1) / W * nbytes / (out["aggregate_us"] * 1e-6) / 1e9
         out["two_shot"] = bool(getattr(self.coll, "last_two_shot", False))
         self._round_mark = {"images": self.images_seen, "t": now, "ms": {k: dict(v) for k, v in summ.items()}}
         return out

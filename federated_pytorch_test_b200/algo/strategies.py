@@ -103,18 +103,31 @@ class FedAvg(Strategy):
     block visit as the server model, i.e. the replicas' common value, instead of 0 (Q6), so the ``dual`` of the first round
     of a visit differs from plain FedAvg.  The round metrics gain ``dp_clipped`` (workers clipped), ``dp_update_norm``
     (mean pre-clip update norm over the K workers), ``dp_clip_norm`` (``C``) and ``dp_epsilon`` (spent so far at
-    ``dp_delta``)."""
+    ``dp_delta``).
+
+    ``compress_bits`` 8 or 4 compresses the workers' uploads (QSGD / FedPAQ; ``algo/compress.py``): with ``z`` the server
+    model the round started from, worker ``k`` sends ``u_k = x_k - z`` (``+ e_k`` with ``compress_ef``) as stochastically
+    rounded codes with one scale per 128 coordinates, and ``z <- z + (1/K) sum_k q_k s_k``, written back into every
+    replica in fp32.  With error feedback ``e_k <- u_k - q_k s_k`` belongs to the worker and the block and persists across
+    the block's visits for the whole run.  The rounding of compressed round ``t`` (``t`` counts the compressed rounds of
+    the run and lives in device memory) is keyed by ``(seed, k, t, coordinate)``.  A round is one launch on the fused
+    collective.  As with DP, ``z`` starts each block visit as the replicas' common value instead of 0 (Q6), so the
+    ``dual`` of the first round of a visit differs from plain FedAvg.  The round metrics gain ``q_bits``, ``q_bytes``
+    (payload bytes per worker: ``N bits / 8 + 4 ceil(N / 128)``) and ``q_rel_err``
+    (``sqrt(sum_k ||u_k - q_k s_k||^2 / sum_k ||u_k||^2)``)."""
 
     name = "fedavg"
     write_back = True
 
     def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1, dp_clip: float = 0.0,
-                 dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0):
-        from ..config import check_aggregator, check_dp, trim_count
+                 dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
+                 compress_ef: bool = False):
+        from ..config import check_aggregator, check_compress, check_dp, trim_count
 
         super().__init__(collective, topo)
         check_aggregator(aggregator, trim_fraction, topo.K)
         check_dp(dp_clip, dp_noise, dp_delta, aggregator)
+        check_compress(compress_bits, compress_ef, dp_clip, aggregator)
         self.aggregator = aggregator
         self.trim_b = trim_count(trim_fraction, topo.K) if aggregator == "trimmed_mean" else 0
         if aggregator != "mean" and hasattr(collective, "warm_robust"):
@@ -130,11 +143,78 @@ class FedAvg(Strategy):
             self.dp_layouts: Dict[int, torch.Tensor] = {}     # block index -> parameter layout (DPRound.valid)
             if hasattr(collective, "warm_dp"):
                 collective.warm_dp = True
+        self.q_bits, self.q_ef_on = int(compress_bits), bool(compress_ef)
+        self.q_rounds = 0                      # host mirror of the device round counter q_t
+        if self.q_bits:
+            from .compress import compress_key
+
+            self.q_key = compress_key(seed)
+            self.q_t = torch.zeros(1, dtype=torch.int64, device=topo.device)
+            self.q_payload: List = []                          # (codes, scales) per local replica, current block
+            self.q_ef: Dict[int, List[torch.Tensor]] = {}      # block index -> error feedback per local replica
+            self._q_restored: Dict[int, torch.Tensor] = {}     # error feedback read from a resume record, installed at the visit
+            if hasattr(collective, "warm_compress"):
+                collective.warm_compress = self.q_bits
 
     def begin_block(self, ci: int, N: int, xs: List[torch.Tensor]) -> None:
         super().begin_block(ci, N, xs)
-        if self.dp:                            # the server model: the replicas are equal here, so a local copy suffices
+        if self.dp or self.q_bits:             # the server model: the replicas are equal here, so a local copy suffices
             self.z.copy_(xs[0])
+        if self.q_bits:
+            self.q_payload = [self.coll.payload_like_block(x, self.q_bits) for x in xs]
+            if self.q_ef_on and ci not in self.q_ef:
+                self.q_ef[ci] = [torch.zeros_like(x) for x in xs]
+                if ci in self._q_restored:
+                    self._install_ef(ci, self._q_restored.pop(ci))
+
+    # -- compressed updates -------------------------------------------------------------------------------------------
+    def _q_kw(self) -> Dict[str, object]:
+        """The compression argument of the aggregation."""
+        if not self.q_bits:
+            return {}
+        from ..parallel.collective import QuantRound
+
+        self.q_rounds += 1
+        return {"compress": QuantRound(self.q_bits, self.q_key, self.q_t, [c for c, _ in self.q_payload],
+                                       [s for _, s in self.q_payload], self.q_ef.get(self.ci))}
+
+    def _with_q(self, metrics: Dict[str, float]) -> Dict[str, float]:
+        if self.q_bits:
+            from .compress import payload_bytes, relative_error
+
+            err, nrm = self.coll.last_q
+            metrics.update(q_bits=float(self.q_bits), q_bytes=float(payload_bytes(self.N, self.q_bits)),
+                           q_rel_err=relative_error(float(err), float(nrm)))
+        return metrics
+
+    def _install_ef(self, ci: int, ef: torch.Tensor) -> None:
+        for dst, src in zip(self.q_ef[ci], ef):
+            dst.copy_(src.to(dst.device))
+
+    def _q_state(self) -> Dict[str, object]:
+        if not self.q_bits:
+            return {}
+        st: Dict[str, object] = {"compress": (self.q_bits, self.q_ef_on, self.q_key), "q_t": self.q_rounds}
+        if self.q_ef_on:                       # this process' workers; blocks restored but not visited yet keep their record
+            ef = dict(self._q_restored)
+            ef.update({ci: torch.stack(v) for ci, v in self.q_ef.items()})
+            st["q_ef"] = ef
+        return st
+
+    def _check_q_state(self, st: Dict[str, object]) -> None:
+        got = tuple(st["compress"]) if st.get("compress") is not None else None
+        want = self._q_state().get("compress")
+        if got != want:
+            raise ValueError("resume record holds compression settings (compress_bits, compress_ef, key) %r, this run uses "
+                             "%r" % (got, want))
+        if self.q_bits:
+            self.q_rounds = int(st["q_t"])
+            self.q_t.fill_(self.q_rounds)
+            for ci, ef in (st.get("q_ef") or {}).items():
+                if ci in self.q_ef:
+                    self._install_ef(ci, ef)
+                else:
+                    self._q_restored[ci] = ef
 
     # -- DP -------------------------------------------------------------------------------------------------------
     def set_param_layout(self, ci: int, chunk_counts: List[int]) -> None:
@@ -172,15 +252,15 @@ class FedAvg(Strategy):
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         if self.aggregator == "mean":
-            dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw())
+            dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw(), **self._q_kw())
         else:
             dual_sq = self.coll.robust_(self.xs, self.z, self.aggregator, self.trim_b)
-        return self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})
+        return self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             if self.aggregator == "mean":
-                self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw())
+                self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw(), **self._q_kw())
             else:
                 self.coll.launch_robust_(self.xs, self.z, self.aggregator, self.trim_b)
             return ("pending", self.N)
@@ -189,7 +269,7 @@ class FedAvg(Strategy):
     def aggregate_end(self, token) -> Dict[str, float]:
         if token[0] == "done":
             return token[1]
-        return self._with_dp({"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]})
+        return self._with_q(self._with_dp({"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]}))
 
     def _robust_state(self) -> Dict[str, object]:
         return {} if self.aggregator == "mean" else {"aggregator": self.aggregator, "trim_b": self.trim_b}
@@ -216,11 +296,12 @@ class FedAvg(Strategy):
             self.dp_t.fill_(self.dp_rounds)
 
     def state(self) -> Dict[str, object]:
-        return {"z": self.z, **self._robust_state(), **self._dp_state()}
+        return {"z": self.z, **self._robust_state(), **self._dp_state(), **self._q_state()}
 
     def load_state(self, st: Dict[str, object]) -> None:
         self._check_robust_state(st)
         self._check_dp_state(st)
+        self._check_q_state(st)
         self.z.copy_(st["z"].to(self.z.device))
 
 
@@ -240,17 +321,21 @@ class FedOpt(FedAvg):
     round with the same ``z``, ``m`` and ``v``.  With a robust ``aggregator`` its aggregate replaces the mean in ``d``
     (e.g. robust FedAdam); the server model at the start of a visit stays the mean (the replicas are equal then).  With DP
     (``dp_clip > 0``) the noised mean of the clipped workers replaces the mean in ``d`` (DP-FedAdam etc.: post-processing),
-    and the server model at the start of a visit is the replicas' common value, copied locally (no launch)."""
+    and the server model at the start of a visit is the replicas' common value, copied locally (no launch).  With
+    compressed updates (``compress_bits``) ``d`` is the dequantized mean update itself (FedPAQ with a server optimizer),
+    and the server model at the start of a visit is again the replicas' common value."""
 
     name = "fedopt"
 
     def __init__(self, collective, topo, kind: str = "adam", lr: float = 0.0, momentum: float = 0.9, beta1: float = 0.9,
                  beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1,
-                 dp_clip: float = 0.0, dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0):
+                 dp_clip: float = 0.0, dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
+                 compress_ef: bool = False):
         from ..config import check_server_opt
         from ..parallel.collective import FEDOPT_KINDS
 
-        super().__init__(collective, topo, aggregator, trim_fraction, dp_clip, dp_noise, dp_delta, seed)
+        super().__init__(collective, topo, aggregator, trim_fraction, dp_clip, dp_noise, dp_delta, seed, compress_bits,
+                         compress_ef)
         if kind not in FEDOPT_KINDS:
             raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
         check_server_opt(kind, lr, momentum, beta1, beta2, tau)
@@ -276,7 +361,7 @@ class FedOpt(FedAvg):
             if ci in self._restored:
                 self._install(ci, *self._restored.pop(ci))
         self.m, self.v = self.ms[ci], self.vs.get(ci)
-        if not self.dp:                                           # (DP: FedAvg.begin_block copied the replicas' value)
+        if not (self.dp or self.q_bits):                          # (else FedAvg.begin_block copied the replicas' value)
             self.coll.fedavg_(xs, self.z, write_back=False)      # the server model: the replicas' mean, no write-back
 
     def _hyper(self):
@@ -286,12 +371,14 @@ class FedOpt(FedAvg):
         return {} if self.aggregator == "mean" else {"agg": self.aggregator, "trim_b": self.trim_b}
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
-        dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw())
-        return self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})
+        dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
+                                    **self._q_kw())
+        return self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
-            self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw())
+            self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
+                                     **self._q_kw())
             return ("pending", self.N)
         return ("done", self.aggregate(nadmm))
 
@@ -302,7 +389,8 @@ class FedOpt(FedAvg):
         vs = {ci: v for ci, (_, v) in self._restored.items() if v is not None}
         ms.update(self.ms)
         vs.update(self.vs)
-        return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state(), **self._dp_state()}
+        return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state(), **self._dp_state(),
+                **self._q_state()}
 
     def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
         self.ms[ci].copy_(m.to(self.ms[ci].device))
@@ -314,6 +402,7 @@ class FedOpt(FedAvg):
             raise ValueError("resume record holds server optimizer %r, this run uses %r" % (st.get("server_opt"), self.kind))
         self._check_robust_state(st)
         self._check_dp_state(st)
+        self._check_q_state(st)
         self.z.copy_(st["z"].to(self.z.device))
         vs = st.get("v") or {}
         for ci, m in (st.get("m") or {}).items():

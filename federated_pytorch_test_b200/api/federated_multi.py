@@ -15,6 +15,11 @@ signflip|gaussian|nan --attack_scale s`` turns the last b workers into simulated
 ``--dp_clip c --dp_noise sigma --dp_delta delta`` makes the mean DP-FedAvg (client-level differential privacy, with or
 without a server optimizer): every worker's block update is clipped to ``c sqrt(N)`` and Gaussian noise is added to the
 mean (``algo/privacy.py``).  The root logs ``dp: ...`` lines with the planned and the spent epsilon.
+
+``--compress_bits 8|4 [--compress_ef]`` compresses what every worker uploads (QSGD / FedPAQ, with or without a server
+optimizer): its block update ``x_k - z`` as stochastically rounded codes with one scale per 128 coordinates, optionally
+with error feedback (``algo/compress.py``); the new model is still broadcast in fp32.  Round metrics gain ``q_bits``,
+``q_bytes`` and ``q_rel_err``.
 """
 from __future__ import annotations
 
@@ -31,6 +36,8 @@ def make_strategy(cfg: Config, coll, topo):
     robust = {} if cfg.aggregator == "mean" else dict(aggregator=cfg.aggregator, trim_fraction=cfg.trim_fraction)
     if cfg.dp_clip > 0.0:
         robust.update(dp_clip=cfg.dp_clip, dp_noise=cfg.dp_noise, dp_delta=cfg.dp_delta, seed=cfg.seed)
+    if cfg.compress_bits:
+        robust.update(compress_bits=cfg.compress_bits, compress_ef=cfg.compress_ef, seed=cfg.seed)
     if cfg.server_opt == "none":
         return FedAvg(coll, topo, **robust)
     return FedOpt(coll, topo, cfg.server_opt, cfg.server_lr, cfg.server_momentum, cfg.server_beta1, cfg.server_beta2,

@@ -133,6 +133,19 @@ def check_dp(dp_clip: float, dp_noise: float, dp_delta: float, aggregator: str) 
                          % (aggregator,))
 
 
+def check_compress(compress_bits: int, compress_ef: bool, dp_clip: float, aggregator: str) -> None:
+    """Raise ``ValueError`` unless the update-compression settings of :class:`FederatedConfig` are valid."""
+    if compress_bits not in (0, 8, 4):
+        raise ValueError("compress_bits must be 0 (off), 8 or 4, got %r" % (compress_bits,))
+    if compress_ef and not compress_bits:
+        raise ValueError("compress_ef needs compress_bits 8 or 4 (error feedback of uncompressed updates is always 0)")
+    if compress_bits and dp_clip > 0.0:
+        raise ValueError("compress_bits cannot be combined with dp_clip > 0 (quantized updates no longer have the clipped "
+                         "sensitivity), got dp_clip %r" % (dp_clip,))
+    if compress_bits and aggregator != "mean":
+        raise ValueError("compress_bits needs aggregator 'mean', got aggregator %r" % (aggregator,))
+
+
 @dataclass
 class FederatedConfig(CommonConfig):
     lambda1: float = 0.0001
@@ -156,6 +169,10 @@ class FederatedConfig(CommonConfig):
     dp_clip: float = 0.0            # 0 = off
     dp_noise: float = 1.0           # noise multiplier sigma (0 = clipping only)
     dp_delta: float = 1e-5          # delta at which epsilon is reported
+    # compressed client updates (QSGD / FedPAQ): every worker uploads its block update as stochastically rounded codes with
+    # one float32 scale per 128 coordinates (algo/compress.py); the new model is still broadcast in fp32
+    compress_bits: int = 0          # 0 = off | 8 | 4
+    compress_ef: bool = False       # error feedback: each worker carries its quantization error into its next update
 
     def __post_init__(self):
         check_server_opt(self.server_opt, self.server_lr, self.server_momentum, self.server_beta1, self.server_beta2,
@@ -163,6 +180,7 @@ class FederatedConfig(CommonConfig):
         check_aggregator(self.aggregator, self.trim_fraction, self.K)
         check_byzantine(self.byzantine, self.attack, self.attack_scale, self.K)
         check_dp(self.dp_clip, self.dp_noise, self.dp_delta, self.aggregator)
+        check_compress(self.compress_bits, self.compress_ef, self.dp_clip, self.aggregator)
 
 
 @dataclass

@@ -609,6 +609,40 @@ static void set_dp(fb::CommArgs& a, double dp_std, int64_t dp_key, const c10::op
     a.dp_valid = dp_valid->data_ptr<uint8_t>();
   }
 }
+// Compressed rounds (q_bits 8 or 4): the group size (must be Q_GROUP), key of the rounding stream, the device round
+// counter (int64), the payload pointer tables of ALL K workers (codes, scales; local or peer-mapped), the error-feedback
+// slices of the local replicas (empty: off) and the per-CTA statistics buffer.
+static void set_q(fb::CommArgs& a, const std::vector<int64_t>& local_idx, int64_t q_bits, int64_t q_group, int64_t q_key,
+                  const c10::optional<Tensor>& q_t, const std::vector<int64_t>& q_code_ptrs,
+                  const std::vector<int64_t>& q_scale_ptrs, const std::vector<Tensor>& q_ef,
+                  const c10::optional<Tensor>& q_part) {
+  if (q_bits == 0) return;
+  TORCH_CHECK(q_bits == 8 || q_bits == 4, "compressed rounds take 8 or 4 bits, got ", q_bits);
+  TORCH_CHECK(q_group == fb::Q_GROUP, "compressed rounds use groups of ", fb::Q_GROUP, " coordinates, got ", q_group);
+  TORCH_CHECK(q_t.has_value() && q_t->defined() && q_t->is_cuda() && q_t->scalar_type() == at::kLong && q_t->numel() >= 1,
+              "compressed round counter: int64 CUDA tensor");
+  TORCH_CHECK(q_part.has_value() && q_part->defined() && q_part->numel() >= fb::Q_PART_FLOATS, "compressed rounds need the statistics buffer");
+  CHECK_F32_CUDA((*q_part));
+  TORCH_CHECK((int)q_code_ptrs.size() == a.K && (int)q_scale_ptrs.size() == a.K, "compressed rounds need K payload pointers");
+  TORCH_CHECK(q_ef.empty() || (int)q_ef.size() == a.n_local, "error feedback: one slice per local replica");
+  a.qbits = (int)q_bits;
+  a.q_key = (unsigned long long)q_key;
+  a.q_t = reinterpret_cast<long long*>(q_t->data_ptr<int64_t>());
+  a.q_part = q_part->data_ptr<float>();
+  for (int k = 0; k < a.K; ++k) {
+    TORCH_CHECK(q_code_ptrs[k] % 16 == 0 && q_scale_ptrs[k] % 4 == 0, "payload slices must be 16-byte aligned");
+    a.q_codes[k] = reinterpret_cast<unsigned char*>(q_code_ptrs[k]);
+    a.q_scales[k] = reinterpret_cast<float*>(q_scale_ptrs[k]);
+  }
+  for (int j = 0; j < a.n_local; ++j) {
+    a.q_worker[j] = (int)local_idx[j];
+    if (!q_ef.empty()) {
+      CHECK_F32_CUDA(q_ef[j]); CHECK_CONTIG(q_ef[j]);
+      TORCH_CHECK(q_ef[j].numel() == a.n, "error feedback slices must have the block's length");
+      a.q_ef[j] = q_ef[j].data_ptr<float>();
+    }
+  }
+}
 static void fill_ctrl(uint32_t** dst, const std::vector<int64_t>& ctrl_ptrs, int world) {
   for (int p = 0; p < world && p < (int)ctrl_ptrs.size(); ++p) dst[p] = reinterpret_cast<uint32_t*>(ctrl_ptrs[p]);
 }
@@ -617,7 +651,10 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
                   std::vector<int64_t> ctrl_ptrs, Tensor sync, int64_t world, int64_t rank, int64_t mc_x, int64_t mc_y,
                   int64_t mc_z, std::vector<int64_t> xw_ptrs, std::vector<int64_t> zw_ptrs, bool two_shot,
                   int64_t max_blocks, double timeout_s, int64_t agg, int64_t trim_b, double dp_std, int64_t dp_key,
-                  c10::optional<Tensor> dp_t, c10::optional<Tensor> dp_stats, c10::optional<Tensor> dp_valid) {
+                  c10::optional<Tensor> dp_t, c10::optional<Tensor> dp_stats, c10::optional<Tensor> dp_valid,
+                  int64_t q_bits, int64_t q_group, int64_t q_key,
+                  c10::optional<Tensor> q_t, std::vector<int64_t> q_code_ptrs, std::vector<int64_t> q_scale_ptrs,
+                  std::vector<Tensor> q_ef, c10::optional<Tensor> q_part) {
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch);
   TORCH_CHECK(out.numel() >= fb::COMM_OUT_FLOATS && scratch.numel() >= fb::COMM_SCRATCH_FLOATS, "out / scratch too small");
   c10::cuda::CUDAGuard guard(z.device());
@@ -656,6 +693,7 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
   a.timeout_cycles = (long long)(timeout_s * 1.9e9);
   a.agg = (int)agg; a.trim_b = (int)trim_b;
   set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
+  set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
   fb::block_reduce_launch(a, cur_stream());
 }
 
@@ -668,7 +706,9 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
                          std::vector<int64_t> mw_ptrs, std::vector<int64_t> vw_ptrs, bool two_shot, int64_t max_blocks,
                          double timeout_s, int64_t agg, int64_t trim_b, double dp_std, int64_t dp_key,
                          c10::optional<Tensor> dp_t, c10::optional<Tensor> dp_stats,
-                         c10::optional<Tensor> dp_valid) {
+                         c10::optional<Tensor> dp_valid, int64_t q_bits, int64_t q_group, int64_t q_key,
+                         c10::optional<Tensor> q_t, std::vector<int64_t> q_code_ptrs, std::vector<int64_t> q_scale_ptrs,
+                         std::vector<Tensor> q_ef, c10::optional<Tensor> q_part) {
   TORCH_CHECK(opt >= fb::FEDOPT_AVGM && opt <= fb::FEDOPT_YOGI, "block_reduce_fedopt: unknown server optimizer ", opt);
   const bool adaptive = opt != fb::FEDOPT_AVGM;
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch); CHECK_F32_CUDA(m); CHECK_CONTIG(m);
@@ -712,6 +752,7 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
   a.v = adaptive ? v->data_ptr<float>() : nullptr;
   a.agg = (int)agg; a.trim_b = (int)trim_b;
   set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
+  set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
   fb::block_reduce_launch(a, cur_stream());
 }
 

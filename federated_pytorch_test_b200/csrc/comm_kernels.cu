@@ -26,7 +26,8 @@
 // mode: 0 = FedAvg (z = sum x / K, write-back), 1 = FedProx (no write-back), 2 = ADMM (z = sum(y + rho x)/(K rho)).
 // A second instantiation (FEDOPT) runs FedAvg with a server optimizer (FedAvgM / FedAdagrad / FedAdam / FedYogi) between
 // the reduction and the write-back.  DP instantiations add DP-FedAvg's Gaussian noise to the mean, after dp_clip_kernel
-// (end of file) has clipped the workers' updates.
+// (end of file) has clipped the workers' updates.  Compressed instantiations (QBITS) reduce stochastically rounded 8- / 4-bit
+// codes of the workers' updates, which every rank encodes for its own replicas before barrier A.
 // Reference sites: /root/reference/src/federated_multi.py:203-217, fedprox_multi.py:211-232, consensus_multi.py:242-299.
 #include "fedb200.h"
 
@@ -308,6 +309,274 @@ __device__ __forceinline__ float dp_noised_f32(const CommArgs& a, int i, float m
   return fmaf(dp_std_at(a, size_t(i)), (i & 1) ? g.y : g.x, mean);
 }
 
+// ---- compressed client updates: stochastic QBITS-bit codes with one scale per Q_GROUP coordinates ----------------------
+// (QSGD, Alistarh et al. 2017; FedPAQ, Reisizadeh et al. 2020; error feedback, Seide et al. 2014, Karimireddy et al. 2019)
+// Worker k's update u = x_k - z (+ e_k) is cut into groups of Q_GROUP coordinates counted from the block start.  A group's
+// scale is s = max|u| / L (L = 127 or 7) and its codes are q = clamp(floor(u / s + U), -L, L), U in [0, 1) the
+// counter-based uniform of (key, k, t, i), so E[q s] = u.  A group holding a non-finite u gets s = NaN (fmaxf alone would
+// drop a NaN) and codes 0: its dequantized values are NaN and the NaN guard fires.  An all-zero group gets s = 0, codes 0.
+// Every float operation that decides a code is correctly rounded (the extension is built with --use_fast_math), so the
+// codes equal the float32 numpy oracle (algo/compress.py: quantize) bit for bit.
+// Coordinates 2p and 2p + 1 share the word w = F(F(F(key + (t + 1) G) + (k + 1) G) + (p + 1) G) (F, G as for the DP
+// noise):  U_2p = w[63:40] 2^-24,  U_2p+1 = w[23:0] 2^-24.
+//
+// Work is split in tiles of COMM_THREADS * Q_SEG coordinates (64 groups) from the start of each slice (slices are whole
+// groups); CTA b takes tiles b, b + grid, ... and thread i the Q_SEG coordinates at 16 i of a tile in the encoder, in the
+// reduction and in the write-back alike.  So CTA b of every rank encodes exactly the groups CTA b of any peer reads, and
+// the per-CTA barriers A and B cover the payload as they cover the floats.
+constexpr int Q_TILE = COMM_THREADS * Q_SEG;
+static_assert(Q_GROUP % Q_SEG == 0 && Q_TILE % Q_GROUP == 0, "a tile must hold whole groups");
+
+__device__ __forceinline__ uint4 ld_sys_u32x4(const void* p) {
+  uint4 v;
+  asm volatile("ld.relaxed.sys.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint2 ld_sys_u32x2(const void* p) {
+  uint2 v;
+  asm volatile("ld.relaxed.sys.global.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p) : "memory");
+  return v;
+}
+// float4 at coordinate c (a multiple of 4) of a length-n slice: coordinates >= n read as 0 and are never written
+__device__ __forceinline__ float4 q_ld4(const float* p, int c, int n) {
+  if (c + 4 <= n) return *reinterpret_cast<const float4*>(p + c);
+  float v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) v[i] = c + i < n ? p[c + i] : 0.f;
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+__device__ __forceinline__ float4 q_ld4_sys(const float* p, int c, int n) {
+  if (c + 4 <= n) return ld_sys_v4(p + c);
+  float v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) v[i] = c + i < n ? ld_sys_f32(p + c + i) : 0.f;
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+__device__ __forceinline__ void q_st4(float* p, int c, int n, float4 v) {
+  if (c + 4 <= n) {
+    *reinterpret_cast<float4*>(p + c) = v;
+    return;
+  }
+  const float w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    if (c + i < n) p[c + i] = w[i];
+}
+// two-shot broadcast of a float4 into every rank: multimem.st when a multicast address is bound, else P2P stores
+__device__ __forceinline__ void q_bcast4(float* mc, float* const* w, int world, int c, int n, float4 v) {
+  if (c + 4 <= n) {
+    if (mc != nullptr) multimem_st_v4(mc + c, v);
+    else for (int p = 0; p < world; ++p) st_sys_v4(w[p] + c, v);
+    return;
+  }
+  const float s[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    if (c + i < n) for (int p = 0; p < world; ++p) st_sys_f32(w[p] + c + i, s[i]);
+}
+__device__ __forceinline__ float4 q_f4(const float* v, int q) { return make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]); }
+__device__ __forceinline__ void q_unf4(float* v, int q, float4 t) { v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w; }
+
+// Slice s of a compressed round: whole groups, coordinates [lo, hi).
+struct QSlice {
+  int lo, hi;
+};
+__device__ __forceinline__ QSlice q_slice(const CommArgs& a, int s) {
+  const int ng = (a.n + Q_GROUP - 1) / Q_GROUP;
+  const int per = a.two_shot ? (ng + a.world - 1) / a.world : ng;
+  return {min(a.n, s * per * Q_GROUP), min(a.n, (s + 1) * per * Q_GROUP)};
+}
+
+// Phase 0: encode the local replicas' updates on this CTA's tiles of every slice, update e_j, and accumulate this
+// thread's part of sum_j ||u_j - q_j s_j||^2 (err) and sum_j ||u_j||^2 (nrm).
+template <int QBITS>
+__device__ __forceinline__ void q_encode(const CommArgs& a, int nslices, float& err, float& nrm) {
+  constexpr float L = QBITS == 8 ? 127.f : 7.f;
+  const float inf = __int_as_float(0x7f800000);
+  for (int s = 0; s < nslices; ++s) {
+    const QSlice sl = q_slice(a, s);
+    for (int tb = sl.lo + blockIdx.x * Q_TILE; tb < sl.hi; tb += gridDim.x * Q_TILE) {   // uniform across the CTA
+      const int c0 = tb + Q_SEG * threadIdx.x;
+      const bool active = c0 < sl.hi;
+      float zv[Q_SEG];
+#pragma unroll
+      for (int q = 0; q < Q_SEG / 4; ++q) q_unf4(zv, q, active ? q_ld4(a.z, c0 + 4 * q, a.n) : make_float4(0.f, 0.f, 0.f, 0.f));
+      for (int j = 0; j < a.n_local; ++j) {
+        const int k = a.q_worker[j];
+        float* ef = a.q_ef[j];
+        float u[Q_SEG];
+        float amax = 0.f;                          // +inf: the group holds a non-finite u
+#pragma unroll
+        for (int q = 0; q < Q_SEG / 4; ++q) {
+          const float4 xv = active ? q_ld4(a.xl[j], c0 + 4 * q, a.n) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 ev = active && ef != nullptr ? q_ld4(ef, c0 + 4 * q, a.n) : make_float4(0.f, 0.f, 0.f, 0.f);
+          u[4 * q + 0] = __fadd_rn(__fsub_rn(xv.x, zv[4 * q + 0]), ev.x);
+          u[4 * q + 1] = __fadd_rn(__fsub_rn(xv.y, zv[4 * q + 1]), ev.y);
+          u[4 * q + 2] = __fadd_rn(__fsub_rn(xv.z, zv[4 * q + 2]), ev.z);
+          u[4 * q + 3] = __fadd_rn(__fsub_rn(xv.w, zv[4 * q + 3]), ev.w);
+        }
+#pragma unroll
+        for (int i = 0; i < Q_SEG; ++i) amax = isfinite(u[i]) ? fmaxf(amax, fabsf(u[i])) : inf;
+        // the Q_GROUP / Q_SEG = 8 threads of a group are adjacent lanes of one warp
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
+        const float sc = amax == inf ? __int_as_float(0x7fc00000) : __fdiv_rn(amax, L);
+        const bool coded = sc > 0.f && sc != inf;  // false for s = 0 and s = NaN: codes 0
+        const uint64_t wkey = dp_mix(dp_mix(a.q_key + uint64_t(*a.q_t + 1) * DP_GAMMA) + uint64_t(k + 1) * DP_GAMMA);
+        uint32_t packed[QBITS * Q_SEG / 32];
+#pragma unroll
+        for (int w = 0; w < QBITS * Q_SEG / 32; ++w) packed[w] = 0u;
+#pragma unroll
+        for (int p = 0; p < Q_SEG / 2; ++p) {
+          const uint64_t w = dp_mix(wkey + uint64_t((c0 >> 1) + p + 1) * DP_GAMMA);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int i = 2 * p + h;
+            const float U = float(uint32_t(h ? (w & 0xFFFFFFull) : (w >> 40))) * 5.9604644775390625e-8f;   // exact
+            int q = 0;
+            if (coded) q = int(fminf(fmaxf(floorf(__fadd_rn(__fdiv_rn(u[i], sc), U)), -L), L));
+            const float e = __fsub_rn(u[i], __fmul_rn(float(q), sc));
+            err = fmaf(e, e, err);
+            nrm = fmaf(u[i], u[i], nrm);
+            u[i] = e;
+            packed[i * QBITS / 32] |= (uint32_t(q) & ((1u << QBITS) - 1u)) << ((i * QBITS) % 32);
+          }
+        }
+        if (!active) continue;
+        if constexpr (QBITS == 8)
+          *reinterpret_cast<uint4*>(a.q_codes[k] + c0) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
+        else
+          *reinterpret_cast<uint2*>(a.q_codes[k] + c0 / 2) = make_uint2(packed[0], packed[1]);
+        if ((threadIdx.x & (Q_GROUP / Q_SEG - 1)) == 0) a.q_scales[k][c0 / Q_GROUP] = sc;
+        if (ef != nullptr) {
+#pragma unroll
+          for (int q = 0; q < Q_SEG / 4; ++q) q_st4(ef, c0 + 4 * q, a.n, q_f4(u, q));
+        }
+      }
+    }
+  }
+}
+
+// sum over the K workers, in worker order, of their dequantized codes q_k s_k at this thread's Q_SEG coordinates c0..
+template <int QBITS>
+__device__ __forceinline__ void q_gather(const CommArgs& a, int c0, float (&acc)[Q_SEG]) {
+#pragma unroll
+  for (int i = 0; i < Q_SEG; ++i) acc[i] = 0.f;
+#pragma unroll 4
+  for (int k = 0; k < a.K; ++k) {
+    const float sc = ld_sys_f32(a.q_scales[k] + c0 / Q_GROUP);
+    uint32_t wd[QBITS * Q_SEG / 32];
+    if constexpr (QBITS == 8) {                    // 16 bytes per peer and load
+      const uint4 v = ld_sys_u32x4(a.q_codes[k] + c0);
+      wd[0] = v.x; wd[1] = v.y; wd[2] = v.z; wd[3] = v.w;
+    } else {                                       // 8 bytes
+      const uint2 v = ld_sys_u32x2(a.q_codes[k] + c0 / 2);
+      wd[0] = v.x; wd[1] = v.y;
+    }
+#pragma unroll
+    for (int i = 0; i < Q_SEG; ++i) {
+      const int q = int(wd[i * QBITS / 32] << (32 - QBITS - (i * QBITS) % 32)) >> (32 - QBITS);   // sign-extended code
+      acc[i] = __fadd_rn(acc[i], __fmul_rn(float(q), sc));
+    }
+  }
+}
+
+// Server optimizer step from the pseudo-gradient d itself (compressed rounds: d is the dequantized mean update, not
+// formed as (z + d) - z).  FedAvgM: z + lr m, which is z + d when beta = 0 and lr = 1.
+__device__ __forceinline__ float fedopt_step_d(const CommArgs& a, float z, float d, float& m, float& v) {
+  if (a.opt == FEDOPT_AVGM) {
+    m = fmaf(a.beta1, m, d);
+    return fmaf(a.lr, m, z);
+  }
+  m = fmaf(a.beta1, m, (1.f - a.beta1) * d);
+  const float d2 = d * d;
+  if (a.opt == FEDOPT_ADAGRAD) {
+    v += d2;
+  } else if (a.opt == FEDOPT_ADAM) {
+    v = fmaf(a.beta2, v, (1.f - a.beta2) * d2);
+  } else {
+    const float s = v > d2 ? 1.f : (v < d2 ? -1.f : 0.f);
+    v = fmaf(-(1.f - a.beta2) * d2, s, v);
+  }
+  return fmaf(a.lr, m / (sqrtf(v) + a.tau), z);
+}
+
+// Pass 1 of a compressed round on this CTA's tiles of slice my_slice: z' = z + (1/K) sum_k q_k s_k (or the server step
+// along that d); one-shot stores z' (and m, v) locally, two-shot broadcasts them into every rank.
+template <bool FEDOPT, int QBITS>
+__device__ __forceinline__ void q_reduce(const CommArgs& a, int my_slice, float inv_k, float& dual, float& bad) {
+  const QSlice sl = q_slice(a, my_slice);
+  const bool adaptive = FEDOPT && a.opt != FEDOPT_AVGM;
+  for (int tb = sl.lo + blockIdx.x * Q_TILE; tb < sl.hi; tb += gridDim.x * Q_TILE) {
+    const int c0 = tb + Q_SEG * threadIdx.x;
+    if (c0 >= sl.hi) continue;
+    float acc[Q_SEG];
+    q_gather<QBITS>(a, c0, acc);
+#pragma unroll
+    for (int q = 0; q < Q_SEG / 4; ++q) {
+      const int c = c0 + 4 * q;
+      if (c >= a.n) break;
+      const float4 zo = q_ld4(a.z, c, a.n);
+      float4 d = q_f4(acc, q);
+      d = make_float4(__fmul_rn(d.x, inv_k), __fmul_rn(d.y, inv_k), __fmul_rn(d.z, inv_k), __fmul_rn(d.w, inv_k));
+      float4 zs, mv, vv;
+      if constexpr (FEDOPT) {
+        mv = q_ld4(a.m, c, a.n);
+        vv = adaptive ? q_ld4(a.v, c, a.n) : make_float4(0.f, 0.f, 0.f, 0.f);
+        zs = make_float4(fedopt_step_d(a, zo.x, d.x, mv.x, vv.x), fedopt_step_d(a, zo.y, d.y, mv.y, vv.y),
+                         fedopt_step_d(a, zo.z, d.z, mv.z, vv.z), fedopt_step_d(a, zo.w, d.w, mv.w, vv.w));
+      } else {
+        zs = make_float4(__fadd_rn(zo.x, d.x), __fadd_rn(zo.y, d.y), __fadd_rn(zo.z, d.z), __fadd_rn(zo.w, d.w));
+      }
+      if (!a.two_shot) {
+        const float dx = zo.x - zs.x, dy = zo.y - zs.y, dz = zo.z - zs.z, dw = zo.w - zs.w;
+        dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
+        if (!(isfinite(zs.x) && isfinite(zs.y) && isfinite(zs.z) && isfinite(zs.w))) bad += 1.f;
+        q_st4(a.z, c, a.n, zs);
+        if constexpr (FEDOPT) {
+          q_st4(a.m, c, a.n, mv);
+          if (adaptive) q_st4(a.v, c, a.n, vv);
+        }
+      } else {                                     // dual + NaN check from the landed weights in pass 2
+        q_bcast4(a.mc_x, a.xw, a.world, c, a.n, zs);
+        if constexpr (FEDOPT) {
+          q_bcast4(a.mc_m, a.mw, a.world, c, a.n, mv);
+          if (adaptive) q_bcast4(a.mc_v, a.vw, a.world, c, a.n, vv);
+        }
+      }
+    }
+  }
+}
+
+// Pass 2 of a compressed round (FedAvg's, on the compressed tiling): one-shot writes z into every local replica,
+// two-shot copies the broadcast weights of every slice into z and takes the dual residual and NaN count from them.
+__device__ __forceinline__ void q_write_back(const CommArgs& a, int nslices, float& dual, float& bad) {
+  for (int s = 0; s < nslices; ++s) {
+    const QSlice sl = q_slice(a, s);
+    for (int tb = sl.lo + blockIdx.x * Q_TILE; tb < sl.hi; tb += gridDim.x * Q_TILE) {
+      const int c0 = tb + Q_SEG * threadIdx.x;
+      if (c0 >= sl.hi) continue;
+#pragma unroll
+      for (int q = 0; q < Q_SEG / 4; ++q) {
+        const int c = c0 + 4 * q;
+        if (c >= a.n) break;
+        if (a.two_shot) {
+          const float4 zn = q_ld4_sys(a.xl[0], c, a.n);
+          const float4 zo = q_ld4(a.z, c, a.n);
+          const float dx = zo.x - zn.x, dy = zo.y - zn.y, dz = zo.z - zn.z, dw = zo.w - zn.w;
+          dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
+          if (!(isfinite(zn.x) && isfinite(zn.y) && isfinite(zn.z) && isfinite(zn.w))) bad += 1.f;
+          q_st4(a.z, c, a.n, zn);
+        } else {
+          const float4 zv = q_ld4(a.z, c, a.n);
+          for (int j = 0; j < a.n_local; ++j) q_st4(a.xl[j], c, a.n, zv);
+        }
+      }
+    }
+  }
+}
+
 // FEDOPT = false: FedAvg / FedProx / ADMM (a.mode).  FEDOPT = true: FedAvg (mode 0) whose new model is a server optimizer
 // step from z instead of the plain mean.  Pass 1 forms the step from the reduced mean, z and the state m (and v): one-shot
 // stores z, m, v locally; two-shot rank r broadcasts slice r of the new weights, of m and of v into every rank, so every rank
@@ -317,7 +586,10 @@ __device__ __forceinline__ float dp_noised_f32(const CommArgs& a, int i, float m
 // DP: the DP-FedAvg instantiations (mode 0, the mean, AGG_PAD = 0): pass 1 adds dp_std * xi to the mean before the optional
 // server step (one-shot, two-shot and the scalar tail alike); phase C exchanges the clip statistics of dp_clip_kernel
 // across ranks, and the last CTA advances the round counter dp_t.
-template <bool FEDOPT, int AGG_PAD, bool DP = false>
+// QBITS = 8 / 4: the compressed instantiations (mode 0, the mean): phase 0, before barrier A, encodes the local replicas'
+// updates into the payload arenas; pass 1 reduces the K workers' payloads instead of their floats, and both passes walk the
+// compressed tiling (no separate scalar tail); phase C exchanges the quantization statistics and advances q_t.
+template <bool FEDOPT, int AGG_PAD, bool DP = false, int QBITS = 0>
 __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const CommArgs a) {
   __shared__ float sm[32];
   __shared__ int s_abort;
@@ -335,12 +607,27 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   const int t0 = blockIdx.x * blockDim.x + threadIdx.x;
   const bool use_mc = a.mc_x != nullptr && (a.mode != 2 || a.mc_y != nullptr);
 
+  // ---- 0 (compressed rounds): encode the local replicas' updates; per-CTA partial statistics in CTA order ------
+  if constexpr (QBITS != 0) {
+    float err = 0.f, nrm = 0.f;
+    q_encode<QBITS>(a, nslices, err, nrm);
+    err = block_add(err, sm);                      // (its barriers also make the CTA's payload visible to all its threads)
+    nrm = block_add(nrm, sm);
+    if (threadIdx.x == 0) {
+      a.q_part[2 * blockIdx.x + 0] = err;
+      a.q_part[2 * blockIdx.x + 1] = nrm;
+    }
+    if (a.world > 1) __threadfence_system();
+  }
+
   // ---- A: inputs of every rank are final (their producers precede this kernel in stream order) ----------------
   cta_peer_barrier(a.ctrl, a.world, a.rank, PAD_FLAG_A, epoch, a.timeout_cycles, a.out + OUT_STATUS, &s_abort);
 
   // ---- 1: reduce, scale, new z, dual residual ---------------------------------------------------------------------
   float dual = 0.f, bad = 0.f;
-  {
+  if constexpr (QBITS != 0) {
+    q_reduce<FEDOPT, QBITS>(a, my_slice, inv_scale, dual, bad);
+  } else {
     const int lo = my_slice * chunk4;
     const int hi = min(n4, lo + chunk4);
     // two elements per thread and iteration: their (remote) loads are issued back to back, so twice as many bytes are in
@@ -405,7 +692,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   }
   // scalar tail (n % 4 elements): every rank reduces it for itself, one-shot style
   const int tail0 = n4 << 2;
-  if (blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
+  if (QBITS == 0 && blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
     const int i = tail0 + threadIdx.x;
     float acc = 0.f;
     if constexpr (AGG_PAD > 0) {
@@ -440,7 +727,8 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   float pr[COMM_MAX_LOCAL];
 #pragma unroll
   for (int j = 0; j < COMM_MAX_LOCAL; ++j) pr[j] = 0.f;
-  for (int s = 0; s < nslices; ++s) {
+  if constexpr (QBITS != 0) q_write_back(a, nslices, dual, bad);
+  for (int s = 0; s < (QBITS == 0 ? nslices : 0); ++s) {
     const int lo = s * chunk4;
     const int hi = min(n4, lo + chunk4);
     for (int i = lo + t0; i < hi; i += stride) {
@@ -475,7 +763,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       }
     }
   }
-  if (blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
+  if (QBITS == 0 && blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
     const int i = tail0 + threadIdx.x;
     const float zv = a.z[i];
 #pragma unroll
@@ -600,6 +888,50 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       *a.dp_t += 1;                                // every CTA has read t: the next round (or graph replay) draws t + 1
     }
   }
+  // compressed rounds (mode 0): the per-CTA partial statistics in CTA order, then over the ranks in rank order, so every
+  // rank reports the same values
+  if constexpr (QBITS != 0) {
+    __shared__ float s_q[2];
+    if (threadIdx.x == 0) {
+      float e = 0.f, u = 0.f;
+      for (int b = 0; b < int(gridDim.x); ++b) {
+        e += __ldcg(a.q_part + 2 * b + 0);
+        u += __ldcg(a.q_part + 2 * b + 1);
+      }
+      s_q[0] = e;
+      s_q[1] = u;
+    }
+    __syncthreads();
+    if (a.world > 1) {
+      if (threadIdx.x < a.world) {
+        float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_Q_PAYLOAD) + 2 * a.rank;
+        st_sys_f32(pay + 0, s_q[0]);
+        st_sys_f32(pay + 1, s_q[1]);
+        __threadfence_system();
+        st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_C + a.rank, epoch);
+        if (s_abort == 0 && !wait_flag(a.ctrl[a.rank] + PAD_FLAG_C + threadIdx.x, epoch, a.timeout_cycles)) {
+          a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
+          atomicExch(&s_abort, 1);
+        }
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_Q_PAYLOAD);
+        float e = 0.f, u = 0.f;
+        for (int r = 0; r < a.world; ++r) {
+          e += ld_sys_f32(pay + 2 * r + 0);
+          u += ld_sys_f32(pay + 2 * r + 1);
+        }
+        s_q[0] = e;
+        s_q[1] = u;
+      }
+    }
+    if (threadIdx.x == 0) {
+      a.out[OUT_Q_ERR_SQ] = s_q[0];
+      a.out[OUT_Q_NORM_SQ] = s_q[1];
+      *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) draws t + 1
+    }
+  }
   if (threadIdx.x == 0) {
     a.out[OUT_DUAL_SQ] = dual_sq;
     a.out[OUT_PRIMAL] = primal;
@@ -649,18 +981,29 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   }
   if (args.dp && (args.agg != AGG_MEAN || args.mode != 0 || args.dp_t == nullptr || args.dp_stats == nullptr))
     throw std::runtime_error("fedb200: block_reduce: DP needs mode 0, the mean, a round counter and clip statistics");
+  if (args.qbits != 0) {
+    if (args.qbits != 8 && args.qbits != 4) throw std::runtime_error("fedb200: block_reduce: compressed rounds take 8 or 4 bits");
+    if (args.agg != AGG_MEAN || args.mode != 0 || args.dp || args.q_t == nullptr || args.q_part == nullptr)
+      throw std::runtime_error("fedb200: block_reduce: compression needs mode 0, the mean without DP, a round counter and "
+                               "a statistics buffer");
+    if (args.two_shot && (args.xw[args.world - 1] == nullptr || (args.opt != FEDOPT_NONE && args.mw[args.world - 1] == nullptr)))
+      throw std::runtime_error("fedb200: block_reduce: two-shot compressed rounds need P2P broadcast targets");
+  }
   const bool fo = args.opt != FEDOPT_NONE;
-  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean]
-  const void* kernels[2][5] = {
+  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean, 8-bit codes, 4-bit codes]
+  const void* kernels[2][7] = {
       {(const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
        (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>,
-       (const void*)block_reduce_kernel<false, 0, true>},
+       (const void*)block_reduce_kernel<false, 0, true>, (const void*)block_reduce_kernel<false, 0, false, 8>,
+       (const void*)block_reduce_kernel<false, 0, false, 4>},
       {(const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
        (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>,
-       (const void*)block_reduce_kernel<true, 0, true>}};
-  const int pad = args.dp ? 4 : args.agg == AGG_MEAN ? 0 : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
+       (const void*)block_reduce_kernel<true, 0, true>, (const void*)block_reduce_kernel<true, 0, false, 8>,
+       (const void*)block_reduce_kernel<true, 0, false, 4>}};
+  const int pad = args.qbits == 8 ? 5 : args.qbits == 4 ? 6 : args.dp ? 4 : args.agg == AGG_MEAN ? 0
+                : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
   const void* kernel = kernels[fo][pad];
-  static int max_blocks[2][5] = {};
+  static int max_blocks[2][7] = {};
   int& mb = max_blocks[fo][pad];
   if (mb == 0) mb = comm_max_blocks(kernel);
   int cap = mb;
@@ -668,6 +1011,11 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   const int n4 = args.n >> 2;
   const int work4 = args.two_shot ? (n4 + args.world - 1) / args.world : n4;
   int want = (work4 + COMM_THREADS - 1) / COMM_THREADS;
+  if (args.qbits != 0) {                               // one tile of COMM_THREADS * Q_SEG coordinates per CTA and step
+    const int ng = (args.n + Q_GROUP - 1) / Q_GROUP;
+    const int per = args.two_shot ? (ng + args.world - 1) / args.world : ng;
+    want = (per * Q_GROUP + Q_TILE - 1) / Q_TILE;
+  }
   int grid = want < 1 ? 1 : (want > cap ? cap : want);
   if (args.timeout_cycles <= 0) args.timeout_cycles = 240000000000LL;   // ~2 min at 2 GHz
   void* kargs[] = {(void*)&args};

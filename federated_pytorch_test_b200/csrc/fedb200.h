@@ -186,13 +186,16 @@ constexpr int PAD_FLAG_D = PAD_FLAG_C + COMM_MAX_WORLD;                       //
 constexpr int PAD_PAYLOAD = PAD_FLAG_D + COMM_MAX_WORLD;                      // [COMM_MAX_WORLD][4] floats: dual^2 part, primal part, #non-finite
 constexpr int PAD_BBROWS = PAD_PAYLOAD + 4 * COMM_MAX_WORLD;                  // [COMM_MAX_K][8] floats: six dots per worker
 constexpr int PAD_DP_PAYLOAD = PAD_BBROWS + 8 * COMM_MAX_K;                   // [COMM_MAX_WORLD][2] floats: #clipped, sum of norms
+constexpr int PAD_Q_PAYLOAD = PAD_DP_PAYLOAD + 2 * COMM_MAX_WORLD;            // [COMM_MAX_WORLD][2] floats: quantization statistics
 constexpr int COMM_PAD_WORDS = 8192;
-static_assert(PAD_DP_PAYLOAD + 2 * COMM_MAX_WORLD <= COMM_PAD_WORDS, "control pad too small");
+static_assert(PAD_Q_PAYLOAD + 2 * COMM_MAX_WORLD <= COMM_PAD_WORDS, "control pad too small");
 
 // out record of an aggregation (floats): what the host reads back, once per round.  DP rounds add the number of clipped
-// workers and the sum of their pre-clip update norms, over all K.
+// workers and the sum of their pre-clip update norms, over all K; compressed rounds the sums over all K of
+// ||u_k - q_k s_k||^2 and ||u_k||^2.
 constexpr int OUT_DUAL_SQ = 0, OUT_PRIMAL = 1, OUT_NONFINITE = 2, OUT_STATUS = 3, OUT_RHO = 4, OUT_EPOCH = 5, OUT_TWO_SHOT = 6;
 constexpr int OUT_DP_CLIPPED = 8, OUT_DP_NORM_SUM = 9;
+constexpr int OUT_Q_ERR_SQ = 10, OUT_Q_NORM_SQ = 11;
 constexpr int COMM_OUT_FLOATS = 12;
 // device scratch (floats): [0] dual^2, [1] #non-finite, [2] ticket (as uint), [4 + j] per-replica primal^2; self-cleaning
 constexpr int COMM_SCRATCH_FLOATS = 4 + COMM_MAX_LOCAL;
@@ -245,7 +248,22 @@ struct CommArgs {
   // per DP_CHUNK-float chunk of the slice, how many of its leading floats are parameters (the rest is the arena's
   // alignment padding, which gets no noise and stays zero); nullptr: every float is a parameter
   const unsigned char* dp_valid;
+  // ---- compressed client updates (QSGD / FedPAQ, mode 0 with the mean, with or without a server optimizer): before barrier
+  // A every rank quantizes its local replicas' updates u_k = x_k - z (+ e_k) into payload arenas — one scale per Q_GROUP
+  // coordinates, stochastically rounded qbits-bit codes — and pass 1 reads the K workers' payloads instead of their floats.
+  int qbits;                         // 0 selects the instantiations above; 8 or 4
+  unsigned long long q_key;          // key of the run's rounding stream
+  long long* q_t;                    // device: index t of this compressed round over the run; the last CTA increments it
+  int q_worker[COMM_MAX_LOCAL];      // global worker id k of local replica j (keys the rounding draw)
+  unsigned char* q_codes[COMM_MAX_K];   // codes of ALL workers (local or peer-mapped): one byte per coordinate (8-bit)
+                                        // or two codes per byte, the even coordinate in the low nibble (4-bit)
+  float* q_scales[COMM_MAX_K];       // one scale per group of Q_GROUP coordinates, counted from the block start
+  float* q_ef[COMM_MAX_LOCAL];       // error feedback e_j of local replica j (in/out), or nullptr (off)
+  float* q_part;                     // [Q_PART_FLOATS] per-CTA partial statistics (each launch overwrites what it reads)
 };
+constexpr int Q_GROUP = 128;                             // coordinates per scale
+constexpr int Q_SEG = 16;                                // coordinates per thread and tile in the compressed instantiations
+constexpr int Q_PART_FLOATS = 2 * COMM_MAX_BLOCKS;
 constexpr int DP_CHUNK = 32;
 constexpr int FEDOPT_NONE = 0, FEDOPT_AVGM = 1, FEDOPT_ADAGRAD = 2, FEDOPT_ADAM = 3, FEDOPT_YOGI = 4;
 constexpr int AGG_MEAN = 0, AGG_MEDIAN = 1, AGG_TRIMMED = 2;

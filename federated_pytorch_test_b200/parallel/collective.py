@@ -7,7 +7,9 @@ one device):
   (/root/reference/src/federated_multi.py:204-217); with a server optimizer (``fedopt_``) ``z'`` is its step from ``z``
   along ``mean_k x_k - z`` instead of the plain mean; with a robust rule (``robust_``) ``z'`` is the coordinate-wise
   median or trimmed mean of the K workers instead of their mean; with DP (``dp_clip_`` first, then ``dp=`` on
-  ``fedavg_`` / ``fedopt_``) the workers' updates are clipped and Gaussian noise is added to the mean (DP-FedAvg)
+  ``fedavg_`` / ``fedopt_``) the workers' updates are clipped and Gaussian noise is added to the mean (DP-FedAvg); with
+  ``compress=`` on ``fedavg_`` / ``fedopt_`` every worker uploads its update ``x_k - z`` as stochastically rounded 8- or
+  4-bit codes with one scale per group (``algo/compress.py``), and ``z' = z + mean_k q_k s_k``
 * X2 FedProx ``z' = mean``; ``dual``; ``primal = sum_k ||rho (x_k - z')||``; no write-back
   (fedprox_multi.py:211-232)
 * X3 ADMM    ``z' = sum_k (y_k + rho x_k) / (K rho)``; ``dual``; ``y_k += rho (x_k - z')``;
@@ -65,6 +67,21 @@ class DPRound:
         return (i % 32) < self.valid.long()[i // 32]
 
 
+@dataclass
+class QuantRound:
+    """The compression of one round (``algo/compress.py``): ``bits`` (8 or 4), the key of the rounding stream and ``t``, a
+    one-element int64 tensor on the block's device holding the index of the compressed round over the run (advanced by the
+    round).  ``codes`` / ``scales`` are the local replicas' payload slices (:meth:`TorchCollective.payload_like_block`;
+    on the fused collective peers read them), ``ef`` the local replicas' error-feedback vectors (in / out; None = off)."""
+
+    bits: int
+    key: int
+    t: torch.Tensor
+    codes: List[torch.Tensor]
+    scales: List[torch.Tensor]
+    ef: Optional[List[torch.Tensor]] = None
+
+
 class TorchCollective:
     """ATen + torch.distributed implementation (baseline / oracle / CPU)."""
 
@@ -75,6 +92,7 @@ class TorchCollective:
         self.topo = topo
         self.launches = 0  # number of framework-owned kernels launched (0 here: library path)
         self.last_dp = (0.0, 0.0)   # DP rounds: (#clipped workers, sum of their pre-clip update norms) over all K
+        self.last_q = (0.0, 0.0)    # compressed rounds: (sum_k ||u_k - q_k s_k||^2, sum_k ||u_k||^2) over all K
 
     # -- arena hooks ------------------------------------------------------
     def arena_allocator(self) -> Optional[Callable]:
@@ -87,6 +105,17 @@ class TorchCollective:
         """Zeroed companion vector of block slice ``x`` (ADMM duals).  The fused backend returns a slice of a
         symmetric arena so that peers can read it."""
         return torch.zeros_like(x)
+
+    def payload_like_block(self, x: torch.Tensor, bits: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Zeroed payload buffers of block slice ``x`` for ``bits``-bit codes: the codes (uint8, ``bits / 8`` bytes per
+        coordinate, two 4-bit codes per byte with the even coordinate in the low nibble, whole segments of 16
+        coordinates) and the scales (float32, one per group of ``compress.GROUP``).  The fused backend hands out slices of
+        symmetric arenas so that peers can read them."""
+        from ..algo.compress import GROUP
+
+        n = x.numel()
+        return (torch.zeros(-(-n // 16) * 2 * bits, dtype=torch.uint8, device=x.device),
+                torch.zeros(-(-n // GROUP), dtype=torch.float32, device=x.device))
 
     # -- primitives -------------------------------------------------------
     def _allreduce(self, t: torch.Tensor) -> torch.Tensor:
@@ -181,12 +210,64 @@ class TorchCollective:
             mean.add_(xi.mul_(dp.std))
         dp.t.add_(1)
 
+    @staticmethod
+    def quantize_(u: torch.Tensor, bits: int, key: int, k: int, t: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Codes (int8) and scales (float32) of update ``u`` of worker ``k`` in compressed round ``t``
+        (``algo/compress.py: quantize``), on ``u``'s device."""
+        from ..algo.compress import quantize
+
+        codes, scales = quantize(u.detach().float().cpu().numpy(), bits, key, k, t)
+        return torch.from_numpy(codes).to(u.device), torch.from_numpy(scales).to(u.device)
+
+    @staticmethod
+    def dequantize(codes: torch.Tensor, scales: torch.Tensor) -> torch.Tensor:
+        """``q s`` per coordinate (float32)."""
+        from ..algo.compress import GROUP
+
+        return codes.float() * scales.repeat_interleave(GROUP)[: codes.numel()]
+
+    @torch.no_grad()
+    def _compressed_update(self, xs: List[torch.Tensor], z: torch.Tensor, q: QuantRound) -> torch.Tensor:
+        """``d = (1/K) sum_k q_k s_k`` of a compressed round, summed in float32 in worker order ``k = 0 .. K-1``: every
+        local replica is quantized (updating its error feedback and its payload slices), then the K dequantized updates
+        are gathered.  Advances ``q.t``; the statistics go to :attr:`last_q`."""
+        from ..algo.compress import pack4
+
+        t = int(q.t.item())
+        deqs, stats = [], torch.zeros(2, dtype=torch.float64, device=z.device)
+        for j, (x, ck) in enumerate(zip(xs, self.topo.local_workers)):
+            u = x - z
+            if q.ef is not None:
+                u = u + q.ef[j]
+            codes, scales = self.quantize_(u, q.bits, q.key, ck, t)
+            deq = self.dequantize(codes, scales)
+            e = u - deq
+            if q.ef is not None:
+                q.ef[j].copy_(e)
+            stats[0] += e.double().square().sum()
+            stats[1] += u.double().square().sum()
+            raw = codes.view(torch.uint8) if q.bits == 8 else torch.from_numpy(pack4(codes.cpu().numpy())).to(z.device)
+            q.codes[j][: raw.numel()].copy_(raw)
+            q.scales[j][: scales.numel()].copy_(scales)
+            deqs.append(deq)
+        full = self.gather_blocks(deqs)
+        acc = full[0].clone()
+        for k in range(1, self.topo.K):
+            acc.add_(full[k])
+        self.last_q = tuple(self.sum_scalars(stats).tolist())
+        q.t.add_(1)
+        return acc.mul_(1.0 / self.topo.K)
+
     @torch.no_grad()
     def fedavg_(self, xs: List[torch.Tensor], z: torch.Tensor, write_back: bool = True,
-                dp: Optional[DPRound] = None) -> torch.Tensor:
+                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> torch.Tensor:
         """In place: ``z <- mean_k x_k``, optionally ``x_k <- z``; returns ``||z_old - z_new||^2`` (0-dim).  With ``dp``
-        the mean is noised (:class:`DPRound`; clip the replicas with :meth:`dp_clip_` first)."""
-        znew = self.sum_blocks(xs).div_(self.topo.K)
+        the mean is noised (:class:`DPRound`; clip the replicas with :meth:`dp_clip_` first).  With ``compress``
+        (:class:`QuantRound`) ``z <- z + (1/K) sum_k q_k s_k``, the workers' updates as uploaded."""
+        if compress is not None:
+            znew = z + self._compressed_update(xs, z, compress)
+        else:
+            znew = self.sum_blocks(xs).div_(self.topo.K)
         if dp is not None:
             self._add_dp_noise_(znew, dp)
         diff = z - znew
@@ -214,22 +295,28 @@ class TorchCollective:
     @torch.no_grad()
     def fedopt_(self, xs: List[torch.Tensor], z: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], kind: str,
                 lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean", trim_b: int = 0,
-                dp: Optional[DPRound] = None) -> torch.Tensor:
+                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> torch.Tensor:
         """FedAvg with a server optimizer, in place: ``d = mean_k x_k - z`` is the pseudo-gradient of server optimizer
         ``kind`` (one of :data:`FEDOPT_KINDS`; ``beta1`` is the momentum of 'avgm'), whose state ``m`` (and ``v``, unused
         by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``.
         With a robust rule ``agg`` (one of :data:`ROBUST_AGGS`) its aggregate replaces the mean in ``d``; with ``dp`` the
-        noised mean does (DP-FedOpt: post-processing)."""
-        if agg == "mean":
+        noised mean does (DP-FedOpt: post-processing); with ``compress`` ``d`` is the dequantized mean update itself
+        (FedPAQ with a server optimizer)."""
+        mean = None
+        if compress is not None:
+            d = self._compressed_update(xs, z, compress)
+        elif agg == "mean":
             mean = self.sum_blocks(xs).div_(self.topo.K)
             if dp is not None:
                 self._add_dp_noise_(mean, dp)
         else:
             mean = self.robust_aggregate(xs, agg, trim_b)
-        d = mean - z
+        if mean is not None:
+            d = mean - z
         if kind == "avgm":
             m.mul_(beta1).add_(d)
-            znew = mean + (lr * m - d)          # = z + lr m; exactly the mean when beta = 0 and lr = 1 (FedAvg)
+            # = z + lr m; from the mean exactly the mean when beta = 0 and lr = 1 (FedAvg)
+            znew = z + lr * m if mean is None else mean + (lr * m - d)
         else:
             m.mul_(beta1).add_(d, alpha=1.0 - beta1)
             d2 = d * d

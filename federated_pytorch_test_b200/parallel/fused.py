@@ -35,6 +35,12 @@ DP-FedAvg (client-level differential privacy) is two launches per round, in stre
 clip kernel on each rank's own replicas (no peer memory), then DP instantiations of the aggregation kernel, which add
 the counter-based Gaussian noise to the mean and advance the device-resident round counter, so a graph-captured round
 draws fresh noise on every replay.
+
+Compressed rounds (stochastic 8- / 4-bit codes with one scale per group, optional error feedback) are one launch of the
+compressed instantiations: before barrier A every rank encodes its own replicas' updates into symmetric payload arenas
+(:meth:`FusedCollective.payload_like_block`), and pass 1 reads the K workers' codes and scales over P2P (there is no
+in-switch reduction of codes with per-group scales; the two-shot broadcast may still use ``multimem.st``), so a rank pulls
+about 4x (8-bit) or 7.5x (4-bit) fewer bytes from its peers.  The rounding counter lives in device memory as the DP one.
 """
 from __future__ import annotations
 
@@ -45,7 +51,7 @@ import torch
 import torch.distributed as dist
 
 from ..ops import cuda_ops
-from .collective import FEDOPT_KINDS, ROBUST_AGGS, DPRound, TorchCollective, check_robust
+from .collective import FEDOPT_KINDS, ROBUST_AGGS, DPRound, QuantRound, TorchCollective, check_robust
 from .topology import Topology
 
 _MAX_LOCAL = 16
@@ -54,9 +60,12 @@ _SCRATCH_FLOATS = 4 + _MAX_LOCAL
 _MAX_BLOCKS = 160                                         # csrc/fedb200.h: COMM_MAX_BLOCKS
 _DP_STATS_FLOATS = 2 * _MAX_LOCAL * _MAX_BLOCKS + 2 * _MAX_LOCAL      # DP_STATS_FLOATS: double partials, norms, flags
 _BB_SCRATCH_FLOATS = 8 * _MAX_LOCAL + 8 + _MAX_LOCAL
+_Q_PART_FLOATS = 2 * _MAX_BLOCKS                          # Q_PART_FLOATS: per-CTA partial statistics
+_Q_GROUP = 128                                            # Q_GROUP (algo/compress.py: GROUP)
 _PAD_WORDS = 8192
 OUT_DUAL_SQ, OUT_PRIMAL, OUT_NONFINITE, OUT_STATUS, OUT_RHO, OUT_EPOCH, OUT_TWO_SHOT = range(7)
 OUT_DP_CLIPPED, OUT_DP_NORM_SUM = 8, 9
+OUT_Q_ERR_SQ, OUT_Q_NORM_SQ = 10, 11
 
 TWO_SHOT_MIN_BYTES = int(os.environ.get("FEDB200_TWO_SHOT_BYTES", str(256 * 1024)))
 TWO_SHOT_MODE = os.environ.get("FEDB200_TWO_SHOT", "auto")          # 'auto' | '0' (never) | '1' (whenever legal)
@@ -160,6 +169,7 @@ class FusedCollective(TorchCollective):
         self.scratch = torch.zeros(_SCRATCH_FLOATS, dtype=torch.float32, device=dev)
         self.bb_scratch = torch.zeros(_BB_SCRATCH_FLOATS, dtype=torch.float32, device=dev)
         self.dp_stats = torch.zeros(_DP_STATS_FLOATS, dtype=torch.float32, device=dev)
+        self.q_part = torch.zeros(_Q_PART_FLOATS, dtype=torch.float32, device=dev)
         self.bb_log = torch.zeros(8 * max(topo.K, 1), dtype=torch.float32, device=dev)
         self.sync = torch.zeros(4, dtype=torch.int32, device=dev)
         self._host_out = torch.zeros(self.out.numel(), dtype=torch.float32).pin_memory()
@@ -168,6 +178,7 @@ class FusedCollective(TorchCollective):
         self.ctrl = self.heap.alloc(_PAD_WORDS, dtype=torch.int32)
         self.ctrl_ptrs = list(self.heap.locate(self.ctrl)[0]["peer_ptrs"])
         self._aux: Dict[Tuple[int, str], torch.Tensor] = {}
+        self._payload: Dict[Tuple[int, int], Tuple[torch.Tensor, torch.Tensor]] = {}   # (arena base, bits) -> code / scale arenas
         # in-switch reduction pays from 4 peers on; between 2 GPUs there is nothing to reduce in the switch and the P2P variant of
         # the same kernel is used.  FEDB200_MULTIMEM=0|1 forces either.
         mm = os.environ.get("FEDB200_MULTIMEM", "auto")
@@ -182,13 +193,15 @@ class FusedCollective(TorchCollective):
         self.warm_fedopt = False          # set by the FedOpt strategy: warm the server-optimizer instantiation too
         self.warm_robust = False          # set by robust strategies: warm the robust instantiation(s) for this K too
         self.warm_dp = False              # set by DP strategies: warm the clip kernel and the DP instantiation(s) too
+        self.warm_compress = 0            # set by compressing strategies to their bit width: warm those instantiations too
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
         cross-rank handshake happen here, at engine construction, not inside the first training round (the first launch
         is far slower than the ones after it).  The server-optimizer kernel is warmed only when ``warm_fedopt`` is set, the
         robust kernels (of this K; with the server optimizer if both are set) only when ``warm_robust`` is set, the DP
-        kernels (likewise) only when ``warm_dp`` is set.
+        kernels (likewise) only when ``warm_dp`` is set, the compressed ones of ``warm_compress`` bits (likewise) only when
+        that is set.
         Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
@@ -200,6 +213,10 @@ class FusedCollective(TorchCollective):
         rho = torch.full((1,), 0.5, dtype=torch.float32, device=self.topo.device)
         if self.warm_fedopt:
             m, v = self.zeros_like_block(xs[0], "srv_m"), self.zeros_like_block(xs[0], "srv_v")
+        if self.warm_compress:
+            pay = [self.payload_like_block(x, self.warm_compress) for x in xs]
+            qr = QuantRound(self.warm_compress, 0, torch.zeros(1, dtype=torch.int64, device=self.topo.device),
+                            [c for c, _ in pay], [sc for _, sc in pay])
         keep = self.two_shot_mode
         for mode_2shot in ("0", "1"):
             self.two_shot_mode = mode_2shot
@@ -218,6 +235,10 @@ class FusedCollective(TorchCollective):
                 self._launch(0, xs, None, z, 0.0, dp=dp)
                 if self.warm_fedopt:
                     self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, dp=dp)
+            if self.warm_compress:
+                self._launch(0, xs, None, z, 0.0, compress=qr)
+                if self.warm_fedopt:
+                    self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, compress=qr)
         self.two_shot_mode = keep
         x0 = [torch.zeros_like(x) for x in xs]
         yh = [torch.zeros_like(x) for x in xs]
@@ -245,6 +266,28 @@ class FusedCollective(TorchCollective):
         sl = buf[off // 4: off // 4 + x.numel()]
         sl.zero_()
         return sl
+
+    def payload_like_block(self, x: torch.Tensor, bits: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The payload slices of block slice ``x`` for ``bits``-bit codes (layout: :meth:`TorchCollective.payload_like_block`)
+        in symmetric arenas that mirror ``x``'s arena: the codes of the arena's float ``i`` at byte ``i bits / 8``, the
+        scale of a group starting at float ``i`` at float ``i / 32`` of a scale arena.  So every block slice has its own
+        payload at the same offset in every rank.  ``x`` must start at a multiple of 32 floats (the arenas' alignment)."""
+        a, off = self.heap.locate(x)
+        i0 = off // 4
+        if i0 % 32:
+            raise ValueError("compressed rounds need block slices that start at a multiple of 32 floats, got %d" % i0)
+        key = (a["base"], int(bits))
+        bufs = self._payload.get(key)
+        if bufs is None:
+            nf = a["nbytes"] // 4
+            bufs = (self.heap.alloc(nf * bits // 8 + 64, dtype=torch.uint8), self.heap.alloc(nf // 32 + 2))
+            self._payload[key] = bufs
+        n = x.numel()
+        codes = bufs[0][i0 * bits // 8: i0 * bits // 8 + -(-n // 16) * 2 * bits]
+        scales = bufs[1][i0 // 32: i0 // 32 + -(-n // _Q_GROUP)]
+        codes.zero_()
+        scales.zero_()
+        return codes, scales
 
     # -- pointer tables -------------------------------------------------------------
     def _tables(self, slices: List[torch.Tensor]):
@@ -286,12 +329,25 @@ class FusedCollective(TorchCollective):
         key = int(dp.key) & ((1 << 64) - 1)
         return float(dp.std), key - (1 << 64) if key >= 1 << 63 else key, dp.t, self.dp_stats, dp.valid
 
+    def _q_args(self, q: Optional[QuantRound]):
+        """The compression arguments of the aggregation bindings: bits, group size, key (as a signed 64-bit int), counter,
+        the K workers' code and scale pointers, the local error-feedback slices, the statistics buffer."""
+        if q is None:
+            return 0, _Q_GROUP, 0, None, [], [], [], None
+        key = int(q.key) & ((1 << 64) - 1)
+        cp, _, _ = self._tables(q.codes)
+        sp, _, _ = self._tables(q.scales)
+        return (int(q.bits), _Q_GROUP, key - (1 << 64) if key >= 1 << 63 else key, q.t, cp, sp,
+                list(q.ef) if q.ef is not None else [], self.q_part)
+
     def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None, agg: str = "mean", trim_b: int = 0,
-                dp: Optional[DPRound] = None) -> None:
+                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> None:
         """Modes 0 / 1 take a robust rule ``agg`` (:data:`ROBUST_AGGS`) in place of the mean; mode 0 with the mean takes
-        the noise of a DP round (``dp``; after :meth:`dp_clip_`)."""
+        the noise of a DP round (``dp``; after :meth:`dp_clip_`) or compresses the workers' updates (``compress``)."""
         if dp is not None and (mode != 0 or agg != "mean"):
             raise ValueError("DP aggregation needs FedAvg with the mean")
+        if compress is not None and (mode != 0 or agg != "mean" or dp is not None):
+            raise ValueError("compressed aggregation needs FedAvg with the mean, without DP")
         code = self._agg_code(agg, trim_b)
         n = xs[0].numel()
         if any(t.numel() != n for t in xs) or z.numel() != n:
@@ -314,19 +370,22 @@ class FusedCollective(TorchCollective):
                     mcz = za["mc_ptr"] + zoff
         self.ext.block_reduce(mode, xp, yp, local_idx, z, n, float(rho), rho_dev, self.out, self.scratch, self.ctrl_ptrs,
                               self.sync, W, self.topo.rank, mcx, mcy, mcz, xw, zw, bool(two), self.max_blocks,
-                              self.timeout_s, code, int(trim_b), *self._dp_args(dp))
+                              self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress))
         self.launches += 1
         self.last_two_shot = bool(two)
 
     def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                       trim_b: int = 0, dp: Optional[DPRound] = None) -> None:
+                       trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> None:
         """FedAvg with a server optimizer: mode 0 of the kernel's FedOpt instantiation.  Two-shot, rank r broadcasts slice r
         of the new weights, of ``m`` and of ``v`` into every rank, so ``m`` / ``v`` must be symmetric slices then
         (:meth:`zeros_like_block`).  A robust rule ``agg`` replaces the mean as the aggregate the step is taken towards; a
-        DP round (``dp``, mean only) noises the mean first."""
+        DP round (``dp``, mean only) noises the mean first; a compressed round (``compress``, mean only) steps along the
+        dequantized mean update."""
         code = self._agg_code(agg, trim_b)
         if dp is not None and agg != "mean":
             raise ValueError("DP aggregation needs the mean")
+        if compress is not None and (agg != "mean" or dp is not None):
+            raise ValueError("compressed aggregation needs the mean, without DP")
         n = xs[0].numel()
         adaptive = kind != "avgm"
         if any(t.numel() != n for t in xs) or z.numel() != n or m.numel() != n or (adaptive and v.numel() != n):
@@ -344,7 +403,7 @@ class FusedCollective(TorchCollective):
         self.ext.block_reduce_fedopt(FEDOPT_KINDS.index(kind) + 1, float(lr), float(beta1), float(beta2), float(tau), m,
                                      v if adaptive else None, xp, local_idx, z, n, self.out, self.scratch, self.ctrl_ptrs,
                                      self.sync, W, self.topo.rank, mcx, mcm, mcv, xw, mw, vw, bool(two), self.max_blocks,
-                                     self.timeout_s, code, int(trim_b), *self._dp_args(dp))
+                                     self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress))
         self.launches += 1
         self.last_two_shot = bool(two)
 
@@ -359,13 +418,14 @@ class FusedCollective(TorchCollective):
             self._out_event.record()
             self._out_pending = True
 
-    def launch_fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None) -> None:
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp)
+    def launch_fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
+                       compress: Optional[QuantRound] = None) -> None:
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress)
         self._record_async()
 
     def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                       trim_b: int = 0, dp: Optional[DPRound] = None) -> None:
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp)
+                       trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> None:
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress)
         self._record_async()
 
     @torch.no_grad()
@@ -405,12 +465,14 @@ class FusedCollective(TorchCollective):
         self.last_nonfinite = vals[OUT_NONFINITE]
         self.last_rho = vals[OUT_RHO]
         self.last_dp = (vals[OUT_DP_CLIPPED], vals[OUT_DP_NORM_SUM])
+        self.last_q = (vals[OUT_Q_ERR_SQ], vals[OUT_Q_NORM_SQ])
         return vals
 
     # -- operators ----------------------------------------------------------------------
     @torch.no_grad()
-    def fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None):
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp)
+    def fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
+                compress: Optional[QuantRound] = None):
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
@@ -420,8 +482,8 @@ class FusedCollective(TorchCollective):
 
     @torch.no_grad()
     def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                trim_b: int = 0, dp: Optional[DPRound] = None):
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp)
+                trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None):
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
