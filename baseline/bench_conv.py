@@ -11,10 +11,15 @@ Each shape is timed with CUDA events around ``--iters`` back-to-back launches (d
 median of ``--reps`` such windows is reported.  FLOPs are 2 * pixels * C_out * kh * kw * C_in from the shape; the share of
 peak is against the 495 TFLOP/s dense TF32 figure of the H100 SXM data sheet (a card with a lower power limit or clock
 cannot reach it).  ``--orient row,pixel`` times both tile orientations of the kernel per shape (alternated), where the
-extension offers the choice; ``auto`` is what the convolution selects by itself.  Prints a table, the device name, power
-limit and max SM clock, then one JSON line.  Writes nothing to disk.
+extension offers the choice; ``auto`` is what the convolution selects by itself.  ``pixel`` runs the window-reuse main loop
+where the shape allows it (``conv_window_reuse``: one input box per filter column serves all three filter rows) and the
+per-tap loop elsewhere; ``pixel_pertap`` always runs the per-tap loop, so ``--orient pixel,pixel_pertap`` compares the two.
 
-    python baseline/bench_conv.py [--batch 128] [--orient auto|row|pixel|row,pixel] [--iters 200] [--reps 5]
+The ``L2->SM MB`` column is the modelled operand traffic of one launch: TMA box bytes x boxes, computed from the shape and
+the loop that runs (operand tiles x k-blocks x (activation box + weight boxes)); ``GB/s`` is that over the kernel time.
+Prints a table, the device name, power limit and max SM clock, then one JSON line.  Writes nothing to disk.
+
+    python baseline/bench_conv.py [--batch 128] [--orient auto|row|pixel|pixel_pertap|row,pixel] [--iters 200] [--reps 5]
 """
 from __future__ import annotations
 
@@ -32,7 +37,8 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 PEAK_TF32 = 495e12
-ORIENT = {"auto": -1, "row": 0, "pixel": 1}
+ORIENT = {"auto": -1, "row": 0, "pixel": 1, "pixel_pertap": 2}
+ROW_M, PIX_M, ROW_BYTES = 128, 256, 128        # output pixels per tile (row-major / pixel-major); bytes per operand row (32 fp32)
 
 # (name, kind, H_in, C_in, C_out, k, stride, pad, sites): the distinct shapes of ResNet18 on 32 x 32 inputs and how often
 # one forward (fwd, shortcut) or one backward (dgrad) runs each
@@ -68,8 +74,32 @@ def _card() -> dict:
     return out
 
 
+def _k_blocks(cin, k):
+    """k-blocks of the per-tap loops: one per (tap, 32-channel block), or 32 / cw taps per k-block when C_in <= 16 is packed."""
+    if cin <= 16 and cin % 4 == 0:
+        cw = 8 if cin <= 8 else 16
+        return -(-k * k // (32 // cw))
+    return k * k * -(-cin // 32)
+
+
+def operand_bytes(e, orient, B, Ho, Wo, cin, cout, k, stride) -> tuple:
+    """(loop that runs, modelled L2 -> shared-memory operand bytes of one launch): TMA box bytes x boxes."""
+    M = B * Ho * Wo
+    if orient < 0:
+        orient = e.conv_orientation(B, Ho, Wo, cout, stride)
+    if orient == 0:
+        bn = 32 if cout <= 32 else (64 if cout <= 64 else 128)
+        tiles = -(-M // ROW_M) * -(-cout // bn)
+        return "row", tiles * _k_blocks(cin, k) * (ROW_M + bn) * ROW_BYTES
+    tiles = -(-M // PIX_M)
+    if orient == 1 and e.conv_window_reuse(Ho, Wo, cin, cout, k, stride, 1):
+        rows = PIX_M // Wo                 # per (filter column, channel block): one (rows + k - 1)-row window + k weight boxes
+        return "window", tiles * k * -(-cin // 32) * ((rows + k - 1) * Wo + k * cout) * ROW_BYTES
+    return "pertap", tiles * _k_blocks(cin, k) * (PIX_M + cout) * ROW_BYTES
+
+
 def _case(e, kind, B, H, Ci, Co, k, s, p, dev):
-    """Inputs and a closure launching the convolution once; (closure, FLOPs of one launch, output channels)."""
+    """Inputs and a closure launching the convolution once; (closure, FLOPs of one launch, output channels, geometry)."""
     g = torch.Generator(device=dev).manual_seed(B + H + Ci + Co + k)
     Ho = (H + 2 * p - k) // s + 1
     if kind == "dgrad":                 # dy [B, H, W, Co] * rotated filter [Ci, k, k, Co] -> dx [B, H, W, Ci]
@@ -82,13 +112,14 @@ def _case(e, kind, B, H, Ci, Co, k, s, p, dev):
         stats, cin, cout, pad = torch.zeros(2 * Co, device=dev), Ci, Co, p
     flops = 2.0 * B * Ho * Ho * cout * k * k * cin
     stride = 1 if kind == "dgrad" else s
+    geom = (B, Ho, Ho, cin, cout, k, stride)
 
     def run(orient):
         if orient < 0:
             return e.conv2d_nhwc(x, w, stats, stride, pad, 1)
         return e.conv2d_nhwc(x, w, stats, stride, pad, 1, orient)
 
-    return run, flops, cout
+    return run, flops, cout, geom
 
 
 def _time(run, orient, iters) -> float:
@@ -113,7 +144,7 @@ def main(argv=None) -> dict:
         raise SystemExit("bench_conv.py measures the GPU path: no CUDA device")
     orients = [o.strip() for o in args.orient.split(",") if o.strip()]
     if any(o not in ORIENT for o in orients):
-        raise SystemExit("--orient takes auto, row, pixel")
+        raise SystemExit("--orient takes auto, row, pixel, pixel_pertap")
 
     from federated_pytorch_test_b200.ops import cuda_ops
 
@@ -123,8 +154,8 @@ def main(argv=None) -> dict:
     rows = []
     with torch.no_grad():
         for name, kind, H, Ci, Co, k, s, p, sites in SHAPES:
-            run, flops, cout = _case(e, kind, args.batch, H, Ci, Co, k, s, p, dev)
-            avail = [o for o in orients if o != "pixel" or cout in (64, 128)]   # pixel-major tiles: C_out 64 / 128 only
+            run, flops, cout, geom = _case(e, kind, args.batch, H, Ci, Co, k, s, p, dev)
+            avail = [o for o in orients if not o.startswith("pixel") or cout in (64, 128)]   # pixel-major tiles: C_out 64 / 128 only
             for o in avail:
                 for _ in range(args.warmup):
                     run(ORIENT[o])
@@ -135,17 +166,21 @@ def main(argv=None) -> dict:
                     times[o].append(_time(run, ORIENT[o], args.iters))
             for o in avail:
                 t = statistics.median(times[o])
-                rows.append({"shape": name, "kind": kind, "orient": o, "sites": sites, "us": t * 1e6,
+                loop, nbytes = operand_bytes(e, ORIENT[o], *geom)
+                rows.append({"shape": name, "kind": kind, "orient": o, "loop": loop, "sites": sites, "us": t * 1e6,
+                             "l2_sm_bytes": nbytes, "l2_sm_GBs": nbytes / t / 1e9,
                              "us_min_max": [min(times[o]) * 1e6, max(times[o]) * 1e6], "gflop": flops / 1e9,
                              "tflops": flops / t / 1e12, "share_of_peak": flops / t / PEAK_TF32})
     print("device: %s  power limit: %s  max SM clock: %s" % (card["device"], card["power_limit"], card["max_sm_clock"]))
-    print("%-26s %-8s %-6s %5s %9s %8s %7s %6s" % ("shape", "kind", "orient", "sites", "us", "GFLOP", "TFLOP/s", "peak"))
+    print("%-26s %-8s %-12s %-6s %5s %9s %8s %7s %6s %10s %7s" % ("shape", "kind", "orient", "loop", "sites", "us", "GFLOP",
+                                                                  "TFLOP/s", "peak", "L2->SM MB", "GB/s"))
     for r in rows:
-        print("%-26s %-8s %-6s %5d %9.1f %8.2f %7.1f %5.1f%%" % (r["shape"], r["kind"], r["orient"], r["sites"], r["us"],
-                                                              r["gflop"], r["tflops"], 100 * r["share_of_peak"]))
+        print("%-26s %-8s %-12s %-6s %5d %9.1f %8.2f %7.1f %5.1f%% %10.1f %7.0f" % (
+            r["shape"], r["kind"], r["orient"], r["loop"], r["sites"], r["us"], r["gflop"], r["tflops"],
+            100 * r["share_of_peak"], r["l2_sm_bytes"] / 1e6, r["l2_sm_GBs"]))
     for o in orients:
         tot = sum(r["us"] * r["sites"] for r in rows if r["orient"] == o)
-        print("  %-6s step total over the sites above: %.1f us" % (o, tot))
+        print("  %-12s step total over the sites above: %.1f us" % (o, tot))
     res = dict(card, batch=args.batch, iters=args.iters, reps=args.reps, rows=rows)
     print(json.dumps(res))
     return res

@@ -257,8 +257,13 @@ bool conv_supported(int64_t H_out, int64_t W_out, int64_t C_in, int64_t stride) 
 int64_t conv_orientation(int64_t NB, int64_t H_out, int64_t W_out, int64_t C_out, int64_t stride) {
   return fb::pick_conv_orientation((int)NB, (int)H_out, (int)W_out, (int)C_out, (int)stride);
 }
+// Whether pixel-major tiles of this shape run the window-reuse main loop (else the per-tap loop)
+bool conv_window_reuse(int64_t H_out, int64_t W_out, int64_t C_in, int64_t C_out, int64_t kh, int64_t stride, int64_t dil) {
+  return fb::conv_window_reuse((int)H_out, (int)W_out, (int)C_in, (int)C_out, (int)kh, (int)stride, (int)dil);
+}
 // x: [N,H,W,Ci] contiguous; w: [Co,kh,kw,Ci] contiguous.  Returns y [N,Ho,Wo,Co]; stats (2*Co) accumulated if given.
-// orient: -1 = chosen from the shape, 0 = row-major tiles, 1 = pixel-major tiles (C_out 64 / 128).
+// orient: -1 = chosen from the shape, 0 = row-major tiles, 1 = pixel-major tiles (C_out 64 / 128; window reuse where
+// conv_window_reuse allows it), 2 = pixel-major tiles with the per-tap main loop (A/B comparisons).
 Tensor conv2d_nhwc(Tensor x, Tensor w, c10::optional<Tensor> stats, int64_t stride, int64_t pad, int64_t dil, int64_t orient) {
   CHECK_F32_CUDA(x); CHECK_F32_CUDA(w); CHECK_CONTIG(x); CHECK_CONTIG(w);
   TORCH_CHECK(x.dim() == 4 && w.dim() == 4 && x.size(3) == w.size(3), "conv2d_nhwc: x [N,H,W,Ci], w [Co,kh,kw,Ci]");
@@ -862,6 +867,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("linear_tf32", &linear_tf32);
   m.def("conv_supported", &conv_supported);
   m.def("conv_orientation", &conv_orientation);
+  m.def("conv_window_reuse", &conv_window_reuse, py::arg("H_out"), py::arg("W_out"), py::arg("C_in"), py::arg("C_out"), py::arg("kh"),
+        py::arg("stride") = 1, py::arg("dil") = 1);
   m.def("conv2d_nhwc", &conv2d_nhwc, py::arg("x"), py::arg("w"), py::arg("stats"), py::arg("stride"), py::arg("pad"), py::arg("dil"),
         py::arg("orient") = -1);
   m.def("conv2d_nhwc_sized", &conv2d_nhwc_sized);

@@ -46,10 +46,15 @@ void linear_tf32(const float* x, const float* w, const float* bias, float* out, 
                  int ldo, int act, cudaStream_t stream);
 bool conv_geometry_supported(int H_out, int W_out, int C_in, int stride);
 // Tile orientation of the convolution kernel: ROW = 128 pixels x BLOCK_N channels (igemm_wgmma_kernel), PIXEL = 64 / 128
-// channels x 256 pixels (igemm_wgmma_pix_kernel, C_out 64 or 128); AUTO = the choice of pick_conv_orientation.
-enum { CONV_ORIENT_AUTO = -1, CONV_ORIENT_ROW = 0, CONV_ORIENT_PIXEL = 1 };
+// channels x 256 pixels (igemm_wgmma_pix_kernel, C_out 64 or 128); AUTO = the choice of pick_conv_orientation.  PIXEL runs
+// the window-reuse main loop where conv_window_reuse allows it and the per-tap loop elsewhere; PIXEL_PERTAP always runs the
+// per-tap loop (A/B tests and benchmarks).
+enum { CONV_ORIENT_AUTO = -1, CONV_ORIENT_ROW = 0, CONV_ORIENT_PIXEL = 1, CONV_ORIENT_PIXEL_PERTAP = 2 };
 // The orientation conv2d_nhwc_tf32 / conv2d_nhwc_accumulate_tf32 use by themselves for this shape (stride-1/2, no split-K).
 int pick_conv_orientation(int NB, int H_out, int W_out, int C_out, int stride);
+// Whether a pixel-major convolution of this shape runs the window-reuse main loop (one input box per filter column serves
+// all kh filter rows).
+bool conv_window_reuse(int H_out, int W_out, int C_in, int C_out, int kh, int stride, int dil);
 void conv2d_nhwc_tf32(const float* x, const float* w, float* y, float* stats, int NB, int H, int W, int C_in, int C_out,
                       int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream,
                       int orient = CONV_ORIENT_AUTO);

@@ -150,15 +150,25 @@ static void dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const
   else dispatch_tile<false>(bn, ta, tb, p, s);
 }
 
-// Pixel-major kernel (C_out = 64 / 128): 4 stages of [256 pixels | C_out weight rows] x 32 channels next to 32 KB of staging.
-template <int CO>
+// Pixel-major kernel (C_out = 64 / 128): per-tap loop: 4 stages of [256 pixels | C_out weight rows] x 32 channels next to
+// 32 KB of staging; window reuse (C_out = 64, WIN_KH = 3: 3 x 3 filters): 3 stages of [window | 3 weight boxes], 225 KB in all
+// for layer 1 of ResNet18.  At C_out = 128 only 2 stages of 84 KB fit, and that ring measured slower than the per-tap loop
+// (H100 SXM, 400 W: 44.7 against 36.6 us for layer 2 of ResNet18), so 128 channels keep the per-tap loop.
+constexpr int PIX_STAGES = 4;
+constexpr int PIX_WIN_STAGES = 3;
+constexpr int PIX_WIN_KH = 3;
+
+template <int CO, int WIN_KH>
 static void launch_pix(const CUtensorMap& ta, const CUtensorMap& tb, IgemmParams p, cudaStream_t stream) {
-  constexpr int ST = 4;
+  constexpr bool WINDOW = WIN_KH > 0;
+  static_assert(!WINDOW || CO == 64, "window reuse serves 64 output channels");
+  constexpr int ST = WINDOW ? PIX_WIN_STAGES : PIX_STAGES;
   using S = PixSmem<CO, ST>;
-  auto kernel = igemm_wgmma_pix_kernel<CO, ST>;
+  auto kernel = igemm_wgmma_pix_kernel<CO, ST, WIN_KH>;
+  const int smem = WINDOW ? S::window_total(p.win_stage_bytes) : S::TOTAL;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WINDOW ? 227 * 1024 : S::TOTAL);
     if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: cudaFuncSetAttribute(igemm_pix): ") + cudaGetErrorString(e));
     configured = true;
   }
@@ -168,7 +178,7 @@ static void launch_pix(const CUtensorMap& ta, const CUtensorMap& tb, IgemmParams
   p.tma_store = 1;
   const CUtensorMap tc = make_tmap_out(p.out, p.M, p.N, p.ldo, 32);
   const int grid = std::min(p.total_tiles, num_sms());
-  cudaError_t e = launch_pdl(kernel, dim3(grid), dim3(IG_THREADS), S::TOTAL, stream, ta, tb, tc, p);
+  cudaError_t e = launch_pdl(kernel, dim3(grid), dim3(IG_THREADS), smem, stream, ta, tb, tc, p);
   if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: igemm_pix launch: ") + cudaGetErrorString(e));
   count_launch();
 }
@@ -231,6 +241,22 @@ static bool pix_geometry_supported(int H_out, int W_out, int stride) {
   const int rows = PX_BLOCK_M / W_out;
   if (rows <= H_out ? (H_out % rows) != 0 : (rows % H_out) != 0) return false;
   return (rows <= H_out ? rows : H_out) * stride <= 256;
+}
+
+// Window reuse of the pixel-major kernel: C_out = 64, stride 1, dilation 1, 3 filter rows (the instantiated count), C_in a
+// multiple of 32 (one tap per k-block), tiles of whole rows of ONE image, image rows of whole 1024-byte swizzle atoms
+// (W_out % 8 == 0), and the stages fit in shared memory.  Returns the bytes of one stage, 0 when the per-tap loop serves it.
+static int pix_window_stage_bytes(int H_out, int W_out, int C_in, int C_out, int kh, int stride, int dil) {
+  if (C_out != 64 || stride != 1 || dil != 1 || kh != PIX_WIN_KH || C_in % IG_BLOCK_K != 0) return 0;
+  if (!pix_geometry_supported(H_out, W_out, 1) || PX_BLOCK_M / W_out > H_out || (W_out * IG_BLOCK_K * 4) % 1024 != 0) return 0;
+  const int win_rows = PX_BLOCK_M / W_out + kh - 1;
+  if (win_rows > 256) return 0;                                          // TMA box dimension
+  const int stage = (win_rows * W_out + kh * C_out) * IG_BLOCK_K * 4;
+  return PixSmem<64, PIX_WIN_STAGES>::window_total(stage) <= 227 * 1024 ? stage : 0;
+}
+
+bool conv_window_reuse(int H_out, int W_out, int C_in, int C_out, int kh, int stride, int dil) {
+  return pix_window_stage_bytes(H_out, W_out, C_in, C_out, kh, stride, dil) > 0;
 }
 
 // Pixel-major tiles for C_out 64 / 128 when the 256-pixel tiles alone come close to one per SM (the 128-pixel tiles of
@@ -305,11 +331,13 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
                            cudaStream_t stream, int accumulate, const BnEvalArgs* eval_bn, int orient) {
   if (!conv_geometry_supported(H_out, W_out, C_in, stride))
     throw std::runtime_error("fedb200: conv geometry not supported by the wgmma path");
-  const bool pix = orient == CONV_ORIENT_PIXEL;
+  const bool pix = orient == CONV_ORIENT_PIXEL || orient == CONV_ORIENT_PIXEL_PERTAP;
   if (pix && ((C_out != 64 && C_out != 128) || bias != nullptr || act != 0 || eval_bn != nullptr ||
               !pix_geometry_supported(H_out, W_out, stride) || (reinterpret_cast<uintptr_t>(y) & 15) != 0))
     throw std::runtime_error("fedb200: pixel-major convolution needs C_out 64 / 128, a plain, statistics or accumulate epilogue, "
                              "whole-row 256-pixel tiles and a 16-byte aligned output");
+  // pixel-major: the window-reuse loop wherever the geometry allows it (CONV_ORIENT_PIXEL_PERTAP keeps the per-tap loop)
+  const int win_stage = orient == CONV_ORIENT_PIXEL ? pix_window_stage_bytes(H_out, W_out, C_in, C_out, kh, stride, dil) : 0;
   const int tile_m = pix ? PX_BLOCK_M : IG_BLOCK_M;
   const int rows = tile_m / W_out;
   const int boxH = rows <= H_out ? rows : H_out;
@@ -317,7 +345,8 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
   const int M = NB * H_out * W_out;
   const int bn = pix ? C_out : pick_block_n(M, C_out);
   const int cw = pick_tap_pack(C_in);
-  CUtensorMap ta = make_tmap_nhwc(x, NB, H, W, C_in, boxN, boxH, W_out, stride, cw);
+  // window reuse: the box spans the tile's rows plus the kh - 1 halo rows the lower filter rows read
+  CUtensorMap ta = make_tmap_nhwc(x, NB, H, W, C_in, boxN, win_stage ? boxH + kh - 1 : boxH, W_out, stride, cw);
   CUtensorMap tb = make_tmap_2d(w, C_out, uint64_t(kh) * kw * C_in, uint64_t(kh) * kw * C_in, bn, cw);
   IgemmParams p{};
   p.M = M; p.N = C_out;
@@ -334,9 +363,18 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
   p.out = y; p.ldo = C_out; p.bias = bias; p.act = act; p.stats = stats;
   p.k_splits = 1; p.kb_per_split = p.num_k_blocks;
   p.accumulate = accumulate;
+  if (win_stage) {
+    p.num_k_blocks = kw * p.cblocks;          // one unit per (filter column, channel block)
+    p.kb_per_split = p.num_k_blocks;
+    p.win_rows = boxH + kh - 1;
+    p.win_a_bytes = p.win_rows * W_out * IG_BLOCK_K * 4;
+    p.win_stage_bytes = win_stage;
+    launch_pix<64, PIX_WIN_KH>(ta, tb, p, stream);
+    return;
+  }
   if (pix) {
-    if (C_out == 64) launch_pix<64>(ta, tb, p, stream);
-    else launch_pix<128>(ta, tb, p, stream);
+    if (C_out == 64) launch_pix<64, 0>(ta, tb, p, stream);
+    else launch_pix<128, 0>(ta, tb, p, stream);
     return;
   }
   if (bias == nullptr && (act == 0 || eval_bn != nullptr)) {   // bias / activation must see the complete sum

@@ -72,6 +72,11 @@ struct IgemmParams {
   float bn_eps;
   const float* residual; // [M, ldr] (NHWC, like the output) or nullptr; ldr even, 8-byte aligned
   int ldr;
+  // window reuse (igemm_wgmma_pix_kernel<CO, STAGES, WIN_KH > 0>): a k-block is one (filter column s, 32-channel block) unit
+  // whose stage is [win_rows x W_out pixels x 128 B | WIN_KH weight boxes of C_out rows x 128 B]; num_k_blocks = kw * cblocks.
+  int win_rows;          // image rows per window: tile rows + WIN_KH - 1
+  int win_a_bytes;       // win_rows * W_out * 128
+  int win_stage_bytes;   // win_a_bytes + WIN_KH * C_out * 128 (a multiple of 1024)
 };
 
 template <int BLOCK_N, int STAGES>
@@ -422,6 +427,15 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 // The [channel][pixel] fragment is transposed through 128B-swizzled 32 x 32 staging boxes into NHWC bulk tensor stores.
 // Requires k_splits == 1, no bias / activation / eval-mode BatchNorm, and a 16-byte aligned output with ldo == C_out.
 // ================================================================================================================
+//
+// Window reuse (WIN_KH = kh > 0; stride 1, dilation 1, C_in a multiple of 32, a tile = whole rows of one image, W_out * 128 B a
+// multiple of the 1024-byte swizzle atom): filter rows r and r + 1 read the same pixels one image row apart, so a k-block is one
+// (filter column s, 32-channel block) unit.  Its stage holds ONE box of tile rows + kh - 1 image rows at column shift s - pad
+// (rows above / below the image zero-filled by the TMA unit) and the kh weight boxes of taps (0, s) .. (kh - 1, s); filter
+// row r reads the window from image row r on, i.e. the wgmma B descriptor starts r * W_out * 128 B (whole swizzle atoms) later.
+// Layer 1 of ResNet18 (64 channels, 32 x 32) moves 384 KB from L2 per tile instead of 720 KB.  The host runs it for C_out = 64
+// (3 stages fit; at 128 channels 2 stages of 84 KB measured slower than the per-tap loop).
+// ================================================================================================================
 constexpr int PX_BLOCK_M = 256;     // output pixels per tile
 
 template <int CO, int STAGES>
@@ -432,23 +446,59 @@ struct PixSmem {
   static constexpr int STAGING_BYTES = 2 * 2 * 2 * 32 * 32 * 4; // per consumer warpgroup: two buffers of two 32 x 32 boxes
   static constexpr int BAR_BYTES = 2 * STAGES * 8;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + STAGING_BYTES + BAR_BYTES + 1024;  // + align slack
+  // window reuse: the stage size depends on the shape (IgemmParams::win_stage_bytes)
+  static constexpr int window_total(int stage_bytes) { return STAGES * stage_bytes + STAGING_BYTES + BAR_BYTES + 1024; }
 };
 
-template <int CO, int STAGES>
+// Window-reuse producer (one thread): per tile, per unit (s, cb): one 4-D box {32, W_out, win_rows, 1} of the input at
+// (cb * 32, s - pad, h0 - pad, img) and KH 2-D weight boxes [C_out x 32] of taps (r, s), r = 0 .. KH - 1.
+template <int CO, int STAGES, int KH>
+__device__ __forceinline__ void igemm_produce_window(const IgemmParams& p, uint8_t* tiles, uint64_t* full_bar, uint64_t* empty_bar,
+                                                     const CUtensorMap* tmap_a, const CUtensorMap* tmap_b) {
+  constexpr uint32_t W_BOX = CO * IG_BLOCK_K * 4;
+  const uint32_t stage_bytes = uint32_t(p.win_stage_bytes);
+  int s = 0;
+  uint32_t ph = 0;
+  for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+    const TileCoord c = decode_tile(p, t, PX_BLOCK_M, CO);
+    const int img = c.m0 / p.HW_out;
+    const int h0 = (c.m0 - img * p.HW_out) / p.W_out - p.pad;
+    for (int sx = 0; sx < p.taps_w; ++sx) {
+      for (int cb = 0; cb < p.cblocks; ++cb) {
+        mbar_wait(&empty_bar[s], ph ^ 1);
+        uint8_t* a_dst = tiles + s * stage_bytes;
+        uint8_t* b_dst = a_dst + p.win_a_bytes;
+        mbar_arrive_expect_tx(&full_bar[s], stage_bytes);
+        tma_load_4d(a_dst, tmap_a, &full_bar[s], cb * IG_BLOCK_K, sx - p.pad, h0, img);
+#pragma unroll
+        for (int r = 0; r < KH; ++r)
+          tma_load_2d(b_dst + r * W_BOX, tmap_b, &full_bar[s], (r * p.taps_w + sx) * p.b_cols_per_tap + cb * IG_BLOCK_K, 0);
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+    }
+  }
+}
+
+// WIN_KH = 0: the per-tap main loop; WIN_KH = kh > 0: window reuse for filters of kh rows (a compile-time count, so the
+// kh x 4 MMAs of a unit are one unrolled run that ptxas issues back to back).
+template <int CO, int STAGES, int WIN_KH>
 __global__ void __launch_bounds__(IG_THREADS, 1)
 igemm_wgmma_pix_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const __grid_constant__ CUtensorMap tmap_c, const IgemmParams p) {
   using S = PixSmem<CO, STAGES>;
+  constexpr bool WINDOW = WIN_KH > 0;
   static_assert(CO == 64 || CO == 128, "pixel-major tiles serve 64 or 128 output channels");
-  static_assert(S::TOTAL <= 227 * 1024, "shared memory budget");
+  static_assert(WINDOW || S::TOTAL <= 227 * 1024, "shared memory budget");   // window reuse: checked by the host
   static_assert(S::STAGE_BYTES % 1024 == 0, "stages must keep the 1024-byte swizzle alignment");
   constexpr bool PINGPONG = CO == 64;
+  // bytes per ring stage; window reuse: [window | kh weight boxes]
+  const uint32_t stage_bytes = WINDOW ? uint32_t(p.win_stage_bytes) : uint32_t(S::STAGE_BYTES);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* tiles = smem;
-  float* staging = reinterpret_cast<float*>(smem + STAGES * S::STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES + S::STAGING_BYTES);
+  float* staging = reinterpret_cast<float*>(smem + STAGES * stage_bytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes + S::STAGING_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int wg = threadIdx.x >> 7;
@@ -470,8 +520,10 @@ igemm_wgmma_pix_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
-    if (threadIdx.x == 0)
-      igemm_produce<PX_BLOCK_M, CO, STAGES, S::A_BYTES, S::STAGE_BYTES>(p, tiles, full_bar, empty_bar, &tmap_a, &tmap_b);
+    if (threadIdx.x == 0) {
+      if constexpr (WINDOW) igemm_produce_window<CO, STAGES, WIN_KH>(p, tiles, full_bar, empty_bar, &tmap_a, &tmap_b);
+      else igemm_produce<PX_BLOCK_M, CO, STAGES, S::A_BYTES, S::STAGE_BYTES>(p, tiles, full_bar, empty_bar, &tmap_a, &tmap_b);
+    }
     return;
   }
   setmaxnreg_inc<232>();
@@ -482,7 +534,8 @@ igemm_wgmma_pix_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   const uint32_t cwq = (p.cw == 8 || p.cw == 16) ? uint32_t(p.cw) : uint32_t(IG_BLOCK_K);
   const uint32_t mma_per_sub = cwq / IG_MMA_K;
   // wgmma A = the weight rows of this warpgroup's channels, wgmma B = the 256 pixel rows
-  const uint64_t adesc0 = make_kmajor_desc(smem_u32(tiles) + uint32_t(S::A_BYTES) + uint32_t(ch_wg) * cwq * 4u, cwq * 4u);
+  const uint32_t a_bytes = WINDOW ? uint32_t(p.win_a_bytes) : uint32_t(S::A_BYTES);
+  const uint64_t adesc0 = make_kmajor_desc(smem_u32(tiles) + a_bytes + uint32_t(ch_wg) * cwq * 4u, cwq * 4u);
   const uint64_t bdesc0 = make_kmajor_desc(smem_u32(tiles), cwq * 4u);
   uint32_t a_off[IG_BLOCK_K / IG_MMA_K], b_off[IG_BLOCK_K / IG_MMA_K];
 #pragma unroll
@@ -500,23 +553,36 @@ igemm_wgmma_pix_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   const int step = PINGPONG ? 2 : 1;
   for (int j = PINGPONG ? g : 0, t = blockIdx.x + j * gridDim.x; t < p.total_tiles; j += step, t += step * gridDim.x) {
     const TileCoord c = decode_tile(p, t, PX_BLOCK_M, CO);
-    // ring position of this tile's first k-block: every tile has num_k_blocks of them (no split-K)
+    // ring position of this tile's first k-block (window reuse: unit): every tile has num_k_blocks of them (no split-K)
     const uint32_t pos = uint32_t(j) * uint32_t(c.kb_count);
     int s = int(pos % STAGES);
     uint32_t ph = (pos / STAGES) & 1u;
     // Ping-pong: the main loops take turns (named barrier 3 + g: "warpgroup g may start").  A full-barrier parity wait
     // only tells the last two fills of a stage apart, so a warpgroup may wait on its k-blocks only once every k-block
-    // before them has been waited on, i.e. once the other warpgroup's main loop has passed its last wait.
+    // before them has been waited on, i.e. once the other warpgroup's main loop has passed its last wait.  This holds
+    // for any number of stages: the producer refills a stage only after the one consumer of its previous fill released it.
     if (PINGPONG && j > 0) named_bar_sync(3 + uint32_t(g), 256);
     int prev = -1;
     for (int i = 0; i < c.kb_count; ++i) {
       mbar_wait(&full_bar[s], ph);
-      const uint64_t so = uint64_t(uint32_t(s) * uint32_t(S::STAGE_BYTES >> 4));
+      const uint64_t so = uint64_t(uint32_t(s) * (stage_bytes >> 4));
       wgmma_fence();
       wgmma_fence_acc(acc);
+      if constexpr (WINDOW) {
+        // filter row r: weight box r, and the window from image row r on (W_out * 128 B per row, in 16-byte units)
+        const uint32_t px_row = uint32_t(p.W_out) * 8u;
 #pragma unroll
-      for (int k = 0; k < IG_BLOCK_K / IG_MMA_K; ++k)
-        wgmma_tf32_n256(acc, adesc0 + so + a_off[k], bdesc0 + so + b_off[k], (i > 0 || k > 0) ? 1u : 0u);
+        for (int r = 0; r < WIN_KH; ++r) {
+          const uint64_t ao = so + uint32_t(r) * uint32_t(CO * 8), bo = so + uint32_t(r) * px_row;
+#pragma unroll
+          for (int k = 0; k < IG_BLOCK_K / IG_MMA_K; ++k)
+            wgmma_tf32_n256(acc, adesc0 + ao + a_off[k], bdesc0 + bo + b_off[k], (i > 0 || r > 0 || k > 0) ? 1u : 0u);
+        }
+      } else {
+#pragma unroll
+        for (int k = 0; k < IG_BLOCK_K / IG_MMA_K; ++k)
+          wgmma_tf32_n256(acc, adesc0 + so + a_off[k], bdesc0 + so + b_off[k], (i > 0 || k > 0) ? 1u : 0u);
+      }
       wgmma_commit();
       wgmma_fence_acc(acc);
       wgmma_wait<1>();

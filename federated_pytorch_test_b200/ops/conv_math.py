@@ -210,3 +210,39 @@ def shuffle_store_oracle(y_packed: torch.Tensor) -> torch.Tensor:
             chunk = rows[row0: row0 + nrow, pc: pc + 32].reshape(nrow // Wo, Wo, 32)
             view5[hon0: hon0 + nrow // Wo, ph, :, pw, ci0: ci0 + 32] = chunk
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Window reuse (csrc/igemm_wgmma.cuh: igemm_wgmma_pix_kernel with WIN_KH > 0): for a stride-1, dilation-1 convolution a
+# 256-pixel tile of `rows` whole output rows of one image (first row h0) is
+#     y_tile = sum_{s, cb} sum_{r < kh} window_{s,cb}[r : r + rows] @ W[:, r, s, cb * 32 : cb * 32 + 32]^T
+# where window_{s,cb} is ONE box of rows + kh - 1 input rows starting at h0 - pad, columns shifted by s - pad and channels
+# [cb * 32, cb * 32 + 32), zero outside the image (the TMA zero fill): filter row r reads the same box from row r on.
+# ------------------------------------------------------------------------------------------------
+def window_reuse_conv_oracle(x_nhwc: torch.Tensor, w_krsc: torch.Tensor, pad: int, rows: int) -> torch.Tensor:
+    """Stride-1 convolution of ``x [N, H, W, Ci]`` with ``w [Co, kh, kw, Ci]`` evaluated tile by tile and window by window
+    exactly as the window-reuse kernel accumulates it; ``rows`` output rows per tile (must divide H_out)."""
+    N, H, W, Ci = x_nhwc.shape
+    Co, kh, kw, _ = w_krsc.shape
+    Ho, Wo = H + 2 * pad - kh + 1, W + 2 * pad - kw + 1
+    assert Ho % rows == 0, "a tile is whole output rows of one image"
+    win_rows = rows + kh - 1
+    y = x_nhwc.new_zeros(N, Ho, Wo, Co)
+    for n in range(N):
+        for h0 in range(0, Ho, rows):
+            acc = x_nhwc.new_zeros(rows * Wo, Co)
+            for s in range(kw):
+                for c0 in range(0, Ci, 32):
+                    c1 = min(c0 + 32, Ci)
+                    window = x_nhwc.new_zeros(win_rows, Wo, c1 - c0)           # out-of-image rows / columns stay zero
+                    for i in range(win_rows):
+                        hi = h0 - pad + i
+                        if not 0 <= hi < H:
+                            continue
+                        w_lo, w_hi = max(0, s - pad), min(W, s - pad + Wo)       # input columns inside the image
+                        if w_lo < w_hi:
+                            window[i, w_lo - (s - pad): w_hi - (s - pad)] = x_nhwc[n, hi, w_lo:w_hi, c0:c1]
+                    for r in range(kh):
+                        acc = acc + window[r: r + rows].reshape(rows * Wo, c1 - c0) @ w_krsc[:, r, s, c0:c1].t()
+            y[n, h0: h0 + rows] = acc.view(rows, Wo, Co)
+    return y
