@@ -21,7 +21,10 @@ What differs from the reference by construction:
   (replica, block) as a CUDA graph and replayed (``graphs=True``), which removes
   the ~400 eager launches and the per-step host sync of the reference;
 * the diagnostics loss is accumulated on the device; it is read back once per
-  round (or per minibatch only when ``be_verbose``).
+  round (or per minibatch only when ``be_verbose``);
+* with client sampling, replicas outside the round's participant set
+  (``Strategy.participates``) take no step: their loaders, optimizer state and
+  ``images_seen`` do not move, and the aggregation writes the new model into them.
 
 A *task* (``api/*.py``) supplies models, data, loss, schedule and evaluation.
 """
@@ -366,21 +369,23 @@ class Engine:
         """One pass over the local replicas' shards.  One replica: plain loop.  Several co-resident replicas (K > #GPUs;
         the reference's default K = 10): minibatch-major order with every replica on its own CUDA stream, so replica
         j+1's kernels are queued while replica j's run and small layers of different replicas overlap on the SMs
-        (SURVEY §2.8).  Replicas are independent between aggregations, so the order does not change any result."""
+        (SURVEY §2.8).  Replicas are independent between aggregations, so the order does not change any result.
+        Replicas that sit out the round (client sampling) are skipped: their loaders are not even iterated."""
         cfg = self.cfg
         reps = self.replicas
+        active = [i for i in range(len(reps)) if self.strategy.participates(i)]
         multi = (cfg.streams and len(reps) > 1 and self.topo.device.type == "cuda" and not cfg.be_verbose)
         if not multi:
-            for i_rep, rep in enumerate(reps):
-                self._run_shard(rep, self.optimizers[i_rep], visit, self.strategy.penalty(i_rep), nloop, epoch, N)
+            for i_rep in active:
+                self._run_shard(reps[i_rep], self.optimizers[i_rep], visit, self.strategy.penalty(i_rep), nloop, epoch, N)
                 if self.stop_requested:
                     return
             return
         cur = torch.cuda.current_stream(self.topo.device)
-        iters = [iter(enumerate(self.task.batches(rep, visit, epoch))) for rep in reps]
+        iters = {i: iter(enumerate(self.task.batches(reps[i], visit, epoch))) for i in active}
         pens = [self.strategy.penalty(i) for i in range(len(reps))]
         running = [None] * len(reps)
-        live = list(range(len(reps)))
+        live = list(active)               # unequal shards: a replica leaves the list when its shard is exhausted
         for i in live:
             self._stream_of(i).wait_stream(cur)
         while live and not self.stop_requested:
@@ -398,10 +403,9 @@ class Engine:
                 if self.stop_requested:
                     break
             live = nxt
-        for i in range(len(reps)):
+        for i in active:
             cur.wait_stream(self._stream_of(i))
-        for i, rep in enumerate(reps):
-            rep.running_loss = running[i]
+            reps[i].running_loss = running[i]
 
     def _one_step(self, rep: Replica, opt, visit: Visit, batch, pen: Penalty, running, i: int, epoch: int, nloop: int, N: int):
         cfg, task = self.cfg, self.task
@@ -444,6 +448,10 @@ class Engine:
         # (only a collective with asynchronous entry points actually defers: FusedCollective; the others answer "done")
         defer = (cfg.deferred_rounds and not cfg.check_results and not cfg.be_verbose
                  and not cfg.resume_path and env != "0" and (env == "1" or self.topo.world_size <= 4))
+        if self._pending_round is not None:
+            # the previous round is still deferred when no local replica took a step since (all of them sat out a sampled
+            # round): finish it here, before its record is overwritten
+            self._finish_round()
         if self.attack is not None:
             self.attack(self)
         with nvtx_range("fedb200:aggregate"), self.timers.phase("aggregate"):

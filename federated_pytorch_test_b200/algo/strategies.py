@@ -13,6 +13,10 @@ object driven by the block-coordinate engine:
 All vector work is delegated to a collective (``parallel.collective``), i.e. to
 one fused NVLink kernel per aggregation on the GPU.
 
+With client sampling (``FedAvg`` / ``FedOpt`` with ``client_n``) only the round's
+participants train: the engine asks ``strat.participates(i)`` before the round's
+steps and skips the others.
+
 Preserved reference behaviour (SURVEY §2.12): ``z`` (and ``y``) start at 0 for
 every block visit (Q6); FedProx/ADMM never write ``z`` back (Q7); ``rho`` is an
 ``[L,3]`` table of which only column 0 is used, shared by all workers and
@@ -23,7 +27,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import torch
 
@@ -59,6 +63,10 @@ class Strategy:
 
     def penalty(self, i: int) -> Penalty:
         return Penalty()
+
+    def participates(self, i: int) -> bool:
+        """Whether local replica ``i`` trains in the current round (every replica, unless the strategy samples clients)."""
+        return True
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         raise NotImplementedError
@@ -114,15 +122,22 @@ class FedAvg(Strategy):
     collective.  As with DP, ``z`` starts each block visit as the replicas' common value instead of 0 (Q6), so the
     ``dual`` of the first round of a visit differs from plain FedAvg.  The round metrics gain ``q_bits``, ``q_bytes``
     (payload bytes per worker: ``N bits / 8 + 4 ceil(N / 128)``) and ``q_rel_err``
-    (``sqrt(sum_k ||u_k - q_k s_k||^2 / sum_k ||u_k||^2)``)."""
+    (``sqrt(sum_k ||u_k - q_k s_k||^2 / sum_k ||u_k||^2)``).
+
+    ``client_n`` (the K workers' sample counts) makes it sample-weighted FedAvg with client sampling (McMahan et al.
+    2017, Algorithm 1; ``algo/sampling.py``): sampled round ``t`` (``t`` counts the sampled rounds of the run and lives in
+    device memory) trains only its ``clients_per_round`` participants (0 = all K), drawn uniformly from ``(seed, t)``, and
+    ``z <- sum_{k in P} w_k x_k`` with ``w_k = n_k / sum_{j in P} n_j``, written back into every replica, participant or
+    not.  Workers that sit out are never read.  A round is one launch on the fused collective.  The round metrics gain
+    ``participants`` (the worker ids) and ``participant_samples`` (``sum_{k in P} n_k``)."""
 
     name = "fedavg"
     write_back = True
 
     def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1, dp_clip: float = 0.0,
                  dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
-                 compress_ef: bool = False):
-        from ..config import check_aggregator, check_compress, check_dp, trim_count
+                 compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None):
+        from ..config import check_aggregator, check_compress, check_dp, check_sampling, trim_count
 
         super().__init__(collective, topo)
         check_aggregator(aggregator, trim_fraction, topo.K)
@@ -155,6 +170,23 @@ class FedAvg(Strategy):
             self._q_restored: Dict[int, torch.Tensor] = {}     # error feedback read from a resume record, installed at the visit
             if hasattr(collective, "warm_compress"):
                 collective.warm_compress = self.q_bits
+        self.sampled = client_n is not None
+        self.samp_rounds = 0                   # host mirror of the device round counter samp_t
+        if self.sampled:
+            from .sampling import sample_key
+
+            check_sampling(clients_per_round, topo.K, "dirichlet", aggregator, dp_clip, compress_bits)
+            if len(client_n) != topo.K or min(client_n) < 1:
+                raise ValueError("client_n needs one sample count >= 1 per worker, got %r" % (list(client_n),))
+            self.samp_S = int(clients_per_round) or topo.K
+            self.samp_key = sample_key(seed)
+            self.client_n = [int(v) for v in client_n]
+            self.samp_t = torch.zeros(1, dtype=torch.int64, device=topo.device)
+            self.samp_n = torch.tensor(self.client_n, dtype=torch.int32, device=topo.device)
+            self._round_ids = (-1, None)                          # (t, participants of sampled round t)
+            self._last_ids: List[int] = []
+            if hasattr(collective, "warm_sample"):
+                collective.warm_sample = True
 
     def begin_block(self, ci: int, N: int, xs: List[torch.Tensor]) -> None:
         super().begin_block(ci, N, xs)
@@ -166,6 +198,52 @@ class FedAvg(Strategy):
                 self.q_ef[ci] = [torch.zeros_like(x) for x in xs]
                 if ci in self._q_restored:
                     self._install_ef(ci, self._q_restored.pop(ci))
+
+    # -- client sampling -------------------------------------------------------------------------------------------------
+    def round_participants(self) -> List[int]:
+        """The workers of the round in progress (all K without sampling)."""
+        if not self.sampled:
+            return list(range(self.topo.K))
+        if self._round_ids[0] != self.samp_rounds:
+            from .sampling import participants
+
+            self._round_ids = (self.samp_rounds, [int(k) for k in participants(self.samp_key, self.samp_rounds,
+                                                                                self.topo.K, self.samp_S)])
+        return self._round_ids[1]
+
+    def participates(self, i: int) -> bool:
+        return not self.sampled or self.topo.local_workers[i] in self.round_participants()
+
+    def _samp_kw(self) -> Dict[str, object]:
+        """The sampling argument of the aggregation (which advances the round counter)."""
+        if not self.sampled:
+            return {}
+        from ..parallel.collective import SampleRound
+
+        self._last_ids = self.round_participants()
+        self.samp_rounds += 1
+        return {"sample": SampleRound(self.samp_S, self.samp_key, self.samp_t, self.samp_n)}
+
+    def _with_samp(self, metrics: Dict[str, float]) -> Dict[str, float]:
+        if self.sampled:
+            metrics.update(participants=list(self._last_ids),
+                           participant_samples=float(sum(self.client_n[k] for k in self._last_ids)))
+        return metrics
+
+    def _samp_state(self) -> Dict[str, object]:
+        if not self.sampled:
+            return {}
+        return {"sample": (self.samp_S, self.samp_key, tuple(self.client_n)), "samp_t": self.samp_rounds}
+
+    def _check_samp_state(self, st: Dict[str, object]) -> None:
+        got = tuple(st["sample"]) if st.get("sample") is not None else None
+        want = self._samp_state().get("sample")
+        if got != want:
+            raise ValueError("resume record holds client-sampling settings (clients_per_round, key, shard sizes) %r, this "
+                             "run uses %r" % (got, want))
+        if self.sampled:
+            self.samp_rounds = int(st["samp_t"])
+            self.samp_t.fill_(self.samp_rounds)
 
     # -- compressed updates -------------------------------------------------------------------------------------------
     def _q_kw(self) -> Dict[str, object]:
@@ -252,15 +330,16 @@ class FedAvg(Strategy):
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         if self.aggregator == "mean":
-            dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw(), **self._q_kw())
+            dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw(), **self._q_kw(),
+                                        **self._samp_kw())
         else:
             dual_sq = self.coll.robust_(self.xs, self.z, self.aggregator, self.trim_b)
-        return self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))
+        return self._with_samp(self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             if self.aggregator == "mean":
-                self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw(), **self._q_kw())
+                self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw(), **self._q_kw(), **self._samp_kw())
             else:
                 self.coll.launch_robust_(self.xs, self.z, self.aggregator, self.trim_b)
             return ("pending", self.N)
@@ -269,7 +348,8 @@ class FedAvg(Strategy):
     def aggregate_end(self, token) -> Dict[str, float]:
         if token[0] == "done":
             return token[1]
-        return self._with_q(self._with_dp({"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]}))
+        return self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]})))
 
     def _robust_state(self) -> Dict[str, object]:
         return {} if self.aggregator == "mean" else {"aggregator": self.aggregator, "trim_b": self.trim_b}
@@ -296,12 +376,13 @@ class FedAvg(Strategy):
             self.dp_t.fill_(self.dp_rounds)
 
     def state(self) -> Dict[str, object]:
-        return {"z": self.z, **self._robust_state(), **self._dp_state(), **self._q_state()}
+        return {"z": self.z, **self._robust_state(), **self._dp_state(), **self._q_state(), **self._samp_state()}
 
     def load_state(self, st: Dict[str, object]) -> None:
         self._check_robust_state(st)
         self._check_dp_state(st)
         self._check_q_state(st)
+        self._check_samp_state(st)
         self.z.copy_(st["z"].to(self.z.device))
 
 
@@ -323,19 +404,21 @@ class FedOpt(FedAvg):
     (``dp_clip > 0``) the noised mean of the clipped workers replaces the mean in ``d`` (DP-FedAdam etc.: post-processing),
     and the server model at the start of a visit is the replicas' common value, copied locally (no launch).  With
     compressed updates (``compress_bits``) ``d`` is the dequantized mean update itself (FedPAQ with a server optimizer),
-    and the server model at the start of a visit is again the replicas' common value."""
+    and the server model at the start of a visit is again the replicas' common value.  With client sampling
+    (``client_n``) the participants' sample-weighted mean replaces the mean in ``d``; the server model at the start of a
+    visit stays the unsampled mean of the (equal) replicas and does not advance the sampling counter."""
 
     name = "fedopt"
 
     def __init__(self, collective, topo, kind: str = "adam", lr: float = 0.0, momentum: float = 0.9, beta1: float = 0.9,
                  beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1,
                  dp_clip: float = 0.0, dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
-                 compress_ef: bool = False):
+                 compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None):
         from ..config import check_server_opt
         from ..parallel.collective import FEDOPT_KINDS
 
         super().__init__(collective, topo, aggregator, trim_fraction, dp_clip, dp_noise, dp_delta, seed, compress_bits,
-                         compress_ef)
+                         compress_ef, clients_per_round, client_n)
         if kind not in FEDOPT_KINDS:
             raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
         check_server_opt(kind, lr, momentum, beta1, beta2, tau)
@@ -372,13 +455,13 @@ class FedOpt(FedAvg):
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
-                                    **self._q_kw())
-        return self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))
+                                    **self._q_kw(), **self._samp_kw())
+        return self._with_samp(self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
-                                     **self._q_kw())
+                                     **self._q_kw(), **self._samp_kw())
             return ("pending", self.N)
         return ("done", self.aggregate(nadmm))
 
@@ -390,7 +473,7 @@ class FedOpt(FedAvg):
         ms.update(self.ms)
         vs.update(self.vs)
         return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state(), **self._dp_state(),
-                **self._q_state()}
+                **self._q_state(), **self._samp_state()}
 
     def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
         self.ms[ci].copy_(m.to(self.ms[ci].device))
@@ -403,6 +486,7 @@ class FedOpt(FedAvg):
         self._check_robust_state(st)
         self._check_dp_state(st)
         self._check_q_state(st)
+        self._check_samp_state(st)
         self.z.copy_(st["z"].to(self.z.device))
         vs = st.get("v") or {}
         for ci, m in (st.get("m") or {}).items():

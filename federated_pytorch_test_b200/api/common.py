@@ -16,8 +16,9 @@ import torch.nn as nn
 
 from .. import models
 from ..algo.engine import Engine, EngineConfig, Replica, Task, Visit
-from ..config import CommonConfig
-from ..data.cifar import CifarData, ShardLoader, augment_key, shard_ranges, worker_norm
+from ..config import CommonConfig, check_partition
+from ..data.cifar import (CifarData, ShardLoader, augment_key, class_histogram, dirichlet_shards, shard_ranges,
+                          worker_norm)
 from ..ops import functional as FX
 from ..ops import losses
 from ..parallel.collective import make_collective
@@ -30,6 +31,12 @@ _MODEL_FACTORIES = {
     "Net": models.Net, "Net1": models.Net1, "Net2": models.Net2,
     "ResNet18": models.ResNet18, "ResNet9": models.ResNet9,
 }
+
+
+def require_iid(cfg: CommonConfig, driver: str) -> None:
+    """The unsupervised drivers (VAE, VAE-CL, CPC) train without labels and accept only the default split."""
+    if getattr(cfg, "partition", "iid") != "iid":
+        raise ValueError("%s supports only partition 'iid', got partition %r" % (driver, cfg.partition))
 
 
 def setup_runtime(cfg: CommonConfig) -> Tuple[Topology, object]:
@@ -78,7 +85,17 @@ class ClassifierTask(Task):
         self.model_name = name
         self.factory = _MODEL_FACTORIES[name]
         self.data = load_cifar(cfg, topo.device)
-        self.shards = shard_ranges(cfg.K, self.data.train_images.shape[0], drop_last_sample=not cfg.fix_shard_off_by_one)
+        partition = getattr(cfg, "partition", "iid")
+        check_partition(partition, getattr(cfg, "dirichlet_alpha", 0.5))
+        self.partition_row = None              # the metrics row describing a non-default split
+        if partition == "dirichlet":
+            self.shards = [torch.from_numpy(s) for s in dirichlet_shards(
+                self.data.train_labels, cfg.K, cfg.dirichlet_alpha, cfg.data_seed, cfg.default_batch)]
+            self.partition_row = dict(kind="partition", partition=partition, alpha=float(cfg.dirichlet_alpha),
+                                      shard_sizes=self.shard_sizes(),
+                                      class_histogram=class_histogram(self.data.train_labels, self.shards))
+        else:
+            self.shards = shard_ranges(cfg.K, self.data.train_images.shape[0], drop_last_sample=not cfg.fix_shard_off_by_one)
         self.channels_last = bool(cfg.fast and topo.device.type == "cuda" and name.startswith("ResNet"))
         self._loaders: Dict[int, ShardLoader] = {}
         self._test_loaders: Dict[int, ShardLoader] = {}
@@ -93,6 +110,10 @@ class ClassifierTask(Task):
             for idx, (pname, p) in enumerate(probe.named_parameters()):
                 if p.dim() == 2:
                     self.dense_param_ids.update((idx, idx + 1))
+
+    def shard_sizes(self) -> List[int]:
+        """``n_k``: the number of training samples of every worker's shard."""
+        return [len(s) for s in self.shards]
 
     # -- replicas -------------------------------------------------------------
     def build_replica(self, ck: int, device: torch.device, allocator) -> Replica:
@@ -231,6 +252,8 @@ def run_engine(cfg: CommonConfig, task: Task, topo: Topology, coll, strategy, ec
     metrics = MetricsLog(cfg.metrics_path or None)
     engine = Engine(task, topo, strategy, coll, ecfg or engine_config(cfg), log=log, metrics=metrics)
     engine.attack = attack
+    if getattr(task, "partition_row", None) and topo.is_root:
+        metrics.write(task.partition_row)
     if cfg.resume:
         ckpt.load_resume(cfg.resume, engine)
     engine.run()

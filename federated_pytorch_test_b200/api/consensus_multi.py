@@ -4,6 +4,9 @@ Reference: /root/reference/src/consensus_multi.py (x/z/y updates, spectral penal
 ``bb_period_T`` rounds, primal/dual residuals).  z-update + dual ascent + both residuals
 are one fused kernel; the BB rule is replayed deterministically on every rank from six
 dot products per worker (SURVEY §7.3(2)).
+
+``--partition dirichlet`` gives the workers label-skewed shards of unequal size; the z-update stays the unweighted
+average of the K workers, as in the reference (sample-count weights and client sampling are ``federated_multi``'s).
 """
 from __future__ import annotations
 

@@ -20,24 +20,35 @@ mean (``algo/privacy.py``).  The root logs ``dp: ...`` lines with the planned an
 optimizer): its block update ``x_k - z`` as stochastically rounded codes with one scale per 128 coordinates, optionally
 with error feedback (``algo/compress.py``); the new model is still broadcast in fp32.  Round metrics gain ``q_bits``,
 ``q_bytes`` and ``q_rel_err``.
+
+``--clients_per_round S`` trains and averages a uniform random subset of S of the K workers in every round (FedAvg's
+partial participation, with or without a server optimizer); ``--partition dirichlet --dirichlet_alpha a`` splits the
+training set with Dirichlet label skew into unequal shards.  Either one makes the aggregate the sample-weighted mean
+``sum_{k in P} n_k x_k / sum_{k in P} n_k`` of the round's participants P (all K without ``--clients_per_round``), one
+fused launch that reads only the participants (``algo/sampling.py``); workers that sit out take no step and receive the
+new model.  Round metrics gain ``participants`` and ``participant_samples``; the root writes a ``partition`` row with the
+shard sizes and per-worker class counts.
 """
 from __future__ import annotations
 
 from ..algo.byzantine import ByzantineAttack
 from ..algo.privacy import dp_line
 from ..algo.strategies import FedAvg, FedOpt
-from ..config import FederatedConfig, parse_config
+from ..config import FederatedConfig, parse_config, sampled_rounds
 from . import common
 
 Config = FederatedConfig
 
 
-def make_strategy(cfg: Config, coll, topo):
+def make_strategy(cfg: Config, coll, topo, client_n=None):
+    """The run's strategy.  ``client_n``: the workers' sample counts, which weight sampled rounds (default: equal)."""
     robust = {} if cfg.aggregator == "mean" else dict(aggregator=cfg.aggregator, trim_fraction=cfg.trim_fraction)
     if cfg.dp_clip > 0.0:
         robust.update(dp_clip=cfg.dp_clip, dp_noise=cfg.dp_noise, dp_delta=cfg.dp_delta, seed=cfg.seed)
     if cfg.compress_bits:
         robust.update(compress_bits=cfg.compress_bits, compress_ef=cfg.compress_ef, seed=cfg.seed)
+    if sampled_rounds(cfg.clients_per_round, cfg.K, cfg.partition):
+        robust.update(clients_per_round=cfg.clients_per_round, client_n=client_n or [1] * cfg.K, seed=cfg.seed)
     if cfg.server_opt == "none":
         return FedAvg(coll, topo, **robust)
     return FedOpt(coll, topo, cfg.server_opt, cfg.server_lr, cfg.server_momentum, cfg.server_beta1, cfg.server_beta2,
@@ -54,7 +65,7 @@ def make_attack(cfg: Config):
 def run(cfg: Config, log=print):
     topo, coll = common.setup_runtime(cfg)
     task = common.ClassifierTask(cfg, topo, cfg.lambda1, cfg.lambda2)
-    strategy = make_strategy(cfg, coll, topo)
+    strategy = make_strategy(cfg, coll, topo, task.shard_sizes())
     dp_log = strategy.dp and topo.is_root
     if dp_log:
         planned = cfg.Nloop * len(list(task.visits(0))) * cfg.Nadmm * cfg.Nepoch

@@ -4,6 +4,9 @@ Reference: /root/reference/src/fedprox_multi.py (local loss + mu/2 ||x - z||^2 w
 mu = ``admm_rho0`` = 1.0, z = mean, no write-back, primal/dual residuals).  The proximal
 gradient is closed-form inside the optimizer kernel; the aggregation kernel also returns
 both residual norms.
+
+``--partition dirichlet`` gives the workers label-skewed shards of unequal size; z stays the unweighted mean of the K
+workers, as in the reference (sample-count weights and client sampling are ``federated_multi``'s).
 """
 from __future__ import annotations
 

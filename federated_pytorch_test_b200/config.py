@@ -61,6 +61,10 @@ class CommonConfig:
     resume: str = ""                # path of a true-resume record written by this framework: re-enter the schedule there
     resume_out: str = ""            # write the true-resume record here after every aggregation round ('' = never)
     streams: bool = True            # co-resident replicas (K > #GPUs) step concurrently on their own CUDA streams
+    # training-set split over the K workers (classifier drivers): 'iid' = equal contiguous shards (the reference) |
+    # 'dirichlet' = label skew, each class split in proportions p ~ Dir(dirichlet_alpha 1_K) (data/cifar.py: dirichlet_shards)
+    partition: str = "iid"
+    dirichlet_alpha: float = 0.5    # smaller = more skewed
 
 
 @dataclass
@@ -133,6 +137,40 @@ def check_dp(dp_clip: float, dp_noise: float, dp_delta: float, aggregator: str) 
                          % (aggregator,))
 
 
+PARTITIONS = ("iid", "dirichlet")
+
+
+def check_partition(partition: str, dirichlet_alpha: float) -> None:
+    """Raise ``ValueError`` unless the training-set split of :class:`CommonConfig` is valid."""
+    if partition not in PARTITIONS:
+        raise ValueError("partition must be one of %s, got %r" % (", ".join(PARTITIONS), partition))
+    if not (math.isfinite(dirichlet_alpha) and dirichlet_alpha > 0.0):
+        raise ValueError("dirichlet_alpha must be finite and > 0, got %r" % (dirichlet_alpha,))
+
+
+def sampled_rounds(clients_per_round: int, K: int, partition: str) -> bool:
+    """Whether federated averaging runs its sampled, sample-weighted rounds: a strict subset of the workers per round,
+    or unequal (Dirichlet) shards, whose sample counts weight the average."""
+    return 0 < clients_per_round < K or partition == "dirichlet"
+
+
+def check_sampling(clients_per_round: int, K: int, partition: str, aggregator: str, dp_clip: float,
+                   compress_bits: int) -> None:
+    """Raise ``ValueError`` unless the client-sampling settings of :class:`FederatedConfig` are valid."""
+    if not 0 <= clients_per_round <= K:
+        raise ValueError("clients_per_round must lie in [0, K] = [0, %d] (0 = all), got %r" % (K, clients_per_round))
+    if not sampled_rounds(clients_per_round, K, partition):
+        return
+    what = "clients_per_round %d" % clients_per_round if 0 < clients_per_round < K else "partition 'dirichlet'"
+    if aggregator != "mean":
+        raise ValueError("%s needs aggregator 'mean' (sample-weighted averaging), got aggregator %r" % (what, aggregator))
+    if dp_clip > 0.0:
+        raise ValueError("%s cannot be combined with dp_clip > 0 (the accountant has no privacy amplification by "
+                         "subsampling), got dp_clip %r" % (what, dp_clip))
+    if compress_bits:
+        raise ValueError("%s cannot be combined with compress_bits, got compress_bits %r" % (what, compress_bits))
+
+
 def check_compress(compress_bits: int, compress_ef: bool, dp_clip: float, aggregator: str) -> None:
     """Raise ``ValueError`` unless the update-compression settings of :class:`FederatedConfig` are valid."""
     if compress_bits not in (0, 8, 4):
@@ -173,6 +211,9 @@ class FederatedConfig(CommonConfig):
     # one float32 scale per 128 coordinates (algo/compress.py); the new model is still broadcast in fp32
     compress_bits: int = 0          # 0 = off | 8 | 4
     compress_ef: bool = False       # error feedback: each worker carries its quantization error into its next update
+    # client sampling (FedAvg partial participation): each round trains and averages a uniform random subset of this many
+    # workers, weighted by their sample counts (algo/sampling.py); 0 = all K.  --partition dirichlet weights all K by n_k
+    clients_per_round: int = 0
 
     def __post_init__(self):
         check_server_opt(self.server_opt, self.server_lr, self.server_momentum, self.server_beta1, self.server_beta2,
@@ -181,6 +222,8 @@ class FederatedConfig(CommonConfig):
         check_byzantine(self.byzantine, self.attack, self.attack_scale, self.K)
         check_dp(self.dp_clip, self.dp_noise, self.dp_delta, self.aggregator)
         check_compress(self.compress_bits, self.compress_ef, self.dp_clip, self.aggregator)
+        check_partition(self.partition, self.dirichlet_alpha)
+        check_sampling(self.clients_per_round, self.K, self.partition, self.aggregator, self.dp_clip, self.compress_bits)
 
 
 @dataclass

@@ -648,6 +648,20 @@ static void set_q(fb::CommArgs& a, const std::vector<int64_t>& local_idx, int64_
     }
   }
 }
+// Sampled rounds (samp_S > 0): participants per round, key of the sampling stream, the device round counter (int64) and
+// the K workers' sample counts (int32, on the device).
+static void set_samp(fb::CommArgs& a, int64_t samp_S, int64_t samp_key, const c10::optional<Tensor>& samp_t,
+                     const c10::optional<Tensor>& client_n) {
+  if (samp_S == 0) return;
+  TORCH_CHECK(samp_t.has_value() && samp_t->defined() && samp_t->is_cuda() && samp_t->scalar_type() == at::kLong &&
+                  samp_t->numel() >= 1, "sampled round counter: int64 CUDA tensor");
+  TORCH_CHECK(client_n.has_value() && client_n->defined() && client_n->is_cuda() && client_n->scalar_type() == at::kInt &&
+                  client_n->is_contiguous() && client_n->numel() == a.K, "sample counts: one int32 CUDA value per worker");
+  a.samp_S = (int)samp_S;
+  a.samp_key = (unsigned long long)samp_key;
+  a.samp_t = reinterpret_cast<long long*>(samp_t->data_ptr<int64_t>());
+  a.client_n = client_n->data_ptr<int>();
+}
 static void fill_ctrl(uint32_t** dst, const std::vector<int64_t>& ctrl_ptrs, int world) {
   for (int p = 0; p < world && p < (int)ctrl_ptrs.size(); ++p) dst[p] = reinterpret_cast<uint32_t*>(ctrl_ptrs[p]);
 }
@@ -659,7 +673,8 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
                   c10::optional<Tensor> dp_t, c10::optional<Tensor> dp_stats, c10::optional<Tensor> dp_valid,
                   int64_t q_bits, int64_t q_group, int64_t q_key,
                   c10::optional<Tensor> q_t, std::vector<int64_t> q_code_ptrs, std::vector<int64_t> q_scale_ptrs,
-                  std::vector<Tensor> q_ef, c10::optional<Tensor> q_part) {
+                  std::vector<Tensor> q_ef, c10::optional<Tensor> q_part, int64_t samp_S, int64_t samp_key,
+                  c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n) {
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch);
   TORCH_CHECK(out.numel() >= fb::COMM_OUT_FLOATS && scratch.numel() >= fb::COMM_SCRATCH_FLOATS, "out / scratch too small");
   c10::cuda::CUDAGuard guard(z.device());
@@ -699,6 +714,7 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
   a.agg = (int)agg; a.trim_b = (int)trim_b;
   set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
   set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
+  set_samp(a, samp_S, samp_key, samp_t, client_n);
   fb::block_reduce_launch(a, cur_stream());
 }
 
@@ -713,7 +729,8 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
                          c10::optional<Tensor> dp_t, c10::optional<Tensor> dp_stats,
                          c10::optional<Tensor> dp_valid, int64_t q_bits, int64_t q_group, int64_t q_key,
                          c10::optional<Tensor> q_t, std::vector<int64_t> q_code_ptrs, std::vector<int64_t> q_scale_ptrs,
-                         std::vector<Tensor> q_ef, c10::optional<Tensor> q_part) {
+                         std::vector<Tensor> q_ef, c10::optional<Tensor> q_part, int64_t samp_S, int64_t samp_key,
+                         c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n) {
   TORCH_CHECK(opt >= fb::FEDOPT_AVGM && opt <= fb::FEDOPT_YOGI, "block_reduce_fedopt: unknown server optimizer ", opt);
   const bool adaptive = opt != fb::FEDOPT_AVGM;
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch); CHECK_F32_CUDA(m); CHECK_CONTIG(m);
@@ -758,6 +775,7 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
   a.agg = (int)agg; a.trim_b = (int)trim_b;
   set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
   set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
+  set_samp(a, samp_S, samp_key, samp_t, client_n);
   fb::block_reduce_launch(a, cur_stream());
 }
 

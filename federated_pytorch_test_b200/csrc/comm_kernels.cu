@@ -27,7 +27,8 @@
 // A second instantiation (FEDOPT) runs FedAvg with a server optimizer (FedAvgM / FedAdagrad / FedAdam / FedYogi) between
 // the reduction and the write-back.  DP instantiations add DP-FedAvg's Gaussian noise to the mean, after dp_clip_kernel
 // (end of file) has clipped the workers' updates.  Compressed instantiations (QBITS) reduce stochastically rounded 8- / 4-bit
-// codes of the workers' updates, which every rank encodes for its own replicas before barrier A.
+// codes of the workers' updates, which every rank encodes for its own replicas before barrier A.  Sampled instantiations
+// (SAMP) average only the round's participants, weighted by their sample counts, reading them over P2P.
 // Reference sites: /root/reference/src/federated_multi.py:203-217, fedprox_multi.py:211-232, consensus_multi.py:242-299.
 #include "fedb200.h"
 
@@ -577,6 +578,76 @@ __device__ __forceinline__ void q_write_back(const CommArgs& a, int nslices, flo
   }
 }
 
+// ---- client sampling: the participant set of round t and its sample-count weights --------------------------------------
+// Worker k draws h_k = F(F(key + (t + 1) G) + (k + 1) G) (F, G as for the DP noise); the round takes the samp_S workers
+// with the smallest (h_k, k), by integer ranks.  w_k = n_k / sum_{j in P} n_j, the integer sum rounded once to float and
+// the quotient correctly rounded (__fdiv_rn: the extension is built with --use_fast_math), so the set and the weights equal
+// algo/sampling.py (participants, weights) exactly.  Every CTA computes them for itself, in shared memory.
+struct SampSet {
+  const float* const* x;             // [np] the participants' slices, in worker order
+  const float* w;                    // [np] their weights
+  int np;
+};
+__device__ __forceinline__ SampSet samp_select(const CommArgs& a) {
+  __shared__ unsigned long long s_h[COMM_MAX_K];
+  __shared__ int s_in[COMM_MAX_K];
+  __shared__ const float* s_x[COMM_MAX_K];
+  __shared__ float s_w[COMM_MAX_K];
+  __shared__ int s_np;
+  const int k = threadIdx.x;
+  if (k < a.K) {
+    const uint64_t rk = dp_mix(a.samp_key + uint64_t(*a.samp_t + 1) * DP_GAMMA);
+    s_h[k] = dp_mix(rk + uint64_t(k + 1) * DP_GAMMA);
+  }
+  __syncthreads();
+  if (k < a.K) {
+    const unsigned long long h = s_h[k];
+    int rank = 0;
+    for (int j = 0; j < a.K; ++j) rank += (s_h[j] < h || (s_h[j] == h && j < k)) ? 1 : 0;
+    s_in[k] = rank < a.samp_S ? 1 : 0;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long total = 0;
+    int np = 0;
+    for (int j = 0; j < a.K; ++j) {
+      if (!s_in[j]) continue;
+      total += a.client_n[j];
+      s_x[np++] = a.x[j];
+    }
+    const float ft = float(total);
+    for (int j = 0, i = 0; j < a.K; ++j)
+      if (s_in[j]) s_w[i++] = __fdiv_rn(float(a.client_n[j]), ft);
+    s_np = np;
+  }
+  __syncthreads();
+  return {s_x, s_w, s_np};
+}
+// sum_{k in P} w_k x_k at float4 index `off` / coordinate i, in worker order; each term rounded, then added (no fma), as
+// the ATen oracle forms it.  Non-participants are not read.
+__device__ __forceinline__ float4 samp_gather_v4(const SampSet& ss, size_t off) {
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 4
+  for (int i = 0; i < ss.np; ++i) {
+    const float w = ss.w[i];
+    const float4 xv = ld_sys_v4(ss.x[i] + off);
+    acc.x = __fadd_rn(acc.x, __fmul_rn(w, xv.x)); acc.y = __fadd_rn(acc.y, __fmul_rn(w, xv.y));
+    acc.z = __fadd_rn(acc.z, __fmul_rn(w, xv.z)); acc.w = __fadd_rn(acc.w, __fmul_rn(w, xv.w));
+  }
+  return acc;
+}
+__device__ __forceinline__ float samp_gather_f32(const SampSet& ss, int i) {
+  float acc = 0.f;
+  for (int p = 0; p < ss.np; ++p) acc = __fadd_rn(acc, __fmul_rn(ss.w[p], ld_sys_f32(ss.x[p] + i)));
+  return acc;
+}
+// pass 1's aggregate at float4 index `off`: the weighted sum of the participants (SAMP) or reduce_v4's
+template <int AGG_PAD, bool SAMP>
+__device__ __forceinline__ float4 pass1_v4(const CommArgs& a, size_t off, float rho, bool use_mc, const SampSet& ss) {
+  if constexpr (SAMP) return samp_gather_v4(ss, off);
+  else return reduce_v4<AGG_PAD>(a, off, rho, use_mc);
+}
+
 // FEDOPT = false: FedAvg / FedProx / ADMM (a.mode).  FEDOPT = true: FedAvg (mode 0) whose new model is a server optimizer
 // step from z instead of the plain mean.  Pass 1 forms the step from the reduced mean, z and the state m (and v): one-shot
 // stores z, m, v locally; two-shot rank r broadcasts slice r of the new weights, of m and of v into every rank, so every rank
@@ -589,23 +660,30 @@ __device__ __forceinline__ void q_write_back(const CommArgs& a, int nslices, flo
 // QBITS = 8 / 4: the compressed instantiations (mode 0, the mean): phase 0, before barrier A, encodes the local replicas'
 // updates into the payload arenas; pass 1 reduces the K workers' payloads instead of their floats, and both passes walk the
 // compressed tiling (no separate scalar tail); phase C exchanges the quantization statistics and advances q_t.
-template <bool FEDOPT, int AGG_PAD, bool DP = false, int QBITS = 0>
+// SAMP: the client-sampling instantiations (mode 0, the mean, AGG_PAD = 0): every CTA selects round *samp_t's participants
+// and their weights first; pass 1 (one-shot, two-shot and the scalar tail) forms the weighted sum of the participants out of
+// peer memory with P2P loads only (multimem.ld_reduce would add every bound device with weight 1; the two-shot broadcast
+// may still use multimem.st); pass 2 is FedAvg's, so every replica, participant or not, receives z; the last CTA advances
+// samp_t.
+template <bool FEDOPT, int AGG_PAD, bool DP = false, int QBITS = 0, bool SAMP = false>
 __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const CommArgs a) {
   __shared__ float sm[32];
   __shared__ int s_abort;
   __shared__ int s_last;
   if (threadIdx.x == 0) { s_abort = 0; s_last = 0; }
   __syncthreads();
+  SampSet ss{};
+  if constexpr (SAMP) ss = samp_select(a);
   const uint32_t epoch = a.sync[0] + 1;
   const float rho = a.rho_dev != nullptr ? __ldg(a.rho_dev) : a.rho;
-  const float inv_scale = AGG_PAD > 0 ? 1.f : a.mode == 2 ? 1.f / (float(a.K) * rho) : 1.f / float(a.K);
+  const float inv_scale = (AGG_PAD > 0 || SAMP) ? 1.f : a.mode == 2 ? 1.f / (float(a.K) * rho) : 1.f / float(a.K);
   const int n4 = a.n >> 2;
   const int nslices = a.two_shot ? a.world : 1;
   const int chunk4 = a.two_shot ? (n4 + a.world - 1) / a.world : n4;
   const int my_slice = a.two_shot ? a.rank : 0;
   const int stride = gridDim.x * blockDim.x;
   const int t0 = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool use_mc = a.mc_x != nullptr && (a.mode != 2 || a.mc_y != nullptr);
+  const bool use_mc = !SAMP && a.mc_x != nullptr && (a.mode != 2 || a.mc_y != nullptr);
 
   // ---- 0 (compressed rounds): encode the local replicas' updates; per-CTA partial statistics in CTA order ------
   if constexpr (QBITS != 0) {
@@ -637,8 +715,8 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       const bool has1 = i1 < hi;
       const size_t off0 = 4 * size_t(i), off1 = 4 * size_t(has1 ? i1 : i);
       float4 accs[2];
-      accs[0] = reduce_v4<AGG_PAD>(a, off0, rho, use_mc);
-      accs[1] = has1 ? reduce_v4<AGG_PAD>(a, off1, rho, use_mc) : accs[0];
+      accs[0] = pass1_v4<AGG_PAD, SAMP>(a, off0, rho, use_mc, ss);
+      accs[1] = has1 ? pass1_v4<AGG_PAD, SAMP>(a, off1, rho, use_mc, ss) : accs[0];
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
         if (u == 1 && !has1) break;
@@ -697,6 +775,8 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
     float acc = 0.f;
     if constexpr (AGG_PAD > 0) {
       acc = robust_gather_f32<AGG_PAD>(a, i);
+    } else if constexpr (SAMP) {
+      acc = samp_gather_f32(ss, i);
     } else if (use_mc) {
       acc = multimem_ld_reduce_f32(a.mc_x + i);
       if (a.mode == 2) acc = fmaf(rho, acc, multimem_ld_reduce_f32(a.mc_y + i));
@@ -932,6 +1012,9 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) draws t + 1
     }
   }
+  if constexpr (SAMP) {
+    if (threadIdx.x == 0) *a.samp_t += 1;          // every CTA has selected: the next round (or graph replay) samples t + 1
+  }
   if (threadIdx.x == 0) {
     a.out[OUT_DUAL_SQ] = dual_sq;
     a.out[OUT_PRIMAL] = primal;
@@ -989,21 +1072,30 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
     if (args.two_shot && (args.xw[args.world - 1] == nullptr || (args.opt != FEDOPT_NONE && args.mw[args.world - 1] == nullptr)))
       throw std::runtime_error("fedb200: block_reduce: two-shot compressed rounds need P2P broadcast targets");
   }
+  const bool samp = args.samp_S != 0 || args.samp_t != nullptr;
+  if (samp) {
+    if (args.samp_S < 1 || args.samp_S > args.K)
+      throw std::runtime_error("fedb200: block_reduce: client sampling needs 1 <= S <= K participants");
+    if (args.samp_t == nullptr || args.client_n == nullptr)
+      throw std::runtime_error("fedb200: block_reduce: client sampling needs a round counter and the sample counts");
+    if (args.mode != 0 || args.agg != AGG_MEAN || args.dp || args.qbits != 0)
+      throw std::runtime_error("fedb200: block_reduce: client sampling needs mode 0 and the mean, without DP or compression");
+  }
   const bool fo = args.opt != FEDOPT_NONE;
-  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean, 8-bit codes, 4-bit codes]
-  const void* kernels[2][7] = {
+  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean, 8-bit codes, 4-bit codes, sampled weighted mean]
+  const void* kernels[2][8] = {
       {(const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
        (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>,
        (const void*)block_reduce_kernel<false, 0, true>, (const void*)block_reduce_kernel<false, 0, false, 8>,
-       (const void*)block_reduce_kernel<false, 0, false, 4>},
+       (const void*)block_reduce_kernel<false, 0, false, 4>, (const void*)block_reduce_kernel<false, 0, false, 0, true>},
       {(const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
        (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>,
        (const void*)block_reduce_kernel<true, 0, true>, (const void*)block_reduce_kernel<true, 0, false, 8>,
-       (const void*)block_reduce_kernel<true, 0, false, 4>}};
-  const int pad = args.qbits == 8 ? 5 : args.qbits == 4 ? 6 : args.dp ? 4 : args.agg == AGG_MEAN ? 0
+       (const void*)block_reduce_kernel<true, 0, false, 4>, (const void*)block_reduce_kernel<true, 0, false, 0, true>}};
+  const int pad = samp ? 7 : args.qbits == 8 ? 5 : args.qbits == 4 ? 6 : args.dp ? 4 : args.agg == AGG_MEAN ? 0
                 : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
   const void* kernel = kernels[fo][pad];
-  static int max_blocks[2][7] = {};
+  static int max_blocks[2][8] = {};
   int& mb = max_blocks[fo][pad];
   if (mb == 0) mb = comm_max_blocks(kernel);
   int cap = mb;

@@ -265,6 +265,14 @@ struct CommArgs {
   float* q_scales[COMM_MAX_K];       // one scale per group of Q_GROUP coordinates, counted from the block start
   float* q_ef[COMM_MAX_LOCAL];       // error feedback e_j of local replica j (in/out), or nullptr (off)
   float* q_part;                     // [Q_PART_FLOATS] per-CTA partial statistics (each launch overwrites what it reads)
+  // ---- client sampling with sample-count weights (FedAvg partial participation, McMahan et al. 2017; mode 0 with the
+  // mean, with or without a server optimizer, without DP or compression): round t = *samp_t takes the samp_S workers with
+  // the smallest (h_k, k), h_k = F(F(samp_key + (t + 1) G) + (k + 1) G), and z = sum_{k in P} w_k x_k with
+  // w_k = n_k / sum_{j in P} n_j.  Only participants are read (over P2P); every replica receives z.
+  int samp_S;                        // 0 selects the instantiations above; else 1..K participants per round
+  unsigned long long samp_key;       // key of the run's sampling stream
+  long long* samp_t;                 // device: index t of this sampled round over the run; the last CTA increments it
+  const int* client_n;               // device: [K] sample counts n_k of the workers' shards
 };
 constexpr int Q_GROUP = 128;                             // coordinates per scale
 constexpr int Q_SEG = 16;                                // coordinates per thread and tile in the compressed instantiations
@@ -273,6 +281,8 @@ constexpr int DP_CHUNK = 32;
 constexpr int FEDOPT_NONE = 0, FEDOPT_AVGM = 1, FEDOPT_ADAGRAD = 2, FEDOPT_ADAM = 3, FEDOPT_YOGI = 4;
 constexpr int AGG_MEAN = 0, AGG_MEDIAN = 1, AGG_TRIMMED = 2;
 constexpr int COMM_MAX_K_ROBUST = 16;
+// block_reduce_launch picks the instantiation: the mean, a robust rule, DP, compressed codes (qbits) or client sampling
+// (samp_S); it rejects combinations the kernel does not implement.
 void block_reduce_launch(const CommArgs& args, cudaStream_t s);
 
 // DP-FedAvg update clipping on the local replicas, as ONE cooperative kernel touching no peer memory: ||x_j - z|| per

@@ -100,6 +100,46 @@ def shard_ranges(K: int, n: int = TRAIN_SIZE, drop_last_sample: bool = True) -> 
     return out
 
 
+DIRICHLET_MAX_DRAWS = 100
+
+
+def dirichlet_shards(labels, K: int, alpha: float, seed: int, min_size: int) -> List[np.ndarray]:
+    """Label-skewed shards of the K workers (Hsu et al. 2019): sorted int64 index arrays, disjoint, covering every sample.
+
+    One ``numpy.random.Generator(PCG64(seed))`` draws everything.  For each class ``c`` in ascending order, the class's
+    sample indices are shuffled, ``p ~ Dir(alpha 1_K)`` is drawn and the shuffled indices are cut at
+    ``floor(cumsum(p) n_c)`` (worker ``k`` gets the ``k``-th piece).  If a shard ends up with fewer than ``min_size``
+    samples, the whole partition is drawn again from the same generator; after ``DIRICHLET_MAX_DRAWS`` draws a
+    ``ValueError`` names ``alpha`` and ``K``.  Every rank computes the full partition, so every rank knows every shard size.
+    """
+    lab = np.asarray(labels.cpu().numpy() if torch.is_tensor(labels) else labels).astype(np.int64)
+    if not (K >= 1 and alpha > 0.0):
+        raise ValueError("dirichlet_shards needs K >= 1 and alpha > 0, got K = %r, alpha = %r" % (K, alpha))
+    rng = np.random.Generator(np.random.PCG64(int(seed)))
+    classes = np.unique(lab)
+    for _ in range(DIRICHLET_MAX_DRAWS):
+        parts: List[List[np.ndarray]] = [[] for _ in range(K)]
+        for c in classes:
+            idx = np.flatnonzero(lab == c)
+            rng.shuffle(idx)
+            p = rng.dirichlet(np.full(K, float(alpha)))
+            cuts = np.floor(np.cumsum(p) * idx.size).astype(np.int64)
+            cuts[-1] = idx.size                       # cumsum(p) may end a rounding error below 1
+            for k, piece in enumerate(np.split(idx, cuts[:-1])):
+                parts[k].append(piece)
+        shards = [np.sort(np.concatenate(p)) for p in parts]
+        if min(s.size for s in shards) >= min_size:
+            return shards
+    raise ValueError("dirichlet_shards: no partition with at least %d samples per worker in %d draws at alpha = %g, "
+                     "K = %d; raise dirichlet_alpha or lower K" % (min_size, DIRICHLET_MAX_DRAWS, alpha, K))
+
+
+def class_histogram(labels, shards: Sequence[np.ndarray], num_classes: int = NUM_CLASSES) -> List[List[int]]:
+    """Per-worker sample counts of every class: ``[K][num_classes]``."""
+    lab = np.asarray(labels.cpu().numpy() if torch.is_tensor(labels) else labels).astype(np.int64)
+    return [np.bincount(lab[np.asarray(s, dtype=np.int64)], minlength=num_classes).tolist() for s in shards]
+
+
 def worker_norm(ck: int, biased: bool = True) -> Tuple[Tuple[float, float, float], Tuple[float, float, float]]:
     """(mean, std) applied after scaling pixels to [0,1]; mean == std in the reference."""
     if biased:

@@ -9,7 +9,9 @@ one device):
   median or trimmed mean of the K workers instead of their mean; with DP (``dp_clip_`` first, then ``dp=`` on
   ``fedavg_`` / ``fedopt_``) the workers' updates are clipped and Gaussian noise is added to the mean (DP-FedAvg); with
   ``compress=`` on ``fedavg_`` / ``fedopt_`` every worker uploads its update ``x_k - z`` as stochastically rounded 8- or
-  4-bit codes with one scale per group (``algo/compress.py``), and ``z' = z + mean_k q_k s_k``
+  4-bit codes with one scale per group (``algo/compress.py``), and ``z' = z + mean_k q_k s_k``; with ``sample=`` on
+  ``fedavg_`` / ``fedopt_`` only the round's ``S`` sampled workers are averaged, weighted by their sample counts
+  (``z' = sum_{k in P} n_k x_k / sum_{k in P} n_k``, ``algo/sampling.py``), and every replica receives ``z'``
 * X2 FedProx ``z' = mean``; ``dual``; ``primal = sum_k ||rho (x_k - z')||``; no write-back
   (fedprox_multi.py:211-232)
 * X3 ADMM    ``z' = sum_k (y_k + rho x_k) / (K rho)``; ``dual``; ``y_k += rho (x_k - z')``;
@@ -80,6 +82,19 @@ class QuantRound:
     codes: List[torch.Tensor]
     scales: List[torch.Tensor]
     ef: Optional[List[torch.Tensor]] = None
+
+
+@dataclass
+class SampleRound:
+    """Client sampling of one round (``algo/sampling.py``): the ``S`` participants of sampled round ``t`` under ``key``
+    are averaged with the weights ``n_k / sum_{j in P} n_j``.  ``t`` is a one-element int64 tensor on the block's device
+    (the index of the sampled round over the run, advanced by the round), ``n`` the K workers' sample counts (int32, on
+    the block's device)."""
+
+    S: int
+    key: int
+    t: torch.Tensor
+    n: torch.Tensor
 
 
 class TorchCollective:
@@ -259,12 +274,34 @@ class TorchCollective:
         return acc.mul_(1.0 / self.topo.K)
 
     @torch.no_grad()
+    def _sampled_mean(self, xs: List[torch.Tensor], s: SampleRound) -> torch.Tensor:
+        """``sum_{k in P} w_k x_k`` of sampled round ``t = s.t`` (``algo/sampling.py``), summed in float32 in worker order,
+        each term rounded before it is added; the K blocks are gathered, only the participants' rows are used.
+        Advances ``s.t``."""
+        from ..algo import sampling
+
+        K = self.topo.K
+        m = sampling.mask(s.key, int(s.t.item()), K, s.S)
+        w = sampling.weights(s.n.cpu().numpy(), m)
+        full = self.gather_blocks(xs)
+        acc = torch.zeros_like(full[0])
+        for k in range(K):
+            if m[k]:
+                acc = acc + full[k] * torch.tensor(w[k], dtype=full.dtype, device=full.device)
+        s.t.add_(1)
+        return acc
+
+    @torch.no_grad()
     def fedavg_(self, xs: List[torch.Tensor], z: torch.Tensor, write_back: bool = True,
-                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> torch.Tensor:
+                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
+                sample: Optional[SampleRound] = None) -> torch.Tensor:
         """In place: ``z <- mean_k x_k``, optionally ``x_k <- z``; returns ``||z_old - z_new||^2`` (0-dim).  With ``dp``
         the mean is noised (:class:`DPRound`; clip the replicas with :meth:`dp_clip_` first).  With ``compress``
-        (:class:`QuantRound`) ``z <- z + (1/K) sum_k q_k s_k``, the workers' updates as uploaded."""
-        if compress is not None:
+        (:class:`QuantRound`) ``z <- z + (1/K) sum_k q_k s_k``, the workers' updates as uploaded.  With ``sample``
+        (:class:`SampleRound`) ``z <-`` the sample-weighted mean of the round's participants; every replica receives it."""
+        if sample is not None:
+            znew = self._sampled_mean(xs, sample)
+        elif compress is not None:
             znew = z + self._compressed_update(xs, z, compress)
         else:
             znew = self.sum_blocks(xs).div_(self.topo.K)
@@ -295,15 +332,18 @@ class TorchCollective:
     @torch.no_grad()
     def fedopt_(self, xs: List[torch.Tensor], z: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], kind: str,
                 lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean", trim_b: int = 0,
-                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> torch.Tensor:
+                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
+                sample: Optional[SampleRound] = None) -> torch.Tensor:
         """FedAvg with a server optimizer, in place: ``d = mean_k x_k - z`` is the pseudo-gradient of server optimizer
         ``kind`` (one of :data:`FEDOPT_KINDS`; ``beta1`` is the momentum of 'avgm'), whose state ``m`` (and ``v``, unused
         by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``.
         With a robust rule ``agg`` (one of :data:`ROBUST_AGGS`) its aggregate replaces the mean in ``d``; with ``dp`` the
         noised mean does (DP-FedOpt: post-processing); with ``compress`` ``d`` is the dequantized mean update itself
-        (FedPAQ with a server optimizer)."""
+        (FedPAQ with a server optimizer); with ``sample`` the sample-weighted mean of the round's participants does."""
         mean = None
-        if compress is not None:
+        if sample is not None:
+            mean = self._sampled_mean(xs, sample)
+        elif compress is not None:
             d = self._compressed_update(xs, z, compress)
         elif agg == "mean":
             mean = self.sum_blocks(xs).div_(self.topo.K)

@@ -41,6 +41,11 @@ compressed instantiations: before barrier A every rank encodes its own replicas'
 (:meth:`FusedCollective.payload_like_block`), and pass 1 reads the K workers' codes and scales over P2P (there is no
 in-switch reduction of codes with per-group scales; the two-shot broadcast may still use ``multimem.st``), so a rank pulls
 about 4x (8-bit) or 7.5x (4-bit) fewer bytes from its peers.  The rounding counter lives in device memory as the DP one.
+
+Sampled rounds (client sampling with sample-count weights) are one launch of the sampled instantiations: every CTA
+selects the round's participants from the device-resident round counter, and pass 1 forms their weighted sum with P2P
+loads of the participants only (``multimem.ld_reduce`` sums every bound device with weight 1; the two-shot broadcast may
+still use ``multimem.st``).  A worker that sits out is never read, and receives the new model in pass 2.
 """
 from __future__ import annotations
 
@@ -51,7 +56,7 @@ import torch
 import torch.distributed as dist
 
 from ..ops import cuda_ops
-from .collective import FEDOPT_KINDS, ROBUST_AGGS, DPRound, QuantRound, TorchCollective, check_robust
+from .collective import FEDOPT_KINDS, ROBUST_AGGS, DPRound, QuantRound, SampleRound, TorchCollective, check_robust
 from .topology import Topology
 
 _MAX_LOCAL = 16
@@ -194,6 +199,7 @@ class FusedCollective(TorchCollective):
         self.warm_robust = False          # set by robust strategies: warm the robust instantiation(s) for this K too
         self.warm_dp = False              # set by DP strategies: warm the clip kernel and the DP instantiation(s) too
         self.warm_compress = 0            # set by compressing strategies to their bit width: warm those instantiations too
+        self.warm_sample = False          # set by sampling strategies: warm the sampled instantiation(s) too
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
@@ -201,7 +207,8 @@ class FusedCollective(TorchCollective):
         is far slower than the ones after it).  The server-optimizer kernel is warmed only when ``warm_fedopt`` is set, the
         robust kernels (of this K; with the server optimizer if both are set) only when ``warm_robust`` is set, the DP
         kernels (likewise) only when ``warm_dp`` is set, the compressed ones of ``warm_compress`` bits (likewise) only when
-        that is set.
+        that is set, the sampled ones (likewise) only when ``warm_sample`` is set; their round counters are throwaway
+        tensors, so warm-up advances no counter of the run.
         Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
@@ -217,6 +224,9 @@ class FusedCollective(TorchCollective):
             pay = [self.payload_like_block(x, self.warm_compress) for x in xs]
             qr = QuantRound(self.warm_compress, 0, torch.zeros(1, dtype=torch.int64, device=self.topo.device),
                             [c for c, _ in pay], [sc for _, sc in pay])
+        if self.warm_sample:
+            sr = SampleRound(1, 0, torch.zeros(1, dtype=torch.int64, device=self.topo.device),
+                             torch.ones(self.topo.K, dtype=torch.int32, device=self.topo.device))
         keep = self.two_shot_mode
         for mode_2shot in ("0", "1"):
             self.two_shot_mode = mode_2shot
@@ -239,6 +249,10 @@ class FusedCollective(TorchCollective):
                 self._launch(0, xs, None, z, 0.0, compress=qr)
                 if self.warm_fedopt:
                     self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, compress=qr)
+            if self.warm_sample:
+                self._launch(0, xs, None, z, 0.0, sample=sr)
+                if self.warm_fedopt:
+                    self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, sample=sr)
         self.two_shot_mode = keep
         x0 = [torch.zeros_like(x) for x in xs]
         yh = [torch.zeros_like(x) for x in xs]
@@ -340,14 +354,26 @@ class FusedCollective(TorchCollective):
         return (int(q.bits), _Q_GROUP, key - (1 << 64) if key >= 1 << 63 else key, q.t, cp, sp,
                 list(q.ef) if q.ef is not None else [], self.q_part)
 
+    def _samp_args(self, s: Optional[SampleRound]):
+        """The sampling arguments of the aggregation bindings: participants per round, key (as a signed 64-bit int),
+        counter, sample counts."""
+        if s is None:
+            return 0, 0, None, None
+        key = int(s.key) & ((1 << 64) - 1)
+        return int(s.S), key - (1 << 64) if key >= 1 << 63 else key, s.t, s.n
+
     def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None, agg: str = "mean", trim_b: int = 0,
-                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> None:
+                dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
+                sample: Optional[SampleRound] = None) -> None:
         """Modes 0 / 1 take a robust rule ``agg`` (:data:`ROBUST_AGGS`) in place of the mean; mode 0 with the mean takes
-        the noise of a DP round (``dp``; after :meth:`dp_clip_`) or compresses the workers' updates (``compress``)."""
+        the noise of a DP round (``dp``; after :meth:`dp_clip_`), compresses the workers' updates (``compress``) or
+        averages the sampled participants of the round (``sample``)."""
         if dp is not None and (mode != 0 or agg != "mean"):
             raise ValueError("DP aggregation needs FedAvg with the mean")
         if compress is not None and (mode != 0 or agg != "mean" or dp is not None):
             raise ValueError("compressed aggregation needs FedAvg with the mean, without DP")
+        if sample is not None and (mode != 0 or agg != "mean" or dp is not None or compress is not None):
+            raise ValueError("sampled aggregation needs FedAvg with the mean, without DP or compression")
         code = self._agg_code(agg, trim_b)
         n = xs[0].numel()
         if any(t.numel() != n for t in xs) or z.numel() != n:
@@ -370,22 +396,26 @@ class FusedCollective(TorchCollective):
                     mcz = za["mc_ptr"] + zoff
         self.ext.block_reduce(mode, xp, yp, local_idx, z, n, float(rho), rho_dev, self.out, self.scratch, self.ctrl_ptrs,
                               self.sync, W, self.topo.rank, mcx, mcy, mcz, xw, zw, bool(two), self.max_blocks,
-                              self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress))
+                              self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress),
+                              *self._samp_args(sample))
         self.launches += 1
         self.last_two_shot = bool(two)
 
     def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                       trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> None:
+                       trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
+                       sample: Optional[SampleRound] = None) -> None:
         """FedAvg with a server optimizer: mode 0 of the kernel's FedOpt instantiation.  Two-shot, rank r broadcasts slice r
         of the new weights, of ``m`` and of ``v`` into every rank, so ``m`` / ``v`` must be symmetric slices then
         (:meth:`zeros_like_block`).  A robust rule ``agg`` replaces the mean as the aggregate the step is taken towards; a
         DP round (``dp``, mean only) noises the mean first; a compressed round (``compress``, mean only) steps along the
-        dequantized mean update."""
+        dequantized mean update; a sampled round (``sample``, mean only) steps towards the participants' weighted mean."""
         code = self._agg_code(agg, trim_b)
         if dp is not None and agg != "mean":
             raise ValueError("DP aggregation needs the mean")
         if compress is not None and (agg != "mean" or dp is not None):
             raise ValueError("compressed aggregation needs the mean, without DP")
+        if sample is not None and (agg != "mean" or dp is not None or compress is not None):
+            raise ValueError("sampled aggregation needs the mean, without DP or compression")
         n = xs[0].numel()
         adaptive = kind != "avgm"
         if any(t.numel() != n for t in xs) or z.numel() != n or m.numel() != n or (adaptive and v.numel() != n):
@@ -403,7 +433,8 @@ class FusedCollective(TorchCollective):
         self.ext.block_reduce_fedopt(FEDOPT_KINDS.index(kind) + 1, float(lr), float(beta1), float(beta2), float(tau), m,
                                      v if adaptive else None, xp, local_idx, z, n, self.out, self.scratch, self.ctrl_ptrs,
                                      self.sync, W, self.topo.rank, mcx, mcm, mcv, xw, mw, vw, bool(two), self.max_blocks,
-                                     self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress))
+                                     self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress),
+                                     *self._samp_args(sample))
         self.launches += 1
         self.last_two_shot = bool(two)
 
@@ -419,13 +450,14 @@ class FusedCollective(TorchCollective):
             self._out_pending = True
 
     def launch_fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
-                       compress: Optional[QuantRound] = None) -> None:
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress)
+                       compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None) -> None:
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample)
         self._record_async()
 
     def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                       trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None) -> None:
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress)
+                       trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
+                       sample: Optional[SampleRound] = None) -> None:
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample)
         self._record_async()
 
     @torch.no_grad()
@@ -471,8 +503,8 @@ class FusedCollective(TorchCollective):
     # -- operators ----------------------------------------------------------------------
     @torch.no_grad()
     def fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
-                compress: Optional[QuantRound] = None):
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress)
+                compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None):
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
@@ -482,8 +514,9 @@ class FusedCollective(TorchCollective):
 
     @torch.no_grad()
     def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
-                trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None):
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress)
+                trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
+                sample: Optional[SampleRound] = None):
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
