@@ -129,15 +129,26 @@ class FedAvg(Strategy):
     device memory) trains only its ``clients_per_round`` participants (0 = all K), drawn uniformly from ``(seed, t)``, and
     ``z <- sum_{k in P} w_k x_k`` with ``w_k = n_k / sum_{j in P} n_j``, written back into every replica, participant or
     not.  Workers that sit out are never read.  A round is one launch on the fused collective.  The round metrics gain
-    ``participants`` (the worker ids) and ``participant_samples`` (``sum_{k in P} n_k``)."""
+    ``participants`` (the worker ids) and ``participant_samples`` (``sum_{k in P} n_k``).
+
+    ``secagg`` makes it secure aggregation (SecAgg, Bonawitz et al. 2017; ``algo/secagg.py``): with ``z`` the server model
+    the round started from, worker ``k`` uploads ``u_k = x_k - z`` as int32 fixed-point codes ``rint(clamp(u, -R, R) 2^f)``
+    (``R = secagg_clip``) plus pairwise ChaCha20 masks keyed by pair keys derived from ``seed`` (or ``secagg_keys``) and
+    the run's secure-aggregation round ``t`` (in device memory), which cancel in the sum; ``z <- z + (sum_k q_k) 2^-f / K``,
+    written back into every replica.  Integer sums are exact, so the new model does not depend on the process layout.  A
+    round is one launch on the fused collective.  As with DP, ``z`` starts each block visit as the replicas' common value
+    instead of 0 (Q6), so the ``dual`` of the first round of a visit differs from plain FedAvg.  The round metrics gain
+    ``sa_frac_bits`` (``f``) and ``sa_clipped`` (coordinates clipped, over all K); a non-finite update coordinate codes to
+    0 and is reported as ``nonfinite``, so the NaN guard fires."""
 
     name = "fedavg"
     write_back = True
 
     def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1, dp_clip: float = 0.0,
                  dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
-                 compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None):
-        from ..config import check_aggregator, check_compress, check_dp, check_sampling, trim_count
+                 compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None,
+                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None):
+        from ..config import check_aggregator, check_compress, check_dp, check_sampling, check_secagg, trim_count
 
         super().__init__(collective, topo)
         check_aggregator(aggregator, trim_fraction, topo.K)
@@ -187,11 +198,33 @@ class FedAvg(Strategy):
             self._last_ids: List[int] = []
             if hasattr(collective, "warm_sample"):
                 collective.warm_sample = True
+        self.sa = bool(secagg)
+        self.sa_rounds = 0                     # host mirror of the device round counter sa_t (the masks' nonce)
+        if self.sa:
+            import numpy as np
+
+            from . import secagg as sa
+
+            check_secagg(True, secagg_clip, topo.K, aggregator, dp_clip, compress_bits, clients_per_round,
+                         "dirichlet" if client_n is not None else "iid")
+            self.sa_clip = float(np.float32(secagg_clip))
+            self.sa_f = sa.frac_bits(secagg_clip, topo.K)
+            keys = sa.pair_keys(seed, topo.K) if secagg_keys is None else np.asarray(secagg_keys, dtype=np.uint32)
+            if keys.shape != (topo.K * (topo.K - 1) // 2, 8):
+                raise ValueError("secagg_keys needs one row of 8 words per worker pair, got shape %r" % (keys.shape,))
+            self.sa_digest = sa.key_digest(keys)
+            self.sa_keys = torch.from_numpy(keys.view(np.int32).copy()).to(topo.device)
+            self.sa_t = torch.zeros(1, dtype=torch.int64, device=topo.device)
+            self.sa_payload: List[torch.Tensor] = []                 # per local replica, current block
+            if hasattr(collective, "warm_secagg"):
+                collective.warm_secagg = True
 
     def begin_block(self, ci: int, N: int, xs: List[torch.Tensor]) -> None:
         super().begin_block(ci, N, xs)
-        if self.dp or self.q_bits:             # the server model: the replicas are equal here, so a local copy suffices
+        if self.dp or self.q_bits or self.sa:  # the server model: the replicas are equal here, so a local copy suffices
             self.z.copy_(xs[0])
+        if self.sa:
+            self.sa_payload = [self.coll.payload32_like_block(x) for x in xs]
         if self.q_bits:
             self.q_payload = [self.coll.payload_like_block(x, self.q_bits) for x in xs]
             if self.q_ef_on and ci not in self.q_ef:
@@ -244,6 +277,39 @@ class FedAvg(Strategy):
         if self.sampled:
             self.samp_rounds = int(st["samp_t"])
             self.samp_t.fill_(self.samp_rounds)
+
+    # -- secure aggregation ---------------------------------------------------------------------------------------------
+    def _sa_kw(self) -> Dict[str, object]:
+        """The secure-aggregation argument of the aggregation (which advances the round counter)."""
+        if not self.sa:
+            return {}
+        from ..parallel.collective import SecAggRound
+
+        self.sa_rounds += 1
+        return {"secagg": SecAggRound(self.sa_clip, self.sa_f, self.sa_keys, self.sa_t, self.sa_payload)}
+
+    def _with_sa(self, metrics: Dict[str, float]) -> Dict[str, float]:
+        if self.sa:
+            clipped, nonfinite = self.coll.last_sa
+            metrics.update(sa_frac_bits=float(self.sa_f), sa_clipped=float(clipped))
+            if nonfinite:
+                metrics["nonfinite"] = float(nonfinite)
+        return metrics
+
+    def _sa_state(self) -> Dict[str, object]:
+        if not self.sa:
+            return {}
+        return {"secagg": (self.sa_clip, self.sa_f, self.sa_digest), "sa_t": self.sa_rounds}
+
+    def _check_sa_state(self, st: Dict[str, object]) -> None:
+        got = tuple(st["secagg"]) if st.get("secagg") is not None else None
+        want = self._sa_state().get("secagg")
+        if got != want:
+            raise ValueError("resume record holds secure-aggregation settings (secagg_clip, f, SHA-256 of the pair keys) %r, "
+                             "this run uses %r" % (got, want))
+        if self.sa:
+            self.sa_rounds = int(st["sa_t"])
+            self.sa_t.fill_(self.sa_rounds)
 
     # -- compressed updates -------------------------------------------------------------------------------------------
     def _q_kw(self) -> Dict[str, object]:
@@ -331,15 +397,17 @@ class FedAvg(Strategy):
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         if self.aggregator == "mean":
             dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw(), **self._q_kw(),
-                                        **self._samp_kw())
+                                        **self._samp_kw(), **self._sa_kw())
         else:
             dual_sq = self.coll.robust_(self.xs, self.z, self.aggregator, self.trim_b)
-        return self._with_samp(self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))
+        return self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             if self.aggregator == "mean":
-                self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw(), **self._q_kw(), **self._samp_kw())
+                self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw(), **self._q_kw(), **self._samp_kw(),
+                                         **self._sa_kw())
             else:
                 self.coll.launch_robust_(self.xs, self.z, self.aggregator, self.trim_b)
             return ("pending", self.N)
@@ -348,8 +416,8 @@ class FedAvg(Strategy):
     def aggregate_end(self, token) -> Dict[str, float]:
         if token[0] == "done":
             return token[1]
-        return self._with_samp(self._with_q(self._with_dp(
-            {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]})))
+        return self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]}))))
 
     def _robust_state(self) -> Dict[str, object]:
         return {} if self.aggregator == "mean" else {"aggregator": self.aggregator, "trim_b": self.trim_b}
@@ -376,13 +444,15 @@ class FedAvg(Strategy):
             self.dp_t.fill_(self.dp_rounds)
 
     def state(self) -> Dict[str, object]:
-        return {"z": self.z, **self._robust_state(), **self._dp_state(), **self._q_state(), **self._samp_state()}
+        return {"z": self.z, **self._robust_state(), **self._dp_state(), **self._q_state(), **self._samp_state(),
+                **self._sa_state()}
 
     def load_state(self, st: Dict[str, object]) -> None:
         self._check_robust_state(st)
         self._check_dp_state(st)
         self._check_q_state(st)
         self._check_samp_state(st)
+        self._check_sa_state(st)
         self.z.copy_(st["z"].to(self.z.device))
 
 
@@ -406,19 +476,22 @@ class FedOpt(FedAvg):
     compressed updates (``compress_bits``) ``d`` is the dequantized mean update itself (FedPAQ with a server optimizer),
     and the server model at the start of a visit is again the replicas' common value.  With client sampling
     (``client_n``) the participants' sample-weighted mean replaces the mean in ``d``; the server model at the start of a
-    visit stays the unsampled mean of the (equal) replicas and does not advance the sampling counter."""
+    visit stays the unsampled mean of the (equal) replicas and does not advance the sampling counter.  With secure
+    aggregation (``secagg``) ``d`` is the decoded sum of the masked updates, and the server model at the start of a visit
+    is the replicas' common value."""
 
     name = "fedopt"
 
     def __init__(self, collective, topo, kind: str = "adam", lr: float = 0.0, momentum: float = 0.9, beta1: float = 0.9,
                  beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1,
                  dp_clip: float = 0.0, dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
-                 compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None):
+                 compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None,
+                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None):
         from ..config import check_server_opt
         from ..parallel.collective import FEDOPT_KINDS
 
         super().__init__(collective, topo, aggregator, trim_fraction, dp_clip, dp_noise, dp_delta, seed, compress_bits,
-                         compress_ef, clients_per_round, client_n)
+                         compress_ef, clients_per_round, client_n, secagg, secagg_clip, secagg_keys)
         if kind not in FEDOPT_KINDS:
             raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
         check_server_opt(kind, lr, momentum, beta1, beta2, tau)
@@ -444,7 +517,7 @@ class FedOpt(FedAvg):
             if ci in self._restored:
                 self._install(ci, *self._restored.pop(ci))
         self.m, self.v = self.ms[ci], self.vs.get(ci)
-        if not (self.dp or self.q_bits):                          # (else FedAvg.begin_block copied the replicas' value)
+        if not (self.dp or self.q_bits or self.sa):               # (else FedAvg.begin_block copied the replicas' value)
             self.coll.fedavg_(xs, self.z, write_back=False)      # the server model: the replicas' mean, no write-back
 
     def _hyper(self):
@@ -455,13 +528,14 @@ class FedOpt(FedAvg):
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
-                                    **self._q_kw(), **self._samp_kw())
-        return self._with_samp(self._with_q(self._with_dp({"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))
+                                    **self._q_kw(), **self._samp_kw(), **self._sa_kw())
+        return self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
-                                     **self._q_kw(), **self._samp_kw())
+                                     **self._q_kw(), **self._samp_kw(), **self._sa_kw())
             return ("pending", self.N)
         return ("done", self.aggregate(nadmm))
 
@@ -473,7 +547,7 @@ class FedOpt(FedAvg):
         ms.update(self.ms)
         vs.update(self.vs)
         return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state(), **self._dp_state(),
-                **self._q_state(), **self._samp_state()}
+                **self._q_state(), **self._samp_state(), **self._sa_state()}
 
     def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
         self.ms[ci].copy_(m.to(self.ms[ci].device))
@@ -487,6 +561,7 @@ class FedOpt(FedAvg):
         self._check_dp_state(st)
         self._check_q_state(st)
         self._check_samp_state(st)
+        self._check_sa_state(st)
         self.z.copy_(st["z"].to(self.z.device))
         vs = st.get("v") or {}
         for ci, m in (st.get("m") or {}).items():

@@ -28,6 +28,12 @@ training set with Dirichlet label skew into unequal shards.  Either one makes th
 fused launch that reads only the participants (``algo/sampling.py``); workers that sit out take no step and receive the
 new model.  Round metrics gain ``participants`` and ``participant_samples``; the root writes a ``partition`` row with the
 shard sizes and per-worker class counts.
+
+``--secagg [--secagg_clip R]`` makes every round secure aggregation (SecAgg, with or without a server optimizer): each
+worker uploads its block update ``x_k - z`` as int32 fixed-point codes of ``clamp(u, -R, R)`` masked with pairwise
+ChaCha20 keystreams that cancel in the sum (``algo/secagg.py``), so the server learns only the sum.  The pair keys are
+derived from ``--seed`` in place of a key agreement: whoever knows the seed can unmask.  Round metrics gain
+``sa_frac_bits`` and ``sa_clipped``.
 """
 from __future__ import annotations
 
@@ -49,6 +55,8 @@ def make_strategy(cfg: Config, coll, topo, client_n=None):
         robust.update(compress_bits=cfg.compress_bits, compress_ef=cfg.compress_ef, seed=cfg.seed)
     if sampled_rounds(cfg.clients_per_round, cfg.K, cfg.partition):
         robust.update(clients_per_round=cfg.clients_per_round, client_n=client_n or [1] * cfg.K, seed=cfg.seed)
+    if cfg.secagg:
+        robust.update(secagg=True, secagg_clip=cfg.secagg_clip, seed=cfg.seed)
     if cfg.server_opt == "none":
         return FedAvg(coll, topo, **robust)
     return FedOpt(coll, topo, cfg.server_opt, cfg.server_lr, cfg.server_momentum, cfg.server_beta1, cfg.server_beta2,

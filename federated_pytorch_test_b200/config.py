@@ -184,6 +184,28 @@ def check_compress(compress_bits: int, compress_ef: bool, dp_clip: float, aggreg
         raise ValueError("compress_bits needs aggregator 'mean', got aggregator %r" % (aggregator,))
 
 
+def check_secagg(secagg: bool, secagg_clip: float, K: int, aggregator: str, dp_clip: float, compress_bits: int,
+                 clients_per_round: int, partition: str) -> None:
+    """Raise ``ValueError`` unless the secure-aggregation settings of :class:`FederatedConfig` are valid."""
+    if not secagg:
+        return
+    from .algo.secagg import frac_bits
+
+    frac_bits(secagg_clip, max(K, 2))                 # names secagg_clip: not finite and > 0, or no scale 2^f in range
+    if K < 2:
+        raise ValueError("secagg needs K >= 2 (a lone worker's payload is unmasked), got K = %d" % K)
+    if aggregator != "mean":
+        raise ValueError("secagg needs aggregator 'mean' (the server sees only the sum), got aggregator %r" % (aggregator,))
+    if dp_clip > 0.0:
+        raise ValueError("secagg cannot be combined with dp_clip > 0, got dp_clip %r" % (dp_clip,))
+    if compress_bits:
+        raise ValueError("secagg cannot be combined with compress_bits, got compress_bits %r" % (compress_bits,))
+    if sampled_rounds(clients_per_round, K, partition):
+        what = "clients_per_round %d" % clients_per_round if 0 < clients_per_round < K else "partition 'dirichlet'"
+        raise ValueError("secagg cannot be combined with sampled rounds (every worker takes part in every round), got %s"
+                         % what)
+
+
 @dataclass
 class FederatedConfig(CommonConfig):
     lambda1: float = 0.0001
@@ -214,6 +236,10 @@ class FederatedConfig(CommonConfig):
     # client sampling (FedAvg partial participation): each round trains and averages a uniform random subset of this many
     # workers, weighted by their sample counts (algo/sampling.py); 0 = all K.  --partition dirichlet weights all K by n_k
     clients_per_round: int = 0
+    # secure aggregation (SecAgg): every worker uploads its block update as int32 fixed-point codes of clamp(u, -R, R)
+    # masked with pairwise ChaCha20 keystreams that cancel in the sum (algo/secagg.py); pair keys are derived from --seed
+    secagg: bool = False
+    secagg_clip: float = 1.0        # R
 
     def __post_init__(self):
         check_server_opt(self.server_opt, self.server_lr, self.server_momentum, self.server_beta1, self.server_beta2,
@@ -224,6 +250,8 @@ class FederatedConfig(CommonConfig):
         check_compress(self.compress_bits, self.compress_ef, self.dp_clip, self.aggregator)
         check_partition(self.partition, self.dirichlet_alpha)
         check_sampling(self.clients_per_round, self.K, self.partition, self.aggregator, self.dp_clip, self.compress_bits)
+        check_secagg(self.secagg, self.secagg_clip, self.K, self.aggregator, self.dp_clip, self.compress_bits,
+                     self.clients_per_round, self.partition)
 
 
 @dataclass

@@ -662,6 +662,34 @@ static void set_samp(fb::CommArgs& a, int64_t samp_S, int64_t samp_key, const c1
   a.samp_t = reinterpret_cast<long long*>(samp_t->data_ptr<int64_t>());
   a.client_n = client_n->data_ptr<int>();
 }
+// Secure-aggregation rounds (sa_t given): f, the clip R, the pair-key table (int32 [K (K - 1) / 2, 8], on the device),
+// the device round counter (int64: the nonce), the payload pointers of ALL K workers (4 bytes per coordinate, local or
+// peer-mapped) and the per-CTA statistics buffer.
+static void set_sa(fb::CommArgs& a, const std::vector<int64_t>& local_idx, int64_t sa_frac_bits, double sa_clip,
+                   const c10::optional<Tensor>& sa_keys, const c10::optional<Tensor>& sa_t,
+                   const std::vector<int64_t>& sa_pay_ptrs, const c10::optional<Tensor>& sa_part) {
+  if (!sa_t.has_value() || !sa_t->defined()) return;
+  TORCH_CHECK(sa_t->is_cuda() && sa_t->scalar_type() == at::kLong && sa_t->numel() >= 1,
+              "secure-aggregation round counter: int64 CUDA tensor");
+  TORCH_CHECK(sa_keys.has_value() && sa_keys->defined() && sa_keys->is_cuda() && sa_keys->scalar_type() == at::kInt &&
+                  sa_keys->is_contiguous() && sa_keys->numel() == (int64_t)a.K * (a.K - 1) / 2 * 8,
+              "secure-aggregation pair keys: int32 CUDA tensor [K (K - 1) / 2, 8]");
+  TORCH_CHECK(sa_part.has_value() && sa_part->defined() && sa_part->numel() >= fb::Q_PART_FLOATS,
+              "secure-aggregation rounds need the statistics buffer");
+  CHECK_F32_CUDA((*sa_part));
+  TORCH_CHECK((int)sa_pay_ptrs.size() == a.K, "secure-aggregation rounds need K payload pointers");
+  a.sa = 1;
+  a.sa_frac_bits = (int)sa_frac_bits;
+  a.sa_clip = (float)sa_clip;
+  a.sa_keys = reinterpret_cast<const uint32_t*>(sa_keys->data_ptr<int>());
+  a.q_t = reinterpret_cast<long long*>(sa_t->data_ptr<int64_t>());
+  a.q_part = sa_part->data_ptr<float>();
+  for (int k = 0; k < a.K; ++k) {
+    TORCH_CHECK(sa_pay_ptrs[k] % 16 == 0, "payload slices must be 16-byte aligned");
+    a.q_codes[k] = reinterpret_cast<unsigned char*>(sa_pay_ptrs[k]);
+  }
+  for (int j = 0; j < a.n_local; ++j) a.q_worker[j] = (int)local_idx[j];
+}
 static void fill_ctrl(uint32_t** dst, const std::vector<int64_t>& ctrl_ptrs, int world) {
   for (int p = 0; p < world && p < (int)ctrl_ptrs.size(); ++p) dst[p] = reinterpret_cast<uint32_t*>(ctrl_ptrs[p]);
 }
@@ -674,7 +702,9 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
                   int64_t q_bits, int64_t q_group, int64_t q_key,
                   c10::optional<Tensor> q_t, std::vector<int64_t> q_code_ptrs, std::vector<int64_t> q_scale_ptrs,
                   std::vector<Tensor> q_ef, c10::optional<Tensor> q_part, int64_t samp_S, int64_t samp_key,
-                  c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n) {
+                  c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n, int64_t sa_frac_bits, double sa_clip,
+                  c10::optional<Tensor> sa_keys, c10::optional<Tensor> sa_t, std::vector<int64_t> sa_pay_ptrs,
+                  c10::optional<Tensor> sa_part) {
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch);
   TORCH_CHECK(out.numel() >= fb::COMM_OUT_FLOATS && scratch.numel() >= fb::COMM_SCRATCH_FLOATS, "out / scratch too small");
   c10::cuda::CUDAGuard guard(z.device());
@@ -715,6 +745,7 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
   set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
   set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
   set_samp(a, samp_S, samp_key, samp_t, client_n);
+  set_sa(a, local_idx, sa_frac_bits, sa_clip, sa_keys, sa_t, sa_pay_ptrs, sa_part);
   fb::block_reduce_launch(a, cur_stream());
 }
 
@@ -730,7 +761,9 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
                          c10::optional<Tensor> dp_valid, int64_t q_bits, int64_t q_group, int64_t q_key,
                          c10::optional<Tensor> q_t, std::vector<int64_t> q_code_ptrs, std::vector<int64_t> q_scale_ptrs,
                          std::vector<Tensor> q_ef, c10::optional<Tensor> q_part, int64_t samp_S, int64_t samp_key,
-                         c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n) {
+                         c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n, int64_t sa_frac_bits,
+                         double sa_clip, c10::optional<Tensor> sa_keys, c10::optional<Tensor> sa_t,
+                         std::vector<int64_t> sa_pay_ptrs, c10::optional<Tensor> sa_part) {
   TORCH_CHECK(opt >= fb::FEDOPT_AVGM && opt <= fb::FEDOPT_YOGI, "block_reduce_fedopt: unknown server optimizer ", opt);
   const bool adaptive = opt != fb::FEDOPT_AVGM;
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch); CHECK_F32_CUDA(m); CHECK_CONTIG(m);
@@ -776,6 +809,7 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
   set_dp(a, dp_std, dp_key, dp_t, dp_stats, dp_valid);
   set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
   set_samp(a, samp_S, samp_key, samp_t, client_n);
+  set_sa(a, local_idx, sa_frac_bits, sa_clip, sa_keys, sa_t, sa_pay_ptrs, sa_part);
   fb::block_reduce_launch(a, cur_stream());
 }
 

@@ -28,7 +28,8 @@
 // the reduction and the write-back.  DP instantiations add DP-FedAvg's Gaussian noise to the mean, after dp_clip_kernel
 // (end of file) has clipped the workers' updates.  Compressed instantiations (QBITS) reduce stochastically rounded 8- / 4-bit
 // codes of the workers' updates, which every rank encodes for its own replicas before barrier A.  Sampled instantiations
-// (SAMP) average only the round's participants, weighted by their sample counts, reading them over P2P.
+// (SAMP) average only the round's participants, weighted by their sample counts, reading them over P2P.  Secure-aggregation
+// instantiations (QBITS = SA_QBITS) sum pairwise ChaCha20-masked fixed-point codes, whose masks cancel in the sum.
 // Reference sites: /root/reference/src/federated_multi.py:203-217, fedprox_multi.py:211-232, consensus_multi.py:242-299.
 #include "fedb200.h"
 
@@ -459,6 +460,125 @@ __device__ __forceinline__ void q_encode(const CommArgs& a, int nslices, float& 
   }
 }
 
+// ---- secure aggregation: pairwise ChaCha20-masked fixed-point updates (SecAgg, Bonawitz et al. 2017) -----------------
+// The instantiations are the compressed ones with QBITS = SA_QBITS: 32-bit codes on the compressed tiling, one ChaCha20
+// block (16 words) per thread, coordinate segment and peer pair.  algo/secagg.py is the numpy oracle; the payloads and the
+// FedAvg model equal it bit for bit.
+constexpr int SA_QBITS = 32;
+static_assert(Q_SEG == 16, "one ChaCha20 block masks one thread's segment");
+
+// ChaCha20 block function (RFC 8439 §2.3) with key `key`, block counter `ctr` and nonce (n0, n1, 0), added to (SIGN = 1)
+// or subtracted from (SIGN = -1) acc, mod 2^32
+#define SA_QR(a, b, c, d)                                                    \
+  a += b; d ^= a; d = __funnelshift_l(d, d, 16);                             \
+  c += d; b ^= c; b = __funnelshift_l(b, b, 12);                             \
+  a += b; d ^= a; d = __funnelshift_l(d, d, 8);                              \
+  c += d; b ^= c; b = __funnelshift_l(b, b, 7);
+__device__ __forceinline__ void sa_chacha_acc(const uint32_t (&key)[8], uint32_t ctr, uint32_t n0, uint32_t n1, bool add,
+                                              uint32_t (&acc)[Q_SEG]) {
+  uint32_t x0 = 0x61707865u, x1 = 0x3320646eu, x2 = 0x79622d32u, x3 = 0x6b206574u;
+  uint32_t x4 = key[0], x5 = key[1], x6 = key[2], x7 = key[3], x8 = key[4], x9 = key[5], x10 = key[6], x11 = key[7];
+  uint32_t x12 = ctr, x13 = n0, x14 = n1, x15 = 0u;
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    SA_QR(x0, x4, x8, x12) SA_QR(x1, x5, x9, x13) SA_QR(x2, x6, x10, x14) SA_QR(x3, x7, x11, x15)
+    SA_QR(x0, x5, x10, x15) SA_QR(x1, x6, x11, x12) SA_QR(x2, x7, x8, x13) SA_QR(x3, x4, x9, x14)
+  }
+  const uint32_t w[Q_SEG] = {x0 + 0x61707865u, x1 + 0x3320646eu, x2 + 0x79622d32u, x3 + 0x6b206574u,
+                             x4 + key[0], x5 + key[1], x6 + key[2], x7 + key[3], x8 + key[4], x9 + key[5], x10 + key[6],
+                             x11 + key[7], x12 + ctr, x13 + n0, x14 + n1, x15};
+#pragma unroll
+  for (int i = 0; i < Q_SEG; ++i) acc[i] = add ? acc[i] + w[i] : acc[i] - w[i];
+}
+#undef SA_QR
+
+// row of pair (i, j), i < j, in the key table: pairs in lexicographic order
+__device__ __forceinline__ int sa_pair_row(int i, int j, int K) { return i * (2 * K - i - 1) / 2 + (j - i - 1); }
+
+// Phase 0 of a SecAgg round: encode and mask the local replicas' updates on this CTA's tiles of every slice, and count
+// this thread's clipped and non-finite coordinates.  The key table is read with uniform loads (every thread of the CTA
+// reads the same 32 bytes).
+__device__ __forceinline__ void sa_encode(const CommArgs& a, int nslices, uint32_t& clipped, uint32_t& nonfinite) {
+  const float R = a.sa_clip;
+  const float scale = __int_as_float((127 + a.sa_frac_bits) << 23);            // 2^f, exact
+  const long long t = *a.q_t;
+  const uint32_t n0 = uint32_t(t), n1 = uint32_t(uint64_t(t) >> 32);
+  for (int s = 0; s < nslices; ++s) {
+    const QSlice sl = q_slice(a, s);
+    for (int tb = sl.lo + blockIdx.x * Q_TILE; tb < sl.hi; tb += gridDim.x * Q_TILE) {
+      const int c0 = tb + Q_SEG * threadIdx.x;
+      if (c0 >= sl.hi) continue;
+      float zv[Q_SEG];
+#pragma unroll
+      for (int q = 0; q < Q_SEG / 4; ++q) q_unf4(zv, q, q_ld4(a.z, c0 + 4 * q, a.n));
+      for (int j = 0; j < a.n_local; ++j) {
+        const int k = a.q_worker[j];
+        uint32_t acc[Q_SEG];
+#pragma unroll
+        for (int q = 0; q < Q_SEG / 4; ++q) {
+          const float4 xv = q_ld4(a.xl[j], c0 + 4 * q, a.n);       // coordinates >= n: u = 0, code 0
+          const float u4[4] = {__fsub_rn(xv.x, zv[4 * q]), __fsub_rn(xv.y, zv[4 * q + 1]), __fsub_rn(xv.z, zv[4 * q + 2]),
+                               __fsub_rn(xv.w, zv[4 * q + 3])};
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float u = u4[i];
+            int code = 0;
+            if (!isfinite(u)) {
+              ++nonfinite;
+            } else {
+              clipped += fabsf(u) > R ? 1u : 0u;
+              code = __float2int_rn(__fmul_rn(fminf(fmaxf(u, -R), R), scale));
+            }
+            acc[4 * q + i] = uint32_t(code);
+          }
+        }
+        const uint32_t ctr = uint32_t(c0 / Q_SEG);
+        for (int p = 0; p < a.K; ++p) {                            // uniform across the CTA
+          if (p == k) continue;
+          const uint4* kp = reinterpret_cast<const uint4*>(a.sa_keys + 8 * sa_pair_row(min(k, p), max(k, p), a.K));
+          const uint4 ka = __ldg(kp), kb = __ldg(kp + 1);
+          const uint32_t key[8] = {ka.x, ka.y, ka.z, ka.w, kb.x, kb.y, kb.z, kb.w};
+          sa_chacha_acc(key, ctr, n0, n1, p > k, acc);
+        }
+        uint4* dst = reinterpret_cast<uint4*>(a.q_codes[k] + 4 * size_t(c0));   // one 64-byte segment per thread
+#pragma unroll
+        for (int q = 0; q < Q_SEG / 4; ++q) dst[q] = make_uint4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+      }
+    }
+  }
+}
+
+// pass 1 of a SecAgg round at this thread's Q_SEG coordinates c0..: S = sum_k y_k mod 2^32 read as int32 (= sum_k q_k),
+// and acc = float(S) 2^-f, correctly rounded
+__device__ __forceinline__ void sa_gather(const CommArgs& a, int c0, float (&acc)[Q_SEG]) {
+  uint32_t s[Q_SEG];
+#pragma unroll
+  for (int i = 0; i < Q_SEG; ++i) s[i] = 0u;
+#pragma unroll 2
+  for (int k = 0; k < a.K; ++k) {
+    const unsigned char* src = a.q_codes[k] + 4 * size_t(c0);
+#pragma unroll
+    for (int q = 0; q < Q_SEG / 4; ++q) {                          // four 16-byte loads per peer
+      const uint4 v = ld_sys_u32x4(src + 16 * q);
+      s[4 * q] += v.x; s[4 * q + 1] += v.y; s[4 * q + 2] += v.z; s[4 * q + 3] += v.w;
+    }
+  }
+  const float inv = __int_as_float((127 - a.sa_frac_bits) << 23);             // 2^-f, exact
+#pragma unroll
+  for (int i = 0; i < Q_SEG; ++i) acc[i] = __fmul_rn(__int2float_rn(int(s[i])), inv);
+}
+
+// the sum over a CTA of a per-thread count, valid in thread 0 (integers: the order does not matter)
+__device__ __forceinline__ uint32_t block_add_u32(uint32_t v, uint32_t* sm) {
+  v = __reduce_add_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+  __syncthreads();
+  uint32_t r = 0u;
+  if (threadIdx.x < 32) r = __reduce_add_sync(0xffffffffu, threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : 0u);
+  __syncthreads();
+  return r;
+}
+
 // sum over the K workers, in worker order, of their dequantized codes q_k s_k at this thread's Q_SEG coordinates c0..
 template <int QBITS>
 __device__ __forceinline__ void q_gather(const CommArgs& a, int c0, float (&acc)[Q_SEG]) {
@@ -513,7 +633,8 @@ __device__ __forceinline__ void q_reduce(const CommArgs& a, int my_slice, float 
     const int c0 = tb + Q_SEG * threadIdx.x;
     if (c0 >= sl.hi) continue;
     float acc[Q_SEG];
-    q_gather<QBITS>(a, c0, acc);
+    if constexpr (QBITS == SA_QBITS) sa_gather(a, c0, acc);
+    else q_gather<QBITS>(a, c0, acc);
 #pragma unroll
     for (int q = 0; q < Q_SEG / 4; ++q) {
       const int c = c0 + 4 * q;
@@ -660,6 +781,9 @@ __device__ __forceinline__ float4 pass1_v4(const CommArgs& a, size_t off, float 
 // QBITS = 8 / 4: the compressed instantiations (mode 0, the mean): phase 0, before barrier A, encodes the local replicas'
 // updates into the payload arenas; pass 1 reduces the K workers' payloads instead of their floats, and both passes walk the
 // compressed tiling (no separate scalar tail); phase C exchanges the quantization statistics and advances q_t.
+// QBITS = SA_QBITS: the secure-aggregation instantiations (mode 0, the mean), on the compressed skeleton: phase 0 encodes
+// and masks the local replicas' updates into 32-bit payloads; pass 1 sums the K payloads as integers mod 2^32 and decodes;
+// phase C exchanges the integer clipped / non-finite counts, adds the latter to the non-finite count and advances q_t.
 // SAMP: the client-sampling instantiations (mode 0, the mean, AGG_PAD = 0): every CTA selects round *samp_t's participants
 // and their weights first; pass 1 (one-shot, two-shot and the scalar tail) forms the weighted sum of the participants out of
 // peer memory with P2P loads only (multimem.ld_reduce would add every bound device with weight 1; the two-shot broadcast
@@ -686,7 +810,17 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   const bool use_mc = !SAMP && a.mc_x != nullptr && (a.mode != 2 || a.mc_y != nullptr);
 
   // ---- 0 (compressed rounds): encode the local replicas' updates; per-CTA partial statistics in CTA order ------
-  if constexpr (QBITS != 0) {
+  if constexpr (QBITS == SA_QBITS) {             // SecAgg: integer counts of clipped and non-finite coordinates
+    uint32_t clipped = 0u, nonfinite = 0u;
+    sa_encode(a, nslices, clipped, nonfinite);
+    clipped = block_add_u32(clipped, reinterpret_cast<uint32_t*>(sm));      // (its barriers also publish the payload)
+    nonfinite = block_add_u32(nonfinite, reinterpret_cast<uint32_t*>(sm));
+    if (threadIdx.x == 0) {
+      reinterpret_cast<uint32_t*>(a.q_part)[2 * blockIdx.x + 0] = clipped;
+      reinterpret_cast<uint32_t*>(a.q_part)[2 * blockIdx.x + 1] = nonfinite;
+    }
+    if (a.world > 1) __threadfence_system();
+  } else if constexpr (QBITS != 0) {
     float err = 0.f, nrm = 0.f;
     q_encode<QBITS>(a, nslices, err, nrm);
     err = block_add(err, sm);                      // (its barriers also make the CTA's payload visible to all its threads)
@@ -704,7 +838,8 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   // ---- 1: reduce, scale, new z, dual residual ---------------------------------------------------------------------
   float dual = 0.f, bad = 0.f;
   if constexpr (QBITS != 0) {
-    q_reduce<FEDOPT, QBITS>(a, my_slice, inv_scale, dual, bad);
+    // SecAgg: 1/K correctly rounded (the extension is built with --use_fast_math), as the oracle's float32(1) / K
+    q_reduce<FEDOPT, QBITS>(a, my_slice, QBITS == SA_QBITS ? __frcp_rn(float(a.K)) : inv_scale, dual, bad);
   } else {
     const int lo = my_slice * chunk4;
     const int hi = min(n4, lo + chunk4);
@@ -968,9 +1103,55 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       *a.dp_t += 1;                                // every CTA has read t: the next round (or graph replay) draws t + 1
     }
   }
+  // SecAgg rounds (mode 0): the per-CTA counts, then over the ranks through the compressed rounds' pad row (as uint32
+  // bit patterns); the non-finite updates join the record's non-finite count, so the NaN guard fires although their
+  // codes are 0
+  if constexpr (QBITS == SA_QBITS) {
+    __shared__ uint32_t s_sa[2];
+    if (threadIdx.x == 0) {
+      uint32_t c = 0u, b = 0u;
+      for (int i = 0; i < int(gridDim.x); ++i) {
+        c += __ldcg(reinterpret_cast<const unsigned int*>(a.q_part) + 2 * i + 0);
+        b += __ldcg(reinterpret_cast<const unsigned int*>(a.q_part) + 2 * i + 1);
+      }
+      s_sa[0] = c;
+      s_sa[1] = b;
+    }
+    __syncthreads();
+    if (a.world > 1) {
+      if (threadIdx.x < a.world) {
+        float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_Q_PAYLOAD) + 2 * a.rank;
+        st_sys_f32(pay + 0, __uint_as_float(s_sa[0]));
+        st_sys_f32(pay + 1, __uint_as_float(s_sa[1]));
+        __threadfence_system();
+        st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_C + a.rank, epoch);
+        if (s_abort == 0 && !wait_flag(a.ctrl[a.rank] + PAD_FLAG_C + threadIdx.x, epoch, a.timeout_cycles)) {
+          a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
+          atomicExch(&s_abort, 1);
+        }
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_Q_PAYLOAD);
+        uint32_t c = 0u, b = 0u;
+        for (int r = 0; r < a.world; ++r) {
+          c += __float_as_uint(ld_sys_f32(pay + 2 * r + 0));
+          b += __float_as_uint(ld_sys_f32(pay + 2 * r + 1));
+        }
+        s_sa[0] = c;
+        s_sa[1] = b;
+      }
+    }
+    if (threadIdx.x == 0) {
+      a.out[OUT_SA_CLIPPED] = __uint_as_float(s_sa[0]);
+      a.out[OUT_SA_NONFINITE] = __uint_as_float(s_sa[1]);
+      nonfinite += float(s_sa[1]);
+      *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) masks with t + 1
+    }
+  }
   // compressed rounds (mode 0): the per-CTA partial statistics in CTA order, then over the ranks in rank order, so every
   // rank reports the same values
-  if constexpr (QBITS != 0) {
+  if constexpr (QBITS != 0 && QBITS != SA_QBITS) {
     __shared__ float s_q[2];
     if (threadIdx.x == 0) {
       float e = 0.f, u = 0.f;
@@ -1081,21 +1262,39 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
     if (args.mode != 0 || args.agg != AGG_MEAN || args.dp || args.qbits != 0)
       throw std::runtime_error("fedb200: block_reduce: client sampling needs mode 0 and the mean, without DP or compression");
   }
+  if (args.sa) {
+    if (args.mode != 0 || args.agg != AGG_MEAN || args.dp || args.qbits != 0 || samp)
+      throw std::runtime_error("fedb200: block_reduce: secure aggregation needs mode 0 and the mean, without DP, "
+                               "compression or sampling");
+    if (args.K < 2) throw std::runtime_error("fedb200: block_reduce: secure aggregation needs at least 2 workers");
+    if (args.sa_keys == nullptr || args.q_t == nullptr || args.q_part == nullptr)
+      throw std::runtime_error("fedb200: block_reduce: secure aggregation needs the pair keys, a round counter and a "
+                               "statistics buffer");
+    if (args.sa_frac_bits < 0 || args.sa_frac_bits > SA_MAX_FRAC_BITS || !(args.sa_clip > 0.f))
+      throw std::runtime_error("fedb200: block_reduce: secure aggregation needs 0 <= f <= 126 and a clip > 0");
+    for (int k = 0; k < args.K; ++k)
+      if (args.q_codes[k] == nullptr) throw std::runtime_error("fedb200: block_reduce: secure aggregation needs K payloads");
+    if (args.two_shot && (args.xw[args.world - 1] == nullptr || (args.opt != FEDOPT_NONE && args.mw[args.world - 1] == nullptr)))
+      throw std::runtime_error("fedb200: block_reduce: two-shot secure aggregation needs P2P broadcast targets");
+  }
   const bool fo = args.opt != FEDOPT_NONE;
-  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean, 8-bit codes, 4-bit codes, sampled weighted mean]
-  const void* kernels[2][8] = {
+  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean, 8-bit codes, 4-bit codes, sampled weighted
+  // mean, secure aggregation]
+  const void* kernels[2][9] = {
       {(const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
        (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>,
        (const void*)block_reduce_kernel<false, 0, true>, (const void*)block_reduce_kernel<false, 0, false, 8>,
-       (const void*)block_reduce_kernel<false, 0, false, 4>, (const void*)block_reduce_kernel<false, 0, false, 0, true>},
+       (const void*)block_reduce_kernel<false, 0, false, 4>, (const void*)block_reduce_kernel<false, 0, false, 0, true>,
+       (const void*)block_reduce_kernel<false, 0, false, SA_QBITS>},
       {(const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
        (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>,
        (const void*)block_reduce_kernel<true, 0, true>, (const void*)block_reduce_kernel<true, 0, false, 8>,
-       (const void*)block_reduce_kernel<true, 0, false, 4>, (const void*)block_reduce_kernel<true, 0, false, 0, true>}};
-  const int pad = samp ? 7 : args.qbits == 8 ? 5 : args.qbits == 4 ? 6 : args.dp ? 4 : args.agg == AGG_MEAN ? 0
+       (const void*)block_reduce_kernel<true, 0, false, 4>, (const void*)block_reduce_kernel<true, 0, false, 0, true>,
+       (const void*)block_reduce_kernel<true, 0, false, SA_QBITS>}};
+  const int pad = args.sa ? 8 : samp ? 7 : args.qbits == 8 ? 5 : args.qbits == 4 ? 6 : args.dp ? 4 : args.agg == AGG_MEAN ? 0
                 : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
   const void* kernel = kernels[fo][pad];
-  static int max_blocks[2][8] = {};
+  static int max_blocks[2][9] = {};
   int& mb = max_blocks[fo][pad];
   if (mb == 0) mb = comm_max_blocks(kernel);
   int cap = mb;
@@ -1103,7 +1302,7 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   const int n4 = args.n >> 2;
   const int work4 = args.two_shot ? (n4 + args.world - 1) / args.world : n4;
   int want = (work4 + COMM_THREADS - 1) / COMM_THREADS;
-  if (args.qbits != 0) {                               // one tile of COMM_THREADS * Q_SEG coordinates per CTA and step
+  if (args.qbits != 0 || args.sa) {                    // one tile of COMM_THREADS * Q_SEG coordinates per CTA and step
     const int ng = (args.n + Q_GROUP - 1) / Q_GROUP;
     const int per = args.two_shot ? (ng + args.world - 1) / args.world : ng;
     want = (per * Q_GROUP + Q_TILE - 1) / Q_TILE;

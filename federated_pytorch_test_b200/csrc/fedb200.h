@@ -201,7 +201,10 @@ static_assert(PAD_Q_PAYLOAD + 2 * COMM_MAX_WORLD <= COMM_PAD_WORDS, "control pad
 constexpr int OUT_DUAL_SQ = 0, OUT_PRIMAL = 1, OUT_NONFINITE = 2, OUT_STATUS = 3, OUT_RHO = 4, OUT_EPOCH = 5, OUT_TWO_SHOT = 6;
 constexpr int OUT_DP_CLIPPED = 8, OUT_DP_NORM_SUM = 9;
 constexpr int OUT_Q_ERR_SQ = 10, OUT_Q_NORM_SQ = 11;
-constexpr int COMM_OUT_FLOATS = 12;
+// secure-aggregation rounds: the number of clipped and of non-finite coordinates over all K, as uint32 bit patterns
+// (integers: float counts stop being exact above 2^24)
+constexpr int OUT_SA_CLIPPED = 12, OUT_SA_NONFINITE = 13;
+constexpr int COMM_OUT_FLOATS = 14;
 // device scratch (floats): [0] dual^2, [1] #non-finite, [2] ticket (as uint), [4 + j] per-replica primal^2; self-cleaning
 constexpr int COMM_SCRATCH_FLOATS = 4 + COMM_MAX_LOCAL;
 
@@ -273,6 +276,16 @@ struct CommArgs {
   unsigned long long samp_key;       // key of the run's sampling stream
   long long* samp_t;                 // device: index t of this sampled round over the run; the last CTA increments it
   const int* client_n;               // device: [K] sample counts n_k of the workers' shards
+  // ---- secure aggregation (SecAgg, Bonawitz et al. 2017; mode 0 with the mean, with or without a server optimizer,
+  // without DP, compression or sampling): before barrier A every rank encodes its local replicas' updates u = x_k - z as
+  // int32 fixed-point codes q = rint(clamp(u, -R, R) 2^f) and uploads y_k = q_k + sum_{j>k} m_kj - sum_{j<k} m_jk
+  // (mod 2^32), m_ij the ChaCha20 keystream of pair key ij under nonce t.  The masks cancel in the sum, so pass 1 decodes
+  // z' = z + (float(sum_k y_k) 2^-f) / K exactly.  The rounds use the compressed rounds' q_codes (as 4-byte words, one
+  // per coordinate), q_t (the nonce t), q_worker and q_part (per-CTA integer counts).
+  int sa;                            // 0 selects the instantiations above
+  int sa_frac_bits;                  // f: K rint(R 2^f) <= 2^31 - 1, 0 <= f <= 126
+  float sa_clip;                     // R
+  const uint32_t* sa_keys;           // device: [K (K - 1) / 2][8] pair keys, pairs (i < j) in lexicographic order
 };
 constexpr int Q_GROUP = 128;                             // coordinates per scale
 constexpr int Q_SEG = 16;                                // coordinates per thread and tile in the compressed instantiations
@@ -281,8 +294,9 @@ constexpr int DP_CHUNK = 32;
 constexpr int FEDOPT_NONE = 0, FEDOPT_AVGM = 1, FEDOPT_ADAGRAD = 2, FEDOPT_ADAM = 3, FEDOPT_YOGI = 4;
 constexpr int AGG_MEAN = 0, AGG_MEDIAN = 1, AGG_TRIMMED = 2;
 constexpr int COMM_MAX_K_ROBUST = 16;
-// block_reduce_launch picks the instantiation: the mean, a robust rule, DP, compressed codes (qbits) or client sampling
-// (samp_S); it rejects combinations the kernel does not implement.
+constexpr int SA_MAX_FRAC_BITS = 126;                   // 2^f and 2^-f stay normal floats
+// block_reduce_launch picks the instantiation: the mean, a robust rule, DP, compressed codes (qbits), client sampling
+// (samp_S) or secure aggregation (sa); it rejects combinations the kernel does not implement.
 void block_reduce_launch(const CommArgs& args, cudaStream_t s);
 
 // DP-FedAvg update clipping on the local replicas, as ONE cooperative kernel touching no peer memory: ||x_j - z|| per

@@ -11,7 +11,9 @@ one device):
   ``compress=`` on ``fedavg_`` / ``fedopt_`` every worker uploads its update ``x_k - z`` as stochastically rounded 8- or
   4-bit codes with one scale per group (``algo/compress.py``), and ``z' = z + mean_k q_k s_k``; with ``sample=`` on
   ``fedavg_`` / ``fedopt_`` only the round's ``S`` sampled workers are averaged, weighted by their sample counts
-  (``z' = sum_{k in P} n_k x_k / sum_{k in P} n_k``, ``algo/sampling.py``), and every replica receives ``z'``
+  (``z' = sum_{k in P} n_k x_k / sum_{k in P} n_k``, ``algo/sampling.py``), and every replica receives ``z'``; with
+  ``secagg=`` on ``fedavg_`` / ``fedopt_`` every worker uploads its update ``x_k - z`` as int32 fixed-point codes masked
+  with pairwise ChaCha20 keystreams that cancel in the sum (``algo/secagg.py``), and ``z' = z + decode(sum_k y_k)``
 * X2 FedProx ``z' = mean``; ``dual``; ``primal = sum_k ||rho (x_k - z')||``; no write-back
   (fedprox_multi.py:211-232)
 * X3 ADMM    ``z' = sum_k (y_k + rho x_k) / (K rho)``; ``dual``; ``y_k += rho (x_k - z')``;
@@ -30,6 +32,7 @@ from __future__ import annotations
 from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -97,6 +100,21 @@ class SampleRound:
     n: torch.Tensor
 
 
+@dataclass
+class SecAggRound:
+    """Secure aggregation of one round (``algo/secagg.py``): clip ``R``, fixed-point bits ``f``, the pair-key table
+    ``keys`` (int32 ``[K (K - 1) / 2, 8]`` on the block's device, the uint32 words of :func:`secagg.pair_keys`) and ``t``,
+    a one-element int64 tensor on the block's device holding the round index over the run (the nonce; advanced by the
+    round).  ``payload`` holds the local replicas' payload slices (int32, 4 bytes per coordinate in whole segments of 16;
+    :meth:`TorchCollective.payload32_like_block`; on the fused collective peers read them)."""
+
+    clip: float
+    f: int
+    keys: torch.Tensor
+    t: torch.Tensor
+    payload: List[torch.Tensor]
+
+
 class TorchCollective:
     """ATen + torch.distributed implementation (baseline / oracle / CPU)."""
 
@@ -108,6 +126,7 @@ class TorchCollective:
         self.launches = 0  # number of framework-owned kernels launched (0 here: library path)
         self.last_dp = (0.0, 0.0)   # DP rounds: (#clipped workers, sum of their pre-clip update norms) over all K
         self.last_q = (0.0, 0.0)    # compressed rounds: (sum_k ||u_k - q_k s_k||^2, sum_k ||u_k||^2) over all K
+        self.last_sa = (0, 0)       # secure-aggregation rounds: (#clipped, #non-finite coordinates) over all K
 
     # -- arena hooks ------------------------------------------------------
     def arena_allocator(self) -> Optional[Callable]:
@@ -131,6 +150,11 @@ class TorchCollective:
         n = x.numel()
         return (torch.zeros(-(-n // 16) * 2 * bits, dtype=torch.uint8, device=x.device),
                 torch.zeros(-(-n // GROUP), dtype=torch.float32, device=x.device))
+
+    def payload32_like_block(self, x: torch.Tensor) -> torch.Tensor:
+        """Zeroed secure-aggregation payload of block slice ``x``: int32, one word per coordinate, whole segments of 16
+        coordinates (one ChaCha20 block each).  The fused backend hands out slices of symmetric arenas."""
+        return torch.zeros(-(-x.numel() // 16) * 16, dtype=torch.int32, device=x.device)
 
     # -- primitives -------------------------------------------------------
     def _allreduce(self, t: torch.Tensor) -> torch.Tensor:
@@ -274,6 +298,28 @@ class TorchCollective:
         return acc.mul_(1.0 / self.topo.K)
 
     @torch.no_grad()
+    def _secagg_update(self, xs: List[torch.Tensor], z: torch.Tensor, sa: SecAggRound) -> torch.Tensor:
+        """``d = decode(sum_k y_k)`` of a secure-aggregation round: every local replica's update is encoded and masked with
+        the oracle (into its payload slice), the K payloads are gathered and summed as integers mod 2^32, then decoded.
+        Advances ``sa.t``; the counts go to :attr:`last_sa`."""
+        from ..algo import secagg
+
+        K, t, n = self.topo.K, int(sa.t.item()), z.numel()
+        keys = sa.keys.cpu().numpy().view(np.uint32)
+        zn = z.detach().float().cpu().numpy()
+        pays, counts = [], torch.zeros(2, dtype=torch.int64)
+        for j, (x, ck) in enumerate(zip(xs, self.topo.local_workers)):
+            q, clipped, nonfinite = secagg.encode(x.detach().float().cpu().numpy() - zn, sa.clip, sa.f)
+            y = torch.from_numpy(secagg.payload(q, keys, K, ck, t).view(np.int32))
+            sa.payload[j][:n].copy_(y)
+            pays.append((y.long() & 0xFFFFFFFF).to(z.device))
+            counts += torch.tensor([clipped, nonfinite])
+        S = self.gather_blocks(pays).sum(dim=0).remainder_(1 << 32).cpu().numpy().astype(np.uint32).view(np.int32)
+        self.last_sa = tuple(int(v) for v in self.sum_scalars(counts.to(z.device)).tolist())
+        sa.t.add_(1)
+        return torch.from_numpy(secagg.decode(S, sa.f, K)).to(z.device)
+
+    @torch.no_grad()
     def _sampled_mean(self, xs: List[torch.Tensor], s: SampleRound) -> torch.Tensor:
         """``sum_{k in P} w_k x_k`` of sampled round ``t = s.t`` (``algo/sampling.py``), summed in float32 in worker order,
         each term rounded before it is added; the K blocks are gathered, only the participants' rows are used.
@@ -294,12 +340,15 @@ class TorchCollective:
     @torch.no_grad()
     def fedavg_(self, xs: List[torch.Tensor], z: torch.Tensor, write_back: bool = True,
                 dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None) -> torch.Tensor:
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> torch.Tensor:
         """In place: ``z <- mean_k x_k``, optionally ``x_k <- z``; returns ``||z_old - z_new||^2`` (0-dim).  With ``dp``
         the mean is noised (:class:`DPRound`; clip the replicas with :meth:`dp_clip_` first).  With ``compress``
         (:class:`QuantRound`) ``z <- z + (1/K) sum_k q_k s_k``, the workers' updates as uploaded.  With ``sample``
-        (:class:`SampleRound`) ``z <-`` the sample-weighted mean of the round's participants; every replica receives it."""
-        if sample is not None:
+        (:class:`SampleRound`) ``z <-`` the sample-weighted mean of the round's participants; every replica receives it.
+        With ``secagg`` (:class:`SecAggRound`) ``z <- z + d``, ``d`` decoded from the sum of the masked payloads."""
+        if secagg is not None:
+            znew = z + self._secagg_update(xs, z, secagg)
+        elif sample is not None:
             znew = self._sampled_mean(xs, sample)
         elif compress is not None:
             znew = z + self._compressed_update(xs, z, compress)
@@ -333,15 +382,18 @@ class TorchCollective:
     def fedopt_(self, xs: List[torch.Tensor], z: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], kind: str,
                 lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean", trim_b: int = 0,
                 dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None) -> torch.Tensor:
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> torch.Tensor:
         """FedAvg with a server optimizer, in place: ``d = mean_k x_k - z`` is the pseudo-gradient of server optimizer
         ``kind`` (one of :data:`FEDOPT_KINDS`; ``beta1`` is the momentum of 'avgm'), whose state ``m`` (and ``v``, unused
         by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``.
         With a robust rule ``agg`` (one of :data:`ROBUST_AGGS`) its aggregate replaces the mean in ``d``; with ``dp`` the
         noised mean does (DP-FedOpt: post-processing); with ``compress`` ``d`` is the dequantized mean update itself
-        (FedPAQ with a server optimizer); with ``sample`` the sample-weighted mean of the round's participants does."""
+        (FedPAQ with a server optimizer); with ``sample`` the sample-weighted mean of the round's participants does; with
+        ``secagg`` ``d`` is the decoded sum of the masked payloads."""
         mean = None
-        if sample is not None:
+        if secagg is not None:
+            d = self._secagg_update(xs, z, secagg)
+        elif sample is not None:
             mean = self._sampled_mean(xs, sample)
         elif compress is not None:
             d = self._compressed_update(xs, z, compress)

@@ -46,21 +46,30 @@ Sampled rounds (client sampling with sample-count weights) are one launch of the
 selects the round's participants from the device-resident round counter, and pass 1 forms their weighted sum with P2P
 loads of the participants only (``multimem.ld_reduce`` sums every bound device with weight 1; the two-shot broadcast may
 still use ``multimem.st``).  A worker that sits out is never read, and receives the new model in pass 2.
+
+Secure-aggregation rounds (pairwise-masked fixed-point updates) are one launch of the SecAgg instantiations, on the
+compressed rounds' tiling: before barrier A every rank encodes its own replicas' updates as int32 codes and adds or
+subtracts the K - 1 ChaCha20 keystreams of its pairs, computed in registers, into 32-bit symmetric payload arenas
+(:meth:`FusedCollective.payload32_like_block`); pass 1 sums the K payloads over P2P as integers mod 2^32, where the masks
+cancel, and decodes.  The sum is exact, so the new model does not depend on the process layout or on one-shot versus
+two-shot.  The nonce counter lives in device memory as the DP one.
 """
 from __future__ import annotations
 
 import os
+import struct
 from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
 
 from ..ops import cuda_ops
-from .collective import FEDOPT_KINDS, ROBUST_AGGS, DPRound, QuantRound, SampleRound, TorchCollective, check_robust
+from .collective import (FEDOPT_KINDS, ROBUST_AGGS, DPRound, QuantRound, SampleRound, SecAggRound, TorchCollective,
+                         check_robust)
 from .topology import Topology
 
 _MAX_LOCAL = 16
-_OUT_FLOATS = 12
+_OUT_FLOATS = 14
 _SCRATCH_FLOATS = 4 + _MAX_LOCAL
 _MAX_BLOCKS = 160                                         # csrc/fedb200.h: COMM_MAX_BLOCKS
 _DP_STATS_FLOATS = 2 * _MAX_LOCAL * _MAX_BLOCKS + 2 * _MAX_LOCAL      # DP_STATS_FLOATS: double partials, norms, flags
@@ -71,6 +80,7 @@ _PAD_WORDS = 8192
 OUT_DUAL_SQ, OUT_PRIMAL, OUT_NONFINITE, OUT_STATUS, OUT_RHO, OUT_EPOCH, OUT_TWO_SHOT = range(7)
 OUT_DP_CLIPPED, OUT_DP_NORM_SUM = 8, 9
 OUT_Q_ERR_SQ, OUT_Q_NORM_SQ = 10, 11
+OUT_SA_CLIPPED, OUT_SA_NONFINITE = 12, 13              # uint32 bit patterns
 
 TWO_SHOT_MIN_BYTES = int(os.environ.get("FEDB200_TWO_SHOT_BYTES", str(256 * 1024)))
 TWO_SHOT_MODE = os.environ.get("FEDB200_TWO_SHOT", "auto")          # 'auto' | '0' (never) | '1' (whenever legal)
@@ -200,6 +210,7 @@ class FusedCollective(TorchCollective):
         self.warm_dp = False              # set by DP strategies: warm the clip kernel and the DP instantiation(s) too
         self.warm_compress = 0            # set by compressing strategies to their bit width: warm those instantiations too
         self.warm_sample = False          # set by sampling strategies: warm the sampled instantiation(s) too
+        self.warm_secagg = False          # set by secure-aggregation strategies: warm the SecAgg instantiation(s) too
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
@@ -207,8 +218,8 @@ class FusedCollective(TorchCollective):
         is far slower than the ones after it).  The server-optimizer kernel is warmed only when ``warm_fedopt`` is set, the
         robust kernels (of this K; with the server optimizer if both are set) only when ``warm_robust`` is set, the DP
         kernels (likewise) only when ``warm_dp`` is set, the compressed ones of ``warm_compress`` bits (likewise) only when
-        that is set, the sampled ones (likewise) only when ``warm_sample`` is set; their round counters are throwaway
-        tensors, so warm-up advances no counter of the run.
+        that is set, the sampled ones (likewise) only when ``warm_sample`` is set, the SecAgg ones (likewise) only when
+        ``warm_secagg`` is set; their round counters are throwaway tensors, so warm-up advances no counter of the run.
         Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
@@ -227,6 +238,11 @@ class FusedCollective(TorchCollective):
         if self.warm_sample:
             sr = SampleRound(1, 0, torch.zeros(1, dtype=torch.int64, device=self.topo.device),
                              torch.ones(self.topo.K, dtype=torch.int32, device=self.topo.device))
+        if self.warm_secagg:
+            K = self.topo.K
+            sa = SecAggRound(1.0, 0, torch.zeros(K * (K - 1) // 2, 8, dtype=torch.int32, device=self.topo.device),
+                             torch.zeros(1, dtype=torch.int64, device=self.topo.device),
+                             [self.payload32_like_block(x) for x in xs])
         keep = self.two_shot_mode
         for mode_2shot in ("0", "1"):
             self.two_shot_mode = mode_2shot
@@ -253,6 +269,10 @@ class FusedCollective(TorchCollective):
                 self._launch(0, xs, None, z, 0.0, sample=sr)
                 if self.warm_fedopt:
                     self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, sample=sr)
+            if self.warm_secagg:
+                self._launch(0, xs, None, z, 0.0, secagg=sa)
+                if self.warm_fedopt:
+                    self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, secagg=sa)
         self.two_shot_mode = keep
         x0 = [torch.zeros_like(x) for x in xs]
         yh = [torch.zeros_like(x) for x in xs]
@@ -302,6 +322,12 @@ class FusedCollective(TorchCollective):
         codes.zero_()
         scales.zero_()
         return codes, scales
+
+    def payload32_like_block(self, x: torch.Tensor) -> torch.Tensor:
+        """The secure-aggregation payload slice of block slice ``x`` (layout: :meth:`TorchCollective.payload32_like_block`):
+        the codes arena of :meth:`payload_like_block` for 32-bit codes, viewed as int32, so the arena's float ``i`` has its
+        word at word ``i`` and every block slice its own payload at the same offset in every rank."""
+        return self.payload_like_block(x, 32)[0].view(torch.int32)
 
     # -- pointer tables -------------------------------------------------------------
     def _tables(self, slices: List[torch.Tensor]):
@@ -362,18 +388,28 @@ class FusedCollective(TorchCollective):
         key = int(s.key) & ((1 << 64) - 1)
         return int(s.S), key - (1 << 64) if key >= 1 << 63 else key, s.t, s.n
 
+    def _sa_args(self, sa: Optional[SecAggRound]):
+        """The secure-aggregation arguments of the aggregation bindings: f, clip, pair keys, counter, the K workers' payload
+        pointers, the statistics buffer."""
+        if sa is None:
+            return 0, 0.0, None, None, [], None
+        pp, _, _ = self._tables(sa.payload)
+        return int(sa.f), float(sa.clip), sa.keys, sa.t, pp, self.q_part
+
     def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None, agg: str = "mean", trim_b: int = 0,
                 dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None) -> None:
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> None:
         """Modes 0 / 1 take a robust rule ``agg`` (:data:`ROBUST_AGGS`) in place of the mean; mode 0 with the mean takes
-        the noise of a DP round (``dp``; after :meth:`dp_clip_`), compresses the workers' updates (``compress``) or
-        averages the sampled participants of the round (``sample``)."""
+        the noise of a DP round (``dp``; after :meth:`dp_clip_`), compresses the workers' updates (``compress``),
+        averages the sampled participants of the round (``sample``) or sums their masked updates (``secagg``)."""
         if dp is not None and (mode != 0 or agg != "mean"):
             raise ValueError("DP aggregation needs FedAvg with the mean")
         if compress is not None and (mode != 0 or agg != "mean" or dp is not None):
             raise ValueError("compressed aggregation needs FedAvg with the mean, without DP")
         if sample is not None and (mode != 0 or agg != "mean" or dp is not None or compress is not None):
             raise ValueError("sampled aggregation needs FedAvg with the mean, without DP or compression")
+        if secagg is not None and (mode != 0 or agg != "mean" or dp is not None or compress is not None or sample is not None):
+            raise ValueError("secure aggregation needs FedAvg with the mean, without DP, compression or sampling")
         code = self._agg_code(agg, trim_b)
         n = xs[0].numel()
         if any(t.numel() != n for t in xs) or z.numel() != n:
@@ -397,18 +433,19 @@ class FusedCollective(TorchCollective):
         self.ext.block_reduce(mode, xp, yp, local_idx, z, n, float(rho), rho_dev, self.out, self.scratch, self.ctrl_ptrs,
                               self.sync, W, self.topo.rank, mcx, mcy, mcz, xw, zw, bool(two), self.max_blocks,
                               self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress),
-                              *self._samp_args(sample))
+                              *self._samp_args(sample), *self._sa_args(secagg))
         self.launches += 1
         self.last_two_shot = bool(two)
 
     def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
                        trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                       sample: Optional[SampleRound] = None) -> None:
+                       sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> None:
         """FedAvg with a server optimizer: mode 0 of the kernel's FedOpt instantiation.  Two-shot, rank r broadcasts slice r
         of the new weights, of ``m`` and of ``v`` into every rank, so ``m`` / ``v`` must be symmetric slices then
         (:meth:`zeros_like_block`).  A robust rule ``agg`` replaces the mean as the aggregate the step is taken towards; a
         DP round (``dp``, mean only) noises the mean first; a compressed round (``compress``, mean only) steps along the
-        dequantized mean update; a sampled round (``sample``, mean only) steps towards the participants' weighted mean."""
+        dequantized mean update; a sampled round (``sample``, mean only) steps towards the participants' weighted mean; a
+        SecAgg round (``secagg``, mean only) steps along the decoded sum of the masked updates."""
         code = self._agg_code(agg, trim_b)
         if dp is not None and agg != "mean":
             raise ValueError("DP aggregation needs the mean")
@@ -416,6 +453,8 @@ class FusedCollective(TorchCollective):
             raise ValueError("compressed aggregation needs the mean, without DP")
         if sample is not None and (agg != "mean" or dp is not None or compress is not None):
             raise ValueError("sampled aggregation needs the mean, without DP or compression")
+        if secagg is not None and (agg != "mean" or dp is not None or compress is not None or sample is not None):
+            raise ValueError("secure aggregation needs the mean, without DP, compression or sampling")
         n = xs[0].numel()
         adaptive = kind != "avgm"
         if any(t.numel() != n for t in xs) or z.numel() != n or m.numel() != n or (adaptive and v.numel() != n):
@@ -434,7 +473,7 @@ class FusedCollective(TorchCollective):
                                      v if adaptive else None, xp, local_idx, z, n, self.out, self.scratch, self.ctrl_ptrs,
                                      self.sync, W, self.topo.rank, mcx, mcm, mcv, xw, mw, vw, bool(two), self.max_blocks,
                                      self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress),
-                                     *self._samp_args(sample))
+                                     *self._samp_args(sample), *self._sa_args(secagg))
         self.launches += 1
         self.last_two_shot = bool(two)
 
@@ -450,14 +489,15 @@ class FusedCollective(TorchCollective):
             self._out_pending = True
 
     def launch_fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
-                       compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None) -> None:
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample)
+                       compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None,
+                       secagg: Optional[SecAggRound] = None) -> None:
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample, secagg=secagg)
         self._record_async()
 
     def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
                        trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                       sample: Optional[SampleRound] = None) -> None:
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample)
+                       sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> None:
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample, secagg)
         self._record_async()
 
     @torch.no_grad()
@@ -498,13 +538,15 @@ class FusedCollective(TorchCollective):
         self.last_rho = vals[OUT_RHO]
         self.last_dp = (vals[OUT_DP_CLIPPED], vals[OUT_DP_NORM_SUM])
         self.last_q = (vals[OUT_Q_ERR_SQ], vals[OUT_Q_NORM_SQ])
+        self.last_sa = struct.unpack("<2I", struct.pack("<2f", vals[OUT_SA_CLIPPED], vals[OUT_SA_NONFINITE]))
         return vals
 
     # -- operators ----------------------------------------------------------------------
     @torch.no_grad()
     def fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
-                compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None):
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample)
+                compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None,
+                secagg: Optional[SecAggRound] = None):
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample, secagg=secagg)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
@@ -515,8 +557,8 @@ class FusedCollective(TorchCollective):
     @torch.no_grad()
     def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
                 trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None):
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample)
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None):
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample, secagg)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
