@@ -8,6 +8,7 @@ batch-statistics BatchNorm ``:108-121`` (Q4, Q5), end-of-run checkpoints ``:226-
 """
 from __future__ import annotations
 
+import functools
 import os
 from typing import Callable, Dict, Iterator, List, Optional, Tuple
 
@@ -16,7 +17,7 @@ import torch.nn as nn
 
 from .. import models
 from ..algo.engine import Engine, EngineConfig, Replica, Task, Visit
-from ..config import CommonConfig, check_partition
+from ..config import CommonConfig, check_norm, check_partition
 from ..data.cifar import (CifarData, ShardLoader, augment_key, class_histogram, dirichlet_shards, shard_ranges,
                           worker_norm)
 from ..ops import functional as FX
@@ -31,6 +32,12 @@ _MODEL_FACTORIES = {
     "Net": models.Net, "Net1": models.Net1, "Net2": models.Net2,
     "ResNet18": models.ResNet18, "ResNet9": models.ResNet9,
 }
+
+
+def require_batch_norm(cfg: CommonConfig, driver: str) -> None:
+    """The VAE, VAE-CL and CPC networks have no GroupNorm variant and accept only the default ``norm``."""
+    if getattr(cfg, "norm", "batch") != "batch":
+        raise ValueError("%s supports only norm 'batch', got norm %r" % (driver, cfg.norm))
 
 
 def require_iid(cfg: CommonConfig, driver: str) -> None:
@@ -83,7 +90,11 @@ class ClassifierTask(Task):
             raise ValueError("eval_bn must be 'batch' or 'running', got %r" % (cfg.eval_bn,))
         name = cfg.model or ("ResNet18" if cfg.use_resnet else "Net")
         self.model_name = name
+        norm = getattr(cfg, "norm", "batch")
+        check_norm(norm, getattr(cfg, "norm_groups", 32), name)
         self.factory = _MODEL_FACTORIES[name]
+        if norm != "batch":
+            self.factory = functools.partial(self.factory, norm=norm, groups=cfg.norm_groups)
         self.data = load_cifar(cfg, topo.device)
         partition = getattr(cfg, "partition", "iid")
         check_partition(partition, getattr(cfg, "dirichlet_alpha", 0.5))
@@ -195,7 +206,8 @@ class ClassifierTask(Task):
         By default networks stay in training mode as in the reference (Q4): BatchNorm
         uses batch statistics and keeps updating its running statistics on test data.
         With ``eval_bn='running'`` each network is evaluated in eval mode (running
-        statistics, left unchanged) and put back into training mode afterwards.  Runs
+        statistics, left unchanged) and put back into training mode afterwards.  A
+        GroupNorm network computes the same in either mode.  Runs
         under ``no_grad`` (no numerical effect).  Counting stays on the device; one
         read per replica.
         """

@@ -61,6 +61,7 @@ class VAETask(common.ClassifierTask):
 
 def run(cfg: Config, log=print):
     common.require_iid(cfg, "federated_vae")
+    common.require_batch_norm(cfg, "federated_vae")
     topo, coll = common.setup_runtime(cfg)
     task = VAETask(cfg, topo)
     engine = common.run_engine(cfg, task, topo, coll, FedAvg(coll, topo), None, log)

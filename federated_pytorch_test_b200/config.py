@@ -48,7 +48,12 @@ class CommonConfig:
     intended_elastic_net_gate: bool = False  # Q2: regularise whenever the block holds dense-layer weights
     diagnostics: str = "post"       # Q17: 'post' (extra forward after the step) | 'pre'
     eval_bn: str = "batch"          # Q4: 'batch' (reference: train-mode BN at evaluation, running stats updated by test data) | 'running' (net.eval())
-                                    # classifier drivers only: the VAE, VAE-CL and CPC networks have no BatchNorm and do not evaluate
+                                    # classifier drivers only: the VAE, VAE-CL and CPC networks have no BatchNorm and do not evaluate;
+                                    # no effect with norm 'group' (GroupNorm has no running statistics)
+    # normalisation of the ResNets: 'batch' (the reference) | 'group' = GroupNorm with norm_groups groups in every layer
+    # (Wu & He 2018), which normalises each sample on its own and mixes no worker's data statistics into the model
+    norm: str = "batch"
+    norm_groups: int = 32           # must divide 64, the narrowest layer
     augment: bool = False           # random 4-pixel-padded crop + horizontal flip of training batches (classifier drivers only)
     nan_guard: str = "raise"        # non-finite aggregation residual: 'raise' | 'warn' | 'off'
     collective: str = "auto"        # 'auto' | 'fused' | 'torch'
@@ -135,6 +140,21 @@ def check_dp(dp_clip: float, dp_noise: float, dp_delta: float, aggregator: str) 
     if dp_clip > 0.0 and aggregator != "mean":
         raise ValueError("dp_clip needs aggregator 'mean' (robust rules have a different sensitivity), got aggregator %r"
                          % (aggregator,))
+
+
+NORMS = ("batch", "group")
+NORM_MODELS = ("ResNet18", "ResNet9")      # the models with a normalisation layer
+
+
+def check_norm(norm: str, norm_groups: int, model: str) -> None:
+    """Raise ``ValueError`` unless the normalisation settings of :class:`CommonConfig` are valid for ``model``."""
+    if norm not in NORMS:
+        raise ValueError("norm must be one of %s, got %r" % (", ".join(NORMS), norm))
+    if not (isinstance(norm_groups, int) and norm_groups >= 1 and 64 % norm_groups == 0):
+        raise ValueError("norm_groups must divide 64 (the narrowest layer), got %r" % (norm_groups,))
+    if norm != "batch" and model not in NORM_MODELS:
+        raise ValueError("norm %r needs a model with normalisation layers (%s), got model %r"
+                         % (norm, ", ".join(NORM_MODELS), model))
 
 
 PARTITIONS = ("iid", "dirichlet")

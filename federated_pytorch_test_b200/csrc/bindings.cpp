@@ -190,6 +190,59 @@ std::vector<Tensor> bn_elu_bwd(Tensor dout, c10::optional<Tensor> out, Tensor y,
                        want_dres ? dres.data_ptr<float>() : nullptr, dg, db, M, C, act ? 1 : 0, persistent ? 1 : 0, cur_stream());
   return {dy, dres};
 }
+// GroupNorm + residual + ELU.  y, residual: [N,H,W,C] contiguous.  Returns (out, mean [N,G], rstd [N,G]).
+static void check_gn(const Tensor& y, const Tensor& gamma, int64_t groups) {
+  CHECK_F32_CUDA(y); CHECK_CONTIG(y);
+  TORCH_CHECK(y.dim() == 4, "GroupNorm kernels: y must be [N,H,W,C]");
+  CHECK_F32_CUDA(gamma); CHECK_CONTIG(gamma);
+  TORCH_CHECK(gamma.numel() == y.size(3), "GroupNorm kernels: gamma must hold C values");
+  TORCH_CHECK(groups >= 1 && y.size(3) % groups == 0, "GroupNorm kernels: the group count must divide C");
+}
+std::vector<Tensor> gn_elu_fwd(Tensor y, Tensor gamma, Tensor beta, c10::optional<Tensor> residual, int64_t groups, double eps,
+                               bool act) {
+  check_gn(y, gamma, groups);
+  CHECK_F32_CUDA(beta); CHECK_CONTIG(beta);
+  if (residual.has_value() && residual->defined()) {
+    CHECK_F32_CUDA((*residual)); CHECK_CONTIG((*residual));
+    TORCH_CHECK(residual->sizes() == y.sizes(), "gn_elu_fwd: residual must have y's shape");
+  }
+  c10::cuda::CUDAGuard guard(y.device());
+  const int N = (int)y.size(0), HW = (int)(y.size(1) * y.size(2)), C = (int)y.size(3), G = (int)groups;
+  auto out = torch::empty_like(y);
+  auto mean = torch::empty({N, G}, y.options()), rstd = torch::empty({N, G}, y.options());
+  auto part = torch::empty({(int64_t)N * fb::gn_splits(N, HW, C) * 2 * C}, y.options());
+  auto table = torch::empty({(int64_t)N * 2 * C}, y.options());
+  fb::gn_elu_fwd(fptr(y), fptr(gamma), fptr(beta), opt_ptr(residual), fptr_mut(out), fptr_mut(mean), fptr_mut(rstd),
+                 fptr_mut(part), fptr_mut(table), N, HW, C, G, (float)eps, act ? 1 : 0, cur_stream());
+  return {out, mean, rstd};
+}
+// Returns (dy, dres or undefined, dgamma or undefined, dbeta or undefined).
+std::vector<Tensor> gn_elu_bwd(Tensor dout, c10::optional<Tensor> out, Tensor y, Tensor mean, Tensor rstd, Tensor gamma,
+                               c10::optional<Tensor> beta, int64_t groups, bool want_dres, bool act, bool want_affine) {
+  check_gn(y, gamma, groups);
+  CHECK_F32_CUDA(dout); CHECK_CONTIG(dout);
+  TORCH_CHECK(dout.sizes() == y.sizes(), "gn_elu_bwd: dout must have y's shape");
+  const int N = (int)y.size(0), HW = (int)(y.size(1) * y.size(2)), C = (int)y.size(3), G = (int)groups;
+  TORCH_CHECK(mean.numel() == (int64_t)N * G && rstd.numel() == (int64_t)N * G && mean.is_contiguous() && rstd.is_contiguous(),
+              "gn_elu_bwd: mean / rstd must be [N, G]");
+  const float* outp = nullptr;
+  if (out.has_value() && out->defined()) {
+    CHECK_CONTIG((*out));
+    TORCH_CHECK(out->sizes() == y.sizes(), "gn_elu_bwd: out must have y's shape");
+    outp = out->data_ptr<float>();
+  }
+  c10::cuda::CUDAGuard guard(y.device());
+  auto part = torch::empty({(int64_t)N * fb::gn_splits(N, HW, C) * 2 * C}, y.options());
+  auto ab = torch::empty({2 * (int64_t)N * G}, y.options());
+  auto dy = torch::empty_like(y);
+  Tensor dres, dgamma, dbeta;
+  if (want_dres) dres = torch::empty_like(y);
+  if (want_affine) { dgamma = torch::empty_like(gamma); dbeta = torch::empty_like(gamma); }
+  fb::gn_elu_bwd(fptr(dout), outp, fptr(y), fptr(mean), fptr(rstd), fptr(gamma), opt_ptr(beta), fptr_mut(part), fptr_mut(ab),
+                 fptr_mut(dy), want_dres ? dres.data_ptr<float>() : nullptr, want_affine ? dgamma.data_ptr<float>() : nullptr,
+                 want_affine ? dbeta.data_ptr<float>() : nullptr, N, HW, C, G, act ? 1 : 0, cur_stream());
+  return {dy, dres, dgamma, dbeta};
+}
 // fused classifier head (experimental): x [N,H,W,C], w [O,C], bias [O] -> (logits [N,O], pooled [N,C])
 std::vector<Tensor> head_fwd(Tensor x, Tensor w, c10::optional<Tensor> bias) {
   CHECK_F32_CUDA(x); CHECK_CONTIG(x); CHECK_F32_CUDA(w); CHECK_CONTIG(w);
@@ -912,6 +965,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("running_mean"), py::arg("running_var"), py::arg("eps"), py::arg("momentum"), py::arg("act"),
         py::arg("self_clean"), py::arg("use_running") = false);
   m.def("bn_elu_bwd", &bn_elu_bwd);
+  m.def("gn_elu_fwd", &gn_elu_fwd, py::arg("y"), py::arg("gamma"), py::arg("beta"), py::arg("residual"), py::arg("groups"),
+        py::arg("eps"), py::arg("act"));
+  m.def("gn_elu_bwd", &gn_elu_bwd, py::arg("dout"), py::arg("out"), py::arg("y"), py::arg("mean"), py::arg("rstd"),
+        py::arg("gamma"), py::arg("beta"), py::arg("groups"), py::arg("want_dres"), py::arg("act"), py::arg("want_affine"));
   m.def("avgpool_nhwc", &avgpool_nhwc);
   m.def("avgpool_nhwc_bwd", &avgpool_nhwc_bwd);
   m.def("weight_flip", &weight_flip);

@@ -131,6 +131,18 @@ void bn_elu_bwd_apply(const float* dout, const float* out, const float* y, const
 bool bn_elu_bwd_fused(const float* dout, const float* out, const float* y, const float* mean, const float* invstd,
                       const float* gamma, const float* beta, float* sums, float* dy, float* dres, float* dgamma,
                       float* dbeta, int M, int C, int act, cudaStream_t s);
+
+// ---- GroupNorm + residual + ELU (norm_kernels.cu) ----------------------------------------------------
+// y, residual, out: [N, HW, C] (NHWC); mean / rstd: [N, G].  Scratch: part [N, S, 2, C] with S = gn_splits(N, HW, C),
+// table [N, 2, C] (scale | shift), ab [2, N, G].  Needs C % 4 == 0, C <= 1024, G | C, G <= 256.
+int gn_splits(int N, int HW, int C);
+void gn_elu_fwd(const float* y, const float* gamma, const float* beta, const float* residual, float* out, float* mean,
+                float* rstd, float* part, float* table, int N, int HW, int C, int G, float eps, int act, cudaStream_t s);
+// out == nullptr (allowed when the layer had no residual input): ELU' is recomputed from y, gamma, beta.  dres, dgamma,
+// dbeta may be nullptr; dgamma / dbeta are overwritten, not accumulated.
+void gn_elu_bwd(const float* dout, const float* out, const float* y, const float* mean, const float* rstd, const float* gamma,
+                const float* beta, float* part, float* ab, float* dy, float* dres, float* dgamma, float* dbeta, int N, int HW,
+                int C, int G, int act, cudaStream_t s);
 // experimental fused classifier head: avg-pool over HW + Linear (true fp32), O <= 32 outputs
 void head_fwd(const float* x, const float* w, const float* bias, float* pooled, float* logits, int NB, int HW, int C, int O,
               cudaStream_t s);

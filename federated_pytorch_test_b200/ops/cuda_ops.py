@@ -10,6 +10,7 @@ Kernel inventory (SURVEY §2.10 ids):
   G1  conv2d_nhwc          wgmma implicit GEMM (TMA 4-D boxes -> smem -> wgmma tf32 -> registers), BN stats in epilogue
   G2/3 bn_elu_fwd/bwd      BatchNorm(train) + residual + ELU fused, two-pass backward
        conv2d_nhwc_bn_eval  conv + BatchNorm(eval, running statistics) + residual + ELU in the conv epilogue (inference)
+       gn_elu_fwd/bwd      GroupNorm + residual + ELU, three kernels each way, no floating-point atomics (norm_kernels.cu)
   G4  avgpool / pool_linear
   G5  linear_tf32          wgmma GEMM with bias+ELU epilogue
   G9  cross_entropy        fused log-softmax/NLL fwd, softmax-minus-onehot bwd
@@ -159,6 +160,13 @@ def _krsc(w: torch.Tensor) -> torch.Tensor:
 
 def _conv_bn_geometry_supported(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d) -> bool:
     if not (isinstance(conv, nn.Conv2d) and isinstance(bn, nn.BatchNorm2d)):
+        return False
+    return _conv_geometry_supported(x, conv)
+
+
+def _conv_geometry_supported(x: torch.Tensor, conv: nn.Conv2d) -> bool:
+    """The bias-free convolutions ``conv2d_nhwc`` runs for a conv + norm (+ residual) (+ ELU) group."""
+    if not isinstance(conv, nn.Conv2d):
         return False
     if conv.bias is not None or conv.groups != 1 or conv.padding_mode != "zeros":
         return False
@@ -436,33 +444,96 @@ class _ConvBnAct(torch.autograd.Function):
         # without a residual input ELU' is recomputed from y (one tensor read less per backward pass)
         dy, dres = e.bn_elu_bwd(dn, out if (has_res or not act) else None, y, mean, invstd, gamma, beta, dgamma, dbeta,
                                 bool(has_res and need_r), act, _bwd_sums_buffer(gamma, gamma.numel()))
-        dx = dw = None
-        kh, kw = wshape[2], wshape[3]
-        if need_x:
-            Ci = xn.shape[3]
-            if stride == 1 and e.conv_supported(xn.shape[1], xn.shape[2], wshape[0], 1) and Ci % 4 == 0:
-                # data gradient of a stride-1 conv = conv of dy with the 180-degree rotated, transposed filter
-                dxn = e.conv2d_nhwc(dy, _flipped_weight(wk, need_w, ctx.w_persistent), None, 1, kh - 1 - pad, 1)
-            elif stride == 2 and _s2_dgrad_supported(e, xn, dy, kh, kw, pad):
-                dxn = _s2_dgrad(e, dy, wk, need_w, ctx.w_persistent)
-            else:
-                dxn = torch.ops.aten.convolution_backward(
-                    dy.permute(0, 3, 1, 2), xn.permute(0, 3, 1, 2), wk.permute(0, 3, 1, 2), None,
-                    [stride, stride], [pad, pad], [1, 1], False, [0, 0], 1, [True, False, False])[0]
-                dxn = _nhwc(dxn)
-            if dxn.shape[3] != cin_logical:
-                dxn = dxn[..., :cin_logical]
-            dx = dxn.permute(0, 3, 1, 2)
-        if need_w:
-            if conv_wgrad_supported(xn, dy, stride):
-                dw = conv_wgrad(xn, dy, kh, kw, cin_logical, stride, pad, 1, ctx.weight_ref)
-            else:
-                dwk = torch.ops.aten.convolution_backward(
-                    dy.permute(0, 3, 1, 2), xn.permute(0, 3, 1, 2), wk.permute(0, 3, 1, 2), None,
-                    [stride, stride], [pad, pad], [1, 1], False, [0, 0], 1, [False, True, False])[1]
-                dw = dwk[:, :cin_logical] if dwk.shape[1] != cin_logical else dwk
+        dx, dw = _conv_backward(e, xn, wk, dy, stride, pad, wshape, cin_logical, need_x, need_w, ctx.w_persistent,
+                                ctx.weight_ref)
         dr = dres.permute(0, 3, 1, 2) if (has_res and need_r and dres is not None) else None
         return dx, dw, dgamma, dbeta, dr, None, None, None, None, None, None, None
+
+
+def _conv_backward(e, xn, wk, dy, stride, pad, wshape, cin_logical, need_x, need_w, w_persistent, weight_ref):
+    """(dx, dW) of the convolution of a conv + norm (+ residual) (+ ELU) group from ``dy`` = dL/d(conv output) [N,Ho,Wo,Co]:
+    the rotated (stride 1) or phase-packed (stride 2) filter for the data gradient, cached for frozen layers, and the wgmma
+    weight gradient, accumulated into ``weight_ref.grad`` inside ``accumulate_into_grad`` (dW is then ``None``)."""
+    dx = dw = None
+    kh, kw = wshape[2], wshape[3]
+    if need_x:
+        Ci = xn.shape[3]
+        if stride == 1 and e.conv_supported(xn.shape[1], xn.shape[2], wshape[0], 1) and Ci % 4 == 0:
+            # data gradient of a stride-1 conv = conv of dy with the 180-degree rotated, transposed filter
+            dxn = e.conv2d_nhwc(dy, _flipped_weight(wk, need_w, w_persistent), None, 1, kh - 1 - pad, 1)
+        elif stride == 2 and _s2_dgrad_supported(e, xn, dy, kh, kw, pad):
+            dxn = _s2_dgrad(e, dy, wk, need_w, w_persistent)
+        else:
+            dxn = torch.ops.aten.convolution_backward(
+                dy.permute(0, 3, 1, 2), xn.permute(0, 3, 1, 2), wk.permute(0, 3, 1, 2), None,
+                [stride, stride], [pad, pad], [1, 1], False, [0, 0], 1, [True, False, False])[0]
+            dxn = _nhwc(dxn)
+        if dxn.shape[3] != cin_logical:
+            dxn = dxn[..., :cin_logical]
+        dx = dxn.permute(0, 3, 1, 2)
+    if need_w:
+        if conv_wgrad_supported(xn, dy, stride):
+            dw = conv_wgrad(xn, dy, kh, kw, cin_logical, stride, pad, 1, weight_ref)
+        else:
+            dwk = torch.ops.aten.convolution_backward(
+                dy.permute(0, 3, 1, 2), xn.permute(0, 3, 1, 2), wk.permute(0, 3, 1, 2), None,
+                [stride, stride], [pad, pad], [1, 1], False, [0, 0], 1, [False, True, False])[1]
+            dw = dwk[:, :cin_logical] if dwk.shape[1] != cin_logical else dwk
+    return dx, dw
+
+
+# ----------------------------------------------------------------------------
+# conv + GroupNorm + residual + ELU group (the GroupNorm ResNets): the same convolution without epilogue statistics, then
+# three GroupNorm kernels forward (per-(sample, channel) statistics, per-(sample, group) merge, one normalise + residual +
+# ELU pass) and three backward (reduce, merge, apply); the convolution's gradients as for BatchNorm (_conv_backward).
+# ----------------------------------------------------------------------------
+def conv_gn_act_supported(x: torch.Tensor, conv: nn.Conv2d, gn: nn.GroupNorm) -> bool:
+    if not isinstance(gn, nn.GroupNorm) or not gn.affine or gn.weight.dtype != torch.float32:
+        return False
+    C, G = gn.num_channels, gn.num_groups
+    if C != getattr(conv, "out_channels", -1) or C % 4 or C > 1024 or G > 256 or C % G:
+        return False
+    return _conv_geometry_supported(x, conv)
+
+
+class _ConvGnAct(torch.autograd.Function):
+    """``act(GroupNorm(conv(x)) + residual)`` with NHWC kernels."""
+
+    @staticmethod
+    def forward(ctx, x, weight, gamma, beta, residual, stride, pad, groups, eps, act):
+        e = ext()
+        xn = _nhwc(x)
+        wk = _krsc(weight)
+        if xn.shape[3] == 3:  # stem: pad 3 -> 4 channels so that the pixel pitch is 16 B (TMA requirement)
+            xn = F.pad(xn, (0, 1))
+            wk = F.pad(wk, (0, 1))
+        y = e.conv2d_nhwc(xn, wk, None, stride, pad, 1)
+        res = _nhwc(residual) if residual is not None else None
+        out, mean, rstd = e.gn_elu_fwd(y, gamma, beta, res, groups, eps, act)
+        ctx.save_for_backward(xn, wk, y, out, mean, rstd, gamma, beta)
+        ctx.cfg = (stride, pad, groups, act, residual is not None, tuple(weight.shape), x.shape[1])
+        ctx.w_persistent = _aliases(wk, weight)
+        ctx.weight_ref = weight
+        return out.permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, dout):
+        e = ext()
+        xn, wk, y, out, mean, rstd, gamma, beta = ctx.saved_tensors
+        stride, pad, groups, act, has_res, wshape, cin_logical = ctx.cfg
+        need_x, need_w, need_g, need_b, need_r = ctx.needs_input_grad[:5]
+        # without a residual input ELU' is recomputed from y, as for BatchNorm
+        dy, dres, dgamma, dbeta = e.gn_elu_bwd(_nhwc(dout), out if has_res else None, y, mean, rstd, gamma, beta, groups,
+                                               bool(has_res and need_r), act, bool(need_g or need_b))
+        dx, dw = _conv_backward(e, xn, wk, dy, stride, pad, wshape, cin_logical, need_x, need_w, ctx.w_persistent,
+                                ctx.weight_ref)
+        dr = dres.permute(0, 3, 1, 2) if (has_res and need_r) else None
+        return dx, dw, (dgamma if need_g else None), (dbeta if need_b else None), dr, None, None, None, None, None
+
+
+def conv_gn_act(x, conv: nn.Conv2d, gn: nn.GroupNorm, residual=None, act: bool = True) -> torch.Tensor:
+    return _ConvGnAct.apply(x, conv.weight, gn.weight, gn.bias, residual, conv.stride[0], conv.padding[0], gn.num_groups,
+                            gn.eps, bool(act))
 
 
 # ----------------------------------------------------------------------------

@@ -49,6 +49,9 @@ def conv_bn_act(
     is in training mode, which in the reference is *always* (SURVEY Q4).  In
     eval mode (``bn.eval()``) the running statistics normalise and stay
     unchanged; without a gradient to compute that runs as one kernel.
+
+    ``bn`` may also be an ``nn.GroupNorm`` (the GroupNorm ResNets): it
+    normalises every sample on its own, in training and eval mode alike.
     """
     if _use_fast(x):
         from . import cuda_ops
@@ -57,6 +60,8 @@ def conv_bn_act(
             return cuda_ops.conv_bn_act_eval(x, conv, bn, residual, act)
         if cuda_ops.conv_bn_act_supported(x, conv, bn):
             return cuda_ops.conv_bn_act(x, conv, bn, residual, act)
+        if cuda_ops.conv_gn_act_supported(x, conv, bn):
+            return cuda_ops.conv_gn_act(x, conv, bn, residual, act)
     y = F.conv2d(x, conv.weight, conv.bias, conv.stride, conv.padding, conv.dilation, conv.groups)
     y = bn(y)
     if residual is not None:
