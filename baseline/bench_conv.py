@@ -1,10 +1,12 @@
 """Per-kernel time of every ResNet18 convolution shape of the training step at batch 128 (CIFAR10, 32 x 32 input).
 
-Three kinds of launch, each on the wgmma implicit-GEMM convolution (``conv2d_nhwc``):
+Four kinds of launch, each on the wgmma implicit-GEMM convolution (``conv2d_nhwc``):
 
   fwd       the forward convolution with the BatchNorm sum / sum-of-squares epilogue (3 x 3, stride 1 or 2; the stem has
             its 3 input channels padded to 4 for the 16-byte pixel pitch, and FLOPs count the 4 channels the kernel multiplies)
   dgrad     the stride-1 data gradient: dy [N, H, W, C_out] convolved with the rotated, transposed filter, plain store
+  dgrad_s2  the stride-2 data gradient of layers 3 and 4: a 2 x 2 stride-1 convolution of dy with the phase-packed filter
+            (4 C_in output columns), stored pixel-shuffled; FLOPs count what that convolution multiplies
   shortcut  the 1 x 1 stride-2 projection of the downsampling blocks, with the statistics epilogue
 
 Each shape is timed with CUDA events around ``--iters`` back-to-back launches (default 200) after ``--warmup`` launches; the
@@ -58,6 +60,8 @@ SHAPES = [
     ("l2 dgrad 128<-128 3x3 16", "dgrad", 16, 128, 128, 3, 1, 1, 3),
     ("l3 dgrad 256<-256 3x3 8", "dgrad", 8, 256, 256, 3, 1, 1, 3),
     ("l4 dgrad 512<-512 3x3 4", "dgrad", 4, 512, 512, 3, 1, 1, 3),
+    ("l3 dgrad 128<-256 3x3 s2", "dgrad_s2", 16, 128, 256, 3, 2, 1, 1),
+    ("l4 dgrad 256<-512 3x3 s2", "dgrad_s2", 8, 256, 512, 3, 2, 1, 1),
 ]
 
 
@@ -102,6 +106,12 @@ def _case(e, kind, B, H, Ci, Co, k, s, p, dev):
     """Inputs and a closure launching the convolution once; (closure, FLOPs of one launch, output channels, geometry)."""
     g = torch.Generator(device=dev).manual_seed(B + H + Ci + Co + k)
     Ho = (H + 2 * p - k) // s + 1
+    if kind == "dgrad_s2":              # dy [B, Ho, Wo, Co] * phase-packed filter [4 Ci, 2, 2, Co] -> dx [B, H, W, Ci]
+        from federated_pytorch_test_b200.ops import conv_math
+        dy = torch.randn(B, Ho, Ho, Co, device=dev, generator=g)
+        wp = conv_math.pack_dgrad_s2_weight(torch.randn(Co, k, k, Ci, device=dev, generator=g) / (k * k * Ci) ** 0.5)
+        flops = 2.0 * B * Ho * Ho * 4 * Ci * 4 * Co
+        return (lambda orient: e.conv2d_nhwc_shuffle(dy, wp, 0, Ho, Ho)), flops, 4 * Ci, (B, Ho, Ho, Co, 4 * Ci, 2, 1)
     if kind == "dgrad":                 # dy [B, H, W, Co] * rotated filter [Ci, k, k, Co] -> dx [B, H, W, Ci]
         x = torch.randn(B, Ho, Ho, Co, device=dev, generator=g)
         w = torch.randn(Ci, k, k, Co, device=dev, generator=g) / (k * k * Co) ** 0.5
@@ -155,7 +165,8 @@ def main(argv=None) -> dict:
     with torch.no_grad():
         for name, kind, H, Ci, Co, k, s, p, sites in SHAPES:
             run, flops, cout, geom = _case(e, kind, args.batch, H, Ci, Co, k, s, p, dev)
-            avail = [o for o in orients if not o.startswith("pixel") or cout in (64, 128)]   # pixel-major tiles: C_out 64 / 128 only
+            # pixel-major tiles: C_out 64 / 128 only; the shuffled stride-2 data gradient runs row-major tiles only
+            avail = [o for o in orients if not o.startswith("pixel") or (cout in (64, 128) and kind != "dgrad_s2")]
             for o in avail:
                 for _ in range(args.warmup):
                     run(ORIENT[o])

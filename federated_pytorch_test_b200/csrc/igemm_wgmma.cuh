@@ -85,7 +85,8 @@ struct IgemmSmem {
   static constexpr int B_BYTES = BLOCK_N * IG_BLOCK_K * 4;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;         // one k-block: [A | B]
   static constexpr int STAGING_BYTES = 2 * 64 * 32 * 4;         // per consumer warpgroup: two 32 x 32 output boxes
-  static constexpr int STATS_BYTES = 2 * BLOCK_N * 4;           // column partials (sum, sumsq) or eval-BN (scale, shift) of the tile
+  // column partials (sum, sumsq) of the tile per consumer warp, or eval-BN (scale, shift) of the tile in the first 2 * BLOCK_N
+  static constexpr int STATS_BYTES = 8 * 2 * BLOCK_N * 4;
   static constexpr int BAR_BYTES = 2 * STAGES * 8;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + STAGING_BYTES + STATS_BYTES + BAR_BYTES + 1024;  // + align slack
 };
@@ -197,7 +198,7 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   uint8_t* tiles = smem;
   float* staging = reinterpret_cast<float*>(smem + STAGES * S::STAGE_BYTES);
   float* colsum = reinterpret_cast<float*>(smem + STAGES * S::STAGE_BYTES + S::STAGING_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(colsum + 2 * BLOCK_N);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(colsum + 8 * 2 * BLOCK_N);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int wg = threadIdx.x >> 7;
@@ -214,7 +215,6 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     }
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < 2 * BLOCK_N; i += IG_THREADS) colsum[i] = 0.f;
   __syncthreads();
   pdl_wait();
 
@@ -322,6 +322,9 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       }
     }
     if (p.stats != nullptr) {
+      // this warp's 16 rows, summed per column, to its own slot: plain stores (a float atomicAdd to shared memory is a
+      // compare-and-swap loop, and eight warps contend for every column)
+      float* wsum = colsum + (4 * g + warp) * 2 * BLOCK_N;
 #pragma unroll
       for (int i = 0; i < NACC / 4; ++i) {
 #pragma unroll
@@ -334,8 +337,8 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             s2 += __shfl_xor_sync(0xffffffffu, s2, o);
           }
           if (lane < 4) {
-            atomicAdd(&colsum[8 * i + col_in + e], s1);
-            atomicAdd(&colsum[BLOCK_N + 8 * i + col_in + e], s2);
+            wsum[8 * i + col_in + e] = s1;
+            wsum[BLOCK_N + 8 * i + col_in + e] = s2;
           }
         }
       }
@@ -399,16 +402,15 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       }
     }
     if (p.stats != nullptr) {
-      named_bar_sync(3, 256);                    // both warpgroups have added their partials
-      for (int cc = threadIdx.x - 128; cc < BLOCK_N; cc += 256) {
-        if (c.n0 + cc < p.N) {
-          atomicAdd(p.stats + c.n0 + cc, colsum[cc]);
-          atomicAdd(p.stats + p.N + c.n0 + cc, colsum[BLOCK_N + cc]);
-        }
-        colsum[cc] = 0.f;
-        colsum[BLOCK_N + cc] = 0.f;
+      named_bar_sync(3, 256);                    // every warp has stored its partials
+      for (int j = threadIdx.x - 128; j < 2 * BLOCK_N; j += 256) {   // j < BLOCK_N: sums, else sums of squares
+        float v = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) v += colsum[w * 2 * BLOCK_N + j];
+        const int cc = j < BLOCK_N ? j : j - BLOCK_N;
+        if (c.n0 + cc < p.N) atomicAdd(p.stats + (j < BLOCK_N ? 0 : p.N) + c.n0 + cc, v);
       }
-      named_bar_sync(3, 256);                    // zeroed before the next tile adds to it
+      named_bar_sync(3, 256);                    // read before the next tile's partials overwrite them
     }
   }
   if (p.tma_store && tid == 0) tma_store_wait_read();   // shared memory must outlive the last bulk store's read
