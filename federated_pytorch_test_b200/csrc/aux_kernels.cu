@@ -2,8 +2,7 @@
 // convolution (those are on wgmma: gemm_wgmma.cu, wgrad_wgmma.cuh):
 //
 //  * gemm_f32_kernel        true-fp32 strided GEMM with bias / ELU / accumulate epilogue: nn.Linear forward, data and
-//                           weight gradients (SURVEY G5; the reference runs nn.Linear in true fp32, so this is the parity
-//                           default — the TF32 tensor-core path is FEDB200_TF32_LINEAR=1)
+//                           weight gradients (SURVEY G5; the reference runs nn.Linear in true fp32, and so does this)
 //  * act_bwd_bias_kernel    dz = dout * ELU'(z) (from the saved output) and db = column sums of dz in one pass
 //  * maxpool2x2 fwd / bwd   NCHW (Net / Net1 / Net2, SURVEY G4)
 //  * argmax_count_kernel    evaluation: argmax over classes, compare with the label, count — on the device (G21)

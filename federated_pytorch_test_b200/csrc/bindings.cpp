@@ -171,8 +171,7 @@ std::vector<Tensor> bn_elu_bwd(Tensor dout, c10::optional<Tensor> out, Tensor y,
   if (out.has_value() && out->defined()) { CHECK_CONTIG((*out)); outp = out->data_ptr<float>(); }
   const float* betap = opt_ptr(beta);
   // sums_buf: a zeroed per-layer [2C + 1] buffer that the apply kernel leaves zeroed again (no memset node per layer)
-  static const bool fused_optin = [] { const char* e = std::getenv("FEDB200_BN_BWD_FUSED"); return e != nullptr && std::atoi(e) != 0; }();
-  const bool persistent = !fused_optin && sums_buf.has_value() && sums_buf->defined();   // the opt-in fused kernel zeroes its own scratch
+  const bool persistent = sums_buf.has_value() && sums_buf->defined();
   if (persistent) TORCH_CHECK(sums_buf->numel() == 2 * C + 1 && sums_buf->is_contiguous(), "bn_elu_bwd: sums buffer must be [2C + 1]");
   auto sums = persistent ? *sums_buf : torch::empty({2 * C + 1}, y.options());
   auto dy = torch::empty_like(y);
@@ -180,10 +179,6 @@ std::vector<Tensor> bn_elu_bwd(Tensor dout, c10::optional<Tensor> out, Tensor y,
   if (want_dres) dres = torch::empty_like(y);
   float* dg = (dgamma.has_value() && dgamma->defined()) ? dgamma->data_ptr<float>() : nullptr;
   float* db = (dbeta.has_value() && dbeta->defined()) ? dbeta->data_ptr<float>() : nullptr;
-  if (fused_optin && fb::bn_elu_bwd_fused(fptr(dout), outp, fptr(y), fptr(mean), fptr(invstd), fptr(gamma), betap, fptr_mut(sums),
-                                          fptr_mut(dy), want_dres ? dres.data_ptr<float>() : nullptr, dg, db, M, C, act ? 1 : 0,
-                                          cur_stream()))
-    return {dy, dres};
   fb::bn_elu_bwd_reduce(fptr(dout), outp, fptr(y), fptr(mean), fptr(invstd), fptr(gamma), betap, fptr_mut(sums), M, C,
                         act ? 1 : 0, persistent ? 1 : 0, cur_stream());
   fb::bn_elu_bwd_apply(fptr(dout), outp, fptr(y), fptr(mean), fptr(invstd), fptr(gamma), betap, fptr_mut(sums), fptr_mut(dy),
@@ -243,7 +238,7 @@ std::vector<Tensor> gn_elu_bwd(Tensor dout, c10::optional<Tensor> out, Tensor y,
                  want_affine ? dbeta.data_ptr<float>() : nullptr, N, HW, C, G, act ? 1 : 0, cur_stream());
   return {dy, dres, dgamma, dbeta};
 }
-// fused classifier head (experimental): x [N,H,W,C], w [O,C], bias [O] -> (logits [N,O], pooled [N,C])
+// fused classifier head: x [N,H,W,C], w [O,C], bias [O] -> (logits [N,O], pooled [N,C])
 std::vector<Tensor> head_fwd(Tensor x, Tensor w, c10::optional<Tensor> bias) {
   CHECK_F32_CUDA(x); CHECK_CONTIG(x); CHECK_F32_CUDA(w); CHECK_CONTIG(w);
   TORCH_CHECK(x.dim() == 4 && w.dim() == 2 && x.size(3) == w.size(1), "head_fwd: x [N,H,W,C], w [O,C]");
@@ -400,21 +395,6 @@ Tensor conv2d_nhwc_multidil(Tensor x, Tensor w, c10::optional<Tensor> bias, bool
   auto y = torch::empty({NB, Ho, Wo, Co}, x.options());
   fb::conv2d_nhwc_multidil_tf32(fptr(x), fptr(w), opt_ptr(bias), act ? 1 : 0, fptr_mut(y), NB, H, W, Ci, Co, B, (int)kh, kw,
                                 (int)stride, d, pd, (int)Ho, (int)Wo, cur_stream());
-  return y;
-}
-
-// y += conv(x, w), in place (experimental)
-Tensor conv2d_nhwc_accumulate(Tensor x, Tensor w, Tensor y, int64_t stride, int64_t pad, int64_t dil, int64_t orient) {
-  CHECK_F32_CUDA(x); CHECK_F32_CUDA(w); CHECK_F32_CUDA(y); CHECK_CONTIG(x); CHECK_CONTIG(w); CHECK_CONTIG(y);
-  TORCH_CHECK(x.dim() == 4 && w.dim() == 4 && y.dim() == 4 && x.size(3) == w.size(3), "conv2d_nhwc_accumulate: x [N,H,W,Ci], w [Co,kh,kw,Ci]");
-  c10::cuda::CUDAGuard guard(x.device());
-  const int NB = (int)x.size(0), H = (int)x.size(1), W = (int)x.size(2), Ci = (int)x.size(3);
-  const int Co = (int)w.size(0), kh = (int)w.size(1), kw = (int)w.size(2);
-  const int Ho = (H + 2 * (int)pad - (int)dil * (kh - 1) - 1) / (int)stride + 1;
-  const int Wo = (W + 2 * (int)pad - (int)dil * (kw - 1) - 1) / (int)stride + 1;
-  TORCH_CHECK(y.size(0) == NB && y.size(1) == Ho && y.size(2) == Wo && y.size(3) == Co, "conv2d_nhwc_accumulate: y must be [N,Ho,Wo,Co]");
-  fb::conv2d_nhwc_accumulate_tf32(fptr(x), fptr(w), fptr_mut(y), NB, H, W, Ci, Co, kh, kw, (int)stride, (int)pad, (int)dil, Ho, Wo,
-                                  cur_stream(), (int)orient);
   return y;
 }
 
@@ -983,8 +963,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv2d_nhwc_sized", &conv2d_nhwc_sized);
   m.def("conv2d_nhwc_bias_act", &conv2d_nhwc_bias_act);
   m.def("conv2d_nhwc_bn_eval", &conv2d_nhwc_bn_eval);
-  m.def("conv2d_nhwc_accumulate", &conv2d_nhwc_accumulate, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("stride"), py::arg("pad"),
-        py::arg("dil"), py::arg("orient") = -1);
   m.def("conv2d_nhwc_shuffle", &conv2d_nhwc_shuffle);
   m.def("conv_shuffle_supported", &conv_shuffle_supported);
   m.def("conv2d_nhwc_multidil", &conv2d_nhwc_multidil);

@@ -34,7 +34,6 @@
 #include "fedb200.h"
 
 #include <cooperative_groups.h>
-#include <cstdlib>
 #include <stdexcept>
 #include <string>
 
@@ -1208,11 +1207,6 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   }
 }
 
-static int env_int_c(const char* name, int dflt) {
-  const char* v = std::getenv(name);
-  return v ? std::atoi(v) : dflt;
-}
-
 static int comm_max_blocks(const void* kernel) {
   int dev = 0, sms = 0, per = 0;
   cudaGetDevice(&dev);
@@ -1220,8 +1214,6 @@ static int comm_max_blocks(const void* kernel) {
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, COMM_THREADS, 0);
   int m = sms * (per < 1 ? 1 : 1);                    // one CTA per SM (132 on an H100 SXM) x 512 threads
   if (m > COMM_MAX_BLOCKS) m = COMM_MAX_BLOCKS;
-  const int cap = env_int_c("FEDB200_COMM_BLOCKS", 0);
-  if (cap > 0 && cap < m) m = cap;
   return m < 1 ? 1 : m;
 }
 
@@ -1311,12 +1303,8 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
   if (args.timeout_cycles <= 0) args.timeout_cycles = 240000000000LL;   // ~2 min at 2 GHz
   void* kargs[] = {(void*)&args};
   // Plain launch: a CTA only ever waits for the SAME-numbered CTA of its peers (never for another CTA of its own grid), so
-  // co-residency of the grid is not required and a cooperative launch only adds launch cost.  FEDB200_COMM_COOP=1 restores
-  // it (A/B runs).
-  static const int coop = env_int_c("FEDB200_COMM_COOP", 0);
-  cudaError_t e;
-  if (coop) e = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
-  else e = cudaLaunchKernel(kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
+  // co-residency of the grid is not required and a cooperative launch would only add launch cost.
+  cudaError_t e = cudaLaunchKernel(kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
   if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: block_reduce launch: ") + cudaGetErrorString(e));
   count_launch();
 }

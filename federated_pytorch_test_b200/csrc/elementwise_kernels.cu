@@ -11,13 +11,8 @@
 //  * avgpool_nhwc (+bwd), weight_krsc_flip (dgrad weights: swap Cin/Cout, rotate taps by 180 degrees)
 #include "fedb200.h"
 
-#include <cstdlib>
-
-#include <cooperative_groups.h>
 #include <stdexcept>
 #include <string>
-
-namespace cg = cooperative_groups;
 
 namespace fedb200 {
 
@@ -200,19 +195,10 @@ __device__ __forceinline__ void block_quad_reduce(const float (&s1)[4], const fl
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(t[0]), "f"(t[1]), "f"(t[2]), "f"(t[3]) : "memory");
   }
 }
-static int reduce_rows_per_thread() {
-  static int rows = -1;
-  if (rows < 0) {
-    const char* v = std::getenv("FEDB200_RED_ROWS");
-    rows = (v != nullptr && std::atoi(v) > 0) ? std::atoi(v) : 4;
-  }
-  return rows;
-}
 static int reduce_grid(int M, int rpi) {
   // One block of four rows in flight per thread, at most two CTAs per SM.  The first version asked for >= 16 rows per thread (few
   // blocks => few same-line atomics), which left the small tensors on 32-64 CTAs, far too few to stream them at DRAM speed.
-  // FEDB200_RED_ROWS=16: old grid.
-  const int rows = reduce_rows_per_thread();
+  constexpr int rows = 4;
   int grid = (M + rpi * rows - 1) / (rpi * rows);
   if (grid > sm_count() * 2) grid = sm_count() * 2;
   return grid < 1 ? 1 : grid;
@@ -542,107 +528,6 @@ void bn_elu_bwd_apply(const float* dout, const float* out, const float* y, const
   check_launch("bn_elu_bwd_apply");
 }
 
-// ------------------------------------------------------------------------------------------------
-// EXPERIMENTAL (opt-in, FEDB200_BN_BWD_FUSED=1): both passes of the
-// BN(+ELU) backward in ONE cooperative kernel for the small layers (layer3 / layer4: 8 / 4 MB per tensor).  The two-pass
-// version costs a memset + 2 launches and reads every tensor twice; here each
-// thread keeps its <= MAXR rows of du and y in registers across a grid barrier, so the tensors are read once.
-// Requires gridDim.x * rows_per_iter * MAXR >= M with all blocks co-resident (cooperative launch).
-// ------------------------------------------------------------------------------------------------
-template <int MODE, int MAXR>
-__global__ void __launch_bounds__(RED_THREADS)
-bn_elu_bwd_fused_kernel(const float* __restrict__ dout, const float* __restrict__ out, const float* __restrict__ y,
-                        const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
-                        const float* __restrict__ beta, float* __restrict__ sums, float* __restrict__ dy,
-                        float* __restrict__ dres, float* __restrict__ dgamma, float* __restrict__ dbeta, int M, int C) {
-  extern __shared__ float sm[];
-  cg::grid_group grid = cg::this_grid();
-  const RowLayout L = row_layout(C, RED_THREADS);
-  const bool active = L.r0 < L.rpi;
-  const int step = gridDim.x * L.rpi;
-  const int r_first = blockIdx.x * L.rpi + L.r0;
-  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-  float4 du[MAXR], v[MAXR];
-  float s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
-  BnBwdCoef k = {};
-  if (active) {
-    k = bn_bwd_coef(mean, invstd, gamma, beta, L.cq);
-#pragma unroll
-    for (int u = 0; u < MAXR; ++u) {
-      const int r = r_first + u * step;
-      const bool ok = r < M;
-      const size_t row = size_t(ok ? r : r_first < M ? r_first : 0);
-      const float4 d = ld4(dout, row, L.q, L.cq);
-      v[u] = ld4(y, row, L.q, L.cq);
-      const float4 o = MODE == 1 ? ld4(out, row, L.q, L.cq) : zero;
-      du[u] = ok ? bn_du<MODE>(d, o, v[u], k) : zero;
-      s1[0] += du[u].x; s1[1] += du[u].y; s1[2] += du[u].z; s1[3] += du[u].w;
-      s2[0] = fmaf(du[u].x, (v[u].x - k.mu[0]) * k.is[0], s2[0]); s2[1] = fmaf(du[u].y, (v[u].y - k.mu[1]) * k.is[1], s2[1]);
-      s2[2] = fmaf(du[u].z, (v[u].z - k.mu[2]) * k.is[2], s2[2]); s2[3] = fmaf(du[u].w, (v[u].w - k.mu[3]) * k.is[3], s2[3]);
-    }
-  }
-  block_quad_reduce(s1, s2, sm, L, sums, sums + C);
-  __threadfence();
-  grid.sync();
-  if (!active) return;
-  float ca[4], cb[4], cc[4];
-  {
-    const float invM = 1.f / float(M);
-    const float4 a = __ldcg(reinterpret_cast<const float4*>(sums) + L.cq);
-    const float4 b = __ldcg(reinterpret_cast<const float4*>(sums + C) + L.cq);
-    const float4 g = reinterpret_cast<const float4*>(gamma)[L.cq];
-    const float sdu[4] = {a.x, a.y, a.z, a.w}, sdx[4] = {b.x, b.y, b.z, b.w}, gg[4] = {g.x, g.y, g.z, g.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float kk = gg[j] * k.is[j];
-      ca[j] = kk;
-      cb[j] = -kk * k.is[j] * sdx[j] * invM;
-      cc[j] = -kk * sdu[j] * invM + kk * k.is[j] * sdx[j] * invM * k.mu[j];
-      if (blockIdx.x == 0 && L.r0 == 0) {
-        if (dgamma != nullptr) dgamma[L.cq * 4 + j] += sdx[j];
-        if (dbeta != nullptr) dbeta[L.cq * 4 + j] += sdu[j];
-      }
-    }
-  }
-#pragma unroll
-  for (int u = 0; u < MAXR; ++u) {
-    const int r = r_first + u * step;
-    if (r < M) {
-      st4(dy, size_t(r), L.q, L.cq,
-          make_float4(fmaf(ca[0], du[u].x, fmaf(cb[0], v[u].x, cc[0])), fmaf(ca[1], du[u].y, fmaf(cb[1], v[u].y, cc[1])),
-                      fmaf(ca[2], du[u].z, fmaf(cb[2], v[u].z, cc[2])), fmaf(ca[3], du[u].w, fmaf(cb[3], v[u].w, cc[3]))));
-      if (dres != nullptr) st4(dres, size_t(r), L.q, L.cq, du[u]);
-    }
-  }
-}
-// returns false (nothing launched) when the tensor does not fit the register-resident scheme
-bool bn_elu_bwd_fused(const float* dout, const float* out, const float* y, const float* mean, const float* invstd,
-                      const float* gamma, const float* beta, float* sums, float* dy, float* dres, float* dgamma,
-                      float* dbeta, int M, int C, int act, cudaStream_t s) {
-  constexpr int MAXR = 8;
-  if ((C & 3) || C > 2 * RED_THREADS) return false;
-  const int rpi = RED_THREADS / (C >> 2);
-  if (rpi < 1) return false;
-  int grid = sm_count();
-  const int need = (M + rpi - 1) / rpi;                 // row groups
-  if (grid > need) grid = need;
-  if ((need + grid - 1) / grid > MAXR) return false;
-  cudaMemsetAsync(sums, 0, 2 * C * sizeof(float), s);
-  const size_t smem = 2 * RED_THREADS * 4 * sizeof(float);
-  void* args[] = {(void*)&dout, (void*)&out, (void*)&y, (void*)&mean, (void*)&invstd, (void*)&gamma, (void*)&beta,
-                  (void*)&sums, (void*)&dy, (void*)&dres, (void*)&dgamma, (void*)&dbeta, (void*)&M, (void*)&C};
-  const void* fn = nullptr;
-  switch (bwd_mode(out, beta, act)) {
-    case 0: fn = (const void*)bn_elu_bwd_fused_kernel<0, MAXR>; break;
-    case 1: fn = (const void*)bn_elu_bwd_fused_kernel<1, MAXR>; break;
-    default: fn = (const void*)bn_elu_bwd_fused_kernel<2, MAXR>; break;
-  }
-  cudaError_t e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RED_THREADS), args, smem, s);
-  if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: bn_elu_bwd_fused: ") + cudaGetErrorString(e));
-  count_launch();
-  return true;
-}
-
 __global__ void __launch_bounds__(256)
 avgpool_kernel(const float* __restrict__ x, float* __restrict__ out, int NB, int HW, int C) {
   pdl_prologue();
@@ -659,7 +544,7 @@ void avgpool_nhwc(const float* x, float* out, int NB, int HW, int C, cudaStream_
   check_launch("avgpool_nhwc");
 }
 // ------------------------------------------------------------------------------------------------
-// Fused classifier head (FEDB200_HEAD_FUSED=0 switches it off):
+// Fused classifier head:
 // avg_pool(window) -> flatten -> Linear in ONE true-fp32 kernel per direction (SURVEY G4 + G5, simple_models.py:213-216).
 // The library path is an avgpool kernel + a SIMT sgemm for a 128x10x512 problem; here one block per sample pools
 // its [HW, C] map into shared memory and eight warps produce the O <= 32 logits with FMA chains + shuffle reductions.

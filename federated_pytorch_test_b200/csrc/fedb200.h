@@ -50,7 +50,7 @@ bool conv_geometry_supported(int H_out, int W_out, int C_in, int stride);
 // the window-reuse main loop where conv_window_reuse allows it and the per-tap loop elsewhere; PIXEL_PERTAP always runs the
 // per-tap loop (A/B tests and benchmarks).
 enum { CONV_ORIENT_AUTO = -1, CONV_ORIENT_ROW = 0, CONV_ORIENT_PIXEL = 1, CONV_ORIENT_PIXEL_PERTAP = 2 };
-// The orientation conv2d_nhwc_tf32 / conv2d_nhwc_accumulate_tf32 use by themselves for this shape (stride-1/2, no split-K).
+// The orientation conv2d_nhwc_tf32 uses by itself for this shape (stride-1/2, no split-K).
 int pick_conv_orientation(int NB, int H_out, int W_out, int C_out, int stride);
 // Whether a pixel-major convolution of this shape runs the window-reuse main loop (one input box per filter column serves
 // all kh filter rows).
@@ -58,10 +58,6 @@ bool conv_window_reuse(int H_out, int W_out, int C_in, int C_out, int kh, int st
 void conv2d_nhwc_tf32(const float* x, const float* w, float* y, float* stats, int NB, int H, int W, int C_in, int C_out,
                       int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream,
                       int orient = CONV_ORIENT_AUTO);
-// y += conv(x, w) (experimental: residual-gradient accumulation fused into the data-gradient convolution)
-void conv2d_nhwc_accumulate_tf32(const float* x, const float* w, float* y, int NB, int H, int W, int C_in, int C_out, int kh,
-                                 int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream,
-                                 int orient = CONV_ORIENT_AUTO);
 // same kernel with bias + optional ELU in the epilogue (no statistics, no split-K): VAE / CPC convolutions
 void conv2d_nhwc_bias_act_tf32(const float* x, const float* w, const float* bias, int act, float* y, int NB, int H, int W,
                                int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
@@ -127,10 +123,6 @@ void bn_elu_bwd_reduce(const float* dout, const float* out, const float* y, cons
 void bn_elu_bwd_apply(const float* dout, const float* out, const float* y, const float* mean, const float* invstd,
                       const float* gamma, const float* beta, float* sums, float* dy, float* dres, float* dgamma,
                       float* dbeta, int M, int C, int act, int self_clean, cudaStream_t s);
-// experimental single-kernel backward for small tensors (returns false when not applicable; sums: [2C] scratch)
-bool bn_elu_bwd_fused(const float* dout, const float* out, const float* y, const float* mean, const float* invstd,
-                      const float* gamma, const float* beta, float* sums, float* dy, float* dres, float* dgamma,
-                      float* dbeta, int M, int C, int act, cudaStream_t s);
 
 // ---- GroupNorm + residual + ELU (norm_kernels.cu) ----------------------------------------------------
 // y, residual, out: [N, HW, C] (NHWC); mean / rstd: [N, G].  Scratch: part [N, S, 2, C] with S = gn_splits(N, HW, C),
@@ -143,7 +135,7 @@ void gn_elu_fwd(const float* y, const float* gamma, const float* beta, const flo
 void gn_elu_bwd(const float* dout, const float* out, const float* y, const float* mean, const float* rstd, const float* gamma,
                 const float* beta, float* part, float* ab, float* dy, float* dres, float* dgamma, float* dbeta, int N, int HW,
                 int C, int G, int act, cudaStream_t s);
-// experimental fused classifier head: avg-pool over HW + Linear (true fp32), O <= 32 outputs
+// fused classifier head: avg-pool over HW + Linear (true fp32), O <= 32 outputs
 void head_fwd(const float* x, const float* w, const float* bias, float* pooled, float* logits, int NB, int HW, int C, int O,
               cudaStream_t s);
 void head_bwd(const float* dlogits, const float* w, float* dx, int NB, int HW, int C, int O, cudaStream_t s);

@@ -34,19 +34,13 @@ static EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// TFLOAT32 makes the TMA unit round fp32 -> tf32 (nearest) on the way into shared memory; FLOAT32 copies the bits and
-// the tensor core truncates the low 13 mantissa bits.  FEDB200_TMAP_F32=1 selects the latter (experiments).
-static CUtensorMapDataType tmap_dtype() {
-  const char* v = std::getenv("FEDB200_TMAP_F32");
-  return (v && std::atoi(v) == 1) ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_TFLOAT32;
-}
-
 static void check_cu(CUresult r, const char* what) {
   if (r != CUDA_SUCCESS) throw std::runtime_error(std::string("fedb200: ") + what + " failed with CUresult " + std::to_string(int(r)));
 }
 
 // fp32 matrix [rows, cols] with row pitch ld (elements): box = [box_rows x 32 cols], 128B swizzle,
-// loaded as TF32 (round-to-nearest on the way into shared memory), out-of-bounds zero-filled.
+// loaded as TF32 (round-to-nearest on the way into shared memory), out-of-bounds zero-filled.  With the FLOAT32 element
+// type the TMA unit would copy the bits and the tensor core would truncate the low 13 mantissa bits instead.
 // cw = channels (K elements) per operand row: 32 (one tap per k-block) or 16 / 8 (tap packing, IgemmParams::cw)
 static CUtensorMapSwizzle swizzle_for(int cw) {
   return cw == 8 ? CU_TENSOR_MAP_SWIZZLE_32B : (cw == 16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B);
@@ -57,7 +51,7 @@ static CUtensorMap make_tmap_2d(const float* ptr, uint64_t rows, uint64_t cols, 
   cuuint64_t strides[1] = {ld * sizeof(float)};
   cuuint32_t box[2] = {uint32_t(cw), box_rows};
   cuuint32_t estr[2] = {1, 1};
-  check_cu(encode_fn()(&m, tmap_dtype(),2, const_cast<float*>(ptr), dims, strides, box, estr,
+  check_cu(encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(cw), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE),
            "cuTensorMapEncodeTiled(2d)");
@@ -86,7 +80,7 @@ static CUtensorMap make_tmap_nhwc(const float* ptr, uint64_t N, uint64_t H, uint
   cuuint64_t strides[3] = {C * sizeof(float), W * C * sizeof(float), H * W * C * sizeof(float)};
   cuuint32_t box[4] = {uint32_t(cw), boxW * stride, boxH * stride, boxN};
   cuuint32_t estr[4] = {1, stride, stride, 1};
-  check_cu(encode_fn()(&m, tmap_dtype(),4, const_cast<float*>(ptr), dims, strides, box, estr,
+  check_cu(encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 4, const_cast<float*>(ptr), dims, strides, box, estr,
                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(cw), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE),
            "cuTensorMapEncodeTiled(nhwc)");
@@ -284,13 +278,12 @@ struct BnEvalArgs {
 // when the convolution runs as one K slice; otherwise bn_elu_fwd does it in place after the split-K convolution.
 static void conv2d_generic(const float* x, const float* w, float* y, float* stats, const float* bias, int act, int NB, int H,
                            int W, int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
-                           cudaStream_t stream, int accumulate = 0, const BnEvalArgs* eval_bn = nullptr,
-                           int orient = CONV_ORIENT_ROW);
+                           cudaStream_t stream, const BnEvalArgs* eval_bn = nullptr, int orient = CONV_ORIENT_ROW);
 
 void conv2d_nhwc_tf32(const float* x, const float* w, float* y, float* stats, int NB, int H, int W, int C_in, int C_out,
                       int kh, int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream, int orient) {
   if (orient == CONV_ORIENT_AUTO) orient = pick_conv_orientation(NB, H_out, W_out, C_out, stride);
-  conv2d_generic(x, w, y, stats, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 0, nullptr,
+  conv2d_generic(x, w, y, stats, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, nullptr,
                  orient);
 }
 
@@ -300,15 +293,6 @@ void conv2d_nhwc_bias_act_tf32(const float* x, const float* w, const float* bias
   conv2d_generic(x, w, y, nullptr, bias, act, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream);
 }
 
-// y += conv(x, w): the residual-gradient accumulation of an identity-shortcut block fused into the data-gradient
-// convolution (experimental, FEDB200_SKIP_FUSED=1): bulk tensor reduce-add epilogue.
-void conv2d_nhwc_accumulate_tf32(const float* x, const float* w, float* y, int NB, int H, int W, int C_in, int C_out, int kh,
-                                 int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream, int orient) {
-  if (orient == CONV_ORIENT_AUTO) orient = pick_conv_orientation(NB, H_out, W_out, C_out, stride);
-  conv2d_generic(x, w, y, nullptr, nullptr, 0, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 1, nullptr,
-                 orient);
-}
-
 // y = act(BN_eval(conv(x, w)) + residual): inference with BatchNorm on its running statistics.  One launch when the
 // convolution needs no split-K; otherwise the split-K convolution into y, then one in-place bn_elu_fwd pass.
 void conv2d_nhwc_bn_eval_tf32(const float* x, const float* w, const float* gamma, const float* beta, const float* mean,
@@ -316,7 +300,7 @@ void conv2d_nhwc_bn_eval_tf32(const float* x, const float* w, const float* gamma
                               int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
                               cudaStream_t stream) {
   const BnEvalArgs args{gamma, beta, mean, var, eps, residual};
-  conv2d_generic(x, w, y, nullptr, nullptr, act, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, 0, &args);
+  conv2d_generic(x, w, y, nullptr, nullptr, act, NB, H, W, C_in, C_out, kh, kw, stride, pad, dil, H_out, W_out, stream, &args);
 }
 
 // Tap packing (IgemmParams::cw): with C_in <= 16 a 32-wide k-block holds 4 (C_in <= 8) or 2 taps instead of one tap padded with
@@ -328,13 +312,13 @@ static int pick_tap_pack(int C_in) {
 
 static void conv2d_generic(const float* x, const float* w, float* y, float* stats, const float* bias, int act, int NB, int H,
                            int W, int C_in, int C_out, int kh, int kw, int stride, int pad, int dil, int H_out, int W_out,
-                           cudaStream_t stream, int accumulate, const BnEvalArgs* eval_bn, int orient) {
+                           cudaStream_t stream, const BnEvalArgs* eval_bn, int orient) {
   if (!conv_geometry_supported(H_out, W_out, C_in, stride))
     throw std::runtime_error("fedb200: conv geometry not supported by the wgmma path");
   const bool pix = orient == CONV_ORIENT_PIXEL || orient == CONV_ORIENT_PIXEL_PERTAP;
   if (pix && ((C_out != 64 && C_out != 128) || bias != nullptr || act != 0 || eval_bn != nullptr ||
               !pix_geometry_supported(H_out, W_out, stride) || (reinterpret_cast<uintptr_t>(y) & 15) != 0))
-    throw std::runtime_error("fedb200: pixel-major convolution needs C_out 64 / 128, a plain, statistics or accumulate epilogue, "
+    throw std::runtime_error("fedb200: pixel-major convolution needs C_out 64 / 128, a plain or statistics epilogue, "
                              "whole-row 256-pixel tiles and a 16-byte aligned output");
   // pixel-major: the window-reuse loop wherever the geometry allows it (CONV_ORIENT_PIXEL_PERTAP keeps the per-tap loop)
   const int win_stage = orient == CONV_ORIENT_PIXEL ? pix_window_stage_bytes(H_out, W_out, C_in, C_out, kh, stride, dil) : 0;
@@ -362,7 +346,6 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
   p.stride = stride; p.pad = pad; p.dil = dil;
   p.out = y; p.ldo = C_out; p.bias = bias; p.act = act; p.stats = stats;
   p.k_splits = 1; p.kb_per_split = p.num_k_blocks;
-  p.accumulate = accumulate;
   if (win_stage) {
     p.num_k_blocks = kw * p.cblocks;          // one unit per (filter column, channel block)
     p.kb_per_split = p.num_k_blocks;
@@ -383,7 +366,7 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
       p.kb_per_split = (p.num_k_blocks + splits - 1) / splits;
       p.k_splits = (p.num_k_blocks + p.kb_per_split - 1) / p.kb_per_split;   // no empty slices
       p.stats = nullptr;
-      if (!accumulate) cudaMemsetAsync(y, 0, size_t(M) * C_out * sizeof(float), stream);
+      cudaMemsetAsync(y, 0, size_t(M) * C_out * sizeof(float), stream);
     }
   }
   if (eval_bn != nullptr) {
@@ -408,7 +391,6 @@ static void conv2d_generic(const float* x, const float* w, float* y, float* stat
 // out[n, 2 ho + ph, 2 wo + pw, ci0 ..] through a 5-D tensor map {ci, pw, wo, ph, n * Ho + ho} over the [N, 2Ho, 2Wo, Ci] result.
 // ------------------------------------------------------------------------------------------------
 bool conv_shuffle_supported(int H_out, int W_out, int C_in, int Ci_out) {
-  if (env_int("FEDB200_SHUFFLE_STORE", 1) == 0) return false;
   if (!conv_geometry_supported(H_out, W_out, C_in, 1)) return false;
   if (Ci_out % 32 != 0) return false;                         // a 32-column box must stay inside one phase
   if (W_out > 32 || (32 % W_out) != 0) return false;          // a 32-row box = whole output rows
@@ -555,11 +537,8 @@ void conv_wgrad_tf32(const float* x, const float* dy, float* dw, int NB, int H, 
   // epilogue), keeping >= 8 k-blocks per CTA.
   const int kb_total = (p.P + WG_BK - 1) / WG_BK;
   const int base = p.j_tiles * p.co_tiles;
-  int splits = env_int("FEDB200_WGRAD_SPLITS", 0);
-  if (splits <= 0) {
-    splits = std::max(1, 2 * num_sms() / base);
-    splits = std::min(splits, std::max(1, kb_total / 8));
-  }
+  int splits = std::max(1, 2 * num_sms() / base);
+  splits = std::min(splits, std::max(1, kb_total / 8));
   splits = std::max(1, std::min(splits, kb_total));
   p.kb_per_split = (kb_total + splits - 1) / splits;
   splits = (kb_total + p.kb_per_split - 1) / p.kb_per_split;       // no empty slices

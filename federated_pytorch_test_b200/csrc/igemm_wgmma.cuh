@@ -17,7 +17,7 @@
 //   * per-channel sum / sum-of-squares of the tile (BatchNorm batch statistics, reduced across the CTA in shared
 //     memory, one atomicAdd per channel per tile), or
 //   * eval-mode BatchNorm from the running statistics + residual + ELU (inference: conv + BN + add + ELU in one launch);
-//   * output through a 128B-swizzled staging tile and bulk tensor stores (reduce-adds for split-K / accumulation), or
+//   * output through a 128B-swizzled staging tile and bulk tensor stores (reduce-adds for split-K), or
 //     direct stores when the row pitch is not 16-byte aligned.
 #pragma once
 #include "sm90.cuh"
@@ -47,7 +47,9 @@ struct IgemmParams {
   int kb_per_split;      // split-K: K slice z handles k-blocks [z*kb_per_split, ...) and reduce-adds into a zeroed output
   int k_splits;          // 1 = plain stores (+ fused stats); > 1 = reduction through L2, stats done by the caller
   int m_tiles, n_tiles, total_tiles;   // tile t -> (t % n_tiles, (t / n_tiles) % m_tiles, K split)
-  int accumulate;        // out += result (bulk reduce-add / atomics) instead of out = result; no memset
+  int shuffle_ci;        // > 0: the N columns are (ph, pw, ci) phase-packed channels of a stride-2 data gradient /
+                         // transposed conv; each 32 x 32 chunk is stored to out[n, 2 ho + ph, 2 wo + pw, ci0 .. ci0 + 31] through a
+                         // 5-D tensor map (no separate pixel-shuffle pass).  shuffle_ci = channels of the shuffled output.
   int tma_store;         // write the output with bulk tensor stores / reduce-adds (needs ldo % 4 == 0)
   int cw;                // convolutions with few input channels: channels per filter tap inside a 32-wide k-block.
                          // 0 / 32 = one tap per k-block (C_in padded to 32 by the TMA zero fill: 4x wasted MMAs at C_in = 8);
@@ -59,9 +61,6 @@ struct IgemmParams {
                          // matrix is block diagonal (branch b owns its own output channels).  The five dilated stem convolutions
                          // of the CPC encoder run as ONE launch writing the concatenated tensor (SURVEY G6).  pad = 0, dil = 1 then.
   unsigned long long ms_dil, ms_pad;
-  int shuffle_ci;        // > 0: the N columns are (ph, pw, ci) phase-packed channels of a stride-2 data gradient /
-                         // transposed conv; each 32 x 32 chunk is stored to out[n, 2 ho + ph, 2 wo + pw, ci0 .. ci0 + 31] through a
-                         // 5-D tensor map (no separate pixel-shuffle pass).  shuffle_ci = channels of the shuffled output.
   // eval-mode BatchNorm (k_splits == 1, stats == nullptr): column c -> v * s_c + t_c with s_c = gamma_c / sqrt(var_c + eps),
   // t_c = beta_c - mean_c * s_c (per tile in shared memory), then + residual, then act.  bn_gamma == nullptr: off (the host
   // launches the EVAL_BN instantiation of the kernel exactly when it is set).
@@ -373,7 +372,7 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
               const int phase = pc / p.shuffle_ci;   // packed channel (ph, pw, ci) of this chunk
               if (p.k_splits > 1) tma_reduce_add_5d(&tmap_c, src, pc - phase * p.shuffle_ci, phase & 1, 0, phase >> 1, row0 / p.W_out);
               else tma_store_5d(&tmap_c, src, pc - phase * p.shuffle_ci, phase & 1, 0, phase >> 1, row0 / p.W_out);
-            } else if (p.k_splits > 1 || p.accumulate) {
+            } else if (p.k_splits > 1) {
               tma_reduce_add_2d(&tmap_c, src, pc, row0);
             } else {
               tma_store_2d(&tmap_c, src, pc, row0);
@@ -395,7 +394,7 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             const int col = c.n0 + 8 * i + col_in + e;
             if (col >= p.N) continue;
             float* dst = p.out + size_t(row) * p.ldo + col;
-            if (p.k_splits > 1 || p.accumulate) atomicAdd(dst, acc[4 * i + 2 * h + e]);
+            if (p.k_splits > 1) atomicAdd(dst, acc[4 * i + 2 * h + e]);
             else *dst = acc[4 * i + 2 * h + e];
           }
         }
@@ -425,7 +424,7 @@ igemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 //   C_out = 64  (ping-pong): each consumer warpgroup owns every other tile (64 ch x 256 px); one warpgroup's main loop
 //               runs while the other one's epilogue does (the ring hands the stages out in tile order).
 //   C_out = 128 (cooperative): warpgroup g computes channels [64 g, 64 g + 64) of every tile.
-// Epilogues: plain store, BatchNorm sum / sum of squares (IgemmParams::stats), or reduce-add (IgemmParams::accumulate).
+// Epilogue: plain store, plus the BatchNorm sum / sum of squares (IgemmParams::stats) when they are asked for.
 // The [channel][pixel] fragment is transposed through 128B-swizzled 32 x 32 staging boxes into NHWC bulk tensor stores.
 // Requires k_splits == 1, no bias / activation / eval-mode BatchNorm, and a 16-byte aligned output with ldo == C_out.
 // ================================================================================================================
@@ -659,10 +658,7 @@ igemm_wgmma_pix_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         const int row0 = c.m0 + 32 * q;
         if (row0 < p.M) {
 #pragma unroll
-          for (int b = 0; b < 2; ++b) {
-            if (p.accumulate) tma_reduce_add_2d(&tmap_c, buf + b * 1024, ch_wg + 32 * b, row0);
-            else tma_store_2d(&tmap_c, buf + b * 1024, ch_wg + 32 * b, row0);
-          }
+          for (int b = 0; b < 2; ++b) tma_store_2d(&tmap_c, buf + b * 1024, ch_wg + 32 * b, row0);
         }
         tma_store_commit();
       }

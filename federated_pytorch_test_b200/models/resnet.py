@@ -78,9 +78,6 @@ class BasicBlock(_Residual):
         self._make_shortcut(in_planes, planes * self.expansion, stride, norm)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if len(self.shortcut) == 0:      # identity shortcut: the input doubles as the residual (see FX.conv_bn_act_skip)
-            h, skip = FX.conv_bn_act_skip(x, self.conv1, self.bn1)
-            return FX.conv_bn_act(h, self.conv2, self.bn2, residual=skip, act=True)
         h = FX.conv_bn_act(x, self.conv1, self.bn1, act=True)
         return FX.conv_bn_act(h, self.conv2, self.bn2, residual=self._skip(x), act=True)
 

@@ -28,7 +28,6 @@ On a CUDA device a missing extension is an error, never a silent fall-back.
 """
 from __future__ import annotations
 
-import os
 from typing import List, Optional, Sequence, Tuple
 
 import torch
@@ -39,7 +38,6 @@ from .. import _ext
 from . import conv_math
 
 _EXT = None
-TF32_LINEAR = os.environ.get("FEDB200_TF32_LINEAR", "0") == "1"
 
 
 def ext():
@@ -317,7 +315,6 @@ def _flipped_weight(wk: torch.Tensor, trainable: bool, persistent: bool = True) 
     return _derived(_FLIP_CACHE, wk, trainable, lambda w: ext().weight_flip(w), persistent)
 
 
-S2_DGRAD = os.environ.get("FEDB200_S2_DGRAD", "1") != "0"
 _S2_CACHE = {}
 
 
@@ -330,7 +327,7 @@ def _packed_s2_weight(wk: torch.Tensor, trainable: bool, persistent: bool = True
 def _s2_dgrad_supported(e, xn: torch.Tensor, dy: torch.Tensor, kh: int, kw: int, pad: int) -> bool:
     H, W, Ci = xn.shape[1], xn.shape[2], xn.shape[3]
     Ho, Wo, Co = dy.shape[1], dy.shape[2], dy.shape[3]
-    if not S2_DGRAD or kh != kw or (kh, pad) not in ((3, 1), (1, 0)):
+    if kh != kw or (kh, pad) not in ((3, 1), (1, 0)):
         return False
     if H != 2 * Ho or W != 2 * Wo or Co % 4 or Ci % 4:
         return False
@@ -358,7 +355,6 @@ def _s2_dgrad(e, dy: torch.Tensor, wk: torch.Tensor, trainable: bool, persistent
 # weight gradient on wgmma (csrc/wgrad_wgmma.cuh): MN-major operands straight from the NHWC activations,
 # split over the pixel range, partial sums red.add-ed into dW
 # ----------------------------------------------------------------------------
-WGRAD = os.environ.get("FEDB200_WGRAD", "1") != "0"
 _ACC_INTO_GRAD = {"on": False}
 
 
@@ -392,7 +388,7 @@ def _grad_buffer_krsc(weight: Optional[torch.Tensor], shape_krsc) -> Optional[to
 
 
 def conv_wgrad_supported(xn: torch.Tensor, dy: torch.Tensor, stride: int) -> bool:
-    return bool(WGRAD and ext().conv_wgrad_supported(xn.shape[3], dy.shape[3], stride, dy.shape[2], dy.shape[1]))
+    return bool(ext().conv_wgrad_supported(xn.shape[3], dy.shape[3], stride, dy.shape[2], dy.shape[1]))
 
 
 def conv_wgrad(xn: torch.Tensor, dy: torch.Tensor, kh: int, kw: int, cw: int, stride: int, pad: int, dil: int,
@@ -537,79 +533,6 @@ def conv_gn_act(x, conv: nn.Conv2d, gn: nn.GroupNorm, residual=None, act: bool =
 
 
 # ----------------------------------------------------------------------------
-# Identity-shortcut blocks: the gradient that reaches the block input is dgrad(conv1) + d(residual).  Autograd adds
-# the two with a separate elementwise kernel (one `add` launch per identity block and step).  Routing the
-# block input through the conv1 Function as a second, pass-through output hands BOTH gradients to one backward call,
-# which lets the data-gradient convolution accumulate straight into the residual gradient (bulk reduce-add epilogue).  Opt-in: FEDB200_SKIP_FUSED=1.
-# ----------------------------------------------------------------------------
-SKIP_FUSED = os.environ.get("FEDB200_SKIP_FUSED", "0") == "1"
-
-
-class _ConvBnActSkip(torch.autograd.Function):
-    """``(ELU(BN_train(conv(x))), x)`` — the second output is the block input itself (no copy)."""
-
-    @staticmethod
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, stride, pad, eps, momentum):
-        e = ext()
-        xn = _nhwc(x)
-        wk = _krsc(weight)
-        Co = weight.shape[0]
-        stats, self_clean = _stats_buffer(weight, Co)
-        y = e.conv2d_nhwc(xn, wk, stats, stride, pad, 1)
-        out, mean, invstd = e.bn_elu_fwd(y, stats, gamma, beta, None, running_mean, running_var, eps, momentum, True, self_clean)
-        ctx.save_for_backward(xn, wk, y, mean, invstd, gamma, beta)
-        ctx.cfg = (stride, pad, tuple(weight.shape))
-        ctx.w_persistent = _aliases(wk, weight)
-        ctx.weight_ref = weight
-        return out.permute(0, 3, 1, 2), x.view_as(x)
-
-    @staticmethod
-    def backward(ctx, dout, dskip):
-        e = ext()
-        xn, wk, y, mean, invstd, gamma, beta = ctx.saved_tensors
-        stride, pad, wshape = ctx.cfg
-        need_x, need_w, need_g, need_b = ctx.needs_input_grad[:4]
-        dgamma = torch.zeros_like(gamma) if need_g else None
-        dbeta = torch.zeros_like(gamma) if need_b else None
-        dy, _ = e.bn_elu_bwd(_nhwc(dout), None, y, mean, invstd, gamma, beta, dgamma, dbeta, False, True,
-                             _bwd_sums_buffer(gamma, gamma.numel()))
-        kh = wshape[2]
-        dx = dw = None
-        if need_x:
-            wf = _flipped_weight(wk, need_w, ctx.w_persistent)
-            if dskip is not None:
-                acc = _nhwc(dskip)                       # the residual gradient of conv2's Function: ours alone
-                if not acc.is_contiguous():
-                    acc = acc.contiguous()
-                dxn = e.conv2d_nhwc_accumulate(dy, wf, acc, 1, kh - 1 - pad, 1)      # acc += dgrad(dy), in place
-            else:
-                dxn = e.conv2d_nhwc(dy, wf, None, 1, kh - 1 - pad, 1)
-            dx = dxn.permute(0, 3, 1, 2)
-        elif dskip is not None:
-            dx = dskip
-        if need_w:
-            if conv_wgrad_supported(xn, dy, stride):
-                dw = conv_wgrad(xn, dy, kh, wshape[3], wshape[1], stride, pad, 1, ctx.weight_ref)
-            else:
-                dw = torch.ops.aten.convolution_backward(
-                    dy.permute(0, 3, 1, 2), xn.permute(0, 3, 1, 2), wk.permute(0, 3, 1, 2), None,
-                    [stride, stride], [pad, pad], [1, 1], False, [0, 0], 1, [False, True, False])[1]
-        return dx, dw, dgamma, dbeta, None, None, None, None, None, None
-
-
-def conv_bn_act_skip_supported(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d) -> bool:
-    if not SKIP_FUSED or not conv_bn_act_supported(x, conv, bn):
-        return False
-    # stride-1 3x3 with matching channel counts (identity shortcut) and a 16-byte pixel pitch
-    return conv.stride[0] == 1 and conv.in_channels == conv.out_channels and conv.in_channels % 4 == 0 and x.requires_grad
-
-
-def conv_bn_act_skip(x, conv: nn.Conv2d, bn: nn.BatchNorm2d):
-    return _ConvBnActSkip.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.stride[0],
-                                conv.padding[0], bn.eps, bn.momentum)
-
-
-# ----------------------------------------------------------------------------
 # conv + bias (+ ELU) of the VAE / CPC networks (SURVEY G6, G7, G8) — forward AND backward on hand-written kernels:
 #   forward   implicit GEMM on wgmma with bias + ELU in the epilogue (transposed convs: 3x3 conv with 4*C_out phase
 #             channels + pixel shuffle, ops/conv_math.py)
@@ -617,13 +540,9 @@ def conv_bn_act_skip(x, conv: nn.Conv2d, bn: nn.BatchNorm2d):
 #   dx        stride-2 4x4: the transposed-conv kernel path with the same weights; stride 1: rotated filter;
 #             transposed conv: the forward stride-2 conv kernel
 #   dw        wgmma weight-gradient kernel (wgrad_wgmma.cuh); for transposed convs with the roles of x and dz swapped
-# FEDB200_CONV_ACT=0 restores the ATen / cuDNN composition (A/B runs).
 # ----------------------------------------------------------------------------
-CONV_ACT = os.environ.get("FEDB200_CONV_ACT", "1") != "0"
-
-
 def conv_act_supported(x: torch.Tensor, conv: nn.Module) -> bool:
-    if not CONV_ACT or not isinstance(conv, nn.Conv2d) or isinstance(conv, nn.ConvTranspose2d):
+    if not isinstance(conv, nn.Conv2d) or isinstance(conv, nn.ConvTranspose2d):
         return False
     if x.dim() != 4 or x.dtype != torch.float32 or conv.groups != 1 or conv.padding_mode != "zeros":
         return False
@@ -718,7 +637,7 @@ def _conv_out(size: int, k: int, s: int, p: int, d: int) -> int:
 def dilated_stem_supported(x: torch.Tensor, convs) -> bool:
     """Several convolutions of the SAME input that differ only in dilation / padding (and own their output channels), followed
     by a channel concatenation: the CPC encoder stem (SURVEY G6, /root/reference/src/simple_models.py:441-451, :455-460)."""
-    if not CONV_ACT or len(convs) < 2 or len(convs) > 8 or x.dim() != 4 or x.dtype != torch.float32 or not x.is_cuda:
+    if len(convs) < 2 or len(convs) > 8 or x.dim() != 4 or x.dtype != torch.float32 or not x.is_cuda:
         return False
     c0 = convs[0]
     k, st = c0.kernel_size[0], c0.stride[0]
@@ -804,7 +723,7 @@ def dilated_stem(x: torch.Tensor, convs, act: bool = True) -> torch.Tensor:
 def conv_transpose_act_supported(x: torch.Tensor, conv: nn.Module) -> bool:
     """ConvTranspose2d(k=4, stride=2, padding=1) of the VAE decoders (SURVEY G7) as one 3x3 convolution with 4*C_out
     phase channels + pixel shuffle (conv_math.pack_convT_s2_weight)."""
-    if not CONV_ACT or not isinstance(conv, nn.ConvTranspose2d) or x.dim() != 4 or x.dtype != torch.float32:
+    if not isinstance(conv, nn.ConvTranspose2d) or x.dim() != 4 or x.dtype != torch.float32:
         return False
     if (tuple(conv.kernel_size), tuple(conv.stride), tuple(conv.padding), tuple(conv.output_padding), tuple(conv.dilation),
             conv.groups) != ((4, 4), (2, 2), (1, 1), (0, 0), (1, 1), 1):
@@ -860,7 +779,7 @@ class _ConvTransposeAct(torch.autograd.Function):
 def conv1x1_supported(x: torch.Tensor, conv: nn.Module) -> bool:
     """1x1 / stride 1 / no padding convolutions on maps the TMA path cannot tile (the 3x3 CPC latent grid, SURVEY G8)
     are plain GEMMs over the [N*H*W, C] pixel rows: they run on the dense-layer kernels."""
-    return (CONV_ACT and isinstance(conv, nn.Conv2d) and not isinstance(conv, nn.ConvTranspose2d) and x.dim() == 4
+    return (isinstance(conv, nn.Conv2d) and not isinstance(conv, nn.ConvTranspose2d) and x.dim() == 4
             and x.dtype == torch.float32 and tuple(conv.kernel_size) == (1, 1) and tuple(conv.stride) == (1, 1)
             and not isinstance(conv.padding, str) and tuple(conv.padding) == (0, 0) and conv.groups == 1)
 
@@ -876,7 +795,7 @@ def unfold_conv_supported(x: torch.Tensor, conv: nn.Module) -> bool:
     """Stride-1 convolutions on tiny maps with many channels (the 2x2 convolutions of the CPC context network on its 3x3 / 4x4
     latent grid, SURVEY G8): im2col rows [N * Ho * Wo, Ci * k * k] x the dense-layer GEMM kernel with the bias + ELU epilogue,
     which keeps far more threads busy than a direct convolution over a 3x3 / 4x4 map."""
-    if not (CONV_ACT and LINEAR_F32) or not isinstance(conv, nn.Conv2d) or isinstance(conv, nn.ConvTranspose2d):
+    if not isinstance(conv, nn.Conv2d) or isinstance(conv, nn.ConvTranspose2d):
         return False
     if x.dim() != 4 or x.dtype != torch.float32 or conv.groups != 1 or conv.padding_mode != "zeros" or isinstance(conv.padding, str):
         return False
@@ -929,9 +848,6 @@ class _AvgPoolNHWC(torch.autograd.Function):
         return dx.permute(0, 3, 1, 2)
 
 
-HEAD_FUSED = os.environ.get("FEDB200_HEAD_FUSED", "1") != "0"   # default on
-
-
 def _dense_wgrad(dz: torch.Tensor, x: torch.Tensor, wparam) -> Optional[torch.Tensor]:
     """dW [N, K] = dz^T x in true fp32: accumulated into ``wparam.grad`` when allowed (returns None), else returned."""
     e = ext()
@@ -973,35 +889,25 @@ class _PoolLinear(torch.autograd.Function):
 
 
 def pool_linear(x, linear: nn.Linear, window: int) -> torch.Tensor:
-    if HEAD_FUSED and linear.out_features <= 32:
+    if linear.out_features <= 32:
         return _PoolLinear.apply(x, linear.weight, linear.bias)
     pooled = _AvgPoolNHWC.apply(x)                     # global average over the window x window map
     return linear_act(pooled, linear, False)
 
 
 # ----------------------------------------------------------------------------
-# dense layers (SURVEY G5).  Default: hand-written TRUE-fp32 kernels (the reference's nn.Linear precision, any shape:
-# 128x10x512 classifier, 400->120->84->10 of Net, the VAE / VAE-CL heads) with bias + ELU in the GEMM epilogue;
-# FEDB200_TF32_LINEAR=1 routes 16-byte aligned layers to the wgmma GEMM (TF32 products) instead.
+# dense layers (SURVEY G5): hand-written TRUE-fp32 kernels (the reference's nn.Linear precision, any shape:
+# 128x10x512 classifier, 400->120->84->10 of Net, the VAE / VAE-CL heads) with bias + ELU in the GEMM epilogue.
 # ----------------------------------------------------------------------------
-LINEAR_F32 = os.environ.get("FEDB200_LINEAR_F32", "1") != "0"
-
-
 def linear_act_supported(x, linear) -> bool:
-    if not (x.dim() == 2 and x.dtype == torch.float32 and isinstance(linear, nn.Linear)):
-        return False
-    return LINEAR_F32 or TF32_LINEAR
+    return x.dim() == 2 and x.dtype == torch.float32 and isinstance(linear, nn.Linear)
 
 
 class _LinearAct(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w, b, act):
-        e = ext()
         xc, wc = x.contiguous(), w.contiguous()
-        if TF32_LINEAR and xc.shape[1] % 4 == 0:
-            out = e.linear_tf32(xc, wc, b, act)
-        else:
-            out = e.linear_f32(xc, wc, b, act)
+        out = ext().linear_f32(xc, wc, b, act)
         ctx.save_for_backward(xc, wc, out)
         ctx.act = act
         ctx.params = (w, b)
@@ -1076,12 +982,11 @@ def vae_loss(recon, x, mu, logvar) -> torch.Tensor:
 # ----------------------------------------------------------------------------
 # InfoNCE (SURVEY G12): normalised Gram + diagonal log-softmax, forward in ONE kernel, closed-form backward
 # ----------------------------------------------------------------------------
-INFO_NCE = os.environ.get("FEDB200_INFO_NCE", "1") != "0"
 _NCE_SCRATCH = {}
 
 
 def info_nce_supported(z) -> bool:
-    return bool(INFO_NCE and z.dim() == 4 and z.dtype == torch.float32 and 1 <= z.shape[2] * z.shape[3] <= ext().info_nce_max_p())
+    return bool(z.dim() == 4 and z.dtype == torch.float32 and 1 <= z.shape[2] * z.shape[3] <= ext().info_nce_max_p())
 
 
 def _nce_scratch(device) -> torch.Tensor:
@@ -1164,11 +1069,8 @@ def max_pool2x2(x: torch.Tensor) -> torch.Tensor:
     return _MaxPool2x2.apply(x)
 
 
-SMALLCONV = os.environ.get("FEDB200_SMALLCONV", "1") != "0"
-
-
 def smallconv_supported(x: torch.Tensor, conv: nn.Module) -> bool:
-    if not SMALLCONV or not isinstance(conv, nn.Conv2d) or isinstance(conv, nn.ConvTranspose2d) or x.dim() != 4:
+    if not isinstance(conv, nn.Conv2d) or isinstance(conv, nn.ConvTranspose2d) or x.dim() != 4:
         return False
     if x.dtype != torch.float32 or conv.groups != 1 or conv.padding_mode != "zeros" or isinstance(conv.padding, str):
         return False

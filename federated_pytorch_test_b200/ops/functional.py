@@ -69,19 +69,6 @@ def conv_bn_act(
     return F.elu(y) if act else y
 
 
-def conv_bn_act_skip(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d):
-    """First group of an identity-shortcut block: returns ``(ELU(BN(conv(x))), x_skip)`` where ``x_skip`` is the block
-    input to be used as the residual of the block's last group (/root/reference/src/simple_models.py:149-153).  On the
-    fused path (``FEDB200_SKIP_FUSED=1``) ``x_skip`` is routed through the same autograd node so that the data gradient
-    of ``conv`` accumulates into the residual gradient instead of being added by a separate kernel."""
-    if _use_fast(x):
-        from . import cuda_ops
-
-        if cuda_ops.conv_bn_act_skip_supported(x, conv, bn):
-            return cuda_ops.conv_bn_act_skip(x, conv, bn)
-    return conv_bn_act(x, conv, bn, act=True), x
-
-
 def pool_linear(x: torch.Tensor, linear: nn.Linear, window: int = 4) -> torch.Tensor:
     """``linear(flatten(avg_pool2d(x, window)))`` (simple_models.py:213-215)."""
     if _use_fast(x):
@@ -160,8 +147,8 @@ def global_avg_pool(x: torch.Tensor) -> torch.Tensor:
 
 
 def linear_act(x: torch.Tensor, linear: nn.Linear, act: bool = True) -> torch.Tensor:
-    """``ELU?(x @ W^T + b)``; on the GPU one hand-written GEMM kernel with the bias + ELU epilogue (true fp32 by default —
-    the reference's nn.Linear precision; FEDB200_TF32_LINEAR=1: wgmma) and hand-written backward kernels."""
+    """``ELU?(x @ W^T + b)``; on the GPU one hand-written GEMM kernel with the bias + ELU epilogue (true fp32, the
+    reference's nn.Linear precision) and hand-written backward kernels."""
     if _use_fast(x):
         from . import cuda_ops
 

@@ -1,25 +1,13 @@
-"""GPU checks of code paths that started as opt-in switches in round 1.
-
-Now DEFAULT (kernel tests, the three VAE / CPC drivers, bench): conv + bias + ELU of the VAE /
-CPC networks and the transposed-conv decomposition, forward AND backward on hand-written kernels (``FEDB200_CONV_ACT``);
-the fused classifier head (``FEDB200_HEAD_FUSED``).  These tests run in every ``-m gpu`` session.
-
-Still opt-in: ``FEDB200_BN_BWD_FUSED=1``,
-``FEDB200_SKIP_FUSED=1``; their tests run only when the switch is set:
-
-    FEDB200_SKIP_FUSED=1 python -m pytest tests/test_gpu_experimental.py -m gpu -q -k "identity_block or accumulating"
+"""GPU checks of code paths that started as opt-in switches in round 1 and now always run: conv + bias + ELU of the
+VAE / CPC networks and the transposed-conv decomposition, forward AND backward on hand-written kernels; the fused
+classifier head.
 """
-import math
-import os
-
 import pytest
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 pytestmark = [pytest.mark.gpu]
-needs_bn_bwd_fused = pytest.mark.skipif(os.environ.get("FEDB200_BN_BWD_FUSED", "0") != "1", reason="opt-in: FEDB200_BN_BWD_FUSED=1")
-needs_skip_fused = pytest.mark.skipif(os.environ.get("FEDB200_SKIP_FUSED", "0") != "1", reason="opt-in: FEDB200_SKIP_FUSED=1")
 
 if not torch.cuda.is_available():
     pytest.skip("CUDA device required", allow_module_level=True)
@@ -92,36 +80,6 @@ def test_dilated_stem_one_launch(B, H, Ci, Co, dils, act):
     assert fwd_launches == 1, "the stem must be one launch of our kernels, got %d" % fwd_launches
 
 
-# run with FEDB200_BN_BWD_FUSED=1: the binding then takes the single-kernel path for tensors that fit in registers
-@needs_bn_bwd_fused
-@pytest.mark.parametrize("C,M,res,act", [(256, 8192, False, True), (256, 8192, True, True), (512, 2048, True, True),
-                                         (512, 2048, False, False), (128, 1000, False, True)])
-def test_fused_bn_backward_equals_two_pass_oracle(C, M, res, act):
-    assert os.environ.get("FEDB200_BN_BWD_FUSED", "0") == "1", "set FEDB200_BN_BWD_FUSED=1 before importing the extension"
-    e = cuda_ops.ext()
-    g = torch.Generator(device=DEV).manual_seed(C + M)
-    y = torch.randn(M, C, device=DEV, generator=g) * 2 + 0.5
-    gamma, beta = torch.rand(C, device=DEV, generator=g) + 0.5, torch.randn(C, device=DEV, generator=g)
-    r = torch.randn(M, C, device=DEV, generator=g) if res else None
-    dout = torch.randn(M, C, device=DEV, generator=g)
-    yr, gr, br = y.clone().requires_grad_(), gamma.clone().requires_grad_(), beta.clone().requires_grad_()
-    rr = r.clone().requires_grad_() if res else None
-    u = F.batch_norm(yr, None, None, gr, br, True, 0.1, 1e-5)
-    if res:
-        u = u + rr
-    o = F.elu(u) if act else u
-    o.backward(dout)
-    mean = y.mean(0)
-    invstd = torch.rsqrt(y.var(0, unbiased=False) + 1e-5)
-    dg, db = torch.zeros(C, device=DEV), torch.zeros(C, device=DEV)
-    dy, dres = e.bn_elu_bwd(dout, o.detach() if (res or not act) else None, y, mean, invstd, gamma, beta, dg, db, res, act, None)
-    torch.testing.assert_close(dy, yr.grad, rtol=2e-3, atol=2e-4)
-    torch.testing.assert_close(dg, gr.grad, rtol=2e-3, atol=2e-2)
-    torch.testing.assert_close(db, br.grad, rtol=2e-3, atol=2e-2)
-    if res:
-        torch.testing.assert_close(dres, rr.grad, rtol=1e-4, atol=1e-5)
-
-
 @pytest.mark.parametrize("B,C,O", [(128, 512, 10), (32, 512, 10), (7, 256, 3)])
 def test_fused_classifier_head(B, C, O):
     torch.manual_seed(B + C)
@@ -135,13 +93,12 @@ def test_fused_classifier_head(B, C, O):
     (rx,) = torch.autograd.grad(ref, x, g)
     dx = e.head_bwd(g.contiguous(), lin.weight, 4, 4).permute(0, 3, 1, 2)
     torch.testing.assert_close(dx, rx, rtol=1e-5, atol=1e-6)
-    if cuda_ops.HEAD_FUSED:
-        y = cuda_ops.pool_linear(x, lin, 4)
-        gx, gw, gb = torch.autograd.grad(y, (x, lin.weight, lin.bias), g)
-        rx2, rw, rb = torch.autograd.grad(F.linear(F.avg_pool2d(x, 4).reshape(B, -1), lin.weight, lin.bias), (x, lin.weight, lin.bias), g)
-        torch.testing.assert_close(gx, rx2, rtol=1e-5, atol=1e-6)
-        torch.testing.assert_close(gw, rw, rtol=1e-4, atol=1e-5)
-        torch.testing.assert_close(gb, rb, rtol=1e-5, atol=1e-5)
+    y = cuda_ops.pool_linear(x, lin, 4)
+    gx, gw, gb = torch.autograd.grad(y, (x, lin.weight, lin.bias), g)
+    rx2, rw, rb = torch.autograd.grad(F.linear(F.avg_pool2d(x, 4).reshape(B, -1), lin.weight, lin.bias), (x, lin.weight, lin.bias), g)
+    torch.testing.assert_close(gx, rx2, rtol=1e-5, atol=1e-6)
+    torch.testing.assert_close(gw, rw, rtol=1e-4, atol=1e-5)
+    torch.testing.assert_close(gb, rb, rtol=1e-5, atol=1e-5)
 
 
 # VAE decoders (simple_models.py:262-265): ConvTranspose2d(k=4, s=2, p=1) = one 3x3 conv with 4*Co phase channels
@@ -161,46 +118,3 @@ def test_conv_transpose_bias_act_forward_backward(B, H, Ci, Co, act):
     gx, gw, gb = torch.autograd.grad(y, (x, conv.weight, conv.bias), g)
     rx, rw, rb = torch.autograd.grad(ref, (x, conv.weight, conv.bias), g)
     assert rel_err(gx, rx) < 5e-3 and rel_err(gw, rw) < 5e-3 and rel_err(gb, rb) < 5e-3
-
-
-# run with FEDB200_SKIP_FUSED=1: identity-shortcut blocks accumulate dgrad(conv1) into the residual gradient in the
-# convolution epilogue (weight-stationary kernel for 64 ch @ 32x32, persistent kernel otherwise)
-@needs_skip_fused
-@pytest.mark.parametrize("planes,H,B", [(64, 32, 8), (128, 16, 8), (256, 8, 16), (512, 4, 16), (64, 32, 3)])
-def test_identity_block_with_fused_residual_gradient(planes, H, B):
-    assert os.environ.get("FEDB200_SKIP_FUSED", "0") == "1", "set FEDB200_SKIP_FUSED=1"
-    from federated_pytorch_test_b200 import models
-    from federated_pytorch_test_b200.ops import functional as FX
-    torch.manual_seed(planes + H)
-    a = models.BasicBlock(planes, planes, 1).to(DEV)
-    b = models.BasicBlock(planes, planes, 1).to(DEV)
-    b.load_state_dict(a.state_dict())
-    x = torch.randn(B, planes, H, H, device=DEV).contiguous(memory_format=torch.channels_last)
-    xa, xb = x.clone().requires_grad_(), x.clone().requires_grad_()
-    FX.set_fast_path(True)
-    oa = a(xa * 1.0)                   # non-leaf block input, as inside the network
-    FX.set_fast_path(False)
-    ob = b(xb * 1.0)
-    FX.set_fast_path(True)
-    assert rel_err(oa, ob) < 5e-3
-    go = torch.randn_like(ob)
-    oa.backward(go)
-    ob.backward(go)
-    assert rel_err(xa.grad, xb.grad) < 2e-2
-    for (n, pa), (_, pb) in zip(a.named_parameters(), b.named_parameters()):
-        assert rel_err(pa.grad, pb.grad) < 2e-2, n
-
-
-def test_accumulating_convolution_kernels():
-    """y += conv(x, w) through both kernels (weight-stationary: 64 ch @ 32x32; persistent: everything else)."""
-    e = cuda_ops.ext()
-    for B, H, C in ((4, 32, 64), (6, 16, 128), (16, 8, 256)):
-        g = torch.Generator(device=DEV).manual_seed(H + C)
-        x = torch.randn(B, H, H, C, device=DEV, generator=g)
-        w = torch.randn(C, 3, 3, C, device=DEV, generator=g) / math.sqrt(9 * C)
-        y0 = torch.randn(B, H, H, C, device=DEV, generator=g)
-        ref = y0.double() + F.conv2d(x.permute(0, 3, 1, 2).double(), w.permute(0, 3, 1, 2).double(), None, 1, 1).permute(0, 2, 3, 1)
-        y = y0.clone()
-        out = e.conv2d_nhwc_accumulate(x, w, y, 1, 1, 1)
-        assert out.data_ptr() == y.data_ptr()
-        assert rel_err(y, ref.float()) < 3e-3

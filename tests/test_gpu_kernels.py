@@ -419,22 +419,12 @@ def test_host_resident_loader_matches_device_resident():
 
 # ------------------------------------------------------------------------------------------ conv kernel variants
 VARIANT_ENVS = [
-    # Switches of the Blackwell kernels that have no Hopper counterpart (KPS, MT, CLUSTER, 2CTA, HALO, WS) select nothing
-    # here: those sets run the default wgmma kernel on the same shapes.
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1"),                       # one K slice: statistics fused in the epilogue
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_KPS="1"),
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_PERSIST="0"),  # one tile per CTA (non-persistent)
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="2", FEDB200_BLOCK_N="64"), # persistent, several tiles per CTA, split-K
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_MT="2"),
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_MT="1"),
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="2", FEDB200_MT="2", FEDB200_BLOCK_N="256"),  # 256: widest tile (128)
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_MT="2", FEDB200_BLOCK_N="64"),
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="4"),                       # split-K with bulk reduce-adds
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_CLUSTER="4"),
-    dict(FEDB200_WS="0", FEDB200_HALO="0", FEDB200_SPLITK="1", FEDB200_2CTA="1"),
-    dict(FEDB200_WS="0", FEDB200_HALO="2"),
-    dict(FEDB200_WS="1"),
-    # choices of the wgmma kernel
+    dict(FEDB200_SPLITK="1"),                                                         # one K slice: statistics fused in the epilogue
+    dict(FEDB200_SPLITK="1", FEDB200_PERSIST="0"),                                    # one tile per CTA (non-persistent)
+    dict(FEDB200_SPLITK="2", FEDB200_BLOCK_N="64"),                                   # persistent, several tiles per CTA, split-K
+    dict(FEDB200_SPLITK="1", FEDB200_BLOCK_N="64"),
+    dict(FEDB200_SPLITK="2"),                                                         # split-K on the widest tile (128)
+    dict(FEDB200_SPLITK="4"),                                                         # split-K with bulk reduce-adds
     dict(),                                                                           # defaults
     dict(FEDB200_SPLITK="8", FEDB200_BLOCK_N="32"),
     dict(FEDB200_SPLITK="1", FEDB200_BLOCK_N="32"),                                   # 64 x 32 wgmma tiles
@@ -451,8 +441,7 @@ VARIANT_ENVS = [
 @pytest.mark.parametrize("B,H,Ci,Co", [(5, 32, 64, 64), (3, 32, 4, 64), (6, 16, 128, 128), (16, 8, 256, 256), (20, 32, 64, 64)])
 def test_conv_kernel_variants(monkeypatch, env, B, H, Ci, Co):
     import os
-    for k in ("FEDB200_WS", "FEDB200_HALO", "FEDB200_SPLITK", "FEDB200_CLUSTER", "FEDB200_2CTA", "FEDB200_BLOCK_N", "FEDB200_KPS",
-              "FEDB200_PERSIST", "FEDB200_MT", "FEDB200_TMA_STORE", "FEDB200_TAP_PACK"):
+    for k in ("FEDB200_SPLITK", "FEDB200_BLOCK_N", "FEDB200_PERSIST", "FEDB200_TMA_STORE", "FEDB200_TAP_PACK"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)

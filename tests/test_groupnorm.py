@@ -101,8 +101,7 @@ def test_skip_group_falls_back_to_the_plain_group():
     torch.manual_seed(0)
     blk = models.BasicBlock(16, 16, 1, lambda c: nn.GroupNorm(4, c))
     x = torch.randn(2, 16, 8, 8)
-    h, skip = FX.conv_bn_act_skip(x, blk.conv1, blk.bn1)
-    assert skip is x
+    h = FX.conv_bn_act(x, blk.conv1, blk.bn1)
     assert torch.equal(h, F.elu(F.group_norm(F.conv2d(x, blk.conv1.weight, None, 1, 1), 4, blk.bn1.weight, blk.bn1.bias)))
 
 
