@@ -17,7 +17,7 @@ What differs from the reference by construction:
 * a block is a zero-copy slice of each replica's flat arena — no pack/unpack, no
   ``torch.cat`` inside closures; penalty gradients are closed-form inside the
   optimizer kernel;
-* the per-minibatch step of the Adam drivers can be captured once per
+* the per-minibatch step of the Adam and SGD drivers can be captured once per
   (replica, block) as a CUDA graph and replayed (``graphs=True``), which removes
   the ~400 eager launches and the per-step host sync of the reference;
 * the diagnostics loss is accumulated on the device; it is read back once per
@@ -41,12 +41,15 @@ import torch.nn as nn
 
 from ..ops import flatops
 from ..optim.block_adam import BlockAdam
+from ..optim.block_sgd import BlockSGD
 from ..optim.lbfgsnew import LBFGSNew
 from ..parallel.topology import Topology
 from ..utils.flat import FlatArena
 from ..utils.metrics import MetricsLog, PhaseTimers, nvtx_range
 from .compress import payload_bytes
 from .strategies import Penalty, Strategy
+
+BLOCK_OPTIMIZERS = (BlockAdam, BlockSGD)   # fused block update: penalty in the kernel, the step graphed
 
 
 @dataclass
@@ -58,7 +61,7 @@ class Visit:
     hi: int                    # last trainable parameter index (inclusive)
     ci: int                    # block index: selects rho[ci], the elastic-net gate, log labels
     label: Tuple[int, int]     # what the legacy log lines print as block=[a,b]
-    optimizer: str = "adam"    # 'adam' | 'lbfgs'
+    optimizer: str = "adam"    # 'adam' | 'sgd' | 'lbfgs'
     opt_kwargs: Dict = field(default_factory=dict)
     lambda1: float = 0.0       # elastic net on the block vector (already gated by the task)
     lambda2: float = 0.0
@@ -157,7 +160,7 @@ class EngineConfig:
     check_results: bool = False
     be_verbose: bool = False
     diagnostics: str = "post"        # 'post' = reference (extra forward after the step, Q17) | 'pre' = reuse closure loss
-    graphs: bool = False             # CUDA-graph the Adam minibatch step
+    graphs: bool = False             # CUDA-graph the Adam / SGD minibatch step
     deferred_rounds: bool = True     # enqueue the next round's first minibatch BEFORE reading the aggregation's record (FedAvg / FedProx
                                      # on the fused collective; not with per-round evaluation, verbose logs or resume records)
     graph_closures: bool = True      # ... and (with graphs=True) the L-BFGS closure: one graph for gradient evaluations, one for probes
@@ -189,7 +192,7 @@ class Engine:
         self.steps_done = 0
         self.last_epoch = 0
         self._graphs: Dict = {}
-        self._adam_cache: Dict = {}
+        self._block_opt_cache: Dict = {}
         self.stop_requested = False
         self.step_hook: Optional[Callable[["Engine"], None]] = None
         self.attack: Optional[Callable[["Engine"], None]] = None   # simulated Byzantine workers, before every aggregation
@@ -214,13 +217,22 @@ class Engine:
         arena = rep.arenas[visit.model]
         if visit.optimizer == "adam":
             key = (rep.ck, visit.model, visit.lo, visit.hi)
-            opt = self._adam_cache.get(key)
+            opt = self._block_opt_cache.get(key)
             lr = visit.opt_kwargs.get("lr", 1e-3)
             if opt is None:
                 opt = BlockAdam(arena, visit.lo, visit.hi, lr=lr)
-                self._adam_cache[key] = opt
+                self._block_opt_cache[key] = opt
             else:
                 opt.reset(lr=lr)  # same as a freshly constructed Adam (Q18), but buffers/graphs persist
+            return opt
+        if visit.optimizer == "sgd":
+            key = ("sgd", rep.ck, visit.model, visit.lo, visit.hi)
+            opt = self._block_opt_cache.get(key)
+            if opt is None:
+                opt = BlockSGD(arena, visit.lo, visit.hi, **visit.opt_kwargs)
+                self._block_opt_cache[key] = opt
+            else:
+                opt.reset(lr=visit.opt_kwargs["lr"])  # a zero momentum buffer, as a fresh SGD (Q18); buffers/graphs persist
             return opt
         if visit.optimizer == "lbfgs":
             return LBFGSNew(arena.params[visit.lo: visit.hi + 1], **visit.opt_kwargs)
@@ -231,7 +243,7 @@ class Engine:
         """One ``opt.step(closure)`` + diagnostics; returns the diagnostics loss (0-dim, on device)."""
         task, cfg = self.task, self.cfg
         pre_loss = [None]
-        if isinstance(opt, BlockAdam):
+        if isinstance(opt, BLOCK_OPTIMIZERS):
             opt.set_penalty(pen.z, pen.y, pen.rho, visit.lambda1, visit.lambda2, pen.rho_dev)
 
             def closure():
@@ -320,6 +332,10 @@ class Engine:
         self.optimizers = [self._make_optimizer(rep, visit) for rep in self.replicas]
         first_round = 0
         if self._resume_pos is not None:          # re-enter the schedule inside this visit (true resume, SURVEY §5.4)
+            held = self._resume_pos.get("optimizer", visit.optimizer)     # records written before SGD did not store it
+            if held != visit.optimizer:
+                raise ValueError("resume record was written with optimizer %r, this run uses optimizer %r"
+                                 % (held, visit.optimizer))
             first_round = int(self._resume_pos.get("round", 0))
             self._restore_visit_state()
             self._resume_pos = None
@@ -342,7 +358,8 @@ class Engine:
                     if cfg.resume_path:
                         from ..utils import ckpt
 
-                        ckpt.save_resume(cfg.resume_path, self, dict(nloop=nloop, visit=vi, round=ri + 1, nadmm=nadmm, epoch=epoch))
+                        ckpt.save_resume(cfg.resume_path, self, dict(nloop=nloop, visit=vi, round=ri + 1, nadmm=nadmm, epoch=epoch,
+                                                                    optimizer=visit.optimizer))
         finally:
             if self._pending_round is not None:      # the last round of the visit (or a stop request): nothing left to overlap with
                 self._finish_round()
@@ -410,7 +427,7 @@ class Engine:
     def _one_step(self, rep: Replica, opt, visit: Visit, batch, pen: Penalty, running, i: int, epoch: int, nloop: int, N: int):
         cfg, task = self.cfg, self.task
         with self.timers.phase("step"):
-            if cfg.graphs and isinstance(opt, BlockAdam) and rep.device.type == "cuda":
+            if cfg.graphs and isinstance(opt, BLOCK_OPTIMIZERS) and rep.device.type == "cuda":
                 loss1 = self._graphed_step(rep, opt, visit, batch, pen)
             else:
                 loss1 = self._train_step(rep, opt, visit, batch, pen)
@@ -530,7 +547,7 @@ class Engine:
         self.log("WARNING: " + msg)
 
     # ------------------------------------------------------------------
-    # CUDA-graphed Adam step
+    # CUDA-graphed block-optimizer step (Adam / SGD)
     # ------------------------------------------------------------------
     def _graphed_closure(self, rep: Replica, opt, visit: Visit, batch):
         """One graphed closure per replica: the graphs of the previous block visit are dropped (their activations pools are
@@ -545,7 +562,7 @@ class Engine:
             self._graphs[slot] = cur
         return cur[1]
 
-    def _graphed_step(self, rep: Replica, opt: BlockAdam, visit: Visit, batch, pen: Penalty) -> torch.Tensor:
+    def _graphed_step(self, rep: Replica, opt, visit: Visit, batch, pen: Penalty) -> torch.Tensor:
         from .graphs import GraphedAdamStep
 
         key = (rep.ck, visit.model, visit.lo, visit.hi, tuple(tuple(t.shape) for t in batch if torch.is_tensor(t)))

@@ -1,16 +1,16 @@
-"""CUDA-graph capture of the per-minibatch Adam step (SURVEY §7.1 ``sched/``, G-launch-bound).
+"""CUDA-graph capture of the per-minibatch block-optimizer step, Adam or SGD (SURVEY §7.1 ``sched/``, G-launch-bound).
 
 The reference's hot loop issues ~400 eager kernel launches per minibatch (forward,
 backward, foreach-Adam, a second diagnostics forward) plus a ``.item()`` host sync
 (/root/reference/src/federated_multi.py:178-197).  Here the whole step
 
-    zero block gradient -> forward -> loss -> backward -> fused Adam(+penalty) -> diagnostics forward
+    zero block gradient -> forward -> loss -> backward -> fused Adam / SGD (+penalty) -> diagnostics forward
 
 is captured ONCE per (replica, block, batch shape) into a ``torch.cuda.CUDAGraph`` on
 static input buffers and replayed with one launch per minibatch.  Everything that
 varies between minibatches lives in device memory (inputs, Adam step counter,
 consensus vectors), so the graph never needs re-capture inside a block visit; across
-visits the optimizer buffers persist (``BlockAdam.reset``) and so do the graphs.
+visits the optimizer buffers persist (``BlockAdam.reset`` / ``BlockSGD.reset``) and so do the graphs.
 
 No tracing compiler is involved: the graph is just the recorded launch sequence of
 the hand-written kernels (and the few ATen ops that remain).
@@ -22,7 +22,6 @@ from typing import List, Optional
 import torch
 
 from ..ops import cuda_ops
-from ..optim.block_adam import BlockAdam
 
 
 
@@ -98,9 +97,13 @@ class GraphedEval:
 
 
 class GraphedAdamStep:
+    """The minibatch step of a block optimizer (``BlockAdam`` or ``BlockSGD``: it only calls ``zero_grad``,
+    ``apply_update`` and ``set_penalty``).  A host-side learning rate is baked into the capture; it does not change within
+    a run."""
+
     WARMUP = 3
 
-    def __init__(self, engine, rep, opt: BlockAdam, visit, batch, pen):
+    def __init__(self, engine, rep, opt, visit, batch, pen):
         self.engine, self.rep, self.opt, self.visit = engine, rep, opt, visit
         self.static = [t.clone() if torch.is_tensor(t) else t for t in batch]
         self.graph: Optional[torch.cuda.CUDAGraph] = None

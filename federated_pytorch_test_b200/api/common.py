@@ -17,7 +17,7 @@ import torch.nn as nn
 
 from .. import models
 from ..algo.engine import Engine, EngineConfig, Replica, Task, Visit
-from ..config import CommonConfig, check_norm, check_partition
+from ..config import ADAM_LR, CommonConfig, check_client_opt, check_norm, check_partition
 from ..data.cifar import (CifarData, ShardLoader, augment_key, class_histogram, dirichlet_shards, shard_ranges,
                           worker_norm)
 from ..ops import functional as FX
@@ -38,6 +38,15 @@ def require_batch_norm(cfg: CommonConfig, driver: str) -> None:
     """The VAE, VAE-CL and CPC networks have no GroupNorm variant and accept only the default ``norm``."""
     if getattr(cfg, "norm", "batch") != "batch":
         raise ValueError("%s supports only norm 'batch', got norm %r" % (driver, cfg.norm))
+
+
+def require_default_client_opt(cfg: CommonConfig, driver: str) -> None:
+    """The VAE, VAE-CL and CPC drivers fix their own optimizers (as the reference does) and accept none of the client-optimizer
+    flags of the classifier drivers."""
+    for name, default in (("lr", 0.0), ("momentum", 0.0), ("nesterov", False), ("weight_decay", 0.0)):
+        if getattr(cfg, name, default) != default:
+            raise ValueError("%s fixes its own optimizer and does not take %s, got %s %r"
+                             % (driver, name, name, getattr(cfg, name)))
 
 
 def require_iid(cfg: CommonConfig, driver: str) -> None:
@@ -92,6 +101,7 @@ class ClassifierTask(Task):
         self.model_name = name
         norm = getattr(cfg, "norm", "batch")
         check_norm(norm, getattr(cfg, "norm_groups", 32), name)
+        check_client_opt(cfg.optimizer, cfg.lr, cfg.momentum, cfg.nesterov, cfg.weight_decay)
         self.factory = _MODEL_FACTORIES[name]
         if norm != "batch":
             self.factory = functools.partial(self.factory, norm=norm, groups=cfg.norm_groups)
@@ -144,8 +154,13 @@ class ClassifierTask(Task):
         return ci in self.linear_ids  # Q2: block index tested against parameter indices
 
     def visits(self, nloop: int):
-        opt_kwargs = dict(lr=1e-3) if self.cfg.optimizer == "adam" else dict(
-            history_size=10, max_iter=4, line_search_fn=True, batch_mode=True)
+        cfg = self.cfg
+        if cfg.optimizer == "adam":
+            opt_kwargs = dict(lr=cfg.lr or ADAM_LR)
+        elif cfg.optimizer == "sgd":
+            opt_kwargs = dict(lr=cfg.lr, momentum=cfg.momentum, nesterov=cfg.nesterov, weight_decay=cfg.weight_decay)
+        else:
+            opt_kwargs = dict(history_size=10, max_iter=4, line_search_fn=True, batch_mode=True)
         if self.whole_model:
             yield Visit("net", 0, self.n_params - 1, 0, (0, self.n_params - 1), self.cfg.optimizer, opt_kwargs)
             return

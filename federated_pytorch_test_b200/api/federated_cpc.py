@@ -108,6 +108,7 @@ class CPCTask(Task):
 def run(cfg: Config, log=print):
     common.require_iid(cfg, "federated_cpc")
     common.require_batch_norm(cfg, "federated_cpc")
+    common.require_default_client_opt(cfg, "federated_cpc")
     topo, coll = common.setup_runtime(cfg)
     task = CPCTask(cfg, topo)
     ecfg = common.engine_config(cfg, Nepoch=1, diagnostics="pre")  # the reference has no diagnostics forward here

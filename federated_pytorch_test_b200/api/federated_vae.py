@@ -30,10 +30,13 @@ class VAETask(common.ClassifierTask):
     def __init__(self, cfg, topo):
         if cfg.augment:     # the loader would crop and flip the VAE's reconstruction targets too
             raise ValueError("augment is supported by the classifier drivers only, not by %s" % type(self).__name__)
-        cfg_model = cfg.model
-        cfg.model = "Net"  # placeholder for the base-class probe; replaced below
-        super().__init__(cfg, topo)
-        cfg.model = cfg_model
+        cfg_model, cfg_optimizer = cfg.model, cfg.optimizer
+        # placeholders for the base-class probe and checks; replaced below (this task fixes its own optimizer)
+        cfg.model, cfg.optimizer = "Net", "adam"
+        try:
+            super().__init__(cfg, topo)
+        finally:
+            cfg.model, cfg.optimizer = cfg_model, cfg_optimizer
         self.factory = models.AutoEncoderCNN
         probe = self.factory()
         self.blocks = probe.train_order_block_ids()
@@ -62,6 +65,7 @@ class VAETask(common.ClassifierTask):
 def run(cfg: Config, log=print):
     common.require_iid(cfg, "federated_vae")
     common.require_batch_norm(cfg, "federated_vae")
+    common.require_default_client_opt(cfg, "federated_vae")
     topo, coll = common.setup_runtime(cfg)
     task = VAETask(cfg, topo)
     engine = common.run_engine(cfg, task, topo, coll, FedAvg(coll, topo), None, log)

@@ -65,6 +65,7 @@ class VAECLTask(federated_vae.VAETask):
 def run(cfg: Config, log=print):
     common.require_iid(cfg, "federated_vae_cl")
     common.require_batch_norm(cfg, "federated_vae_cl")
+    common.require_default_client_opt(cfg, "federated_vae_cl")
     topo, coll = common.setup_runtime(cfg)
     task = VAECLTask(cfg, topo)
     engine = common.run_engine(cfg, task, topo, coll, FedAvg(coll, topo), None, log)

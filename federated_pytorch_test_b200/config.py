@@ -36,7 +36,12 @@ class CommonConfig:
     use_cuda: bool = True
     # ---- new in this framework -------------------------------------------------
     model: str = ""                 # '', 'Net', 'Net1', 'Net2', 'ResNet18', 'ResNet9' ('' = follow use_resnet)
-    optimizer: str = "adam"         # 'adam' | 'lbfgs' (the reference's commented-out alternative)
+    optimizer: str = "adam"         # 'adam' | 'sgd' | 'lbfgs' (the reference's commented-out alternative)
+    # client optimizer (classifier drivers): torch.optim.SGD semantics with dampening 0 (optim/block_sgd.py)
+    lr: float = 0.0                 # 0 = the optimizer's default: 1e-3 for adam; sgd has none and needs lr > 0
+    momentum: float = 0.0           # sgd only, in [0, 1)
+    nesterov: bool = False          # sgd only, needs momentum > 0
+    weight_decay: float = 0.0       # sgd only, >= 0: adds weight_decay * x to the gradient
     seed: int = 69                  # torch.manual_seed(69) at the top of every reference script
     data: str = "synthetic"         # 'synthetic' | 'torchvision' (needs local files, never downloads)
     data_seed: int = 1234
@@ -155,6 +160,32 @@ def check_norm(norm: str, norm_groups: int, model: str) -> None:
     if norm != "batch" and model not in NORM_MODELS:
         raise ValueError("norm %r needs a model with normalisation layers (%s), got model %r"
                          % (norm, ", ".join(NORM_MODELS), model))
+
+
+OPTIMIZERS = ("adam", "sgd", "lbfgs")
+ADAM_LR = 1e-3                      # the reference's client learning rate
+
+
+def check_client_opt(optimizer: str, lr: float, momentum: float, nesterov: bool, weight_decay: float) -> None:
+    """Raise ``ValueError`` unless the client-optimizer settings of :class:`CommonConfig` are valid."""
+    if optimizer not in OPTIMIZERS:
+        raise ValueError("optimizer must be one of %s, got %r" % (", ".join(OPTIMIZERS), optimizer))
+    if not (math.isfinite(lr) and lr >= 0.0):
+        raise ValueError("lr must be finite and >= 0 (0 = the optimizer's default), got %r" % (lr,))
+    if optimizer == "lbfgs" and lr != 0.0:
+        raise ValueError("lr cannot be set with optimizer 'lbfgs' (its line search sets the step length), got lr %r" % (lr,))
+    if optimizer == "sgd" and lr == 0.0:
+        raise ValueError("optimizer 'sgd' has no default learning rate: set lr > 0")
+    if not 0.0 <= momentum < 1.0:
+        raise ValueError("momentum must lie in [0, 1), got %r" % (momentum,))
+    if not (math.isfinite(weight_decay) and weight_decay >= 0.0):
+        raise ValueError("weight_decay must be finite and >= 0, got %r" % (weight_decay,))
+    for name, val, default in (("momentum", momentum, 0.0), ("nesterov", nesterov, False),
+                               ("weight_decay", weight_decay, 0.0)):
+        if val != default and optimizer != "sgd":
+            raise ValueError("%s needs optimizer 'sgd', got optimizer %r" % (name, optimizer))
+    if nesterov and momentum == 0.0:
+        raise ValueError("nesterov needs momentum > 0, got momentum %r" % (momentum,))
 
 
 PARTITIONS = ("iid", "dirichlet")

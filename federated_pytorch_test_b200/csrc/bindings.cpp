@@ -27,6 +27,18 @@ void adam_prox(Tensor x, Tensor g, Tensor m, Tensor v, Tensor step, double lr, d
   fb::adam_prox(fptr_mut(x), fptr(g), fptr_mut(m), fptr_mut(v), step.data_ptr<int>(), (int)x.numel(), (float)lr, (float)b1,
                 (float)b2, (float)eps, opt_ptr(z), opt_ptr(y), (float)rho, (float)l1, (float)l2, cur_stream(), opt_ptr(rho_dev));
 }
+void sgd_prox(Tensor x, Tensor g, c10::optional<Tensor> buf, double lr, double momentum, bool nesterov, double weight_decay,
+              c10::optional<Tensor> z, c10::optional<Tensor> y, double rho, double l1, double l2,
+              c10::optional<Tensor> rho_dev) {
+  CHECK_F32_CUDA(x); CHECK_CONTIG(x); CHECK_CONTIG(g);
+  const bool has_buf = buf.has_value() && buf->defined();
+  TORCH_CHECK(has_buf == (momentum != 0.0), "sgd_prox: a momentum buffer is passed exactly when momentum != 0");
+  if (has_buf) { CHECK_CONTIG(*buf); TORCH_CHECK(buf->numel() == x.numel(), "sgd_prox: buf must have x's length"); }
+  c10::cuda::CUDAGuard guard(x.device());
+  fb::sgd_prox(fptr_mut(x), fptr(g), has_buf ? buf->data_ptr<float>() : nullptr, (int)x.numel(), (float)lr, (float)momentum,
+               nesterov, (float)weight_decay, opt_ptr(z), opt_ptr(y), (float)rho, (float)l1, (float)l2, cur_stream(),
+               opt_ptr(rho_dev));
+}
 void bump_step(Tensor step) {
   c10::cuda::CUDAGuard guard(step.device());
   fb::bump_step(step.data_ptr<int>(), cur_stream());
@@ -927,6 +939,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "federated_pytorch_test_b200: hand-written sm_90a kernels";
   m.def("launch_count", &launch_count);
   m.def("adam_prox", &adam_prox);
+  m.def("sgd_prox", &sgd_prox);
   m.def("bump_step", &bump_step);
   m.def("l1_l2", &l1_l2);
   m.def("make_pair", &make_pair);

@@ -1,5 +1,6 @@
 // Level-1 kernels over flat parameter blocks (SURVEY G14-G16, G20).
 //  * adam_prox_kernel    : Adam update with the FedProx / augmented-Lagrangian / elastic-net gradient folded in
+//  * sgd_prox_kernel     : SGD (momentum, Nesterov, weight decay) update with the same gradient folded in
 //  * l1_l2, make_pair, welford, penalty_value, penalty_grad, multi_dot : one pass + in-kernel reductions,
 //    results stay on the device (callers read several scalars with ONE D2H copy)
 //  * lbfgs_two_loop_kernel: the whole two-loop recursion (2k+2 dependent passes) as ONE cooperative persistent
@@ -145,6 +146,70 @@ void adam_prox(float* x, const float* g, float* m, float* v, const int* step_dev
                const float* rho_dev) {
   adam_prox_kernel<<<grid_for(n), 256, 0, s>>>(x, g, m, v, step_dev, n, lr, b1, b2, eps, z, y, rho, l1, l2, rho_dev);
   check_launch("adam_prox");
+}
+
+// torch.optim.SGD (dampening 0, weight decay added to the gradient) with the same penalty gradient as adam_prox_kernel:
+//   gt = g + y + rho (x - z) + l1 sign(x) + 2 l2 x + wd x;  buf = mu buf + gt;  x -= lr (nesterov ? gt + mu buf : buf)
+// A zeroed buffer gives torch's first step (buf = gt), so no step counter is read.  buf == nullptr <=> mu == 0: the
+// kernel then reads x, g and writes x only.
+template <bool kMomentum>
+__global__ void __launch_bounds__(256)
+sgd_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __restrict__ buf, int n, float lr, float mu,
+                bool nesterov, float wd, const float* __restrict__ z, const float* __restrict__ y, float rho_host, float l1,
+                float l2, const float* __restrict__ rho_dev) {
+  const float rho = rho_dev != nullptr ? __ldg(rho_dev) : rho_host;
+  const int n4 = n >> 2;
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    float4 xv = reinterpret_cast<float4*>(x)[i];
+    const float4 gv = reinterpret_cast<const float4*>(g)[i];
+    float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (kMomentum) bv = reinterpret_cast<float4*>(buf)[i];
+    float4 zv = make_float4(0.f, 0.f, 0.f, 0.f), yv = zv;
+    if (z != nullptr) zv = reinterpret_cast<const float4*>(z)[i];
+    if (y != nullptr) yv = reinterpret_cast<const float4*>(y)[i];
+    float xs[4] = {xv.x, xv.y, xv.z, xv.w}, gs[4] = {gv.x, gv.y, gv.z, gv.w}, bs[4] = {bv.x, bv.y, bv.z, bv.w},
+          zs[4] = {zv.x, zv.y, zv.z, zv.w}, ys[4] = {yv.x, yv.y, yv.z, yv.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float gt = gs[j] + ys[j] + l1 * sgnf(xs[j]) + 2.f * l2 * xs[j];
+      if (z != nullptr) gt += rho * (xs[j] - zs[j]);
+      gt += wd * xs[j];
+      float d = gt;
+      if (kMomentum) {
+        bs[j] = mu * bs[j] + gt;
+        d = nesterov ? gt + mu * bs[j] : bs[j];
+      }
+      xs[j] -= lr * d;
+    }
+    reinterpret_cast<float4*>(x)[i] = make_float4(xs[0], xs[1], xs[2], xs[3]);
+    if (kMomentum) reinterpret_cast<float4*>(buf)[i] = make_float4(bs[0], bs[1], bs[2], bs[3]);
+  }
+  // scalar tail (n not a multiple of 4)
+  for (int i = (n4 << 2) + blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float xi = x[i];
+    float gt = g[i] + (y ? y[i] : 0.f) + l1 * sgnf(xi) + 2.f * l2 * xi;
+    if (z != nullptr) gt += rho * (xi - z[i]);
+    gt += wd * xi;
+    float d = gt;
+    if (kMomentum) {
+      const float bi = mu * buf[i] + gt;
+      buf[i] = bi;
+      d = nesterov ? gt + mu * bi : bi;
+    }
+    x[i] = xi - lr * d;
+  }
+}
+
+void sgd_prox(float* x, const float* g, float* buf, int n, float lr, float momentum, bool nesterov, float weight_decay,
+              const float* z, const float* y, float rho, float l1, float l2, cudaStream_t s, const float* rho_dev) {
+  if (buf != nullptr)
+    sgd_prox_kernel<true><<<grid_for(n), 256, 0, s>>>(x, g, buf, n, lr, momentum, nesterov, weight_decay, z, y, rho, l1,
+                                                      l2, rho_dev);
+  else
+    sgd_prox_kernel<false><<<grid_for(n), 256, 0, s>>>(x, g, nullptr, n, lr, 0.f, false, weight_decay, z, y, rho, l1, l2,
+                                                       rho_dev);
+  check_launch("sgd_prox");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -15,7 +15,7 @@ Kernel inventory (SURVEY §2.10 ids):
   G5  linear_tf32          wgmma GEMM with bias+ELU epilogue
   G9  cross_entropy        fused log-softmax/NLL fwd, softmax-minus-onehot bwd
   G10 vae_loss             single fused reduction fwd, elementwise bwd
-  G14-16 flat ops          adam_prox, penalty, L-BFGS algebra (see flatops.py)
+  G14-16 flat ops          adam_prox, sgd_prox, penalty, L-BFGS algebra (see flatops.py)
   G22 normalize_u8         uint8 NHWC -> normalised float, layout change fused
       augment_normalize_u8 the same with batch gather + random padded crop + horizontal flip fused (training augmentation)
 
@@ -74,6 +74,12 @@ def adam_prox_step(x, g, m, v, step, lr, beta1, beta2, eps, z=None, y=None, rho=
         t.fill_(int(step))
         step = t
     ext().adam_prox(x, g, m, v, step, lr, beta1, beta2, eps, z, y, rho, lambda1, lambda2, rho_dev)
+
+
+def sgd_prox_step(x, g, buf, lr, momentum, nesterov, weight_decay, z=None, y=None, rho=0.0, lambda1=0.0, lambda2=0.0,
+                  rho_dev=None) -> None:
+    """``buf`` is ``None`` exactly when ``momentum == 0``; no host read, so the launch can be graph-captured."""
+    ext().sgd_prox(x, g, buf, lr, momentum, nesterov, weight_decay, z, y, rho, lambda1, lambda2, rho_dev)
 
 
 def bump_step(step: torch.Tensor) -> None:

@@ -182,6 +182,39 @@ def adam_prox_step(
     x.addcdiv_(m, denom, value=-lr / bc1)
 
 
+def sgd_prox_step(
+    x: torch.Tensor, g: torch.Tensor, buf: Optional[torch.Tensor], lr: float, momentum: float = 0.0,
+    nesterov: bool = False, weight_decay: float = 0.0,
+    z: Optional[torch.Tensor] = None, y: Optional[torch.Tensor] = None, rho: float = 0.0,
+    lambda1: float = 0.0, lambda2: float = 0.0, rho_dev: Optional[torch.Tensor] = None,
+) -> None:
+    """One ``torch.optim.SGD`` update (dampening 0) of ``x`` with the penalty gradients of :func:`adam_prox_step`:
+
+    ``gt = penalty_grad(...) + weight_decay*x``; ``buf = momentum*buf + gt``;
+    ``x -= lr * (gt + momentum*buf if nesterov else buf)``.
+
+    ``buf`` starts at zero (which gives torch's first step, ``buf = gt``) and is ``None`` exactly when ``momentum == 0``.
+    """
+    if (buf is None) != (momentum == 0.0):
+        raise ValueError("sgd_prox_step: pass a momentum buffer exactly when momentum != 0, got momentum %r" % (momentum,))
+    if _cuda(x):
+        from . import cuda_ops
+
+        cuda_ops.sgd_prox_step(x, g, buf, lr, momentum, nesterov, weight_decay, z, y, rho, lambda1, lambda2, rho_dev)
+        return
+    if rho_dev is not None:
+        rho = float(rho_dev)
+    gt = penalty_grad(x, g, z, y, rho, lambda1, lambda2)
+    if weight_decay != 0.0:
+        gt.add_(x, alpha=weight_decay)
+    if buf is not None:
+        buf.mul_(momentum).add_(gt)
+        d = gt.add_(buf, alpha=momentum) if nesterov else buf
+    else:
+        d = gt
+    x.add_(d, alpha=-lr)
+
+
 def penalty_grad(x, g, z=None, y=None, rho: float = 0.0, lambda1: float = 0.0, lambda2: float = 0.0) -> torch.Tensor:
     gt = g.clone()
     if z is not None and rho != 0.0:

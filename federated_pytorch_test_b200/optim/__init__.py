@@ -1,4 +1,5 @@
-"""Optimizers: ``LBFGSNew`` (reference-compatible) and the fused block Adam."""
+"""Optimizers: ``LBFGSNew`` (reference-compatible) and the fused block Adam and SGD."""
+from .block_sgd import BlockSGD
 from .lbfgsnew import LBFGSNew
 
-__all__ = ["LBFGSNew"]
+__all__ = ["BlockSGD", "LBFGSNew"]
