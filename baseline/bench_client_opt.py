@@ -1,4 +1,5 @@
-"""Cost of the client SGD update against the client Adam update, on one GPU.
+"""Cost of the client SGD update against the client Adam update, and of the client recipe (AdamW, gradient-norm clipping,
+a device learning rate for the schedule), on one GPU.
 
 1. The fused update kernels alone (``adam_prox`` and ``sgd_prox`` with momentum 0.9 and with momentum 0, each without and
    with the consensus vectors ``z`` / ``y``) at the ten ResNet18 block sizes.  Each variant is launched ``--calls`` times
@@ -6,9 +7,13 @@
    in us per launch and in GB/s of the bytes the update must move per parameter (computed below from what the kernel
    reads and writes: Adam reads x, g, m, v and writes x, m, v = 28 B; SGD with momentum reads x, g, buf and writes x, buf =
    20 B; SGD without momentum reads x, g and writes x = 12 B; z and y add 4 B each).
+   The recipe arms run the gradient-norm kernel and the update together, with the learning rate read from the device:
+   ``adamw_clip`` (AdamW, weight decay 0.05, clip 1.0) against ``adam``, and ``sgd_m0.9_clip`` against ``sgd_m0.9``.
+   Clipping adds one read of g (4 B per parameter), which the byte counts include, and a few KB of per-CTA partials.
 2. A CUDA-graphed training step of ResNet18 at batch 128 with every parameter trainable (forward, backward, fused update):
-   Adam against SGD (momentum 0.9, Nesterov, weight decay 5e-4), alternating window by window, median of ``--windows``
-   windows of ``--steps`` replays.
+   Adam against SGD (momentum 0.9, Nesterov, weight decay 5e-4) and against AdamW + clipping + a cosine schedule (the
+   device learning rate rewritten before every window), alternating window by window, median of ``--windows`` windows
+   of ``--steps`` replays.
 
 Prints the device name, its power limit and max SM clock, a table, then one JSON line.  Writes nothing to disk.
 
@@ -37,19 +42,41 @@ KERNELS = {
     "adam": (28, None, False), "adam_zy": (36, None, True),
     "sgd_m0.9": (20, 0.9, False), "sgd_m0.9_zy": (28, 0.9, True),
     "sgd_m0": (12, 0.0, False), "sgd_m0_zy": (20, 0.0, True),
+    "adamw_clip": (32, None, False), "sgd_m0.9_clip": (24, 0.9, False),
 }
+CLIP = 1.0
 
 
 def _update_call(name: str, n: int, dev):
     """(call, tensors it keeps alive) of one update launch on a fresh block of ``n`` parameters."""
     from federated_pytorch_test_b200.ops import cuda_ops
 
+    from federated_pytorch_test_b200.ops import flatops
+
     _, mom, zy = KERNELS[name]
+    clip = name.endswith("_clip")
     g = torch.Generator(device=dev).manual_seed(n)
     x = torch.randn(n, device=dev, generator=g)
     gr = 1e-3 * torch.randn(n, device=dev, generator=g)
     z, y = (torch.randn(n, device=dev, generator=g), 1e-3 * torch.randn(n, device=dev, generator=g)) if zy else (None, None)
     rho = 0.1 if zy else 0.0
+    if clip:       # the recipe: norm kernel + update, learning rate read from the device
+        ws, ticket = flatops.clip_workspace(x)
+        lr = torch.full((1,), 1e-3, device=dev)
+        if mom is None:
+            m, v, step = torch.zeros(n, device=dev), torch.zeros(n, device=dev), torch.ones(1, dtype=torch.int32, device=dev)
+
+            def call():
+                cuda_ops.grad_norm(gr, ws, ticket, CLIP)
+                cuda_ops.adam_prox_step(x, gr, m, v, step, 0.0, 0.9, 0.999, 1e-8, lr_dev=lr, weight_decay=0.05,
+                                        norm_dev=ws[0:1], clip_norm=CLIP)
+            return call, (x, gr, m, v, step, ws, ticket, lr)
+        buf = torch.zeros(n, device=dev)
+
+        def call():
+            cuda_ops.grad_norm(gr, ws, ticket, CLIP)
+            cuda_ops.sgd_prox_step(x, gr, buf, 0.0, mom, False, 0.0, lr_dev=lr, norm_dev=ws[0:1], clip_norm=CLIP)
+        return call, (x, gr, buf, ws, ticket, lr)
     if mom is None:
         m, v, step = torch.zeros(n, device=dev), torch.zeros(n, device=dev), torch.ones(1, dtype=torch.int32, device=dev)
         return (lambda: cuda_ops.adam_prox_step(x, gr, m, v, step, 1e-3, 0.9, 0.999, 1e-8, z, y, rho, 1e-4, 1e-4)), \
@@ -72,8 +99,12 @@ def _graphed_step(kind: str, dev):
     arena = FlatArena(net, channels_last_weights=True)
     unfreeze_all_layers(net)
     last = len(arena.params) - 1
-    opt = (BlockAdam(arena, 0, last) if kind == "adam"
-           else BlockSGD(arena, 0, last, lr=0.05, momentum=0.9, nesterov=True, weight_decay=5e-4))
+    if kind == "adam":
+        opt = BlockAdam(arena, 0, last)
+    elif kind == "adamw_clip_cosine":
+        opt = BlockAdam(arena, 0, last, adamw=True, weight_decay=0.05, clip_norm=CLIP, device_lr=True)
+    else:
+        opt = BlockSGD(arena, 0, last, lr=0.05, momentum=0.9, nesterov=True, weight_decay=5e-4)
     g = torch.Generator(device=dev).manual_seed(1)
     x = torch.randn(B, 3, 32, 32, device=dev, generator=g).contiguous(memory_format=torch.channels_last)
     y = torch.randint(0, 10, (B,), device=dev, generator=g)
@@ -121,13 +152,17 @@ def main(argv=None) -> dict:
                          GBps={k: round(KERNELS[k][0] * n / (us[k] * 1e-6) / 1e9, 1) for k in KERNELS}))
         del calls
 
-    steps = {k: _graphed_step(k, dev) for k in ("adam", "sgd")}
+    from federated_pytorch_test_b200.optim.schedule import round_lr
+
+    steps = {k: _graphed_step(k, dev) for k in ("adam", "sgd", "adamw_clip_cosine")}
     for graph, _ in steps.values():
         for _ in range(5):
             graph.replay()
     torch.cuda.synchronize()
     step_times = {k: [] for k in steps}
-    for _ in range(args.windows):
+    sched_opt = steps["adamw_clip_cosine"][1][2]
+    for w in range(args.windows):
+        sched_opt.set_lr(round_lr(1e-3, w, args.windows, "cosine"))      # a new round's rate, no re-capture
         for k, (graph, _) in steps.items():
             step_times[k].append(_time(graph.replay, args.steps))
     step_ms = {k: 1e3 * statistics.median(v) for k, v in step_times.items()}
@@ -147,7 +182,7 @@ def main(argv=None) -> dict:
     for r in rows:
         print("    %9d " % r["n"] + " ".join("%10.2f (%7.1f)" % (r["us"][k], r["GBps"][k]) for k in KERNELS))
     for k, v in step_ms.items():
-        print("  ResNet18 graphed step, batch %d, every parameter trainable, %-4s %7.3f ms (median of %d windows)"
+        print("  ResNet18 graphed step, batch %d, every parameter trainable, %-17s %7.3f ms (median of %d windows)"
               % (B, k, v, args.windows))
     print(json.dumps(res))
     return res

@@ -43,6 +43,7 @@ from ..ops import flatops
 from ..optim.block_adam import BlockAdam
 from ..optim.block_sgd import BlockSGD
 from ..optim.lbfgsnew import LBFGSNew
+from ..optim.schedule import round_lr, schedule_active
 from ..parallel.topology import Topology
 from ..utils.flat import FlatArena
 from ..utils.metrics import MetricsLog, PhaseTimers, nvtx_range
@@ -61,7 +62,7 @@ class Visit:
     hi: int                    # last trainable parameter index (inclusive)
     ci: int                    # block index: selects rho[ci], the elastic-net gate, log labels
     label: Tuple[int, int]     # what the legacy log lines print as block=[a,b]
-    optimizer: str = "adam"    # 'adam' | 'sgd' | 'lbfgs'
+    optimizer: str = "adam"    # 'adam' | 'adamw' | 'sgd' | 'lbfgs'
     opt_kwargs: Dict = field(default_factory=dict)
     lambda1: float = 0.0       # elastic net on the block vector (already gated by the task)
     lambda2: float = 0.0
@@ -171,6 +172,17 @@ class EngineConfig:
     resume_path: str = ""            # write a true-resume record here after every aggregation round ('' = never)
     streams: bool = True             # co-resident replicas (K > #GPUs) step concurrently on their own CUDA streams
     round_metrics: bool = True       # per-round JSONL: images/s, step / aggregate / eval device ms, bus GB/s
+    # client learning-rate schedule over the run's rounds (optim/schedule.py); the base rate is the visit's opt_kwargs lr
+    lr_schedule: str = "const"
+    lr_warmup: int = 0
+    lr_gamma: float = 0.1
+    lr_step_rounds: int = 0
+    lr_min: float = 0.0
+
+    def recipe(self, clip_norm: float = 0.0) -> Dict:
+        """The schedule and clipping settings a resume record must match."""
+        return dict(lr_schedule=self.lr_schedule, lr_warmup=self.lr_warmup, lr_gamma=self.lr_gamma,
+                    lr_step_rounds=self.lr_step_rounds, lr_min=self.lr_min, clip_norm=clip_norm)
 
 
 class Engine:
@@ -205,6 +217,18 @@ class Engine:
         self._resume_state: Optional[Dict] = None
         self._round_mark = {"images": 0, "t": time.perf_counter(), "ms": {}}
         self._streams: Dict[int, "torch.cuda.Stream"] = {}
+        self._round_extra: Dict = {}
+        # client learning-rate schedule: round r of T (a pure function of the schedule position)
+        self.scheduled = schedule_active(cfg.lr_schedule, cfg.lr_warmup)
+        self.total_rounds = 0
+        self._visit_base: List[int] = []      # rounds before each nloop's first visit, in visits
+        if self.scheduled:
+            counts = [sum(1 for _ in task.visits(n)) for n in range(cfg.Nloop)]
+            self._visit_base = [sum(counts[:n]) for n in range(cfg.Nloop)]
+            self.total_rounds = sum(counts) * cfg.Nadmm * cfg.Nepoch
+            if cfg.lr_warmup >= self.total_rounds:
+                raise ValueError("lr_warmup must be smaller than the run's number of rounds T = %d (Nloop x block visits x "
+                                 "Nadmm x Nepoch), got lr_warmup %d" % (self.total_rounds, cfg.lr_warmup))
 
     # ------------------------------------------------------------------
     def log(self, msg: str, root_only: bool = False) -> None:
@@ -215,12 +239,15 @@ class Engine:
     # ------------------------------------------------------------------
     def _make_optimizer(self, rep: Replica, visit: Visit):
         arena = rep.arenas[visit.model]
-        if visit.optimizer == "adam":
-            key = (rep.ck, visit.model, visit.lo, visit.hi)
+        if visit.optimizer in ("adam", "adamw"):
+            key = (rep.ck, visit.model, visit.lo, visit.hi) if visit.optimizer == "adam" else \
+                ("adamw", rep.ck, visit.model, visit.lo, visit.hi)
             opt = self._block_opt_cache.get(key)
-            lr = visit.opt_kwargs.get("lr", 1e-3)
+            kw = dict(visit.opt_kwargs)
+            lr = kw.pop("lr", 1e-3)
             if opt is None:
-                opt = BlockAdam(arena, visit.lo, visit.hi, lr=lr)
+                opt = BlockAdam(arena, visit.lo, visit.hi, lr=lr, adamw=visit.optimizer == "adamw",
+                                device_lr=self.scheduled, **kw)
                 self._block_opt_cache[key] = opt
             else:
                 opt.reset(lr=lr)  # same as a freshly constructed Adam (Q18), but buffers/graphs persist
@@ -229,7 +256,7 @@ class Engine:
             key = ("sgd", rep.ck, visit.model, visit.lo, visit.hi)
             opt = self._block_opt_cache.get(key)
             if opt is None:
-                opt = BlockSGD(arena, visit.lo, visit.hi, **visit.opt_kwargs)
+                opt = BlockSGD(arena, visit.lo, visit.hi, device_lr=self.scheduled, **visit.opt_kwargs)
                 self._block_opt_cache[key] = opt
             else:
                 opt.reset(lr=visit.opt_kwargs["lr"])  # a zero momentum buffer, as a fresh SGD (Q18); buffers/graphs persist
@@ -336,10 +363,17 @@ class Engine:
             if held != visit.optimizer:
                 raise ValueError("resume record was written with optimizer %r, this run uses optimizer %r"
                                  % (held, visit.optimizer))
+            want = cfg.recipe(visit.opt_kwargs.get("clip_norm", 0.0))
+            held = self._resume_pos.get("recipe", EngineConfig().recipe())   # records written before schedules: defaults
+            for name, val in want.items():
+                if held.get(name) != val:
+                    raise ValueError("resume record was written with %s %r, this run uses %s %r"
+                                     % (name, held.get(name), name, val))
             first_round = int(self._resume_pos.get("round", 0))
             self._restore_visit_state()
             self._resume_pos = None
         rounds = [(nadmm, epoch) for nadmm in range(cfg.Nadmm) for epoch in range(cfg.Nepoch)]
+        clip = visit.opt_kwargs.get("clip_norm", 0.0) > 0.0
         try:
             for ri, (nadmm, epoch) in enumerate(rounds):
                 if ri < first_round:
@@ -347,6 +381,14 @@ class Engine:
                 self.last_epoch = epoch
                 if cfg.reset_optimizer_each_epoch and epoch > 0:
                     self.optimizers = [self._make_optimizer(rep, visit) for rep in self.replicas]
+                extra: Dict = {}
+                if self.scheduled:
+                    # round r of the whole run; written on the current stream, which the replicas' streams wait on
+                    r = (self._visit_base[nloop] + vi) * len(rounds) + ri
+                    extra["lr"] = round_lr(visit.opt_kwargs["lr"], r, self.total_rounds, cfg.lr_schedule, cfg.lr_warmup,
+                                           cfg.lr_gamma, cfg.lr_step_rounds, cfg.lr_min)
+                    for opt in self.optimizers:
+                        opt.set_lr(extra["lr"])
                 task.on_epoch_start(epoch, self)
                 with nvtx_range("fedb200:steps"):
                     self._run_replicas(visit, nloop, epoch, N)
@@ -354,15 +396,28 @@ class Engine:
                     return
                 last_epoch_of_round = epoch == cfg.Nepoch - 1
                 if cfg.aggregate_in_epoch_loop or last_epoch_of_round:
+                    if clip:
+                        extra["clip"] = self._take_clip_stats()
+                    self._round_extra = extra          # the round row's lr / clip fields, carried with the pending round
                     self._aggregate(visit, nloop, nadmm, epoch if cfg.aggregate_in_epoch_loop else cfg.Nepoch - 1, N)
                     if cfg.resume_path:
                         from ..utils import ckpt
 
                         ckpt.save_resume(cfg.resume_path, self, dict(nloop=nloop, visit=vi, round=ri + 1, nadmm=nadmm, epoch=epoch,
-                                                                    optimizer=visit.optimizer))
+                                                                    optimizer=visit.optimizer,
+                                                                    recipe=cfg.recipe(visit.opt_kwargs.get("clip_norm", 0.0))))
         finally:
             if self._pending_round is not None:      # the last round of the visit (or a stop request): nothing left to overlap with
                 self._finish_round()
+
+    def _take_clip_stats(self) -> torch.Tensor:
+        """``[sum of pre-clip norms, clipped steps, steps]`` over the local optimizers since the last call, and zero their
+        accumulators; in stream order, so a minibatch queued behind a deferred aggregation counts toward the next round."""
+        stats = [opt.clip_stats for opt in self.optimizers]
+        snap = torch.stack(stats).sum(0)
+        for st in stats:
+            st.zero_()
+        return snap
 
     def _restore_visit_state(self) -> None:
         st = self._resume_state or {}
@@ -473,12 +528,13 @@ class Engine:
             self.attack(self)
         with nvtx_range("fedb200:aggregate"), self.timers.phase("aggregate"):
             token = self.strategy.aggregate_begin(nadmm) if defer else ("done", self.strategy.aggregate(nadmm))
-        self._pending_round = (token, visit, nloop, nadmm, epoch, N)
+        self._pending_round = (token, visit, nloop, nadmm, epoch, N, self._round_extra)
+        self._round_extra = {}
         if token[0] == "done":
             self._finish_round()
 
     def _finish_round(self) -> None:
-        token, visit, nloop, nadmm, epoch, N = self._pending_round
+        token, visit, nloop, nadmm, epoch, N, extra = self._pending_round
         self._pending_round = None
         metrics = self.strategy.aggregate_end(token)
         self.aggregations_done += 1
@@ -493,6 +549,12 @@ class Engine:
         if metrics:
             self.task.aggregate_log(visit, metrics, ctx, self)
             row = dict(kind="round", block=visit.ci, label=list(visit.label), model=visit.model, **ctx, **metrics)
+            if "lr" in extra:
+                row["lr"] = extra["lr"]
+            if "clip" in extra:                    # mean pre-clip gradient norm of the round's local steps, clipped share
+                norm_sum, clipped, steps = (float(v) for v in extra["clip"].tolist())
+                row["grad_norm"] = norm_sum / steps if steps else float("nan")
+                row["clip_frac"] = clipped / steps if steps else float("nan")
             if self.cfg.round_metrics:
                 row.update(self._round_perf(N))
             self.metrics.write(row)

@@ -98,8 +98,10 @@ class GraphedEval:
 
 class GraphedAdamStep:
     """The minibatch step of a block optimizer (``BlockAdam`` or ``BlockSGD``: it only calls ``zero_grad``,
-    ``apply_update`` and ``set_penalty``).  A host-side learning rate is baked into the capture; it does not change within
-    a run."""
+    ``apply_update`` and ``set_penalty``).  The graph is captured once per (replica, block, batch shape) and a change of
+    learning rate does not invalidate it: with a schedule the optimizer passes its device ``lr_dev``, which the engine
+    rewrites in stream order at the start of every round, and without one the host rate is constant over the run.
+    With clipping the captured update is two kernels, the gradient norm and the step."""
 
     WARMUP = 3
 

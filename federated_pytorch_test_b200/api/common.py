@@ -17,7 +17,7 @@ import torch.nn as nn
 
 from .. import models
 from ..algo.engine import Engine, EngineConfig, Replica, Task, Visit
-from ..config import ADAM_LR, CommonConfig, check_client_opt, check_norm, check_partition
+from ..config import ADAM_LR, CLIENT_RECIPE_DEFAULTS, CommonConfig, check_client_opt, check_norm, check_partition
 from ..data.cifar import (CifarData, ShardLoader, augment_key, class_histogram, dirichlet_shards, shard_ranges,
                           worker_norm)
 from ..ops import functional as FX
@@ -43,10 +43,12 @@ def require_batch_norm(cfg: CommonConfig, driver: str) -> None:
 def require_default_client_opt(cfg: CommonConfig, driver: str) -> None:
     """The VAE, VAE-CL and CPC drivers fix their own optimizers (as the reference does) and accept none of the client-optimizer
     flags of the classifier drivers."""
-    for name, default in (("lr", 0.0), ("momentum", 0.0), ("nesterov", False), ("weight_decay", 0.0)):
+    for name, default in (("lr", 0.0), ("momentum", 0.0), ("nesterov", False), ("weight_decay", 0.0)) + CLIENT_RECIPE_DEFAULTS:
         if getattr(cfg, name, default) != default:
             raise ValueError("%s fixes its own optimizer and does not take %s, got %s %r"
                              % (driver, name, name, getattr(cfg, name)))
+    if getattr(cfg, "optimizer", "adam") == "adamw":
+        raise ValueError("%s fixes its own optimizer and does not take optimizer 'adamw'" % driver)
 
 
 def require_iid(cfg: CommonConfig, driver: str) -> None:
@@ -72,7 +74,9 @@ def engine_config(cfg: CommonConfig, **kw) -> EngineConfig:
     base = dict(Nloop=cfg.Nloop, Nadmm=cfg.Nadmm, Nepoch=cfg.Nepoch, check_results=cfg.check_results,
                 be_verbose=cfg.be_verbose, diagnostics=cfg.diagnostics, graphs=cfg.graphs,
                 max_minibatches=cfg.max_minibatches or None, nan_guard=getattr(cfg, "nan_guard", "raise"),
-                resume_path=getattr(cfg, "resume_out", ""), streams=getattr(cfg, "streams", True))
+                resume_path=getattr(cfg, "resume_out", ""), streams=getattr(cfg, "streams", True),
+                lr_schedule=cfg.lr_schedule, lr_warmup=cfg.lr_warmup, lr_gamma=cfg.lr_gamma,
+                lr_step_rounds=cfg.lr_step_rounds, lr_min=cfg.lr_min)
     base.update(kw)
     return EngineConfig(**base)
 
@@ -101,7 +105,8 @@ class ClassifierTask(Task):
         self.model_name = name
         norm = getattr(cfg, "norm", "batch")
         check_norm(norm, getattr(cfg, "norm_groups", 32), name)
-        check_client_opt(cfg.optimizer, cfg.lr, cfg.momentum, cfg.nesterov, cfg.weight_decay)
+        check_client_opt(cfg.optimizer, cfg.lr, cfg.momentum, cfg.nesterov, cfg.weight_decay, cfg.lr_schedule, cfg.lr_warmup,
+                         cfg.lr_gamma, cfg.lr_step_rounds, cfg.lr_min, cfg.clip_norm)
         self.factory = _MODEL_FACTORIES[name]
         if norm != "batch":
             self.factory = functools.partial(self.factory, norm=norm, groups=cfg.norm_groups)
@@ -157,10 +162,14 @@ class ClassifierTask(Task):
         cfg = self.cfg
         if cfg.optimizer == "adam":
             opt_kwargs = dict(lr=cfg.lr or ADAM_LR)
+        elif cfg.optimizer == "adamw":
+            opt_kwargs = dict(lr=cfg.lr or ADAM_LR, weight_decay=cfg.weight_decay)
         elif cfg.optimizer == "sgd":
             opt_kwargs = dict(lr=cfg.lr, momentum=cfg.momentum, nesterov=cfg.nesterov, weight_decay=cfg.weight_decay)
         else:
             opt_kwargs = dict(history_size=10, max_iter=4, line_search_fn=True, batch_mode=True)
+        if cfg.clip_norm > 0.0:
+            opt_kwargs["clip_norm"] = cfg.clip_norm
         if self.whole_model:
             yield Visit("net", 0, self.n_params - 1, 0, (0, self.n_params - 1), self.cfg.optimizer, opt_kwargs)
             return

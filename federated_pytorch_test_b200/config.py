@@ -36,12 +36,21 @@ class CommonConfig:
     use_cuda: bool = True
     # ---- new in this framework -------------------------------------------------
     model: str = ""                 # '', 'Net', 'Net1', 'Net2', 'ResNet18', 'ResNet9' ('' = follow use_resnet)
-    optimizer: str = "adam"         # 'adam' | 'sgd' | 'lbfgs' (the reference's commented-out alternative)
-    # client optimizer (classifier drivers): torch.optim.SGD semantics with dampening 0 (optim/block_sgd.py)
-    lr: float = 0.0                 # 0 = the optimizer's default: 1e-3 for adam; sgd has none and needs lr > 0
+    optimizer: str = "adam"         # 'adam' | 'adamw' | 'sgd' | 'lbfgs' (the reference's commented-out alternative)
+    # client optimizer (classifier drivers): torch.optim.SGD semantics with dampening 0 (optim/block_sgd.py), and
+    # torch.optim.AdamW (optim/block_adam.py)
+    lr: float = 0.0                 # 0 = the optimizer's default: 1e-3 for adam / adamw; sgd has none and needs lr > 0
     momentum: float = 0.0           # sgd only, in [0, 1)
     nesterov: bool = False          # sgd only, needs momentum > 0
-    weight_decay: float = 0.0       # sgd only, >= 0: adds weight_decay * x to the gradient
+    weight_decay: float = 0.0       # sgd / adamw, >= 0: sgd adds weight_decay * x to the gradient, adamw decays x by
+                                    # 1 - lr * weight_decay before its step
+    # client learning-rate schedule over communication rounds (optim/schedule.py; adam / adamw / sgd)
+    lr_schedule: str = "const"      # 'const' | 'step' | 'cosine'
+    lr_warmup: int = 0              # linear warmup over the first lr_warmup rounds, with any schedule
+    lr_gamma: float = 0.1           # step only, in (0, 1]: the factor every lr_step_rounds rounds
+    lr_step_rounds: int = 0         # step only, >= 1 (no default: 0 = unset)
+    lr_min: float = 0.0             # cosine only, in [0, 1): the final rate is lr_min * lr
+    clip_norm: float = 0.0          # > 0: clip the block's data-loss gradient to this norm before every step (0 = off)
     seed: int = 69                  # torch.manual_seed(69) at the top of every reference script
     data: str = "synthetic"         # 'synthetic' | 'torchvision' (needs local files, never downloads)
     data_seed: int = 1234
@@ -162,11 +171,17 @@ def check_norm(norm: str, norm_groups: int, model: str) -> None:
                          % (norm, ", ".join(NORM_MODELS), model))
 
 
-OPTIMIZERS = ("adam", "sgd", "lbfgs")
+OPTIMIZERS = ("adam", "adamw", "sgd", "lbfgs")
 ADAM_LR = 1e-3                      # the reference's client learning rate
+LR_SCHEDULES = ("const", "step", "cosine")
+# the client-recipe fields (schedule and clipping) and their defaults
+CLIENT_RECIPE_DEFAULTS = (("lr_schedule", "const"), ("lr_warmup", 0), ("lr_gamma", 0.1), ("lr_step_rounds", 0),
+                          ("lr_min", 0.0), ("clip_norm", 0.0))
 
 
-def check_client_opt(optimizer: str, lr: float, momentum: float, nesterov: bool, weight_decay: float) -> None:
+def check_client_opt(optimizer: str, lr: float, momentum: float, nesterov: bool, weight_decay: float,
+                     lr_schedule: str = "const", lr_warmup: int = 0, lr_gamma: float = 0.1, lr_step_rounds: int = 0,
+                     lr_min: float = 0.0, clip_norm: float = 0.0) -> None:
     """Raise ``ValueError`` unless the client-optimizer settings of :class:`CommonConfig` are valid."""
     if optimizer not in OPTIMIZERS:
         raise ValueError("optimizer must be one of %s, got %r" % (", ".join(OPTIMIZERS), optimizer))
@@ -180,12 +195,39 @@ def check_client_opt(optimizer: str, lr: float, momentum: float, nesterov: bool,
         raise ValueError("momentum must lie in [0, 1), got %r" % (momentum,))
     if not (math.isfinite(weight_decay) and weight_decay >= 0.0):
         raise ValueError("weight_decay must be finite and >= 0, got %r" % (weight_decay,))
-    for name, val, default in (("momentum", momentum, 0.0), ("nesterov", nesterov, False),
-                               ("weight_decay", weight_decay, 0.0)):
+    for name, val, default in (("momentum", momentum, 0.0), ("nesterov", nesterov, False)):
         if val != default and optimizer != "sgd":
             raise ValueError("%s needs optimizer 'sgd', got optimizer %r" % (name, optimizer))
+    if weight_decay != 0.0 and optimizer not in ("sgd", "adamw"):
+        raise ValueError("weight_decay needs optimizer 'sgd' or 'adamw' (coupled L2 decay for Adam is not offered), "
+                         "got optimizer %r" % (optimizer,))
     if nesterov and momentum == 0.0:
         raise ValueError("nesterov needs momentum > 0, got momentum %r" % (momentum,))
+    # learning-rate schedule and clipping
+    if lr_schedule not in LR_SCHEDULES:
+        raise ValueError("lr_schedule must be one of %s, got %r" % (", ".join(LR_SCHEDULES), lr_schedule))
+    if not (isinstance(lr_warmup, int) and lr_warmup >= 0):
+        raise ValueError("lr_warmup must be an integer >= 0, got %r" % (lr_warmup,))
+    if not 0.0 < lr_gamma <= 1.0:
+        raise ValueError("lr_gamma must lie in (0, 1], got %r" % (lr_gamma,))
+    if not (isinstance(lr_step_rounds, int) and lr_step_rounds >= 0):
+        raise ValueError("lr_step_rounds must be an integer >= 0 (0 = unset), got %r" % (lr_step_rounds,))
+    if not 0.0 <= lr_min < 1.0:
+        raise ValueError("lr_min must lie in [0, 1), got %r" % (lr_min,))
+    if not (math.isfinite(clip_norm) and clip_norm >= 0.0):
+        raise ValueError("clip_norm must be finite and >= 0 (0 = off), got %r" % (clip_norm,))
+    if lr_schedule == "step" and lr_step_rounds < 1:
+        raise ValueError("lr_schedule 'step' needs lr_step_rounds >= 1, got lr_step_rounds %r" % (lr_step_rounds,))
+    for name, val, default, owner in (("lr_gamma", lr_gamma, 0.1, "step"), ("lr_step_rounds", lr_step_rounds, 0, "step"),
+                                      ("lr_min", lr_min, 0.0, "cosine")):
+        if val != default and lr_schedule != owner:
+            raise ValueError("%s belongs to lr_schedule %r, got lr_schedule %r" % (name, owner, lr_schedule))
+    if optimizer == "lbfgs":
+        for name, val, default in (("lr_schedule", lr_schedule, "const"), ("lr_warmup", lr_warmup, 0),
+                                   ("clip_norm", clip_norm, 0.0)):
+            if val != default:
+                raise ValueError("%s cannot be set with optimizer 'lbfgs' (its line search sets the step), got %s %r"
+                                 % (name, name, val))
 
 
 PARTITIONS = ("iid", "dirichlet")

@@ -21,15 +21,17 @@ static const float* opt_ptr(const c10::optional<Tensor>& t) { return (t.has_valu
 // ---------------------------------------------------------------------------------------------- flat ops
 void adam_prox(Tensor x, Tensor g, Tensor m, Tensor v, Tensor step, double lr, double b1, double b2, double eps,
                c10::optional<Tensor> z, c10::optional<Tensor> y, double rho, double l1, double l2,
-               c10::optional<Tensor> rho_dev) {
+               c10::optional<Tensor> rho_dev, c10::optional<Tensor> lr_dev, double weight_decay,
+               c10::optional<Tensor> norm_dev, double clip) {
   CHECK_F32_CUDA(x); CHECK_CONTIG(x); CHECK_CONTIG(g); CHECK_CONTIG(m); CHECK_CONTIG(v);
   c10::cuda::CUDAGuard guard(x.device());
   fb::adam_prox(fptr_mut(x), fptr(g), fptr_mut(m), fptr_mut(v), step.data_ptr<int>(), (int)x.numel(), (float)lr, (float)b1,
-                (float)b2, (float)eps, opt_ptr(z), opt_ptr(y), (float)rho, (float)l1, (float)l2, cur_stream(), opt_ptr(rho_dev));
+                (float)b2, (float)eps, opt_ptr(z), opt_ptr(y), (float)rho, (float)l1, (float)l2, cur_stream(), opt_ptr(rho_dev),
+                opt_ptr(lr_dev), (float)weight_decay, opt_ptr(norm_dev), (float)clip);
 }
 void sgd_prox(Tensor x, Tensor g, c10::optional<Tensor> buf, double lr, double momentum, bool nesterov, double weight_decay,
               c10::optional<Tensor> z, c10::optional<Tensor> y, double rho, double l1, double l2,
-              c10::optional<Tensor> rho_dev) {
+              c10::optional<Tensor> rho_dev, c10::optional<Tensor> lr_dev, c10::optional<Tensor> norm_dev, double clip) {
   CHECK_F32_CUDA(x); CHECK_CONTIG(x); CHECK_CONTIG(g);
   const bool has_buf = buf.has_value() && buf->defined();
   TORCH_CHECK(has_buf == (momentum != 0.0), "sgd_prox: a momentum buffer is passed exactly when momentum != 0");
@@ -37,7 +39,18 @@ void sgd_prox(Tensor x, Tensor g, c10::optional<Tensor> buf, double lr, double m
   c10::cuda::CUDAGuard guard(x.device());
   fb::sgd_prox(fptr_mut(x), fptr(g), has_buf ? buf->data_ptr<float>() : nullptr, (int)x.numel(), (float)lr, (float)momentum,
                nesterov, (float)weight_decay, opt_ptr(z), opt_ptr(y), (float)rho, (float)l1, (float)l2, cur_stream(),
-               opt_ptr(rho_dev));
+               opt_ptr(rho_dev), opt_ptr(lr_dev), opt_ptr(norm_dev), (float)clip);
+}
+int64_t grad_norm_blocks(int64_t n) { return fb::grad_norm_blocks((int)n); }
+void grad_norm(Tensor g, Tensor ws, Tensor ticket, double clip) {
+  CHECK_F32_CUDA(g); CHECK_CONTIG(g); CHECK_F32_CUDA(ws); CHECK_CONTIG(ws);
+  TORCH_CHECK(ticket.is_cuda() && ticket.scalar_type() == torch::kInt32 && ticket.numel() == 1,
+              "grad_norm: ticket must be one CUDA int32");
+  TORCH_CHECK(ws.numel() >= fb::kGradNormHeader + fb::grad_norm_blocks((int)g.numel()),
+              "grad_norm: ws needs ", fb::kGradNormHeader, " + grad_norm_blocks(n) floats");
+  c10::cuda::CUDAGuard guard(g.device());
+  fb::grad_norm(fptr(g), (int)g.numel(), fptr_mut(ws), reinterpret_cast<unsigned int*>(ticket.data_ptr<int>()), (float)clip,
+                cur_stream());
 }
 void bump_step(Tensor step) {
   c10::cuda::CUDAGuard guard(step.device());
@@ -940,6 +953,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("launch_count", &launch_count);
   m.def("adam_prox", &adam_prox);
   m.def("sgd_prox", &sgd_prox);
+  m.def("grad_norm_blocks", &grad_norm_blocks);
+  m.def("grad_norm", &grad_norm);
   m.def("bump_step", &bump_step);
   m.def("l1_l2", &l1_l2);
   m.def("make_pair", &make_pair);

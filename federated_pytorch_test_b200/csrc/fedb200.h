@@ -87,10 +87,16 @@ void conv_wgrad_tf32(const float* x, const float* dy, float* dw, int NB, int H, 
 // ---- flat-vector kernels (flat_kernels.cu) ---------------------------------------------------------
 void adam_prox(float* x, const float* g, float* m, float* v, const int* step_dev, int n, float lr, float b1, float b2,
                float eps, const float* z, const float* y, float rho, float l1, float l2, cudaStream_t s,
-               const float* rho_dev = nullptr);
+               const float* rho_dev = nullptr, const float* lr_dev = nullptr, float weight_decay = 0.f,
+               const float* norm_dev = nullptr, float clip = 0.f);
 // buf == nullptr: no momentum (momentum must then be 0)
 void sgd_prox(float* x, const float* g, float* buf, int n, float lr, float momentum, bool nesterov, float weight_decay,
-              const float* z, const float* y, float rho, float l1, float l2, cudaStream_t s, const float* rho_dev);
+              const float* z, const float* y, float rho, float l1, float l2, cudaStream_t s, const float* rho_dev,
+              const float* lr_dev = nullptr, const float* norm_dev = nullptr, float clip = 0.f);
+// gradient norm for clipping: ws = [norm, sum of norms, clipped steps, steps, partials[grad_norm_blocks(n)]]
+constexpr int kGradNormHeader = 4;
+int grad_norm_blocks(int n);
+void grad_norm(const float* g, int n, float* ws, unsigned int* ticket, float clip, cudaStream_t s);
 void bump_step(int* step_dev, cudaStream_t s);
 void l1_l2(const float* g, int n, float* out2, cudaStream_t s);
 void make_pair(const float* g, const float* gprev, const float* d, float t, float trust, float* y, float* sv, int n,

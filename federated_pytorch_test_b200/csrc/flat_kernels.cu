@@ -1,6 +1,7 @@
 // Level-1 kernels over flat parameter blocks (SURVEY G14-G16, G20).
 //  * adam_prox_kernel    : Adam update with the FedProx / augmented-Lagrangian / elastic-net gradient folded in
 //  * sgd_prox_kernel     : SGD (momentum, Nesterov, weight decay) update with the same gradient folded in
+//  * grad_norm_kernel    : the block's gradient norm for client gradient-norm clipping, reduced in a fixed order
 //  * l1_l2, make_pair, welford, penalty_value, penalty_grad, multi_dot : one pass + in-kernel reductions,
 //    results stay on the device (callers read several scalars with ONE D2H copy)
 //  * lbfgs_two_loop_kernel: the whole two-loop recursion (2k+2 dependent passes) as ONE cooperative persistent
@@ -91,13 +92,31 @@ void bump_step(int* step_dev, cudaStream_t s) {
   check_launch("bump_step");
 }
 
+// Client-recipe scalars read from device memory, so a captured step replays with the current round's values:
+//  * lr_dev (when not null) wins over the host lr, as rho_dev does over rho: the learning-rate schedule writes it once
+//    per round;
+//  * norm_dev (when not null) is the gradient norm written by grad_norm_kernel just before the update.  The data-loss
+//    gradient is scaled by clip_grad_norm_'s min(1, c / (norm + 1e-6)) in registers, before the penalty terms are added.
+//    A NaN norm must give a NaN scale, as torch's clamp does: fminf(1, NaN) would be 1, so it is not used here.
+__device__ __forceinline__ float clip_scale(const float* norm_dev, float clip) {
+  if (norm_dev == nullptr) return 1.f;
+  const float s = clip / (__ldg(norm_dev) + 1e-6f);
+  return s >= 1.f ? 1.f : s;
+}
+
+// AdamW (weight_decay != 0): x *= 1 - lr wd before the moment update, with the same (device) lr; the penalty gradient
+// is taken at the undecayed x, where autograd would have taken it.
 __global__ void __launch_bounds__(256)
 adam_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                 const int* __restrict__ step_dev, int n, float lr, float b1, float b2, float eps,
+                 const int* __restrict__ step_dev, int n, float lr_host, float b1, float b2, float eps,
                  const float* __restrict__ z, const float* __restrict__ y, float rho_host, float l1, float l2,
-                 const float* __restrict__ rho_dev) {
+                 const float* __restrict__ rho_dev, const float* __restrict__ lr_dev, float wd,
+                 const float* __restrict__ norm_dev, float clip) {
   // adaptive ADMM keeps the penalty in device memory (written by bb_update_kernel): a captured graph never goes stale
   const float rho = rho_dev != nullptr ? __ldg(rho_dev) : rho_host;
+  const float lr = lr_dev != nullptr ? __ldg(lr_dev) : lr_host;
+  const float gscale = clip_scale(norm_dev, clip);
+  const float decay = 1.f - lr * wd;
   const float t = static_cast<float>(*step_dev);
   const float bc1 = 1.f - powf(b1, t);
   const float bc2 = 1.f - powf(b2, t);
@@ -117,8 +136,9 @@ adam_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __re
           vs[4] = {vv.x, vv.y, vv.z, vv.w}, zs[4] = {zv.x, zv.y, zv.z, zv.w}, ys[4] = {yv.x, yv.y, yv.z, yv.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      float gt = gs[j] + ys[j] + l1 * sgnf(xs[j]) + 2.f * l2 * xs[j];
+      float gt = gs[j] * gscale + ys[j] + l1 * sgnf(xs[j]) + 2.f * l2 * xs[j];
       if (z != nullptr) gt += rho * (xs[j] - zs[j]);
+      if (wd != 0.f) xs[j] *= decay;
       ms[j] = b1 * ms[j] + (1.f - b1) * gt;
       vs[j] = b2 * vs[j] + (1.f - b2) * gt * gt;
       const float denom = sqrtf(vs[j]) * inv_sqrt_bc2 + eps;
@@ -130,9 +150,10 @@ adam_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __re
   }
   // scalar tail (n not a multiple of 4)
   for (int i = (n4 << 2) + blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const float xi = x[i];
-    float gt = g[i] + (y ? y[i] : 0.f) + l1 * sgnf(xi) + 2.f * l2 * xi;
+    float xi = x[i];
+    float gt = g[i] * gscale + (y ? y[i] : 0.f) + l1 * sgnf(xi) + 2.f * l2 * xi;
     if (z != nullptr) gt += rho * (xi - z[i]);
+    if (wd != 0.f) xi *= decay;
     const float mi = b1 * m[i] + (1.f - b1) * gt;
     const float vi = b2 * v[i] + (1.f - b2) * gt * gt;
     m[i] = mi;
@@ -143,8 +164,9 @@ adam_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __re
 
 void adam_prox(float* x, const float* g, float* m, float* v, const int* step_dev, int n, float lr, float b1, float b2,
                float eps, const float* z, const float* y, float rho, float l1, float l2, cudaStream_t s,
-               const float* rho_dev) {
-  adam_prox_kernel<<<grid_for(n), 256, 0, s>>>(x, g, m, v, step_dev, n, lr, b1, b2, eps, z, y, rho, l1, l2, rho_dev);
+               const float* rho_dev, const float* lr_dev, float weight_decay, const float* norm_dev, float clip) {
+  adam_prox_kernel<<<grid_for(n), 256, 0, s>>>(x, g, m, v, step_dev, n, lr, b1, b2, eps, z, y, rho, l1, l2, rho_dev,
+                                               lr_dev, weight_decay, norm_dev, clip);
   check_launch("adam_prox");
 }
 
@@ -154,10 +176,13 @@ void adam_prox(float* x, const float* g, float* m, float* v, const int* step_dev
 // kernel then reads x, g and writes x only.
 template <bool kMomentum>
 __global__ void __launch_bounds__(256)
-sgd_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __restrict__ buf, int n, float lr, float mu,
+sgd_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __restrict__ buf, int n, float lr_host, float mu,
                 bool nesterov, float wd, const float* __restrict__ z, const float* __restrict__ y, float rho_host, float l1,
-                float l2, const float* __restrict__ rho_dev) {
+                float l2, const float* __restrict__ rho_dev, const float* __restrict__ lr_dev,
+                const float* __restrict__ norm_dev, float clip) {
   const float rho = rho_dev != nullptr ? __ldg(rho_dev) : rho_host;
+  const float lr = lr_dev != nullptr ? __ldg(lr_dev) : lr_host;
+  const float gscale = clip_scale(norm_dev, clip);
   const int n4 = n >> 2;
   const int stride = gridDim.x * blockDim.x;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
@@ -172,7 +197,7 @@ sgd_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __res
           zs[4] = {zv.x, zv.y, zv.z, zv.w}, ys[4] = {yv.x, yv.y, yv.z, yv.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      float gt = gs[j] + ys[j] + l1 * sgnf(xs[j]) + 2.f * l2 * xs[j];
+      float gt = gs[j] * gscale + ys[j] + l1 * sgnf(xs[j]) + 2.f * l2 * xs[j];
       if (z != nullptr) gt += rho * (xs[j] - zs[j]);
       gt += wd * xs[j];
       float d = gt;
@@ -188,7 +213,7 @@ sgd_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __res
   // scalar tail (n not a multiple of 4)
   for (int i = (n4 << 2) + blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const float xi = x[i];
-    float gt = g[i] + (y ? y[i] : 0.f) + l1 * sgnf(xi) + 2.f * l2 * xi;
+    float gt = g[i] * gscale + (y ? y[i] : 0.f) + l1 * sgnf(xi) + 2.f * l2 * xi;
     if (z != nullptr) gt += rho * (xi - z[i]);
     gt += wd * xi;
     float d = gt;
@@ -202,14 +227,65 @@ sgd_prox_kernel(float* __restrict__ x, const float* __restrict__ g, float* __res
 }
 
 void sgd_prox(float* x, const float* g, float* buf, int n, float lr, float momentum, bool nesterov, float weight_decay,
-              const float* z, const float* y, float rho, float l1, float l2, cudaStream_t s, const float* rho_dev) {
+              const float* z, const float* y, float rho, float l1, float l2, cudaStream_t s, const float* rho_dev,
+              const float* lr_dev, const float* norm_dev, float clip) {
   if (buf != nullptr)
     sgd_prox_kernel<true><<<grid_for(n), 256, 0, s>>>(x, g, buf, n, lr, momentum, nesterov, weight_decay, z, y, rho, l1,
-                                                      l2, rho_dev);
+                                                      l2, rho_dev, lr_dev, norm_dev, clip);
   else
     sgd_prox_kernel<false><<<grid_for(n), 256, 0, s>>>(x, g, nullptr, n, lr, 0.f, false, weight_decay, z, y, rho, l1, l2,
-                                                       rho_dev);
+                                                       rho_dev, lr_dev, norm_dev, clip);
   check_launch("sgd_prox");
+}
+
+// Gradient norm for client gradient-norm clipping (torch.nn.utils.clip_grad_norm_ over the block).  Every CTA writes the
+// sum of squares of its grid-stride share of g to partials[blockIdx.x]; the CTA that draws the last ticket sums the
+// partials in CTA order and writes sqrt of the sum to ws[0].  No floating-point atomics: with the grid a function of n
+// alone, the norm has the same bits on every run and on every replica.  That CTA also resets the ticket (so the buffers
+// are clean for the next launch and for graph replay) and, as the only writer, adds [norm, norm > clip, 1] to the
+// optimizer's round accumulator ws[1..3].
+//   ws = [norm, sum of norms, clipped steps, steps, partials[grad_norm_blocks(n)]]
+__global__ void __launch_bounds__(256)
+grad_norm_kernel(const float* __restrict__ g, int n, float* __restrict__ ws, unsigned int* __restrict__ ticket,
+                 float clip) {
+  __shared__ float sm[32];
+  __shared__ bool last;
+  float* partials = ws + kGradNormHeader;
+  float acc[1] = {0.f};
+  const int n4 = n >> 2;
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(g) + i);
+    acc[0] += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+  }
+  for (int i = (n4 << 2) + blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) acc[0] += g[i] * g[i];
+  block_reduce<1>(acc, sm);
+  if (threadIdx.x == 0) {
+    partials[blockIdx.x] = acc[0];
+    __threadfence();                                       // the partial is visible before the ticket is drawn
+    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  float tot[1] = {0.f};
+  for (int i = threadIdx.x; i < gridDim.x; i += blockDim.x) tot[0] += __ldcg(partials + i);
+  block_reduce<1>(tot, sm);
+  if (threadIdx.x == 0) {
+    const float norm = sqrtf(tot[0]);
+    ws[0] = norm;
+    ws[1] += norm;
+    ws[2] += norm > clip ? 1.f : 0.f;
+    ws[3] += 1.f;
+    *ticket = 0u;
+  }
+}
+
+int grad_norm_blocks(int n) { return grid_for(n); }
+
+void grad_norm(const float* g, int n, float* ws, unsigned int* ticket, float clip, cudaStream_t s) {
+  grad_norm_kernel<<<grid_for(n), 256, 0, s>>>(g, n, ws, ticket, clip);
+  check_launch("grad_norm");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -15,7 +15,8 @@ Kernel inventory (SURVEY §2.10 ids):
   G5  linear_tf32          wgmma GEMM with bias+ELU epilogue
   G9  cross_entropy        fused log-softmax/NLL fwd, softmax-minus-onehot bwd
   G10 vae_loss             single fused reduction fwd, elementwise bwd
-  G14-16 flat ops          adam_prox, sgd_prox, penalty, L-BFGS algebra (see flatops.py)
+  G14-16 flat ops          adam_prox (Adam / AdamW), sgd_prox, grad_norm (clipping), penalty, L-BFGS algebra
+                           (see flatops.py)
   G22 normalize_u8         uint8 NHWC -> normalised float, layout change fused
       augment_normalize_u8 the same with batch gather + random padded crop + horizontal flip fused (training augmentation)
 
@@ -66,20 +67,40 @@ def _step_tensor(key, device) -> torch.Tensor:
 
 
 def adam_prox_step(x, g, m, v, step, lr, beta1, beta2, eps, z=None, y=None, rho=0.0, lambda1=0.0, lambda2=0.0,
-                   rho_dev=None) -> None:
+                   rho_dev=None, lr_dev=None, weight_decay=0.0, norm_dev=None, clip_norm=0.0) -> None:
     """``step`` is either a CUDA int32 tensor holding the (already incremented) step count
-    (graph-capturable) or a Python int (copied into a per-buffer device counter)."""
+    (graph-capturable) or a Python int (copied into a per-buffer device counter).  ``lr_dev`` (a 1-element device tensor)
+    wins over ``lr``; ``weight_decay`` is AdamW's decoupled decay; ``norm_dev`` is the gradient norm written by
+    :func:`grad_norm`, and the gradient is clipped to ``clip_norm`` with it."""
     if not torch.is_tensor(step):
         t = _step_tensor(m.data_ptr(), x.device)
         t.fill_(int(step))
         step = t
-    ext().adam_prox(x, g, m, v, step, lr, beta1, beta2, eps, z, y, rho, lambda1, lambda2, rho_dev)
+    ext().adam_prox(x, g, m, v, step, lr, beta1, beta2, eps, z, y, rho, lambda1, lambda2, rho_dev, lr_dev, weight_decay,
+                    norm_dev, clip_norm)
 
 
 def sgd_prox_step(x, g, buf, lr, momentum, nesterov, weight_decay, z=None, y=None, rho=0.0, lambda1=0.0, lambda2=0.0,
-                  rho_dev=None) -> None:
-    """``buf`` is ``None`` exactly when ``momentum == 0``; no host read, so the launch can be graph-captured."""
-    ext().sgd_prox(x, g, buf, lr, momentum, nesterov, weight_decay, z, y, rho, lambda1, lambda2, rho_dev)
+                  rho_dev=None, lr_dev=None, norm_dev=None, clip_norm=0.0) -> None:
+    """``buf`` is ``None`` exactly when ``momentum == 0``; no host read, so the launch can be graph-captured.
+    ``lr_dev``, ``norm_dev`` and ``clip_norm`` as for :func:`adam_prox_step`."""
+    ext().sgd_prox(x, g, buf, lr, momentum, nesterov, weight_decay, z, y, rho, lambda1, lambda2, rho_dev, lr_dev, norm_dev,
+                   clip_norm)
+
+
+GRAD_NORM_HEADER = 4     # grad_norm's workspace: [norm, sum of norms, clipped steps, steps, per-CTA partials...]
+
+
+def grad_norm_blocks(n: int) -> int:
+    """CTAs (= partial sums) of :func:`grad_norm` over ``n`` values; a function of ``n`` alone on a given device."""
+    return int(ext().grad_norm_blocks(int(n)))
+
+
+def grad_norm(g, ws, ticket, clip_norm: float) -> None:
+    """``ws[0] = ||g||_2`` in a fixed summation order, and ``ws[1:4] += [norm, norm > clip_norm, 1]``.  ``ws`` holds
+    ``GRAD_NORM_HEADER + grad_norm_blocks(g.numel())`` floats; ``ticket`` is one int32, zero between launches (the kernel
+    resets it).  One launch and no host read, so it can be graph-captured."""
+    ext().grad_norm(g, ws, ticket, clip_norm)
 
 
 def bump_step(step: torch.Tensor) -> None:

@@ -152,11 +152,60 @@ class PairHistory:
 # ----------------------------------------------------------------------------
 # Fused Adam (+ closed-form penalty gradients) over a flat slice — SURVEY G14/G15
 # ----------------------------------------------------------------------------
+def clip_workspace(x: torch.Tensor) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """``(ws, ticket)`` for gradient-norm clipping of a block like ``x``: ``ws = [norm, sum of norms, clipped steps, steps,
+    per-CTA partials of the CUDA norm kernel]`` and one int32 ticket (``None`` on the ATen path).  ``ws[1:4]`` accumulates over
+    the steps until the caller zeroes it."""
+    if _cuda(x):
+        from . import cuda_ops
+
+        n = cuda_ops.GRAD_NORM_HEADER + cuda_ops.grad_norm_blocks(x.numel())
+        return (torch.zeros(n, dtype=torch.float32, device=x.device),
+                torch.zeros(1, dtype=torch.int32, device=x.device))
+    return torch.zeros(4, dtype=torch.float32, device=x.device), None
+
+
+def grad_norm_(g: torch.Tensor, ws: torch.Tensor, ticket: Optional[torch.Tensor], clip_norm: float) -> torch.Tensor:
+    """``ws[0] = ||g||_2`` and ``ws[1:4] += [norm, norm > clip_norm, 1]``; returns ``ws[0:1]``.  The ATen norm is summed
+    in float64, so on the CPU it does not depend on how many threads reduce it."""
+    if _cuda(g):
+        from . import cuda_ops
+
+        cuda_ops.grad_norm(g, ws, ticket, clip_norm)
+        return ws[0:1]
+    norm = g.double().square().sum().sqrt().float()
+    ws[0] = norm
+    ws[1:4] += torch.stack([norm, (norm > clip_norm).float(), torch.ones((), dtype=torch.float32, device=g.device)])
+    return ws[0:1]
+
+
+def _clip_scale(norm: torch.Tensor, clip_norm: float) -> torch.Tensor:
+    """``torch.nn.utils.clip_grad_norm_``'s factor ``min(1, c / (norm + 1e-6))``; a NaN norm gives a NaN factor."""
+    return (clip_norm / (norm + 1e-6)).clamp(max=1.0)
+
+
+def _lr_value(lr) -> float:
+    return float(lr) if torch.is_tensor(lr) else lr
+
+
+def _clipped_grad(x, g, clip_norm: float, clip_ws):
+    """``(g, norm_dev)``: on the CPU the clipped gradient itself, on CUDA the unclipped one and the device norm the update
+    kernel scales it by."""
+    if clip_norm <= 0.0:
+        return g, None
+    ws, ticket = clip_ws if clip_ws is not None else clip_workspace(x)
+    norm = grad_norm_(g, ws, ticket, clip_norm)
+    if _cuda(x):
+        return g, norm
+    return g * _clip_scale(norm, clip_norm), None
+
+
 def adam_prox_step(
     x: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor, step: int,
-    lr: float, beta1: float, beta2: float, eps: float,
+    lr, beta1: float, beta2: float, eps: float,
     z: Optional[torch.Tensor] = None, y: Optional[torch.Tensor] = None, rho: float = 0.0,
     lambda1: float = 0.0, lambda2: float = 0.0, rho_dev: Optional[torch.Tensor] = None,
+    weight_decay: float = 0.0, clip_norm: float = 0.0, clip_ws=None,
 ) -> None:
     """One Adam update of ``x`` with the penalty gradients added in closed form:
 
@@ -165,15 +214,29 @@ def adam_prox_step(
     (the reference builds these terms through autograd on a ``torch.cat`` of the
     block inside every closure, consensus_multi.py:214-220).  Adam follows
     ``torch.optim.Adam`` defaults semantics (no amsgrad, no weight decay).
+
+    ``lr`` is a float or a 1-element tensor (read on the device by the CUDA kernel, so a schedule can change it between
+    graph replays).  ``weight_decay`` makes it ``torch.optim.AdamW``: ``x *= 1 - lr*weight_decay`` before the moment
+    update.  ``clip_norm > 0`` first scales ``g`` (the data-loss gradient only, not the penalty gradient) as
+    ``torch.nn.utils.clip_grad_norm_(block, clip_norm)`` does; ``clip_ws`` is the :func:`clip_workspace` whose
+    accumulator counts the step.
     """
     if _cuda(x):
         from . import cuda_ops
 
-        cuda_ops.adam_prox_step(x, g, m, v, step, lr, beta1, beta2, eps, z, y, rho, lambda1, lambda2, rho_dev)
+        g, norm_dev = _clipped_grad(x, g, clip_norm, clip_ws)
+        lr_dev = lr if torch.is_tensor(lr) else None
+        cuda_ops.adam_prox_step(x, g, m, v, step, 0.0 if lr_dev is not None else lr, beta1, beta2, eps, z, y, rho, lambda1,
+                                lambda2, rho_dev, lr_dev=lr_dev, weight_decay=weight_decay, norm_dev=norm_dev,
+                                clip_norm=clip_norm)
         return
     if rho_dev is not None:
         rho = float(rho_dev)
+    lr = _lr_value(lr)
+    g, _ = _clipped_grad(x, g, clip_norm, clip_ws)
     gt = penalty_grad(x, g, z, y, rho, lambda1, lambda2)
+    if weight_decay != 0.0:
+        x.mul_(1 - lr * weight_decay)
     m.mul_(beta1).add_(gt, alpha=1 - beta1)
     v.mul_(beta2).addcmul_(gt, gt, value=1 - beta2)
     bc1 = 1 - beta1 ** step
@@ -183,10 +246,11 @@ def adam_prox_step(
 
 
 def sgd_prox_step(
-    x: torch.Tensor, g: torch.Tensor, buf: Optional[torch.Tensor], lr: float, momentum: float = 0.0,
+    x: torch.Tensor, g: torch.Tensor, buf: Optional[torch.Tensor], lr, momentum: float = 0.0,
     nesterov: bool = False, weight_decay: float = 0.0,
     z: Optional[torch.Tensor] = None, y: Optional[torch.Tensor] = None, rho: float = 0.0,
     lambda1: float = 0.0, lambda2: float = 0.0, rho_dev: Optional[torch.Tensor] = None,
+    clip_norm: float = 0.0, clip_ws=None,
 ) -> None:
     """One ``torch.optim.SGD`` update (dampening 0) of ``x`` with the penalty gradients of :func:`adam_prox_step`:
 
@@ -194,16 +258,22 @@ def sgd_prox_step(
     ``x -= lr * (gt + momentum*buf if nesterov else buf)``.
 
     ``buf`` starts at zero (which gives torch's first step, ``buf = gt``) and is ``None`` exactly when ``momentum == 0``.
+    ``lr``, ``clip_norm`` and ``clip_ws`` as for :func:`adam_prox_step`.
     """
     if (buf is None) != (momentum == 0.0):
         raise ValueError("sgd_prox_step: pass a momentum buffer exactly when momentum != 0, got momentum %r" % (momentum,))
     if _cuda(x):
         from . import cuda_ops
 
-        cuda_ops.sgd_prox_step(x, g, buf, lr, momentum, nesterov, weight_decay, z, y, rho, lambda1, lambda2, rho_dev)
+        g, norm_dev = _clipped_grad(x, g, clip_norm, clip_ws)
+        lr_dev = lr if torch.is_tensor(lr) else None
+        cuda_ops.sgd_prox_step(x, g, buf, 0.0 if lr_dev is not None else lr, momentum, nesterov, weight_decay, z, y, rho,
+                               lambda1, lambda2, rho_dev, lr_dev=lr_dev, norm_dev=norm_dev, clip_norm=clip_norm)
         return
     if rho_dev is not None:
         rho = float(rho_dev)
+    lr = _lr_value(lr)
+    g, _ = _clipped_grad(x, g, clip_norm, clip_ws)
     gt = penalty_grad(x, g, z, y, rho, lambda1, lambda2)
     if weight_decay != 0.0:
         gt.add_(x, alpha=weight_decay)

@@ -5,7 +5,9 @@ augmented-Lagrangian / elastic-net gradients folded into the update; the sibling
 * one kernel (``flat_kernels.cu: sgd_prox_kernel``) reads ``x, g, buf`` (+ ``z``, ``y``) once and writes ``x, buf``;
 * numerics are ``torch.optim.SGD`` with ``dampening = 0`` and ``maximize = False``.  A zeroed buffer gives torch's first
   step (``buf = g``), so there is no step counter and the update has no host-side state that changes between steps:
-  it replays from a CUDA graph as it is.
+  it replays from a CUDA graph as it is;
+* ``device_lr`` and ``clip_norm`` work as for :class:`~.block_adam.BlockAdam` (a device learning rate that a schedule
+  rewrites between rounds; the gradient-norm kernel before the update).
 
 It subclasses ``torch.optim.Optimizer`` so ``state_dict()`` has the stock SGD layout (``momentum_buffer`` per parameter,
 SGD's param-group keys) for the legacy checkpoint schema.
@@ -23,7 +25,7 @@ from ..utils.flat import FlatArena
 
 class BlockSGD(Optimizer):
     def __init__(self, arena: FlatArena, lo: int, hi: int, lr: float, momentum: float = 0.0, nesterov: bool = False,
-                 weight_decay: float = 0.0):
+                 weight_decay: float = 0.0, clip_norm: float = 0.0, device_lr: bool = False):
         if not lr > 0.0:
             raise ValueError("lr must be > 0 for SGD, got %r" % (lr,))
         if not 0.0 <= momentum < 1.0:
@@ -32,6 +34,8 @@ class BlockSGD(Optimizer):
             raise ValueError("nesterov needs momentum > 0")
         if not weight_decay >= 0.0:
             raise ValueError("weight_decay must be >= 0, got %r" % (weight_decay,))
+        if not clip_norm >= 0.0:
+            raise ValueError("clip_norm must be >= 0, got %r" % (clip_norm,))
         params = arena.params[lo: hi + 1]
         super().__init__(params, dict(lr=lr, momentum=momentum, dampening=0, weight_decay=weight_decay,
                                       nesterov=bool(nesterov), maximize=False, foreach=None, differentiable=False,
@@ -41,6 +45,10 @@ class BlockSGD(Optimizer):
         self._span = (a, b)
         self.buf: Optional[torch.Tensor] = (torch.zeros(b - a, dtype=torch.float32, device=arena.data.device)
                                             if momentum != 0.0 else None)
+        self.clip_norm = float(clip_norm)
+        self.lr_dev: Optional[torch.Tensor] = (torch.full((1,), lr, dtype=torch.float32, device=arena.data.device)
+                                               if device_lr else None)
+        self.clip_ws = flatops.clip_workspace(self.x) if clip_norm > 0.0 else None
         # penalty configuration (set by the aggregation strategy for the current block visit)
         self.z: Optional[torch.Tensor] = None
         self.y: Optional[torch.Tensor] = None
@@ -67,7 +75,18 @@ class BlockSGD(Optimizer):
         if self.buf is not None:
             self.buf.zero_()
         if lr is not None:
-            self.param_groups[0]["lr"] = lr
+            self.set_lr(lr)
+
+    def set_lr(self, lr: float) -> None:
+        """The learning rate of the following steps; with ``device_lr`` written in stream order, no host sync."""
+        self.param_groups[0]["lr"] = lr
+        if self.lr_dev is not None:
+            self.lr_dev.fill_(lr)
+
+    @property
+    def clip_stats(self) -> Optional[torch.Tensor]:
+        """``[sum of pre-clip norms, clipped steps, steps]`` since the last zeroing (device; ``None`` without clipping)."""
+        return self.clip_ws[0][1:4] if self.clip_ws is not None else None
 
     def zero_grad(self, set_to_none: bool = False) -> None:
         self.g.zero_()
@@ -76,8 +95,9 @@ class BlockSGD(Optimizer):
     def apply_update(self) -> None:
         """The update alone (gradients already in the arena); CUDA-graph friendly: no host reads."""
         grp = self.param_groups[0]
-        flatops.sgd_prox_step(self.x, self.g, self.buf, grp["lr"], grp["momentum"], grp["nesterov"], grp["weight_decay"],
-                              self.z, self.y, self.rho, self.lambda1, self.lambda2, self.rho_dev)
+        flatops.sgd_prox_step(self.x, self.g, self.buf, self.lr_dev if self.lr_dev is not None else grp["lr"],
+                              grp["momentum"], grp["nesterov"], grp["weight_decay"], self.z, self.y, self.rho,
+                              self.lambda1, self.lambda2, self.rho_dev, clip_norm=self.clip_norm, clip_ws=self.clip_ws)
 
     def step(self, closure: Optional[Callable] = None):
         loss = None
@@ -105,7 +125,7 @@ class BlockSGD(Optimizer):
                              % (held, (grp["momentum"], grp["nesterov"], grp["weight_decay"])))
         if self.buf is not None:
             self.buf.copy_(rec["buf"].to(self.buf.device))
-        grp["lr"] = rec["lr"]
+        self.set_lr(rec["lr"])
 
     # -- stock-SGD compatible state -------------------------------------------
     def state_dict(self):

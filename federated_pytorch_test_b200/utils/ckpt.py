@@ -81,7 +81,8 @@ def save_resume(path: str, engine, position: Dict) -> str:
     ``EngineConfig.resume_path`` is set: schedule position ``(nloop, visit, round)`` = where to RE-ENTER, consensus
     state of the open block visit (z, y_k, rho table, BB vectors), per-replica weights + BatchNorm buffers, the
     optimizers' flat state (Adam moments + step / SGD momentum buffer + settings / L-BFGS history, direction, Welford
-    statistics), the optimizer's name in the position, loader RNG streams and
+    statistics), the optimizer's name and the learning-rate schedule and clipping settings in the position, loader RNG
+    streams and
     augmentation counters,
     global RNG states and the run counters.  Written atomically (tmp + rename); one file per rank."""
     strat_state = {}
