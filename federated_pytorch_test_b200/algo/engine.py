@@ -178,11 +178,16 @@ class EngineConfig:
     lr_gamma: float = 0.1
     lr_step_rounds: int = 0
     lr_min: float = 0.0
+    # training-loss regularisers of the classifier drivers (label smoothing, mixup, CutMix): part of the resume recipe
+    label_smoothing: float = 0.0
+    mixup_alpha: float = 0.0
+    cutmix_alpha: float = 0.0
 
     def recipe(self, clip_norm: float = 0.0) -> Dict:
-        """The schedule and clipping settings a resume record must match."""
+        """The schedule, clipping and mixing settings a resume record must match."""
         return dict(lr_schedule=self.lr_schedule, lr_warmup=self.lr_warmup, lr_gamma=self.lr_gamma,
-                    lr_step_rounds=self.lr_step_rounds, lr_min=self.lr_min, clip_norm=clip_norm)
+                    lr_step_rounds=self.lr_step_rounds, lr_min=self.lr_min, clip_norm=clip_norm,
+                    label_smoothing=self.label_smoothing, mixup_alpha=self.mixup_alpha, cutmix_alpha=self.cutmix_alpha)
 
 
 class Engine:
@@ -364,11 +369,12 @@ class Engine:
                 raise ValueError("resume record was written with optimizer %r, this run uses optimizer %r"
                                  % (held, visit.optimizer))
             want = cfg.recipe(visit.opt_kwargs.get("clip_norm", 0.0))
-            held = self._resume_pos.get("recipe", EngineConfig().recipe())   # records written before schedules: defaults
+            # records written before schedules (or before mixing) lack the fields: they were run with the defaults
+            held = dict(EngineConfig().recipe(), **self._resume_pos.get("recipe", {}))
             for name, val in want.items():
-                if held.get(name) != val:
+                if held[name] != val:
                     raise ValueError("resume record was written with %s %r, this run uses %s %r"
-                                     % (name, held.get(name), name, val))
+                                     % (name, held[name], name, val))
             first_round = int(self._resume_pos.get("round", 0))
             self._restore_visit_state()
             self._resume_pos = None

@@ -17,8 +17,9 @@ import torch.nn as nn
 
 from .. import models
 from ..algo.engine import Engine, EngineConfig, Replica, Task, Visit
-from ..config import ADAM_LR, CLIENT_RECIPE_DEFAULTS, CommonConfig, check_client_opt, check_norm, check_partition
-from ..data.cifar import (CifarData, ShardLoader, augment_key, class_histogram, dirichlet_shards, shard_ranges,
+from ..config import (ADAM_LR, CLIENT_RECIPE_DEFAULTS, MIX_DEFAULTS, CommonConfig, check_client_opt, check_mix, check_norm,
+                      check_partition)
+from ..data.cifar import (CifarData, ShardLoader, augment_key, class_histogram, dirichlet_shards, mix_key, shard_ranges,
                           worker_norm)
 from ..ops import functional as FX
 from ..ops import losses
@@ -51,6 +52,14 @@ def require_default_client_opt(cfg: CommonConfig, driver: str) -> None:
         raise ValueError("%s fixes its own optimizer and does not take optimizer 'adamw'" % driver)
 
 
+def require_no_mix(cfg: CommonConfig, task: str) -> None:
+    """Label smoothing, mixup and CutMix belong to the classifier drivers' cross-entropy (and mixup / CutMix would blend the
+    VAE's reconstruction targets too)."""
+    for name, default in MIX_DEFAULTS:
+        if getattr(cfg, name, default) != default:
+            raise ValueError("%s is supported by the classifier drivers only, not by %s" % (name, task))
+
+
 def require_iid(cfg: CommonConfig, driver: str) -> None:
     """The unsupervised drivers (VAE, VAE-CL, CPC) train without labels and accept only the default split."""
     if getattr(cfg, "partition", "iid") != "iid":
@@ -76,7 +85,8 @@ def engine_config(cfg: CommonConfig, **kw) -> EngineConfig:
                 max_minibatches=cfg.max_minibatches or None, nan_guard=getattr(cfg, "nan_guard", "raise"),
                 resume_path=getattr(cfg, "resume_out", ""), streams=getattr(cfg, "streams", True),
                 lr_schedule=cfg.lr_schedule, lr_warmup=cfg.lr_warmup, lr_gamma=cfg.lr_gamma,
-                lr_step_rounds=cfg.lr_step_rounds, lr_min=cfg.lr_min)
+                lr_step_rounds=cfg.lr_step_rounds, lr_min=cfg.lr_min, label_smoothing=cfg.label_smoothing,
+                mixup_alpha=cfg.mixup_alpha, cutmix_alpha=cfg.cutmix_alpha)
     base.update(kw)
     return EngineConfig(**base)
 
@@ -107,6 +117,7 @@ class ClassifierTask(Task):
         check_norm(norm, getattr(cfg, "norm_groups", 32), name)
         check_client_opt(cfg.optimizer, cfg.lr, cfg.momentum, cfg.nesterov, cfg.weight_decay, cfg.lr_schedule, cfg.lr_warmup,
                          cfg.lr_gamma, cfg.lr_step_rounds, cfg.lr_min, cfg.clip_norm)
+        check_mix(cfg.label_smoothing, cfg.mixup_alpha, cfg.cutmix_alpha)
         self.factory = _MODEL_FACTORIES[name]
         if norm != "batch":
             self.factory = functools.partial(self.factory, norm=norm, groups=cfg.norm_groups)
@@ -186,7 +197,8 @@ class ClassifierTask(Task):
             ld = ShardLoader(self.data.train_images, self.data.train_labels, self.shards[ck], self.cfg.default_batch,
                              self.topo.device, mean, std, shuffle=True, seed=self.cfg.seed + 1000 * ck,
                              channels_last=self.channels_last, augment=self.cfg.augment,
-                             aug_key=augment_key(self.cfg.seed, ck))
+                             aug_key=augment_key(self.cfg.seed, ck), mixup_alpha=self.cfg.mixup_alpha,
+                             cutmix_alpha=self.cfg.cutmix_alpha, mix_key=mix_key(self.cfg.seed, ck))
             self._loaders[ck] = ld
         return ld
 
@@ -204,8 +216,9 @@ class ClassifierTask(Task):
         return iter(self.loader(rep.ck))
 
     def loss(self, rep: Replica, batch) -> torch.Tensor:
-        x, y = batch
-        return losses.cross_entropy(rep.nets["net"](x), y)
+        x, y = batch[0], batch[1]
+        lam = batch[2] if len(batch) == 3 else None        # a mixed batch carries its lam_eff
+        return losses.cross_entropy(rep.nets["net"](x), y, self.cfg.label_smoothing, lam)
 
     # -- logging / evaluation ----------------------------------------------------
     def after_minibatch(self, rep, visit, batch, i, epoch, nloop, N, loss1, engine) -> None:

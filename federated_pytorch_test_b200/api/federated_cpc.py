@@ -37,6 +37,7 @@ class CPCTask(Task):
     def __init__(self, cfg: Config, topo):
         if cfg.augment:
             raise ValueError("augment is supported by the classifier drivers only, not by CPCTask")
+        common.require_no_mix(cfg, "CPCTask")
         self.cfg, self.topo = cfg, topo
         files = [f for f in cfg.file_list.split(",") if f]
         saps = [s for s in cfg.sap_list.split(",") if s]

@@ -30,6 +30,7 @@ class VAETask(common.ClassifierTask):
     def __init__(self, cfg, topo):
         if cfg.augment:     # the loader would crop and flip the VAE's reconstruction targets too
             raise ValueError("augment is supported by the classifier drivers only, not by %s" % type(self).__name__)
+        common.require_no_mix(cfg, type(self).__name__)
         cfg_model, cfg_optimizer = cfg.model, cfg.optimizer
         # placeholders for the base-class probe and checks; replaced below (this task fixes its own optimizer)
         cfg.model, cfg.optimizer = "Net", "adam"

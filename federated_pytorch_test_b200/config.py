@@ -69,6 +69,11 @@ class CommonConfig:
     norm: str = "batch"
     norm_groups: int = 32           # must divide 64, the narrowest layer
     augment: bool = False           # random 4-pixel-padded crop + horizontal flip of training batches (classifier drivers only)
+    # regularisers of the classifier drivers' training loss (timm's Mixup in batch mode, SoftTargetCrossEntropy): sample i
+    # of a batch is mixed with sample n-1-i (data/cifar.py: mix_draws); 0 = off
+    label_smoothing: float = 0.0    # epsilon in [0, 1): targets (1 - eps) onehot(y) + eps / C
+    mixup_alpha: float = 0.0        # >= 0: mixup with lambda ~ Beta(alpha, alpha)
+    cutmix_alpha: float = 0.0       # >= 0: CutMix with lambda ~ Beta(alpha, alpha); with mixup, one of the two per batch
     nan_guard: str = "raise"        # non-finite aggregation residual: 'raise' | 'warn' | 'off'
     collective: str = "auto"        # 'auto' | 'fused' | 'torch'
     fast: bool = True               # use the hand-written sm_90a kernels on CUDA devices
@@ -228,6 +233,18 @@ def check_client_opt(optimizer: str, lr: float, momentum: float, nesterov: bool,
             if val != default:
                 raise ValueError("%s cannot be set with optimizer 'lbfgs' (its line search sets the step), got %s %r"
                                  % (name, name, val))
+
+
+MIX_DEFAULTS = (("label_smoothing", 0.0), ("mixup_alpha", 0.0), ("cutmix_alpha", 0.0))
+
+
+def check_mix(label_smoothing: float, mixup_alpha: float, cutmix_alpha: float) -> None:
+    """Raise ``ValueError`` unless the label-smoothing, mixup and CutMix settings of :class:`CommonConfig` are valid."""
+    if not 0.0 <= label_smoothing < 1.0:
+        raise ValueError("label_smoothing must lie in [0, 1), got %r" % (label_smoothing,))
+    for name, val in (("mixup_alpha", mixup_alpha), ("cutmix_alpha", cutmix_alpha)):
+        if not (math.isfinite(val) and val >= 0.0):
+            raise ValueError("%s must be finite and >= 0 (0 = off), got %r" % (name, val))
 
 
 PARTITIONS = ("iid", "dirichlet")

@@ -153,6 +153,37 @@ Tensor augment_normalize_u8(Tensor u8, c10::optional<Tensor> rows, int64_t key, 
                            m3, s3, to_nchw ? 1 : 0, cur_stream());
   return out;
 }
+// Mixup / CutMix input stage: returns {batch, lam} with lam a one-float32 tensor holding lam_eff.  key: the augmentation key
+// (used with augment), rows as for augment_normalize_u8.  lam_f / mlam_f / lam_eff arrive as doubles holding float32 values.
+std::vector<Tensor> mix_normalize_u8(Tensor u8, c10::optional<Tensor> rows, bool augment, int64_t key, int64_t counter,
+                                     std::vector<double> mean, std::vector<double> stdv, bool to_nchw, bool cutmix,
+                                     double lam_f, double mlam_f, int64_t y0, int64_t y1, int64_t x0, int64_t x1,
+                                     double lam_eff) {
+  TORCH_CHECK(u8.is_cuda() && u8.scalar_type() == torch::kUInt8 && u8.dim() == 4 && u8.size(3) == 3 && u8.is_contiguous(),
+              "mix_normalize_u8 expects a contiguous CUDA uint8 [N,H,W,3] tensor");
+  TORCH_CHECK(counter >= 0, "mix_normalize_u8: negative counter");
+  c10::cuda::CUDAGuard guard(u8.device());
+  int64_t N = u8.size(0);
+  const int64_t H = u8.size(1), W = u8.size(2);
+  TORCH_CHECK(0 <= y0 && y0 <= y1 && y1 <= H && 0 <= x0 && x0 <= x1 && x1 <= W, "mix_normalize_u8: box outside the image");
+  const int64_t* rp = nullptr;
+  if (rows.has_value() && rows->defined()) {
+    TORCH_CHECK(rows->is_cuda() && rows->device() == u8.device() && rows->scalar_type() == torch::kInt64 && rows->dim() == 1 &&
+                    rows->is_contiguous(),
+                "mix_normalize_u8: rows must be a contiguous int64 vector on the images' device");
+    N = rows->numel();
+    rp = rows->data_ptr<int64_t>();
+  }
+  TORCH_CHECK(N * H * W < (int64_t(1) << 31), "mix_normalize_u8: batch too large");
+  float m3[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s3[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
+  auto opts = torch::TensorOptions().dtype(torch::kFloat32).device(u8.device());
+  Tensor out = to_nchw ? torch::empty({N, 3, H, W}, opts) : torch::empty({N, H, W, 3}, opts);
+  Tensor lam = torch::empty({1}, opts);
+  fb::mix_normalize_u8(u8.data_ptr<uint8_t>(), rp, fptr_mut(out), fptr_mut(lam), (int)N, (int)H, (int)W, augment ? 1 : 0,
+                       (uint64_t)key, (uint64_t)counter, m3, s3, to_nchw ? 1 : 0, cutmix ? 1 : 0, (float)lam_f, (float)mlam_f,
+                       (int)y0, (int)y1, (int)x0, (int)x1, (float)lam_eff, cur_stream());
+  return {out, lam};
+}
 void col_stats(Tensor y, Tensor stats) {
   CHECK_F32_CUDA(y); CHECK_CONTIG(y);
   c10::cuda::CUDAGuard guard(y.device());
@@ -487,6 +518,37 @@ Tensor cross_entropy_bwd(Tensor probs, Tensor labels, Tensor gout) {
   auto g = gout.contiguous();
   fb::cross_entropy_bwd(fptr(probs), (const long long*)labels.data_ptr<int64_t>(), fptr(g), fptr_mut(d), (int)probs.size(0),
                         (int)probs.size(1), cur_stream());
+  return d;
+}
+// lam: optional one-float32 device tensor (absent = 1); the target of sample i mixes labels i and B-1-i.
+static const float* soft_ce_lam(const c10::optional<Tensor>& lam, const Tensor& like) {
+  if (!lam.has_value() || !lam->defined()) return nullptr;
+  TORCH_CHECK(lam->is_cuda() && lam->device() == like.device() && lam->scalar_type() == torch::kFloat32 && lam->numel() == 1,
+              "soft_ce: lam must be a one-element CUDA float32 tensor on the logits' device");
+  return lam->data_ptr<float>();
+}
+std::vector<Tensor> soft_ce_fwd(Tensor logits, Tensor labels, c10::optional<Tensor> lam, double eps) {
+  CHECK_F32_CUDA(logits); CHECK_CONTIG(logits);
+  TORCH_CHECK(logits.dim() == 2 && logits.size(0) >= 1 && logits.size(1) >= 1, "soft_ce_fwd: logits must be [B >= 1, C >= 1]");
+  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.is_cuda() && labels.is_contiguous() &&
+                  labels.numel() == logits.size(0), "soft_ce_fwd: labels must be a contiguous CUDA int64 [B] tensor");
+  TORCH_CHECK(eps >= 0.0 && eps < 1.0, "soft_ce_fwd: eps must lie in [0, 1)");
+  c10::cuda::CUDAGuard guard(logits.device());
+  auto loss = torch::empty({}, logits.options());
+  auto probs = torch::empty_like(logits);
+  fb::soft_ce_fwd(fptr(logits), (const long long*)labels.data_ptr<int64_t>(), soft_ce_lam(lam, logits), (float)eps,
+                  fptr_mut(loss), fptr_mut(probs), (int)logits.size(0), (int)logits.size(1), cur_stream());
+  return {loss, probs};
+}
+Tensor soft_ce_bwd(Tensor probs, Tensor labels, c10::optional<Tensor> lam, double eps, Tensor gout) {
+  CHECK_F32_CUDA(probs); CHECK_CONTIG(probs);
+  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.is_cuda() && labels.is_contiguous() &&
+                  labels.numel() == probs.size(0), "soft_ce_bwd: labels must be a contiguous CUDA int64 [B] tensor");
+  c10::cuda::CUDAGuard guard(probs.device());
+  auto d = torch::empty_like(probs);
+  auto g = gout.contiguous();
+  fb::soft_ce_bwd(fptr(probs), (const long long*)labels.data_ptr<int64_t>(), soft_ce_lam(lam, probs), (float)eps, fptr(g),
+                  fptr_mut(d), (int)probs.size(0), (int)probs.size(1), cur_stream());
   return d;
 }
 Tensor vae_loss_fwd(Tensor recon, Tensor x, Tensor mu, Tensor logvar) {
@@ -966,6 +1028,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("normalize_u8", &normalize_u8);
   m.def("augment_normalize_u8", &augment_normalize_u8, py::arg("u8"), py::arg("rows"), py::arg("key"), py::arg("counter"),
         py::arg("mean"), py::arg("std"), py::arg("to_nchw"));
+  m.def("mix_normalize_u8", &mix_normalize_u8, py::arg("u8"), py::arg("rows"), py::arg("augment"), py::arg("key"),
+        py::arg("counter"), py::arg("mean"), py::arg("std"), py::arg("to_nchw"), py::arg("cutmix"), py::arg("lam_f"),
+        py::arg("mlam_f"), py::arg("y0"), py::arg("y1"), py::arg("x0"), py::arg("x1"), py::arg("lam_eff"));
   m.def("col_stats", &col_stats);
   m.def("head_fwd", &head_fwd);
   m.def("head_bwd", &head_bwd);
@@ -999,6 +1064,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_wgrad_supported", &conv_wgrad_supported);
   m.def("cross_entropy_fwd", &cross_entropy_fwd);
   m.def("cross_entropy_bwd", &cross_entropy_bwd);
+  m.def("soft_ce_fwd", &soft_ce_fwd, py::arg("logits"), py::arg("labels"), py::arg("lam"), py::arg("eps"));
+  m.def("soft_ce_bwd", &soft_ce_bwd, py::arg("probs"), py::arg("labels"), py::arg("lam"), py::arg("eps"), py::arg("gout"));
   m.def("vae_loss_fwd", &vae_loss_fwd);
   m.def("vae_loss_bwd", &vae_loss_bwd);
   m.def("linear_f32", &linear_f32);

@@ -2,6 +2,7 @@
 // 128-bit accesses along the channel axis, per-channel parameters staged in shared memory.
 //  * normalize_u8_nhwc : uint8 NHWC pixels -> (x/255-mean)/std as NHWC (optionally padded to 4 channels) or NCHW
 //  * augment_normalize_u8 : the same with the batch gather, a random padded crop and a random horizontal flip fused in
+//  * mix_normalize_u8  : the same (crop and flip optional) with the mixup blend or CutMix paste of sample n-1-i fused in
 //  * col_stats        : per-channel sum / sum of squares (only for layers whose conv did not emit them)
 //  * bn_elu_fwd        : BatchNorm(batch stats from the conv epilogue) + residual + ELU in ONE pass; block 0 also
 //                        updates the running statistics and stores mean/invstd for the backward pass.  Running-statistics
@@ -131,6 +132,87 @@ void augment_normalize_u8(const uint8_t* in, const int64_t* rows, float* out, in
   augment_normalize_u8_kernel<<<grid, 256, 0, s>>>(in, rows, out, npix, key, counter, mean3[0], mean3[1], mean3[2],
                                                    std3[0], std3[1], std3[2], to_nchw, H, W);
   check_launch("augment_normalize_u8");
+}
+
+// ------------------------------------------------------------------------------------------------
+// Mixup / CutMix fused into the input stage: gather (optional) + crop + flip (AUG: augment_normalize_u8_kernel's draw, per
+// source sample) + normalisation + mix with the partner sample n - 1 - i + layout change, one thread per output pixel.
+// The draw (lam_f, mlam_f, box) is made on the host (data/cifar.py: mix_draws).  Mixup is rn(rn(lam_f a) + rn(mlam_f b))
+// without FMA contraction, i.e. ATen's a * lam + b * (1 - lam) on float32 tensors; CutMix takes the partner's pixel inside
+// [y0, y1) x [x0, x1).  The normalised pixels are augment_normalize_u8_kernel's (normalize_u8_kernel's without AUG).
+template <bool AUG>
+__device__ __forceinline__ float3 mix_source_px(const uint8_t* __restrict__ in, const int64_t* __restrict__ rows, int n,
+                                                int h, int w, int H, int W, uint64_t key, uint64_t counter,
+                                                const float* sc, const float* sh) {
+  constexpr int PAD = 4;
+  int sy = h, sx = w;
+  if (AUG) {
+    const uint64_t z = splitmix64_finaliser(key + (counter + uint64_t(n) + 1ull) * 0x9E3779B97F4A7C15ull);
+    const int dx = int(((z & 0xFFFFFFFFull) * 9ull) >> 32);
+    const int dy = int((((z >> 32) & 0x7FFFFFFFull) * 9ull) >> 31);
+    sy = h + dy - PAD;
+    sx = ((z >> 63) ? W - 1 - w : w) + dx - PAD;
+  }
+  uint8_t c0 = 0, c1 = 0, c2 = 0;
+  if (!AUG || (unsigned(sy) < unsigned(H) && unsigned(sx) < unsigned(W))) {
+    const int64_t row = rows != nullptr ? rows[n] : int64_t(n);
+    const uint8_t* px = in + ((size_t(row) * H + sy) * W + sx) * 3;
+    c0 = px[0];
+    c1 = px[1];
+    c2 = px[2];
+  }
+  return make_float3(fmaf(float(c0), sc[0], sh[0]), fmaf(float(c1), sc[1], sh[1]), fmaf(float(c2), sc[2], sh[2]));
+}
+
+template <bool AUG, bool CUTMIX>
+__global__ void __launch_bounds__(256)
+mix_normalize_u8_kernel(const uint8_t* __restrict__ in, const int64_t* __restrict__ rows, float* __restrict__ out,
+                        float* __restrict__ lam_out, int N, int npix, uint64_t key, uint64_t counter, float m0, float m1,
+                        float m2, float s0, float s1, float s2, int to_nchw, int H, int W, float lam_f, float mlam_f,
+                        int y0, int y1, int x0, int x1, float lam_eff) {
+  const float sc[3] = {1.f / (255.f * s0), 1.f / (255.f * s1), 1.f / (255.f * s2)};
+  const float sh[3] = {-m0 / s0, -m1 / s1, -m2 / s2};
+  const int HW = H * W;
+  if (blockIdx.x == 0 && threadIdx.x == 0) lam_out[0] = lam_eff;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
+    const int n = p / HW, r = p - n * HW, h = r / W, w = r - h * W;
+    const int partner = N - 1 - n;
+    float3 v;
+    if (CUTMIX) {
+      const bool inside = h >= y0 && h < y1 && w >= x0 && w < x1;
+      v = mix_source_px<AUG>(in, rows, inside ? partner : n, h, w, H, W, key, counter, sc, sh);
+    } else {
+      const float3 a = mix_source_px<AUG>(in, rows, n, h, w, H, W, key, counter, sc, sh);
+      const float3 b = mix_source_px<AUG>(in, rows, partner, h, w, H, W, key, counter, sc, sh);
+      v.x = __fadd_rn(__fmul_rn(lam_f, a.x), __fmul_rn(mlam_f, b.x));
+      v.y = __fadd_rn(__fmul_rn(lam_f, a.y), __fmul_rn(mlam_f, b.y));
+      v.z = __fadd_rn(__fmul_rn(lam_f, a.z), __fmul_rn(mlam_f, b.z));
+    }
+    if (to_nchw) {
+      float* o = out + size_t(n) * 3 * HW + r;
+      o[0] = v.x;
+      o[HW] = v.y;
+      o[2 * HW] = v.z;
+    } else {
+      float* o = out + size_t(p) * 3;
+      o[0] = v.x;
+      o[1] = v.y;
+      o[2] = v.z;
+    }
+  }
+}
+void mix_normalize_u8(const uint8_t* in, const int64_t* rows, float* out, float* lam_out, int n, int H, int W, int augment,
+                      uint64_t key, uint64_t counter, const float* mean3, const float* std3, int to_nchw, int cutmix,
+                      float lam_f, float mlam_f, int y0, int y1, int x0, int x1, float lam_eff, cudaStream_t s) {
+  const int npix = n * H * W;
+  int grid = (npix + 255) / 256;
+  if (grid > sm_count() * 16) grid = sm_count() * 16;
+  if (grid < 1) grid = 1;
+  auto kern = augment ? (cutmix ? mix_normalize_u8_kernel<true, true> : mix_normalize_u8_kernel<true, false>)
+                      : (cutmix ? mix_normalize_u8_kernel<false, true> : mix_normalize_u8_kernel<false, false>);
+  kern<<<grid, 256, 0, s>>>(in, rows, out, lam_out, n, npix, key, counter, mean3[0], mean3[1], mean3[2], std3[0], std3[1],
+                            std3[2], to_nchw, H, W, lam_f, mlam_f, y0, y1, x0, x1, lam_eff);
+  check_launch("mix_normalize_u8");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -119,6 +119,13 @@ void normalize_u8_nhwc(const uint8_t* in, float* out, int npix, int c_out, const
 // the n samples.  Sample i draws from (key, counter + i); the draw is documented in data/cifar.py (augment_draws).
 void augment_normalize_u8(const uint8_t* in, const int64_t* rows, float* out, int n, int H, int W, uint64_t key,
                           uint64_t counter, const float* mean3, const float* std3, int to_nchw, cudaStream_t s);
+// n samples mixed with their partners n-1-i (mixup: lam_f a + mlam_f b; cutmix: the partner's pixels inside
+// [y0, y1) x [x0, x1)), after the optional augmentation (augment != 0, drawn from (key, counter + i)) and normalisation,
+// NCHW or NHWC (3 channels) out; lam_out[0] = lam_eff.  rows as for augment_normalize_u8.  The draw is made on the host
+// (data/cifar.py: mix_draws).
+void mix_normalize_u8(const uint8_t* in, const int64_t* rows, float* out, float* lam_out, int n, int H, int W, int augment,
+                      uint64_t key, uint64_t counter, const float* mean3, const float* std3, int to_nchw, int cutmix,
+                      float lam_f, float mlam_f, int y0, int y1, int x0, int x1, float lam_eff, cudaStream_t s);
 void col_stats(const float* y, float* stats, int M, int C, cudaStream_t s);
 // stats: [2C] sums (+ one uint counter behind them when self_clean: the kernel zeroes the buffer after the last read)
 // use_running: eval-mode BatchNorm on running_mean / running_var (read only); stats, save_mean / save_invstd, momentum and
@@ -159,6 +166,12 @@ void cross_entropy_fwd(const float* logits, const long long* labels, float* loss
                        cudaStream_t s);
 void cross_entropy_bwd(const float* probs, const long long* labels, const float* gout, float* dlogits, int B, int C,
                        cudaStream_t s);
+// soft-target cross-entropy: targets lam s(y_i) + (1 - lam) s(y_{B-1-i}), s(y) = (1 - eps) onehot(y) + eps / C; lam is a
+// device scalar (nullptr = 1).  The mean loss is summed in a fixed order (no atomics); dlogits = (p - q) gout / B.
+void soft_ce_fwd(const float* logits, const long long* labels, const float* lam, float eps, float* loss, float* probs, int B,
+                 int C, cudaStream_t s);
+void soft_ce_bwd(const float* probs, const long long* labels, const float* lam, float eps, const float* gout, float* dlogits,
+                 int B, int C, cudaStream_t s);
 void vae_loss_fwd(const float* recon, const float* x, int n, const float* mu, const float* logvar, int nl, float* out,
                   cudaStream_t s);
 void vae_loss_bwd(const float* recon, const float* x, int n, const float* mu, const float* logvar, int nl,

@@ -26,6 +26,11 @@ followed by ``RandomHorizontalFlip(0.5)`` on the raw uint8 image, before normali
 counter-based, not a ``torch.Generator``: sample ``i`` of a batch takes :func:`augment_draws` ``(key, counter + i)``, where
 ``key`` is fixed per worker (:func:`augment_key`) and ``counter`` is the number of samples its loader has handed out.
 So augmentation does not touch the shuffle generator, and a batch does not depend on the process topology.
+
+Mixup and CutMix (opt-in, ``--mixup_alpha`` / ``--cutmix_alpha``) mix sample ``i`` of a training batch with sample
+``n-1-i`` after the crop / flip and the normalisation.  The draw is one per batch, made on the host by :func:`mix_draws`
+from the same loader counter under a second key (:func:`mix_key`); on the CUDA fast path the whole input stage stays one
+launch (:func:`ops.cuda_ops.mix_normalize_u8`), and :func:`mix_batch` is the ATen composition.
 """
 from __future__ import annotations
 
@@ -233,6 +238,141 @@ def augment_batch(u8_nhwc: torch.Tensor, mean, std, channels_last: bool, key: in
 
 
 # ----------------------------------------------------------------------------
+# mixup / CutMix: one draw per batch, sample i mixed with sample n-1-i
+# ----------------------------------------------------------------------------
+MIX_WORDS = 256                      # splitmix64 words per batch sub-stream
+_MIX_TAG = 0x6D69782D63757421       # domain tag: mixing keys never coincide with augmentation keys
+
+
+def mix_key(seed: int, ck: int) -> int:
+    """64-bit mixup / CutMix key of worker ``ck`` in a run seeded with ``seed`` (the :func:`augment_key` input with a domain
+    tag folded in before the finaliser, so the two keys differ)."""
+    z = np.array([(((int(seed) & 0xFFFFFFFF) << 32) | (int(ck) & 0xFFFFFFFF)) ^ _MIX_TAG], dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        return int(_splitmix64_finaliser(z)[0])
+
+
+def _splitmix64_word(key: int, i: int) -> int:
+    z = (key + (i + 1) * _GOLDEN_GAMMA) & _MASK64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _MASK64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _MASK64
+    return z ^ (z >> 31)
+
+
+class _Words:
+    """Uniforms of one batch's sub-stream: word ``j`` is output ``counter * 256 + j`` of splitmix64 seeded with ``key``."""
+
+    def __init__(self, key: int, counter: int, first: int):
+        self.key, self.base, self.j = int(key) & _MASK64, (int(counter) * MIX_WORDS) & _MASK64, first
+
+    def word(self, j: int) -> int:
+        return _splitmix64_word(self.key, (self.base + j) & _MASK64)
+
+    def uniform(self) -> float:
+        """The next word as a float64 in the open interval (0, 1)."""
+        if self.j >= MIX_WORDS:
+            raise RuntimeError("mix_draws: the batch's %d-word sub-stream is exhausted" % MIX_WORDS)
+        w = self.word(self.j)
+        self.j += 1
+        return ((w >> 11) + 0.5) * 2.0 ** -53
+
+    def log_gamma(self, alpha: float) -> float:
+        """log of a Gamma(alpha, 1) variate (Marsaglia & Tsang 2000; for alpha < 1 a Gamma(alpha + 1) variate times
+        U^(1/alpha)).  In logs so that the Beta ratio of two tiny variates is still defined."""
+        boost = 0.0
+        if alpha < 1.0:
+            boost = math.log(self.uniform()) / alpha
+            alpha += 1.0
+        d = alpha - 1.0 / 3.0
+        c = 1.0 / math.sqrt(9.0 * d)
+        while True:
+            x = math.sqrt(-2.0 * math.log(self.uniform())) * math.cos(2.0 * math.pi * self.uniform())   # Box-Muller
+            v = 1.0 + c * x
+            if v <= 0.0:
+                continue
+            v = v * v * v
+            if math.log(self.uniform()) < 0.5 * x * x + d - d * v + d * math.log(v):
+                return math.log(d * v) + boost
+
+
+def mix_draws(key: int, counter: int, n: int, H: int, W: int, mixup_alpha: float,
+              cutmix_alpha: float) -> Tuple[str, float, Tuple[int, int, int, int], float]:
+    """Mixing draw of the batch of ``n`` ``H x W`` samples whose first sample has loader counter ``counter``.
+
+    A pure float64 function of its arguments.  The batch owns the splitmix64 sub-stream of :func:`augment_draws`' generator
+    (same finaliser ``F``) at outputs ``counter * 256 .. counter * 256 + 255``: word ``j`` is
+    ``F(key + (counter * 256 + j + 1) * 0x9E3779B97F4A7C15 mod 2**64)``, and a word ``w`` is the uniform
+    ``((w >> 11) + 1/2) 2**-53`` in (0, 1).  Consecutive batches of a loader have counters at least 1 apart, so their
+    sub-streams never overlap.  Word 0's top bit picks CutMix (1) or mixup (0) when both alphas are > 0; otherwise the
+    mode whose alpha is > 0 is used.  Words 1 and 2 give the CutMix centre ``cy = (w1[63:32] * H) >> 32`` and
+    ``cx = (w2[63:32] * W) >> 32``.  From word 3 on, ``lam = G1 / (G1 + G2) ~ Beta(alpha, alpha)`` with Marsaglia-Tsang
+    Gamma variates (Box-Muller normals; for alpha < 1 boosted by ``U^(1/alpha)``); a draw that would need more than 256
+    words raises ``RuntimeError`` (rejection rates make this practically impossible).
+
+    Mixup: ``x_i = lam a_i + (1 - lam) a_{n-1-i}`` and ``lam_eff = lam``.  CutMix: ``r = sqrt(1 - lam)``,
+    ``cut_h = int(H r)``, ``cut_w = int(W r)``; the box ``[clip(cy - cut_h // 2, 0, H), clip(cy + cut_h // 2, 0, H))`` x
+    the same in x takes its pixels from the partner, and ``lam_eff = 1 - box area / (H W)``.
+
+    Returns ``(mode, lam, (y0, y1, x0, x1), lam_eff)`` with ``mode`` 'mixup' or 'cutmix'; the box is empty for mixup.
+    """
+    if not (mixup_alpha > 0.0 or cutmix_alpha > 0.0):
+        raise ValueError("mix_draws needs mixup_alpha > 0 or cutmix_alpha > 0")
+    words = _Words(key, counter, 3)
+    if mixup_alpha > 0.0 and cutmix_alpha > 0.0:
+        cutmix = bool(words.word(0) >> 63)
+    else:
+        cutmix = cutmix_alpha > 0.0
+    alpha = cutmix_alpha if cutmix else mixup_alpha
+    lg1, lg2 = words.log_gamma(alpha), words.log_gamma(alpha)
+    d = lg2 - lg1
+    lam = 1.0 / (1.0 + math.exp(d)) if d < 700.0 else 0.0
+    if not cutmix:
+        return "mixup", lam, (0, 0, 0, 0), lam
+    cy = ((words.word(1) >> 32) * H) >> 32
+    cx = ((words.word(2) >> 32) * W) >> 32
+    r = math.sqrt(1.0 - lam)
+    cut_h, cut_w = int(H * r), int(W * r)
+    y0, y1 = min(max(cy - cut_h // 2, 0), H), min(max(cy + cut_h // 2, 0), H)
+    x0, x1 = min(max(cx - cut_w // 2, 0), W), min(max(cx + cut_w // 2, 0), W)
+    return "cutmix", lam, (y0, y1, x0, x1), 1.0 - (y1 - y0) * (x1 - x0) / float(H * W)
+
+
+def mix_factors(lam: float) -> Tuple[float, float]:
+    """``(float32(lam), float32(1 - lam))`` rounded from float64, as Python floats: the mixup blend's two factors."""
+    return float(np.float32(lam)), float(np.float32(1.0 - lam))
+
+
+def mix_images(x: torch.Tensor, mode: str, lam: float, box: Tuple[int, int, int, int]) -> torch.Tensor:
+    """Mixup blend or CutMix paste of a normalised ``[n, 3, H, W]`` batch with its reverse ``x.flip(0)``, in ATen ops.
+    Mixup is ``x * lam_f + x.flip(0) * mlam_f`` in float32 (:func:`mix_factors`), which the kernel reproduces bit for bit."""
+    partner = x.flip(0)
+    if mode == "mixup":
+        lam_f, mlam_f = mix_factors(lam)
+        out = x * lam_f + partner * mlam_f
+    else:
+        y0, y1, x0, x1 = box
+        out = x.clone()
+        out[:, :, y0:y1, x0:x1] = partner[:, :, y0:y1, x0:x1]
+    if x.is_contiguous(memory_format=torch.channels_last) and not x.is_contiguous():
+        return out.contiguous(memory_format=torch.channels_last)
+    return out.contiguous()
+
+
+def mix_batch(u8_nhwc: torch.Tensor, mean, std, channels_last: bool, aug_key: Optional[int], key: int, counter: int,
+              mixup_alpha: float, cutmix_alpha: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Mixed training batch and its ``lam_eff`` (a one-float32 tensor on ``u8_nhwc``'s device): crop + flip
+    (:func:`augment_batch`, when ``aug_key`` is not None) or :func:`normalize_batch`, then :func:`mix_images` with the draw
+    :func:`mix_draws` ``(key, counter, ...)``.  The ATen composition used on the CPU and with ``fast=False``."""
+    n, H, W, _ = u8_nhwc.shape
+    if aug_key is None:
+        x = normalize_batch(u8_nhwc, mean, std, channels_last)
+    else:
+        x = augment_batch(u8_nhwc, mean, std, channels_last, aug_key, counter)
+    mode, lam, box, lam_eff = mix_draws(key, counter, n, H, W, mixup_alpha, cutmix_alpha)
+    return mix_images(x, mode, lam, box), torch.tensor([lam_eff], dtype=torch.float32, device=u8_nhwc.device)
+
+
+# ----------------------------------------------------------------------------
 @dataclass
 class CifarData:
     """The four arrays every driver needs."""
@@ -275,13 +415,17 @@ class ShardLoader:
     or in pinned host memory; in the latter case each batch is gathered by the
     native batch assembler and copied H2D asynchronously, double buffered.
 
-    ``augment=True`` crops and flips every sample at random (see the module docstring) with draws keyed by ``aug_key``;
-    ``aug_counter`` counts the samples handed out so far and advances by the batch size with every yielded batch.
+    ``augment=True`` crops and flips every sample at random (see the module docstring) with draws keyed by ``aug_key``.
+    ``mixup_alpha`` / ``cutmix_alpha`` > 0 mix every batch with its reverse (:func:`mix_draws`, keyed by ``mix_key``) and
+    yield ``(x, y, lam)``, ``lam`` a one-float32 tensor holding ``lam_eff`` on the batch's device; unmixed batches are
+    ``(x, y)``.  With augmentation or mixing, ``aug_counter`` counts the samples handed out so far and advances by the batch
+    size with every yielded batch.
     """
 
     def __init__(self, images: torch.Tensor, labels: torch.Tensor, indices: Sequence[int], batch_size: int,
                  device: torch.device, mean, std, shuffle: bool = True, seed: int = 0,
-                 channels_last: bool = False, with_labels: bool = True, augment: bool = False, aug_key: int = 0):
+                 channels_last: bool = False, with_labels: bool = True, augment: bool = False, aug_key: int = 0,
+                 mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0, mix_key: int = 0):
         self.images, self.labels = images, labels
         self.index = torch.as_tensor(list(indices) if not isinstance(indices, torch.Tensor) else indices, dtype=torch.int64)
         self.batch_size = int(batch_size)
@@ -294,6 +438,9 @@ class ShardLoader:
         self.augment = bool(augment)
         self.aug_key = int(aug_key) & _MASK64
         self.aug_counter = 0
+        self.mixup_alpha, self.cutmix_alpha = float(mixup_alpha), float(cutmix_alpha)
+        self.mixing = self.mixup_alpha > 0.0 or self.cutmix_alpha > 0.0
+        self.mix_key = int(mix_key) & _MASK64
         self.prefetch_order = True     # see _device_order(); a loader abandoned mid-epoch simply never prefetches
         self._next_order = None
         self.host_resident = not images.is_cuda and self.device.type == "cuda"
@@ -341,20 +488,29 @@ class ShardLoader:
                 self._next_order = None
                 self._next_order = self._device_order()
             idx = dev_order[b * self.batch_size:(b + 1) * self.batch_size]
-            if self.augment:
+            if self.mixing:
+                x, lam = self._mixed(self.images, idx)
+            elif self.augment:
                 x = self._augmented(self.images, idx)
             else:
                 x = normalize_batch(self.images.index_select(0, idx), self.mean, self.std, self.channels_last)
             y = self.labels.index_select(0, idx)
             if x.device != self.device:
                 x, y = x.to(self.device), y.to(self.device)
-            yield x, y
+            if self.mixing:
+                yield x, y, lam.to(self.device)
+            else:
+                yield x, y
 
     def _iter_host(self, order: torch.Tensor, nb: int):
         asm = self._assembler
         asm.start_epoch(order)
         for b in range(nb):
             u8, lab = asm.next_batch_to(self.device)  # pinned staging -> async H2D on the copy stream
+            if self.mixing:
+                x, lam = self._mixed(u8, None)
+                yield x, lab, lam
+                continue
             if self.augment:
                 x = self._augmented(u8, None)
             else:
@@ -375,3 +531,24 @@ class ShardLoader:
                                                      self.channels_last)   # gather + crop + flip + normalise: one launch
         u8 = images if idx is None else images.index_select(0, idx)
         return augment_batch(u8, self.mean, self.std, self.channels_last, self.aug_key, counter)
+
+    def _mixed(self, images: torch.Tensor, idx: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Mixed (and, with ``augment``, cropped and flipped), normalised batch of ``images[idx]`` (``images`` itself when
+        ``idx`` is None) and its ``lam_eff`` tensor; advances the counter."""
+        counter = self.aug_counter
+        n = images.shape[0] if idx is None else idx.numel()
+        self.aug_counter += n
+        aug_key = self.aug_key if self.augment else None
+        if images.is_cuda:
+            from ..ops import functional as FX
+
+            if FX.fast_path_enabled():
+                from ..ops import cuda_ops
+
+                draw = mix_draws(self.mix_key, counter, n, images.shape[1], images.shape[2], self.mixup_alpha,
+                                 self.cutmix_alpha)
+                return cuda_ops.mix_normalize_u8(images, idx, aug_key, counter, self.mean, self.std, self.channels_last,
+                                                 draw)   # gather + crop + flip + normalise + mix: one launch
+        u8 = images if idx is None else images.index_select(0, idx)
+        return mix_batch(u8, self.mean, self.std, self.channels_last, aug_key, self.mix_key, counter, self.mixup_alpha,
+                         self.cutmix_alpha)

@@ -19,6 +19,8 @@ Kernel inventory (SURVEY §2.10 ids):
                            (see flatops.py)
   G22 normalize_u8         uint8 NHWC -> normalised float, layout change fused
       augment_normalize_u8 the same with batch gather + random padded crop + horizontal flip fused (training augmentation)
+      mix_normalize_u8     the same (crop + flip optional) with the mixup blend / CutMix paste of sample n-1-i fused
+  G9' soft_ce              cross-entropy against label-smoothed / mixed targets built in the kernel, fixed-order mean
 
 Reference call sites these replace (library calls in the reference): conv + BatchNorm + ELU + residual
 ``src/simple_models.py:137-153`` / ``:191-216``, ``avg_pool2d`` + ``linear`` ``:213-216``, cross-entropy
@@ -167,6 +169,27 @@ def augment_normalize_u8(images_u8: torch.Tensor, rows: Optional[torch.Tensor], 
     if channels_last:
         return ext().augment_normalize_u8(u8, rows, k, int(counter), list(mean), list(std), False).permute(0, 3, 1, 2)
     return ext().augment_normalize_u8(u8, rows, k, int(counter), list(mean), list(std), True)
+
+
+def mix_normalize_u8(images_u8: torch.Tensor, rows: Optional[torch.Tensor], aug_key: Optional[int], counter: int, mean, std,
+                     channels_last: bool, draw) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Mixed training batch in one launch: ``images_u8[rows]`` (or ``images_u8`` itself), cropped and flipped as
+    :func:`augment_normalize_u8` when ``aug_key`` is not None, normalised, and mixed with its reverse by ``draw``, the
+    ``(mode, lam, box, lam_eff)`` of ``data.cifar.mix_draws``.  Returns the batch and ``lam``, a one-float32 tensor holding
+    ``lam_eff`` (written by the same kernel)."""
+    from ..data.cifar import mix_factors
+
+    mode, lam, (y0, y1, x0, x1), lam_eff = draw
+    u8 = images_u8.contiguous()
+    k = int(aug_key or 0) & 0xFFFFFFFFFFFFFFFF
+    k = k - (1 << 64) if k >= (1 << 63) else k                           # the key's bit pattern as an int64
+    if rows is not None:
+        rows = rows.to(torch.int64).contiguous()
+    lam_f, mlam_f = mix_factors(lam)
+    out, lam_t = ext().mix_normalize_u8(u8, rows, aug_key is not None, k, int(counter), list(mean), list(std),
+                                        not channels_last, mode == "cutmix", lam_f, mlam_f, y0, y1, x0, x1,
+                                        float(lam_eff))   # rounded to float32 by the binding
+    return (out.permute(0, 3, 1, 2) if channels_last else out), lam_t
 
 
 # ----------------------------------------------------------------------------
@@ -986,6 +1009,27 @@ class _CrossEntropy(torch.autograd.Function):
 
 def cross_entropy(logits, labels) -> torch.Tensor:
     return _CrossEntropy.apply(logits, labels)
+
+
+class _SoftCrossEntropy(torch.autograd.Function):
+    """Mean cross-entropy against ``q_i = lam s(y_i) + (1 - lam) s(y_{B-1-i})``, ``s(y) = (1 - eps) onehot(y) + eps / C``;
+    ``lam`` a one-float32 device tensor or None (= 1).  The targets never exist as a tensor; graph-capturable."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, lam, eps):
+        loss, probs = ext().soft_ce_fwd(logits.contiguous(), labels, lam, eps)
+        ctx.save_for_backward(probs, labels, lam)
+        ctx.eps = eps
+        return loss
+
+    @staticmethod
+    def backward(ctx, gout):
+        probs, labels, lam = ctx.saved_tensors
+        return ext().soft_ce_bwd(probs, labels, lam, ctx.eps, gout.reshape(1).float()), None, None, None
+
+
+def soft_cross_entropy(logits, labels, lam: Optional[torch.Tensor], label_smoothing: float) -> torch.Tensor:
+    return _SoftCrossEntropy.apply(logits, labels, lam, float(label_smoothing))
 
 
 class _VAELoss(torch.autograd.Function):

@@ -11,7 +11,7 @@ transcriptions of the math with loops, kept as test oracles.
 from __future__ import annotations
 
 import math
-from typing import Dict, Tuple
+from typing import Dict, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -22,14 +22,29 @@ from . import functional as FX
 # ----------------------------------------------------------------------------
 # classifier
 # ----------------------------------------------------------------------------
-def cross_entropy(logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
-    """Mean softmax cross-entropy (``nn.CrossEntropyLoss()`` of federated_multi.py:132)."""
+def cross_entropy(logits: torch.Tensor, labels: torch.Tensor, label_smoothing: float = 0.0,
+                  lam: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Mean softmax cross-entropy (``nn.CrossEntropyLoss()`` of federated_multi.py:132).
+
+    With ``label_smoothing`` eps or a mixed batch's ``lam`` (a one-element tensor, ``lam_eff`` of ``data.cifar.mix_draws``)
+    the target of sample ``i`` is ``lam s(y_i) + (1 - lam) s(y_{B-1-i})`` with ``s(y) = (1 - eps) onehot(y) + eps / C``
+    (timm's ``SoftTargetCrossEntropy`` of mixed, smoothed targets), i.e.
+    ``lam CE_eps(z, y) + (1 - lam) CE_eps(z, y.flip(0))``.  Without either the hard-label kernels run as before."""
+    plain = label_smoothing == 0.0 and lam is None
     if logits.is_cuda and FX.fast_path_enabled():
         from . import cuda_ops
 
         if cuda_ops.cross_entropy_supported(logits):
-            return cuda_ops.cross_entropy(logits, labels)
-    return F.cross_entropy(logits, labels)
+            if plain:
+                return cuda_ops.cross_entropy(logits, labels)
+            return cuda_ops.soft_cross_entropy(logits, labels, lam, label_smoothing)
+    if plain:
+        return F.cross_entropy(logits, labels)
+    loss = F.cross_entropy(logits, labels, label_smoothing=label_smoothing)
+    if lam is None:
+        return loss
+    lam = lam.reshape(())
+    return lam * loss + (1.0 - lam) * F.cross_entropy(logits, labels.flip(0), label_smoothing=label_smoothing)
 
 
 # ----------------------------------------------------------------------------
