@@ -17,8 +17,8 @@
 //   2. local epilogue in place: FedAvg writes z back into every local replica (one-shot) or copies the broadcast
 //      weights into z (two-shot); FedProx accumulates ||rho (x - z)||^2; ADMM performs the dual ascent
 //      y += rho (x - z) and accumulates the same norm
-//   C. the last CTA to finish exchanges the scalars (dual part, primal part, #non-finite) through the control pads
-//      and writes the result record.
+//   C. the last CTA to finish exchanges the round's statistics through the control pads (FedProx/ADMM: dual part,
+//      primal part, #non-finite; DP, compressed and SecAgg rounds: their own statistics) and writes the result record.
 //
 // CTA b works on the SAME index set on every rank and in both passes, so barriers A and B only involve CTA b of each
 // rank (threads 0..world-1 signal / poll one peer each): there is no grid-wide barrier in the kernel.
@@ -36,6 +36,7 @@
 #include <cooperative_groups.h>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 namespace cg = cooperative_groups;
 
@@ -126,6 +127,33 @@ __device__ __forceinline__ void cta_peer_barrier(uint32_t* const* ctrl, int worl
     }
   }
   __syncthreads();
+}
+
+// One-off exchange with every peer on flag row `row` (PAD_FLAG_C / PAD_FLAG_D), run by threads 0..world-1 after each has
+// written its payload into peer threadIdx.x's pad: publish the payload, signal that peer, and wait for its signal.
+__device__ __forceinline__ void peer_post_wait(uint32_t* const* ctrl, int rank, int row, uint32_t epoch, long long limit,
+                                               float* status, int* s_abort) {
+  const int peer = threadIdx.x;
+  __threadfence_system();
+  st_release_sys(ctrl[peer] + row + rank, epoch);
+  if (*s_abort == 0 && !wait_flag(ctrl[rank] + row + peer, epoch, limit)) {
+    *status = 100.f + float(peer);
+    atomicExch(s_abort, 1);
+  }
+}
+
+// the dual residual ||zo - zn||^2 and the non-finite count of the new values zn, accumulated over one float4
+__device__ __forceinline__ void dual_nan_v4(float4 zo, float4 zn, float& dual, float& bad) {
+  const float dx = zo.x - zn.x, dy = zo.y - zn.y, dz = zo.z - zn.z, dw = zo.w - zn.w;
+  dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
+  if (!(isfinite(zn.x) && isfinite(zn.y) && isfinite(zn.z) && isfinite(zn.w))) bad += 1.f;
+}
+
+// two-shot broadcast of a float4 into the same offset of every rank: multimem.st when a multicast address is bound, else
+// P2P stores
+__device__ __forceinline__ void bcast_v4(float* mc, float* const* w, int world, size_t off, float4 v) {
+  if (mc != nullptr) multimem_st_v4(mc + off, v);
+  else for (int p = 0; p < world; ++p) st_sys_v4(w[p] + off, v);
 }
 
 // sum over all K workers of x_k (+ y_k / rho-scaled for ADMM) at float4 index `off`: one in-switch reduction or K peer loads
@@ -363,11 +391,10 @@ __device__ __forceinline__ void q_st4(float* p, int c, int n, float4 v) {
   for (int i = 0; i < 4; ++i)
     if (c + i < n) p[c + i] = w[i];
 }
-// two-shot broadcast of a float4 into every rank: multimem.st when a multicast address is bound, else P2P stores
+// bcast_v4 at coordinate c (a multiple of 4) of a length-n slice: coordinates >= n are not written
 __device__ __forceinline__ void q_bcast4(float* mc, float* const* w, int world, int c, int n, float4 v) {
   if (c + 4 <= n) {
-    if (mc != nullptr) multimem_st_v4(mc + c, v);
-    else for (int p = 0; p < world; ++p) st_sys_v4(w[p] + c, v);
+    bcast_v4(mc, w, world, size_t(c), v);
     return;
   }
   const float s[4] = {v.x, v.y, v.z, v.w};
@@ -651,9 +678,7 @@ __device__ __forceinline__ void q_reduce(const CommArgs& a, int my_slice, float 
         zs = make_float4(__fadd_rn(zo.x, d.x), __fadd_rn(zo.y, d.y), __fadd_rn(zo.z, d.z), __fadd_rn(zo.w, d.w));
       }
       if (!a.two_shot) {
-        const float dx = zo.x - zs.x, dy = zo.y - zs.y, dz = zo.z - zs.z, dw = zo.w - zs.w;
-        dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
-        if (!(isfinite(zs.x) && isfinite(zs.y) && isfinite(zs.z) && isfinite(zs.w))) bad += 1.f;
+        dual_nan_v4(zo, zs, dual, bad);
         q_st4(a.z, c, a.n, zs);
         if constexpr (FEDOPT) {
           q_st4(a.m, c, a.n, mv);
@@ -684,10 +709,7 @@ __device__ __forceinline__ void q_write_back(const CommArgs& a, int nslices, flo
         if (c >= a.n) break;
         if (a.two_shot) {
           const float4 zn = q_ld4_sys(a.xl[0], c, a.n);
-          const float4 zo = q_ld4(a.z, c, a.n);
-          const float dx = zo.x - zn.x, dy = zo.y - zn.y, dz = zo.z - zn.z, dw = zo.w - zn.w;
-          dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
-          if (!(isfinite(zn.x) && isfinite(zn.y) && isfinite(zn.z) && isfinite(zn.w))) bad += 1.f;
+          dual_nan_v4(q_ld4(a.z, c, a.n), zn, dual, bad);
           q_st4(a.z, c, a.n, zn);
         } else {
           const float4 zv = q_ld4(a.z, c, a.n);
@@ -768,6 +790,37 @@ __device__ __forceinline__ float4 pass1_v4(const CommArgs& a, size_t off, float 
   else return reduce_v4<AGG_PAD>(a, off, rho, use_mc);
 }
 
+// Phase C (the last CTA, world > 1): every rank posts the NW words w[] of its round statistics into row PAD_PAYLOAD of
+// every peer; thread 0 then replaces w[] by their sums over the ranks in rank order, as T (float, or uint32_t for counts
+// passed as bit patterns), so every rank reports the same values.  w is shared memory, written by thread 0 before the call.
+template <typename T, int NW>
+__device__ __forceinline__ void exchange_sum(const CommArgs& a, uint32_t epoch, float* w, int* s_abort) {
+  __syncthreads();
+  if (threadIdx.x < a.world) {
+    float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_PAYLOAD) + 4 * a.rank;
+    for (int i = 0; i < NW; ++i) st_sys_f32(pay + i, w[i]);
+    peer_post_wait(a.ctrl, a.rank, PAD_FLAG_C, epoch, a.timeout_cycles, a.out + OUT_STATUS, s_abort);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_PAYLOAD);
+    T s[NW] = {};
+    for (int r = 0; r < a.world; ++r) {
+#pragma unroll
+      for (int i = 0; i < NW; ++i) {
+        const float v = ld_sys_f32(pay + 4 * r + i);
+        if constexpr (std::is_same<T, float>::value) s[i] += v;
+        else s[i] += __float_as_uint(v);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < NW; ++i) {
+      if constexpr (std::is_same<T, float>::value) w[i] = s[i];
+      else w[i] = __uint_as_float(s[i]);
+    }
+  }
+}
+
 // FEDOPT = false: FedAvg / FedProx / ADMM (a.mode).  FEDOPT = true: FedAvg (mode 0) whose new model is a server optimizer
 // step from z instead of the plain mean.  Pass 1 forms the step from the reduced mean, z and the state m (and v): one-shot
 // stores z, m, v locally; two-shot rank r broadcasts slice r of the new weights, of m and of v into every rank, so every rank
@@ -842,6 +895,9 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   } else {
     const int lo = my_slice * chunk4;
     const int hi = min(n4, lo + chunk4);
+    const bool adaptive = FEDOPT && a.opt != FEDOPT_AVGM;
+    const bool dual_here = !(a.two_shot && a.mode == 0);   // two-shot FedAvg takes the dual residual and NaN count from
+                                                            // the finished weights in pass 2
     // two elements per thread and iteration: their (remote) loads are issued back to back, so twice as many bytes are in
     // flight per thread — the pass is bound by NVLink round trips, not by issue slots
     for (int i = lo + t0; i < hi; i += 2 * stride) {
@@ -859,45 +915,28 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
         const float4 zn = DP ? dp_noised_v4<DP>(a, off, make_float4(acc.x * inv_scale, acc.y * inv_scale, acc.z * inv_scale,
                                                                      acc.w * inv_scale))
                              : make_float4(acc.x * inv_scale, acc.y * inv_scale, acc.z * inv_scale, acc.w * inv_scale);
+        // the new value zs: the aggregate itself, or the server step from z along it (which also updates m and v)
+        const float4 zo = (FEDOPT || dual_here) ? *reinterpret_cast<const float4*>(a.z + off) : zn;
+        float4 zs = zn, mv, vv;
         if constexpr (FEDOPT) {
-          const bool adaptive = a.opt != FEDOPT_AVGM;
-          const float4 zo = *reinterpret_cast<const float4*>(a.z + off);
-          float4 mv = *reinterpret_cast<const float4*>(a.m + off);
-          float4 vv = adaptive ? *reinterpret_cast<const float4*>(a.v + off) : make_float4(0.f, 0.f, 0.f, 0.f);
-          const float4 zs = fedopt_step_v4(a, zo, zn, mv, vv);
-          if (!a.two_shot) {
-            const float dx = zo.x - zs.x, dy = zo.y - zs.y, dz = zo.z - zs.z, dw = zo.w - zs.w;
-            dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
-            if (!(isfinite(zs.x) && isfinite(zs.y) && isfinite(zs.z) && isfinite(zs.w))) bad += 1.f;
-            *reinterpret_cast<float4*>(a.z + off) = zs;
+          mv = *reinterpret_cast<const float4*>(a.m + off);
+          vv = adaptive ? *reinterpret_cast<const float4*>(a.v + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+          zs = fedopt_step_v4(a, zo, zn, mv, vv);
+        }
+        if (dual_here) dual_nan_v4(zo, zs, dual, bad);
+        if (!a.two_shot) {
+          *reinterpret_cast<float4*>(a.z + off) = zs;
+          if constexpr (FEDOPT) {
             *reinterpret_cast<float4*>(a.m + off) = mv;
             if (adaptive) *reinterpret_cast<float4*>(a.v + off) = vv;
-          } else {                                 // weights, m and v of slice r into every rank (dual + NaN check: pass 2)
-            if (a.mc_x != nullptr) multimem_st_v4(a.mc_x + off, zs);
-            else for (int p = 0; p < a.world; ++p) st_sys_v4(a.xw[p] + off, zs);
-            if (a.mc_m != nullptr) multimem_st_v4(a.mc_m + off, mv);
-            else for (int p = 0; p < a.world; ++p) st_sys_v4(a.mw[p] + off, mv);
-            if (adaptive) {
-              if (a.mc_v != nullptr) multimem_st_v4(a.mc_v + off, vv);
-              else for (int p = 0; p < a.world; ++p) st_sys_v4(a.vw[p] + off, vv);
-            }
           }
-          continue;
-        }
-        if (!(a.two_shot && a.mode == 0)) {       // two-shot FedAvg takes both from the finished weights in pass 2
-          const float4 zo = *reinterpret_cast<const float4*>(a.z + off);
-          const float dx = zo.x - zn.x, dy = zo.y - zn.y, dz = zo.z - zn.z, dw = zo.w - zn.w;
-          dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
-          if (!(isfinite(zn.x) && isfinite(zn.y) && isfinite(zn.z) && isfinite(zn.w))) bad += 1.f;
-        }
-        if (!a.two_shot) {
-          *reinterpret_cast<float4*>(a.z + off) = zn;
-        } else if (a.mode == 0) {                 // broadcast the averaged weights into every rank's replica
-          if (a.mc_x != nullptr) multimem_st_v4(a.mc_x + off, zn);
-          else for (int p = 0; p < a.world; ++p) st_sys_v4(a.xw[p] + off, zn);
-        } else {                                   // broadcast the consensus vector
-          if (a.mc_z != nullptr) multimem_st_v4(a.mc_z + off, zn);
-          else for (int p = 0; p < a.world; ++p) st_sys_v4(a.zw[p] + off, zn);
+        } else {                                   // slice r into every rank: FedAvg's weights, else the consensus vector
+          if (a.mode == 0) bcast_v4(a.mc_x, a.xw, a.world, off, zs);
+          else bcast_v4(a.mc_z, a.zw, a.world, off, zs);
+          if constexpr (FEDOPT) {
+            bcast_v4(a.mc_m, a.mw, a.world, off, mv);
+            if (adaptive) bcast_v4(a.mc_v, a.vw, a.world, off, vv);
+          }
         }
       }
     }
@@ -950,10 +989,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       if (a.mode == 0) {
         if (a.two_shot) {                        // weights already hold the average: keep a copy as next round's z_old,
           const float4 zn = ld_sys_v4(a.xl[0] + off);          // and take the dual residual + NaN check from it (the full vector
-          const float4 zo = *reinterpret_cast<const float4*>(a.z + off);   // is local now: no cross-rank sum needed)
-          const float dx = zo.x - zn.x, dy = zo.y - zn.y, dz = zo.z - zn.z, dw = zo.w - zn.w;
-          dual = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, dual))));
-          if (!(isfinite(zn.x) && isfinite(zn.y) && isfinite(zn.z) && isfinite(zn.w))) bad += 1.f;
+          dual_nan_v4(*reinterpret_cast<const float4*>(a.z + off), zn, dual, bad);   // is local now: no cross-rank sum needed)
           *reinterpret_cast<float4*>(a.z + off) = zn;
         } else {
           const float4 zv = *reinterpret_cast<const float4*>(a.z + off);
@@ -1018,184 +1054,73 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   __syncthreads();
   if (!s_last) return;
 
-  // ---- C: exchange and finish the scalars (one CTA) -------------------------------------------------------------
-  __shared__ float s_vals[3];
+  // ---- C: exchange the round's statistics over the ranks and write the record (one CTA) ---------------------------
+  // A round exchanges one set of words at most: FedProx / ADMM their dual and primal parts and non-finite counts (FedAvg's
+  // are complete on every rank already), DP rounds the clip statistics of the local replicas, compressed rounds the
+  // quantization statistics and SecAgg rounds the clipped / non-finite counts, both summed over the CTAs in CTA order.
+  __shared__ float s_c[3];
+  float dual_sq = 0.f, primal = 0.f, nonfinite = 0.f;   // thread 0
   if (threadIdx.x == 0) {
     __threadfence();
-    float local = 0.f;
-    for (int j = 0; j < a.n_local; ++j) local += sqrtf(__ldcg(a.scratch + 4 + j));
-    s_vals[0] = __ldcg(a.scratch + 0);
-    s_vals[1] = local;
-    s_vals[2] = __ldcg(a.scratch + 1);
+    for (int j = 0; j < a.n_local; ++j) primal += sqrtf(__ldcg(a.scratch + 4 + j));
+    dual_sq = __ldcg(a.scratch + 0);
+    nonfinite = __ldcg(a.scratch + 1);
     for (int j = 0; j < COMM_SCRATCH_FLOATS; ++j) a.scratch[j] = 0.f;      // self-cleaning: no memset per launch
-  }
-  __syncthreads();
-  float dual_sq = s_vals[0], primal = s_vals[1], nonfinite = s_vals[2];
-  if (a.world > 1 && a.mode != 0) {          // FedAvg: every rank already holds the complete dual residual and NaN count
-    if (threadIdx.x < a.world) {
-      float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_PAYLOAD) + 4 * a.rank;
-      st_sys_f32(pay + 0, dual_sq);
-      st_sys_f32(pay + 1, primal);
-      st_sys_f32(pay + 2, nonfinite);
-      __threadfence_system();
-      st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_C + a.rank, epoch);
-      if (s_abort == 0 && !wait_flag(a.ctrl[a.rank] + PAD_FLAG_C + threadIdx.x, epoch, a.timeout_cycles)) {
-        a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
-        atomicExch(&s_abort, 1);
-      }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_PAYLOAD);
-      float d = 0.f, p = 0.f, b = 0.f;
-      for (int r = 0; r < a.world; ++r) {
-        d += ld_sys_f32(pay + 4 * r + 0);
-        p += ld_sys_f32(pay + 4 * r + 1);
-        b += ld_sys_f32(pay + 4 * r + 2);
-      }
-      if (a.two_shot) dual_sq = d;      // one-shot: every rank already holds the full sum
-      primal = p;
-      nonfinite = a.two_shot ? b : nonfinite;
-    }
-  }
-  // DP (mode 0): the clip statistics of dp_clip_kernel, summed over the local replicas and then over the ranks in rank
-  // order, so every rank reports the same values
-  if constexpr (DP) {
-    __shared__ float s_dp[2];
-    if (threadIdx.x == 0) {
+    if constexpr (DP) {
       float clipped = 0.f, norms = 0.f;
       for (int j = 0; j < a.n_local; ++j) {
         norms += a.dp_stats[j];
         clipped += a.dp_stats[COMM_MAX_LOCAL + j];
       }
-      s_dp[0] = clipped;
-      s_dp[1] = norms;
-    }
-    __syncthreads();
-    if (a.world > 1) {
-      if (threadIdx.x < a.world) {
-        float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_DP_PAYLOAD) + 2 * a.rank;
-        st_sys_f32(pay + 0, s_dp[0]);
-        st_sys_f32(pay + 1, s_dp[1]);
-        __threadfence_system();
-        st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_C + a.rank, epoch);
-        if (s_abort == 0 && !wait_flag(a.ctrl[a.rank] + PAD_FLAG_C + threadIdx.x, epoch, a.timeout_cycles)) {
-          a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
-          atomicExch(&s_abort, 1);
-        }
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_DP_PAYLOAD);
-        float c = 0.f, s = 0.f;
-        for (int r = 0; r < a.world; ++r) {
-          c += ld_sys_f32(pay + 2 * r + 0);
-          s += ld_sys_f32(pay + 2 * r + 1);
-        }
-        s_dp[0] = c;
-        s_dp[1] = s;
-      }
-    }
-    if (threadIdx.x == 0) {
-      a.out[OUT_DP_CLIPPED] = s_dp[0];
-      a.out[OUT_DP_NORM_SUM] = s_dp[1];
-      *a.dp_t += 1;                                // every CTA has read t: the next round (or graph replay) draws t + 1
-    }
-  }
-  // SecAgg rounds (mode 0): the per-CTA counts, then over the ranks through the compressed rounds' pad row (as uint32
-  // bit patterns); the non-finite updates join the record's non-finite count, so the NaN guard fires although their
-  // codes are 0
-  if constexpr (QBITS == SA_QBITS) {
-    __shared__ uint32_t s_sa[2];
-    if (threadIdx.x == 0) {
+      s_c[0] = clipped;
+      s_c[1] = norms;
+    } else if constexpr (QBITS == SA_QBITS) {      // integers, as uint32 bit patterns
       uint32_t c = 0u, b = 0u;
       for (int i = 0; i < int(gridDim.x); ++i) {
         c += __ldcg(reinterpret_cast<const unsigned int*>(a.q_part) + 2 * i + 0);
         b += __ldcg(reinterpret_cast<const unsigned int*>(a.q_part) + 2 * i + 1);
       }
-      s_sa[0] = c;
-      s_sa[1] = b;
-    }
-    __syncthreads();
-    if (a.world > 1) {
-      if (threadIdx.x < a.world) {
-        float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_Q_PAYLOAD) + 2 * a.rank;
-        st_sys_f32(pay + 0, __uint_as_float(s_sa[0]));
-        st_sys_f32(pay + 1, __uint_as_float(s_sa[1]));
-        __threadfence_system();
-        st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_C + a.rank, epoch);
-        if (s_abort == 0 && !wait_flag(a.ctrl[a.rank] + PAD_FLAG_C + threadIdx.x, epoch, a.timeout_cycles)) {
-          a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
-          atomicExch(&s_abort, 1);
-        }
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_Q_PAYLOAD);
-        uint32_t c = 0u, b = 0u;
-        for (int r = 0; r < a.world; ++r) {
-          c += __float_as_uint(ld_sys_f32(pay + 2 * r + 0));
-          b += __float_as_uint(ld_sys_f32(pay + 2 * r + 1));
-        }
-        s_sa[0] = c;
-        s_sa[1] = b;
-      }
-    }
-    if (threadIdx.x == 0) {
-      a.out[OUT_SA_CLIPPED] = __uint_as_float(s_sa[0]);
-      a.out[OUT_SA_NONFINITE] = __uint_as_float(s_sa[1]);
-      nonfinite += float(s_sa[1]);
-      *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) masks with t + 1
-    }
-  }
-  // compressed rounds (mode 0): the per-CTA partial statistics in CTA order, then over the ranks in rank order, so every
-  // rank reports the same values
-  if constexpr (QBITS != 0 && QBITS != SA_QBITS) {
-    __shared__ float s_q[2];
-    if (threadIdx.x == 0) {
+      s_c[0] = __uint_as_float(c);
+      s_c[1] = __uint_as_float(b);
+    } else if constexpr (QBITS != 0) {
       float e = 0.f, u = 0.f;
       for (int b = 0; b < int(gridDim.x); ++b) {
         e += __ldcg(a.q_part + 2 * b + 0);
         u += __ldcg(a.q_part + 2 * b + 1);
       }
-      s_q[0] = e;
-      s_q[1] = u;
-    }
-    __syncthreads();
-    if (a.world > 1) {
-      if (threadIdx.x < a.world) {
-        float* pay = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_Q_PAYLOAD) + 2 * a.rank;
-        st_sys_f32(pay + 0, s_q[0]);
-        st_sys_f32(pay + 1, s_q[1]);
-        __threadfence_system();
-        st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_C + a.rank, epoch);
-        if (s_abort == 0 && !wait_flag(a.ctrl[a.rank] + PAD_FLAG_C + threadIdx.x, epoch, a.timeout_cycles)) {
-          a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
-          atomicExch(&s_abort, 1);
-        }
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        const float* pay = reinterpret_cast<const float*>(a.ctrl[a.rank] + PAD_Q_PAYLOAD);
-        float e = 0.f, u = 0.f;
-        for (int r = 0; r < a.world; ++r) {
-          e += ld_sys_f32(pay + 2 * r + 0);
-          u += ld_sys_f32(pay + 2 * r + 1);
-        }
-        s_q[0] = e;
-        s_q[1] = u;
-      }
-    }
-    if (threadIdx.x == 0) {
-      a.out[OUT_Q_ERR_SQ] = s_q[0];
-      a.out[OUT_Q_NORM_SQ] = s_q[1];
-      *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) draws t + 1
+      s_c[0] = e;
+      s_c[1] = u;
+    } else {
+      s_c[0] = dual_sq;
+      s_c[1] = primal;
+      s_c[2] = nonfinite;
     }
   }
-  if constexpr (SAMP) {
-    if (threadIdx.x == 0) *a.samp_t += 1;          // every CTA has selected: the next round (or graph replay) samples t + 1
-  }
+  using Word = typename std::conditional<QBITS == SA_QBITS, uint32_t, float>::type;
+  constexpr int NW = (DP || QBITS != 0) ? 2 : 3;
+  if (a.world > 1 && (DP || QBITS != 0 || a.mode != 0)) exchange_sum<Word, NW>(a, epoch, s_c, &s_abort);
   if (threadIdx.x == 0) {
+    if constexpr (DP) {
+      a.out[OUT_DP_CLIPPED] = s_c[0];
+      a.out[OUT_DP_NORM_SUM] = s_c[1];
+      *a.dp_t += 1;                                // every CTA has read t: the next round (or graph replay) draws t + 1
+    } else if constexpr (QBITS == SA_QBITS) {
+      a.out[OUT_SA_CLIPPED] = s_c[0];
+      a.out[OUT_SA_NONFINITE] = s_c[1];
+      nonfinite += float(__float_as_uint(s_c[1]));  // so the NaN guard fires although the non-finite updates' codes are 0
+      *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) masks with t + 1
+    } else if constexpr (QBITS != 0) {
+      a.out[OUT_Q_ERR_SQ] = s_c[0];
+      a.out[OUT_Q_NORM_SQ] = s_c[1];
+      *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) draws t + 1
+    } else if (a.world > 1 && a.mode != 0) {
+      if (a.two_shot) {                            // one-shot: every rank already holds the full dual residual and NaN count
+        dual_sq = s_c[0];
+        nonfinite = s_c[2];
+      }
+      primal = s_c[1];
+    }
+    if constexpr (SAMP) *a.samp_t += 1;            // every CTA has selected: the next round (or graph replay) samples t + 1
     a.out[OUT_DUAL_SQ] = dual_sq;
     a.out[OUT_PRIMAL] = primal;
     a.out[OUT_NONFINITE] = nonfinite;
@@ -1207,14 +1132,30 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   }
 }
 
-static int comm_max_blocks(const void* kernel) {
-  int dev = 0, sms = 0, per = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, COMM_THREADS, 0);
-  int m = sms * (per < 1 ? 1 : 1);                    // one CTA per SM (132 on an H100 SXM) x 512 threads
-  if (m > COMM_MAX_BLOCKS) m = COMM_MAX_BLOCKS;
-  return m < 1 ? 1 : m;
+// one CTA per SM (132 on an H100 SXM) x 512 threads, at most COMM_MAX_BLOCKS; read once per process
+static int comm_max_blocks() {
+  static const int m = [] {
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms < 1 ? 1 : (sms > COMM_MAX_BLOCKS ? COMM_MAX_BLOCKS : sms);
+  }();
+  return m;
+}
+
+// block_reduce_kernel's instantiation for a round, as an index into the launcher's table: the mean, the robust rules on
+// <= 4, <= 8 and <= 16 workers, the DP mean, 8-bit codes, 4-bit codes, the sampled weighted mean and secure aggregation,
+// plus REDUCE_VARIANTS with a server optimizer
+constexpr int REDUCE_VARIANTS = 9;
+static int reduce_variant(const CommArgs& a) {
+  int v;
+  if (a.sa) v = 8;
+  else if (a.samp_S != 0 || a.samp_t != nullptr) v = 7;
+  else if (a.qbits != 0) v = a.qbits == 8 ? 5 : 6;
+  else if (a.dp) v = 4;
+  else if (a.agg == AGG_MEAN) v = 0;
+  else v = a.K <= 4 ? 1 : a.K <= 8 ? 2 : 3;
+  return (a.opt != FEDOPT_NONE ? REDUCE_VARIANTS : 0) + v;
 }
 
 void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
@@ -1269,27 +1210,19 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
     if (args.two_shot && (args.xw[args.world - 1] == nullptr || (args.opt != FEDOPT_NONE && args.mw[args.world - 1] == nullptr)))
       throw std::runtime_error("fedb200: block_reduce: two-shot secure aggregation needs P2P broadcast targets");
   }
-  const bool fo = args.opt != FEDOPT_NONE;
-  // kernel table: [fedopt][mean, robust on <= 4, <= 8, <= 16 workers, DP mean, 8-bit codes, 4-bit codes, sampled weighted
-  // mean, secure aggregation]
-  const void* kernels[2][9] = {
-      {(const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
-       (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>,
-       (const void*)block_reduce_kernel<false, 0, true>, (const void*)block_reduce_kernel<false, 0, false, 8>,
-       (const void*)block_reduce_kernel<false, 0, false, 4>, (const void*)block_reduce_kernel<false, 0, false, 0, true>,
-       (const void*)block_reduce_kernel<false, 0, false, SA_QBITS>},
-      {(const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
-       (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>,
-       (const void*)block_reduce_kernel<true, 0, true>, (const void*)block_reduce_kernel<true, 0, false, 8>,
-       (const void*)block_reduce_kernel<true, 0, false, 4>, (const void*)block_reduce_kernel<true, 0, false, 0, true>,
-       (const void*)block_reduce_kernel<true, 0, false, SA_QBITS>}};
-  const int pad = args.sa ? 8 : samp ? 7 : args.qbits == 8 ? 5 : args.qbits == 4 ? 6 : args.dp ? 4 : args.agg == AGG_MEAN ? 0
-                : args.K <= 4 ? 1 : args.K <= 8 ? 2 : 3;
-  const void* kernel = kernels[fo][pad];
-  static int max_blocks[2][9] = {};
-  int& mb = max_blocks[fo][pad];
-  if (mb == 0) mb = comm_max_blocks(kernel);
-  int cap = mb;
+  static const void* const kernels[2 * REDUCE_VARIANTS] = {
+      (const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
+      (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>,
+      (const void*)block_reduce_kernel<false, 0, true>, (const void*)block_reduce_kernel<false, 0, false, 8>,
+      (const void*)block_reduce_kernel<false, 0, false, 4>, (const void*)block_reduce_kernel<false, 0, false, 0, true>,
+      (const void*)block_reduce_kernel<false, 0, false, SA_QBITS>,
+      (const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
+      (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>,
+      (const void*)block_reduce_kernel<true, 0, true>, (const void*)block_reduce_kernel<true, 0, false, 8>,
+      (const void*)block_reduce_kernel<true, 0, false, 4>, (const void*)block_reduce_kernel<true, 0, false, 0, true>,
+      (const void*)block_reduce_kernel<true, 0, false, SA_QBITS>};
+  const void* kernel = kernels[reduce_variant(args)];
+  int cap = comm_max_blocks();
   if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;
   const int n4 = args.n >> 2;
   const int work4 = args.two_shot ? (n4 + args.world - 1) / args.world : n4;
@@ -1409,9 +1342,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) dp_clip_kernel(const DPClipAr
 void dp_clip_launch(const DPClipArgs& args, cudaStream_t s) {
   if (args.n_local < 1 || args.n_local > COMM_MAX_LOCAL || args.n < 1)
     throw std::runtime_error("fedb200: dp_clip: bad replica count or block length");
-  static int max_blocks = 0;
-  if (max_blocks == 0) max_blocks = comm_max_blocks((const void*)dp_clip_kernel);
-  int cap = max_blocks;
+  int cap = comm_max_blocks();
   if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;
   const int want = ((args.n >> 2) + COMM_THREADS - 1) / COMM_THREADS;
   const int grid = want < 1 ? 1 : (want > cap ? cap : want);
@@ -1435,7 +1366,6 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) bb_update_kernel(const BBArgs
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
   const int nth = gridDim.x * blockDim.x;
   float* dots = a.scratch;                         // [n_local][8]
-  unsigned* ticket = reinterpret_cast<unsigned*>(a.scratch + 8 * COMM_MAX_LOCAL);
   float* rho_turn = a.scratch + 8 * COMM_MAX_LOCAL + 8;   // [n_local]
 
   if (!a.seed_only) {
@@ -1478,12 +1408,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) bb_update_kernel(const BBArgs
           float* rows = reinterpret_cast<float*>(a.ctrl[threadIdx.x] + PAD_BBROWS);
           for (int j = 0; j < a.n_local; ++j)
             for (int q = 0; q < 6; ++q) st_sys_f32(rows + 8 * a.worker[j] + q, __ldcg(dots + 8 * j + q));
-          __threadfence_system();
-          st_release_sys(a.ctrl[threadIdx.x] + PAD_FLAG_D + a.rank, epoch);
-          if (!wait_flag(a.ctrl[a.rank] + PAD_FLAG_D + threadIdx.x, epoch, a.timeout_cycles)) {
-            a.out[OUT_STATUS] = 100.f + float(threadIdx.x);
-            atomicExch(&s_abort, 1);
-          }
+          peer_post_wait(a.ctrl, a.rank, PAD_FLAG_D, epoch, a.timeout_cycles, a.out + OUT_STATUS, &s_abort);
         }
       } else if (threadIdx.x == 0) {
         for (int j = 0; j < a.n_local; ++j)
@@ -1542,7 +1467,6 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) bb_update_kernel(const BBArgs
   grid.sync();
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     for (int j = 0; j < BB_SCRATCH_FLOATS; ++j) a.scratch[j] = 0.f;
-    (void)ticket;
     __threadfence();
     a.sync[0] = epoch;
   }
@@ -1552,9 +1476,7 @@ void bb_update_launch(const BBArgs& args_in, cudaStream_t s) {
   BBArgs args = args_in;
   if (args.K < 1 || args.K > COMM_MAX_K || args.n_local > COMM_MAX_LOCAL || args.world > COMM_MAX_WORLD)
     throw std::runtime_error("fedb200: bb_update: limits exceeded");
-  static int max_blocks = 0;
-  if (max_blocks == 0) max_blocks = comm_max_blocks((const void*)bb_update_kernel);
-  int cap = max_blocks;
+  int cap = comm_max_blocks();
   if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;
   int want = ((args.n >> 2) + COMM_THREADS - 1) / COMM_THREADS;
   int grid = want < 1 ? 1 : (want > cap ? cap : want);

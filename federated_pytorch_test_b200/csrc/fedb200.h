@@ -210,16 +210,19 @@ constexpr int COMM_MAX_BLOCKS = 160; // CTAs per aggregation kernel (one per SM:
 
 // Control pad (uint32 words; one pad per rank, mapped into every peer).  Flags hold the epoch of the aggregation that
 // last signalled them (monotonic, compared with >=), so nothing is ever reset.
+// Every kind of round posts its statistics into the same PAD_PAYLOAD row (FedProx / ADMM: dual^2 part, primal part,
+// #non-finite; DP: #clipped, sum of norms; compressed: quantization statistics; SecAgg: clipped / non-finite counts).  A
+// rank posts into a peer's row again only in a later round, after passing that round's barrier A with the peer; the
+// peer's kernel for that round started only after its kernel that read the row had finished (launches on a stream run in
+// order), so a round never overwrites words a peer has yet to read, whatever kind either round is.
 constexpr int PAD_FLAG_A = 0;                                                 // [COMM_MAX_BLOCKS][COMM_MAX_WORLD]  per-CTA: inputs final
 constexpr int PAD_FLAG_B = PAD_FLAG_A + COMM_MAX_BLOCKS * COMM_MAX_WORLD;     // [COMM_MAX_BLOCKS][COMM_MAX_WORLD]  per-CTA: reads / broadcasts done
-constexpr int PAD_FLAG_C = PAD_FLAG_B + COMM_MAX_BLOCKS * COMM_MAX_WORLD;     // [COMM_MAX_WORLD]  scalars posted
+constexpr int PAD_FLAG_C = PAD_FLAG_B + COMM_MAX_BLOCKS * COMM_MAX_WORLD;     // [COMM_MAX_WORLD]  statistics posted
 constexpr int PAD_FLAG_D = PAD_FLAG_C + COMM_MAX_WORLD;                       // [COMM_MAX_WORLD]  Barzilai-Borwein rows posted
-constexpr int PAD_PAYLOAD = PAD_FLAG_D + COMM_MAX_WORLD;                      // [COMM_MAX_WORLD][4] floats: dual^2 part, primal part, #non-finite
+constexpr int PAD_PAYLOAD = PAD_FLAG_D + COMM_MAX_WORLD;                      // [COMM_MAX_WORLD][4] words: a round's statistics
 constexpr int PAD_BBROWS = PAD_PAYLOAD + 4 * COMM_MAX_WORLD;                  // [COMM_MAX_K][8] floats: six dots per worker
-constexpr int PAD_DP_PAYLOAD = PAD_BBROWS + 8 * COMM_MAX_K;                   // [COMM_MAX_WORLD][2] floats: #clipped, sum of norms
-constexpr int PAD_Q_PAYLOAD = PAD_DP_PAYLOAD + 2 * COMM_MAX_WORLD;            // [COMM_MAX_WORLD][2] floats: quantization statistics
 constexpr int COMM_PAD_WORDS = 8192;
-static_assert(PAD_Q_PAYLOAD + 2 * COMM_MAX_WORLD <= COMM_PAD_WORDS, "control pad too small");
+static_assert(PAD_BBROWS + 8 * COMM_MAX_K <= COMM_PAD_WORDS, "control pad too small");
 
 // out record of an aggregation (floats): what the host reads back, once per round.  DP rounds add the number of clipped
 // workers and the sum of their pre-clip update norms, over all K; compressed rounds the sums over all K of
@@ -360,7 +363,7 @@ struct BBArgs {
   const float* z;
   float* rho_dev;                    // in/out: the shared penalty of this block
   float* log;                        // [K][8]: d11, d12, d22, alpha, alphaSD, alphaMG, tested(0/1), rho after this worker's turn
-  float* scratch;                    // [8 * COMM_MAX_LOCAL + 8] zero between launches: dots + ticket + rho_turn
+  float* scratch;                    // [BB_SCRATCH_FLOATS] zero between launches: dots, 8 unused words, rho_turn
   uint32_t* ctrl[COMM_MAX_WORLD];
   uint32_t* sync;
   float* out;                        // status goes to out[OUT_STATUS]
