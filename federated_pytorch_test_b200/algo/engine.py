@@ -223,6 +223,7 @@ class Engine:
         self._round_mark = {"images": 0, "t": time.perf_counter(), "ms": {}}
         self._streams: Dict[int, "torch.cuda.Stream"] = {}
         self._round_extra: Dict = {}
+        self._round_steps: Dict[int, int] = {}       # worker id -> local steps since the last aggregation
         # client learning-rate schedule: round r of T (a pure function of the schedule position)
         self.scheduled = schedule_active(cfg.lr_schedule, cfg.lr_warmup)
         self.total_rounds = 0
@@ -498,6 +499,7 @@ class Engine:
         self.last_loss1 = loss1
         self.images_seen += task.batch_size_of(batch)
         self.steps_done += 1
+        self._round_steps[rep.ck] = self._round_steps.get(rep.ck, 0) + 1
         task.after_minibatch(rep, visit, batch, i, epoch, nloop, N, loss1, self)
         if self.step_hook is not None:
             self.step_hook(self)
@@ -532,6 +534,10 @@ class Engine:
             self._finish_round()
         if self.attack is not None:
             self.attack(self)
+        # the round's local step counts (0 for replicas that sat out) and client learning rate, known on the host
+        self.strategy.note_local_steps([self._round_steps.get(rep.ck, 0) for rep in self.replicas],
+                                       self._round_extra.get("lr", visit.opt_kwargs.get("lr")))
+        self._round_steps = {}
         with nvtx_range("fedb200:aggregate"), self.timers.phase("aggregate"):
             token = self.strategy.aggregate_begin(nadmm) if defer else ("done", self.strategy.aggregate(nadmm))
         self._pending_round = (token, visit, nloop, nadmm, epoch, N, self._round_extra)

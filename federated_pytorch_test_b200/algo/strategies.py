@@ -68,6 +68,10 @@ class Strategy:
         """Whether local replica ``i`` trains in the current round (every replica, unless the strategy samples clients)."""
         return True
 
+    def note_local_steps(self, steps: Sequence[int], lr: Optional[float]) -> None:
+        """Called by the engine before every aggregation: the local steps each local replica took since the last one
+        (0 for a replica that sat out) and the round's client learning rate.  Only SCAFFOLD uses them."""
+
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         raise NotImplementedError
 
@@ -139,16 +143,26 @@ class FedAvg(Strategy):
     round is one launch on the fused collective.  As with DP, ``z`` starts each block visit as the replicas' common value
     instead of 0 (Q6), so the ``dual`` of the first round of a visit differs from plain FedAvg.  The round metrics gain
     ``sa_frac_bits`` (``f``) and ``sa_clipped`` (coordinates clipped, over all K); a non-finite update coordinate codes to
-    0 and is reported as ``nonfinite``, so the NaN guard fires."""
+    0 and is reported as ``nonfinite``, so the NaN guard fires.
+
+    ``scaffold`` adds SCAFFOLD control variates (Karimireddy et al. 2020, option II; ``algo/scaffold.py``) to SGD client
+    steps: every local step of worker ``i`` adds ``d_i = c - c_i`` to its gradient (``penalty(i).y``), and every round
+    first updates the ``c_i`` of the workers that trained from their model change, averages ``c`` over all K and forms the
+    next ``d_i`` (three launches), then aggregates the model as without it (mean, sample-weighted mean or server
+    optimizer).  ``c`` and ``c_i`` persist per block for the whole run.  As with DP, ``z`` starts each block visit as the
+    replicas' common value instead of 0 (Q6), so the ``dual`` of the first round of a visit differs from plain FedAvg.  The
+    round metrics gain ``scaffold_corr``, the mean over this process' replicas of ``||c - c_i||``."""
 
     name = "fedavg"
     write_back = True
+    forms_server_model = False      # FedOpt averages the replicas into z at the start of a visit itself
 
     def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1, dp_clip: float = 0.0,
                  dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
                  compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None,
-                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None):
-        from ..config import check_aggregator, check_compress, check_dp, check_sampling, check_secagg, trim_count
+                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None, scaffold: bool = False):
+        from ..config import (check_aggregator, check_compress, check_dp, check_sampling, check_scaffold, check_secagg,
+                              trim_count)
 
         super().__init__(collective, topo)
         check_aggregator(aggregator, trim_fraction, topo.K)
@@ -218,11 +232,20 @@ class FedAvg(Strategy):
             self.sa_payload: List[torch.Tensor] = []                 # per local replica, current block
             if hasattr(collective, "warm_secagg"):
                 collective.warm_secagg = True
+        check_scaffold(scaffold, aggregator, dp_clip, compress_bits, secagg)
+        self.scaffold = None
+        if scaffold:
+            from .scaffold import ControlVariates
+
+            self.scaffold = ControlVariates(collective, topo)
 
     def begin_block(self, ci: int, N: int, xs: List[torch.Tensor]) -> None:
         super().begin_block(ci, N, xs)
-        if self.dp or self.q_bits or self.sa:  # the server model: the replicas are equal here, so a local copy suffices
+        # the server model: the replicas are equal here, so a local copy suffices
+        if self.dp or self.q_bits or self.sa or (self.scaffold is not None and not self.forms_server_model):
             self.z.copy_(xs[0])
+        if self.scaffold is not None:
+            self.scaffold.begin_block(ci, xs)
         if self.sa:
             self.sa_payload = [self.coll.payload32_like_block(x) for x in xs]
         if self.q_bits:
@@ -231,6 +254,36 @@ class FedAvg(Strategy):
                 self.q_ef[ci] = [torch.zeros_like(x) for x in xs]
                 if ci in self._q_restored:
                     self._install_ef(ci, self._q_restored.pop(ci))
+
+    # -- SCAFFOLD --------------------------------------------------------------------------------------------------------
+    def penalty(self, i: int) -> Penalty:
+        return Penalty(y=self.scaffold.correction(i)) if self.scaffold is not None else Penalty()
+
+    def note_local_steps(self, steps: Sequence[int], lr: Optional[float]) -> None:
+        if self.scaffold is not None:
+            self.scaffold.note_local_steps(steps, lr)
+
+    def _scaffold_round(self) -> None:
+        """Steps 1-3 of the control variates, launched before the model aggregation (which overwrites ``z``)."""
+        if self.scaffold is not None:
+            self.scaffold.end_round(self.xs, self.z)
+
+    def _with_scaffold(self, metrics: Dict[str, float]) -> Dict[str, float]:
+        if self.scaffold is not None:
+            metrics["scaffold_corr"] = self.scaffold.corr_norm()
+        return metrics
+
+    def _scaffold_state(self) -> Dict[str, object]:
+        if self.scaffold is None:
+            return {}
+        return {"scaffold": True, **self.scaffold.state()}
+
+    def _check_scaffold_state(self, st: Dict[str, object]) -> None:
+        got, want = bool(st.get("scaffold", False)), self.scaffold is not None
+        if got != want:
+            raise ValueError("resume record was written with scaffold %r, this run uses scaffold %r" % (got, want))
+        if self.scaffold is not None:
+            self.scaffold.load_state(st)
 
     # -- client sampling -------------------------------------------------------------------------------------------------
     def round_participants(self) -> List[int]:
@@ -395,16 +448,18 @@ class FedAvg(Strategy):
         return metrics
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
+        self._scaffold_round()
         if self.aggregator == "mean":
             dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw(), **self._q_kw(),
                                         **self._samp_kw(), **self._sa_kw())
         else:
             dual_sq = self.coll.robust_(self.xs, self.z, self.aggregator, self.trim_b)
-        return self._with_sa(self._with_samp(self._with_q(self._with_dp(
-            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))))
+        return self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
+            self._scaffold_round()
             if self.aggregator == "mean":
                 self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw(), **self._q_kw(), **self._samp_kw(),
                                          **self._sa_kw())
@@ -416,8 +471,8 @@ class FedAvg(Strategy):
     def aggregate_end(self, token) -> Dict[str, float]:
         if token[0] == "done":
             return token[1]
-        return self._with_sa(self._with_samp(self._with_q(self._with_dp(
-            {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]}))))
+        return self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]})))))
 
     def _robust_state(self) -> Dict[str, object]:
         return {} if self.aggregator == "mean" else {"aggregator": self.aggregator, "trim_b": self.trim_b}
@@ -445,7 +500,7 @@ class FedAvg(Strategy):
 
     def state(self) -> Dict[str, object]:
         return {"z": self.z, **self._robust_state(), **self._dp_state(), **self._q_state(), **self._samp_state(),
-                **self._sa_state()}
+                **self._sa_state(), **self._scaffold_state()}
 
     def load_state(self, st: Dict[str, object]) -> None:
         self._check_robust_state(st)
@@ -453,6 +508,7 @@ class FedAvg(Strategy):
         self._check_q_state(st)
         self._check_samp_state(st)
         self._check_sa_state(st)
+        self._check_scaffold_state(st)
         self.z.copy_(st["z"].to(self.z.device))
 
 
@@ -478,20 +534,22 @@ class FedOpt(FedAvg):
     (``client_n``) the participants' sample-weighted mean replaces the mean in ``d``; the server model at the start of a
     visit stays the unsampled mean of the (equal) replicas and does not advance the sampling counter.  With secure
     aggregation (``secagg``) ``d`` is the decoded sum of the masked updates, and the server model at the start of a visit
-    is the replicas' common value."""
+    is the replicas' common value.  With SCAFFOLD (``scaffold``) the control variates are updated before the server step,
+    exactly as for FedAvg; ``avgm`` with ``momentum 0`` and ``lr eta_g`` is the paper's global step size ``eta_g``."""
 
     name = "fedopt"
+    forms_server_model = True
 
     def __init__(self, collective, topo, kind: str = "adam", lr: float = 0.0, momentum: float = 0.9, beta1: float = 0.9,
                  beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1,
                  dp_clip: float = 0.0, dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
                  compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None,
-                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None):
+                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None, scaffold: bool = False):
         from ..config import check_server_opt
         from ..parallel.collective import FEDOPT_KINDS
 
         super().__init__(collective, topo, aggregator, trim_fraction, dp_clip, dp_noise, dp_delta, seed, compress_bits,
-                         compress_ef, clients_per_round, client_n, secagg, secagg_clip, secagg_keys)
+                         compress_ef, clients_per_round, client_n, secagg, secagg_clip, secagg_keys, scaffold)
         if kind not in FEDOPT_KINDS:
             raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
         check_server_opt(kind, lr, momentum, beta1, beta2, tau)
@@ -527,13 +585,15 @@ class FedOpt(FedAvg):
         return {} if self.aggregator == "mean" else {"agg": self.aggregator, "trim_b": self.trim_b}
 
     def aggregate(self, nadmm: int) -> Dict[str, float]:
+        self._scaffold_round()
         dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
                                     **self._q_kw(), **self._samp_kw(), **self._sa_kw())
-        return self._with_sa(self._with_samp(self._with_q(self._with_dp(
-            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))))
+        return self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
+            self._scaffold_round()
             self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
                                      **self._q_kw(), **self._samp_kw(), **self._sa_kw())
             return ("pending", self.N)
@@ -547,7 +607,7 @@ class FedOpt(FedAvg):
         ms.update(self.ms)
         vs.update(self.vs)
         return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state(), **self._dp_state(),
-                **self._q_state(), **self._samp_state(), **self._sa_state()}
+                **self._q_state(), **self._samp_state(), **self._sa_state(), **self._scaffold_state()}
 
     def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
         self.ms[ci].copy_(m.to(self.ms[ci].device))
@@ -562,6 +622,7 @@ class FedOpt(FedAvg):
         self._check_q_state(st)
         self._check_samp_state(st)
         self._check_sa_state(st)
+        self._check_scaffold_state(st)
         self.z.copy_(st["z"].to(self.z.device))
         vs = st.get("v") or {}
         for ci, m in (st.get("m") or {}).items():

@@ -34,6 +34,15 @@ worker uploads its block update ``x_k - z`` as int32 fixed-point codes of ``clam
 ChaCha20 keystreams that cancel in the sum (``algo/secagg.py``), so the server learns only the sum.  The pair keys are
 derived from ``--seed`` in place of a key agreement: whoever knows the seed can unmask.  Round metrics gain
 ``sa_frac_bits`` and ``sa_clipped``.
+
+``--scaffold`` (with ``--optimizer sgd``) adds SCAFFOLD control variates (Karimireddy et al. 2020, option II) against
+client drift on skewed shards, with or without a server optimizer, client sampling or a Dirichlet partition: every local
+SGD step adds ``c - c_i`` to the gradient, and every round updates the workers' ``c_i`` from their model change
+``(z - x_i) / (tau_i lr)``, averages ``c`` over all K workers, then aggregates the model as without it
+(``algo/scaffold.py``).  With momentum that model change is about ``1 / (1 - momentum)`` times the mean gradient; it is
+used unchanged, as in most implementations.  Simulated Byzantine workers (``--byzantine``) attack before the control
+variates are updated, so an attacker's ``c_i`` comes from its attacked model.  Round metrics gain ``scaffold_corr``
+(mean ``||c - c_i||`` over the process' workers).
 """
 from __future__ import annotations
 
@@ -57,6 +66,8 @@ def make_strategy(cfg: Config, coll, topo, client_n=None):
         robust.update(clients_per_round=cfg.clients_per_round, client_n=client_n or [1] * cfg.K, seed=cfg.seed)
     if cfg.secagg:
         robust.update(secagg=True, secagg_clip=cfg.secagg_clip, seed=cfg.seed)
+    if cfg.scaffold:
+        robust.update(scaffold=True)
     if cfg.server_opt == "none":
         return FedAvg(coll, topo, **robust)
     return FedOpt(coll, topo, cfg.server_opt, cfg.server_lr, cfg.server_momentum, cfg.server_beta1, cfg.server_beta2,

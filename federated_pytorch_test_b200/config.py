@@ -316,6 +316,25 @@ def check_secagg(secagg: bool, secagg_clip: float, K: int, aggregator: str, dp_c
                          % what)
 
 
+def check_scaffold(scaffold: bool, aggregator: str, dp_clip: float, compress_bits: int, secagg: bool,
+                   optimizer: Optional[str] = None) -> None:
+    """Raise ``ValueError`` unless the SCAFFOLD settings of :class:`FederatedConfig` are valid.  ``optimizer`` None: not
+    checked (the aggregation strategy does not know the client optimizer)."""
+    if not scaffold:
+        return
+    if optimizer is not None and optimizer != "sgd":
+        raise ValueError("scaffold needs optimizer 'sgd' (its control-variate update assumes SGD local steps), got "
+                         "optimizer %r" % (optimizer,))
+    if aggregator != "mean":
+        raise ValueError("scaffold needs aggregator 'mean' (the control variates are averaged), got aggregator %r"
+                         % (aggregator,))
+    for name, val, on in (("dp_clip", dp_clip, dp_clip > 0.0), ("compress_bits", compress_bits, bool(compress_bits)),
+                          ("secagg", secagg, bool(secagg))):
+        if on:
+            raise ValueError("scaffold cannot be combined with %s (the control-variate update needs the workers' models "
+                             "as trained, which %s changes), got %s %r" % (name, name, name, val))
+
+
 @dataclass
 class FederatedConfig(CommonConfig):
     lambda1: float = 0.0001
@@ -350,6 +369,8 @@ class FederatedConfig(CommonConfig):
     # masked with pairwise ChaCha20 keystreams that cancel in the sum (algo/secagg.py); pair keys are derived from --seed
     secagg: bool = False
     secagg_clip: float = 1.0        # R
+    # SCAFFOLD control variates (algo/scaffold.py): every SGD step adds c - c_i to the gradient, which corrects client drift
+    scaffold: bool = False
 
     def __post_init__(self):
         check_server_opt(self.server_opt, self.server_lr, self.server_momentum, self.server_beta1, self.server_beta2,
@@ -362,6 +383,7 @@ class FederatedConfig(CommonConfig):
         check_sampling(self.clients_per_round, self.K, self.partition, self.aggregator, self.dp_clip, self.compress_bits)
         check_secagg(self.secagg, self.secagg_clip, self.K, self.aggregator, self.dp_clip, self.compress_bits,
                      self.clients_per_round, self.partition)
+        check_scaffold(self.scaffold, self.aggregator, self.dp_clip, self.compress_bits, self.secagg, self.optimizer)
 
 
 @dataclass

@@ -951,6 +951,62 @@ void dp_clip(std::vector<Tensor> xs, Tensor z, double bound, Tensor stats, int64
   fb::dp_clip_launch(a, cur_stream());
 }
 
+// SCAFFOLD control variates of the local replicas; see ScaffoldArgs.
+static fb::ScaffoldArgs scaffold_args(const std::vector<Tensor>& cs, const Tensor& c, const char* name) {
+  TORCH_CHECK(!cs.empty() && cs.size() <= (size_t)fb::COMM_MAX_LOCAL, name, ": 1 to ", fb::COMM_MAX_LOCAL, " replicas");
+  CHECK_F32_CUDA(c); CHECK_CONTIG(c);
+  fb::ScaffoldArgs a{};
+  a.n = (int)c.numel(); a.n_local = (int)cs.size();
+  for (int j = 0; j < a.n_local; ++j) {
+    CHECK_F32_CUDA(cs[j]); CHECK_CONTIG(cs[j]);
+    TORCH_CHECK(cs[j].numel() == a.n, name, ": every vector must have c's length");
+    a.ci[j] = const_cast<float*>(fptr(cs[j]));
+  }
+  a.c = fptr(c);
+  return a;
+}
+static void check_vec4(const std::vector<Tensor>& ts, const char* name) {
+  for (const Tensor& t : ts)
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, name, ": vectors must start at a 16-byte boundary");
+}
+void scaffold_cv(std::vector<Tensor> cs, std::vector<Tensor> xs, Tensor c, Tensor z, std::vector<double> scales) {
+  fb::ScaffoldArgs a = scaffold_args(cs, c, "scaffold_cv");
+  TORCH_CHECK(xs.size() == cs.size() && scales.size() == cs.size(), "scaffold_cv: one x and one scale per c_i");
+  CHECK_F32_CUDA(z); CHECK_CONTIG(z);
+  TORCH_CHECK(z.numel() == a.n, "scaffold_cv: every vector must have c's length");
+  for (int j = 0; j < a.n_local; ++j) {
+    CHECK_F32_CUDA(xs[j]); CHECK_CONTIG(xs[j]);
+    TORCH_CHECK(xs[j].numel() == a.n, "scaffold_cv: every vector must have c's length");
+    a.x[j] = fptr(xs[j]);
+    a.scale[j] = (float)scales[j];
+  }
+  a.z = fptr(z);
+  check_vec4(cs, "scaffold_cv"); check_vec4(xs, "scaffold_cv"); check_vec4({c, z}, "scaffold_cv");
+  c10::cuda::CUDAGuard guard(c.device());
+  fb::scaffold_cv_launch(a, cur_stream());
+}
+int64_t scaffold_corr_blocks(int64_t n) { return fb::scaffold_corr_blocks((int)n); }
+void scaffold_corr(std::vector<Tensor> cs, std::vector<Tensor> ds, Tensor c, Tensor norm_sq, Tensor ws, Tensor tickets) {
+  fb::ScaffoldArgs a = scaffold_args(cs, c, "scaffold_corr");
+  TORCH_CHECK(ds.size() == cs.size(), "scaffold_corr: one d_i per c_i");
+  for (int j = 0; j < a.n_local; ++j) {
+    CHECK_F32_CUDA(ds[j]); CHECK_CONTIG(ds[j]);
+    TORCH_CHECK(ds[j].numel() == a.n, "scaffold_corr: every vector must have c's length");
+    a.d[j] = fptr_mut(ds[j]);
+  }
+  CHECK_F32_CUDA(norm_sq); CHECK_F32_CUDA(ws);
+  TORCH_CHECK(tickets.is_cuda() && tickets.scalar_type() == torch::kInt32, "scaffold_corr: tickets must be CUDA int32");
+  TORCH_CHECK(norm_sq.numel() >= a.n_local && tickets.numel() >= a.n_local &&
+                  ws.numel() >= (int64_t)a.n_local * fb::scaffold_corr_blocks(a.n),
+              "scaffold_corr: norm_sq / tickets need one entry per replica, ws n_local * scaffold_corr_blocks(n) floats");
+  check_vec4(cs, "scaffold_corr"); check_vec4(ds, "scaffold_corr"); check_vec4({c}, "scaffold_corr");
+  a.ws = fptr_mut(ws);
+  a.tickets = reinterpret_cast<unsigned int*>(tickets.data_ptr<int>());
+  a.norm_sq = fptr_mut(norm_sq);
+  c10::cuda::CUDAGuard guard(c.device());
+  fb::scaffold_corr_launch(a, cur_stream());
+}
+
 // Barzilai-Borwein update (consensus_multi.py:242-278) as one kernel; see BBArgs.
 void bb_update(std::vector<Tensor> xs, std::vector<Tensor> ys, std::vector<Tensor> yhat0s, std::vector<Tensor> x0s, Tensor z,
                std::vector<int64_t> workers, int64_t K, Tensor rho_dev, Tensor log, Tensor scratch, Tensor out,
@@ -1017,6 +1073,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sgd_prox", &sgd_prox);
   m.def("grad_norm_blocks", &grad_norm_blocks);
   m.def("grad_norm", &grad_norm);
+  m.def("scaffold_cv", &scaffold_cv);
+  m.def("scaffold_corr_blocks", &scaffold_corr_blocks);
+  m.def("scaffold_corr", &scaffold_corr);
   m.def("bump_step", &bump_step);
   m.def("l1_l2", &l1_l2);
   m.def("make_pair", &make_pair);

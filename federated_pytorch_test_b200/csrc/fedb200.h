@@ -347,6 +347,27 @@ constexpr int DP_CLIPPED = DP_NORM + COMM_MAX_LOCAL;
 constexpr int DP_STATS_FLOATS = DP_CLIPPED + COMM_MAX_LOCAL;
 void dp_clip_launch(const DPClipArgs& args, cudaStream_t s);
 
+// SCAFFOLD control variates (flat_kernels.cu), one launch per step for all local replicas j (blockIdx.y = j):
+//  * scaffold_cv:   c_j <- (c_j - c) + s_j (z - x_j) for the replicas with s_j != 0 (s_j = 0: sat out, not written);
+//  * scaffold_corr: d_j <- c - c_j for every replica, and norm_sq[j] = ||d_j||^2 summed in a fixed order (per-CTA partials
+//    in ws[j * scaffold_corr_blocks(n) + cta], the last CTA of replica j, by its ticket, sums them in CTA order and
+//    resets the ticket).  No floating-point atomics: the same bits on every run.
+struct ScaffoldArgs {
+  int n, n_local;
+  float* ci[COMM_MAX_LOCAL];         // c_j (cv: in/out; corr: in)
+  const float* x[COMM_MAX_LOCAL];    // cv: x_j after the round's local steps
+  float* d[COMM_MAX_LOCAL];          // corr: the correction d_j (out)
+  float scale[COMM_MAX_LOCAL];       // cv: s_j = 1 / (tau_j lr), 0 = sat out
+  const float* c;                    // the server control variate
+  const float* z;                    // cv: the server model the round started from
+  float* ws;                         // corr: [n_local * scaffold_corr_blocks(n)] partials
+  unsigned int* tickets;             // corr: [n_local], zero between launches
+  float* norm_sq;                    // corr: [n_local]
+};
+int scaffold_corr_blocks(int n);
+void scaffold_cv_launch(const ScaffoldArgs& args, cudaStream_t s);
+void scaffold_corr_launch(const ScaffoldArgs& args, cudaStream_t s);
+
 // Barzilai-Borwein / spectral penalty update of consensus ADMM as ONE kernel (SURVEY G20, X4): six dots per worker
 // straight from (x, y, yhat0, x0, z), rows exchanged through the control pads, the reference's sequential
 // accept/reject rule replayed identically on every rank, rho written to device memory, yhat0 / x0 carried forward.

@@ -2,6 +2,8 @@
 //  * adam_prox_kernel    : Adam update with the FedProx / augmented-Lagrangian / elastic-net gradient folded in
 //  * sgd_prox_kernel     : SGD (momentum, Nesterov, weight decay) update with the same gradient folded in
 //  * grad_norm_kernel    : the block's gradient norm for client gradient-norm clipping, reduced in a fixed order
+//  * scaffold_cv_kernel, scaffold_corr_kernel : SCAFFOLD's per-round control-variate update and correction, all local
+//    replicas per launch
 //  * l1_l2, make_pair, welford, penalty_value, penalty_grad, multi_dot : one pass + in-kernel reductions,
 //    results stay on the device (callers read several scalars with ONE D2H copy)
 //  * lbfgs_two_loop_kernel: the whole two-loop recursion (2k+2 dependent passes) as ONE cooperative persistent
@@ -286,6 +288,90 @@ int grad_norm_blocks(int n) { return grid_for(n); }
 void grad_norm(const float* g, int n, float* ws, unsigned int* ticket, float clip, cudaStream_t s) {
   grad_norm_kernel<<<grid_for(n), 256, 0, s>>>(g, n, ws, ticket, clip);
   check_launch("grad_norm");
+}
+
+// SCAFFOLD control variates (see ScaffoldArgs).  The update is rounded operation by operation (no contraction into an
+// FMA), so it equals the ATen expression (c_j - c) + s_j * (z - x_j) bit for bit.
+__device__ __forceinline__ float scaffold_cv1(float ci, float c, float z, float x, float s) {
+  return __fadd_rn(__fsub_rn(ci, c), __fmul_rn(s, __fsub_rn(z, x)));
+}
+
+__global__ void __launch_bounds__(256) scaffold_cv_kernel(const ScaffoldArgs a) {
+  const int j = blockIdx.y;
+  const float s = a.scale[j];
+  if (s == 0.f) return;                                    // sat out: c_j keeps its bits
+  float* __restrict__ ci = a.ci[j];
+  const float* __restrict__ x = a.x[j];
+  const float* __restrict__ c = a.c;
+  const float* __restrict__ z = a.z;
+  const int n4 = a.n >> 2;
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    float4 v = reinterpret_cast<float4*>(ci)[i];
+    const float4 cv = __ldg(reinterpret_cast<const float4*>(c) + i);
+    const float4 zv = __ldg(reinterpret_cast<const float4*>(z) + i);
+    const float4 xv = __ldg(reinterpret_cast<const float4*>(x) + i);
+    v.x = scaffold_cv1(v.x, cv.x, zv.x, xv.x, s);
+    v.y = scaffold_cv1(v.y, cv.y, zv.y, xv.y, s);
+    v.z = scaffold_cv1(v.z, cv.z, zv.z, xv.z, s);
+    v.w = scaffold_cv1(v.w, cv.w, zv.w, xv.w, s);
+    reinterpret_cast<float4*>(ci)[i] = v;
+  }
+  for (int i = (n4 << 2) + blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride)
+    ci[i] = scaffold_cv1(ci[i], c[i], z[i], x[i], s);
+}
+
+__global__ void __launch_bounds__(256) scaffold_corr_kernel(const ScaffoldArgs a) {
+  __shared__ float sm[32];
+  __shared__ bool last;
+  const int j = blockIdx.y;
+  const float* __restrict__ ci = a.ci[j];
+  const float* __restrict__ c = a.c;
+  float* __restrict__ d = a.d[j];
+  float acc[1] = {0.f};
+  const int n4 = a.n >> 2;
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float4 cv = __ldg(reinterpret_cast<const float4*>(c) + i);
+    const float4 iv = __ldg(reinterpret_cast<const float4*>(ci) + i);
+    const float4 dv = make_float4(cv.x - iv.x, cv.y - iv.y, cv.z - iv.z, cv.w - iv.w);
+    reinterpret_cast<float4*>(d)[i] = dv;
+    acc[0] += dv.x * dv.x + dv.y * dv.y + dv.z * dv.z + dv.w * dv.w;
+  }
+  for (int i = (n4 << 2) + blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
+    const float di = c[i] - ci[i];
+    d[i] = di;
+    acc[0] += di * di;
+  }
+  block_reduce<1>(acc, sm);
+  float* partials = a.ws + static_cast<size_t>(j) * gridDim.x;
+  if (threadIdx.x == 0) {
+    partials[blockIdx.x] = acc[0];
+    __threadfence();                                       // the partial is visible before the ticket is drawn
+    last = atomicAdd(a.tickets + j, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  float tot[1] = {0.f};
+  for (int i = threadIdx.x; i < gridDim.x; i += blockDim.x) tot[0] += __ldcg(partials + i);
+  block_reduce<1>(tot, sm);
+  if (threadIdx.x == 0) {
+    a.norm_sq[j] = tot[0];
+    a.tickets[j] = 0u;
+  }
+}
+
+int scaffold_corr_blocks(int n) { return grid_for(n); }
+
+void scaffold_cv_launch(const ScaffoldArgs& args, cudaStream_t s) {
+  scaffold_cv_kernel<<<dim3(grid_for(args.n), args.n_local), 256, 0, s>>>(args);
+  check_launch("scaffold_cv");
+}
+
+void scaffold_corr_launch(const ScaffoldArgs& args, cudaStream_t s) {
+  scaffold_corr_kernel<<<dim3(scaffold_corr_blocks(args.n), args.n_local), 256, 0, s>>>(args);
+  check_launch("scaffold_corr");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -15,8 +15,8 @@ Kernel inventory (SURVEY §2.10 ids):
   G5  linear_tf32          wgmma GEMM with bias+ELU epilogue
   G9  cross_entropy        fused log-softmax/NLL fwd, softmax-minus-onehot bwd
   G10 vae_loss             single fused reduction fwd, elementwise bwd
-  G14-16 flat ops          adam_prox (Adam / AdamW), sgd_prox, grad_norm (clipping), penalty, L-BFGS algebra
-                           (see flatops.py)
+  G14-16 flat ops          adam_prox (Adam / AdamW), sgd_prox, grad_norm (clipping), penalty, L-BFGS algebra,
+                           scaffold_cv / scaffold_corr (SCAFFOLD control variates; see flatops.py)
   G22 normalize_u8         uint8 NHWC -> normalised float, layout change fused
       augment_normalize_u8 the same with batch gather + random padded crop + horizontal flip fused (training augmentation)
       mix_normalize_u8     the same (crop + flip optional) with the mixup blend / CutMix paste of sample n-1-i fused
@@ -103,6 +103,23 @@ def grad_norm(g, ws, ticket, clip_norm: float) -> None:
     ``GRAD_NORM_HEADER + grad_norm_blocks(g.numel())`` floats; ``ticket`` is one int32, zero between launches (the kernel
     resets it).  One launch and no host read, so it can be graph-captured."""
     ext().grad_norm(g, ws, ticket, clip_norm)
+
+
+def scaffold_cv(cs, xs, c, z, scales) -> None:
+    """SCAFFOLD step 1 for all local replicas in one launch: ``c_j <- (c_j - c) + s_j (z - x_j)`` where ``s_j != 0``."""
+    ext().scaffold_cv(list(cs), list(xs), c, z, [float(s) for s in scales])
+
+
+def scaffold_corr_blocks(n: int) -> int:
+    """CTAs per replica (= partial sums per replica) of :func:`scaffold_corr` over ``n`` values."""
+    return int(ext().scaffold_corr_blocks(int(n)))
+
+
+def scaffold_corr(cs, ds, c, norm_sq, ws, tickets) -> None:
+    """SCAFFOLD step 3 for all local replicas in one launch: ``d_j <- c - c_j`` and ``norm_sq[j] = ||d_j||^2`` in a
+    fixed summation order.  ``ws`` holds ``len(cs) * scaffold_corr_blocks(n)`` floats, ``tickets`` ``len(cs)`` int32 that
+    are zero between launches (the kernel resets them)."""
+    ext().scaffold_corr(list(cs), list(ds), c, norm_sq, ws, tickets)
 
 
 def bump_step(step: torch.Tensor) -> None:

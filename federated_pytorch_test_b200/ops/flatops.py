@@ -328,6 +328,50 @@ def penalty_value(x, z=None, y=None, rho: float = 0.0, lambda1: float = 0.0, lam
     return val
 
 
+# ----------------------------------------------------------------------------
+# SCAFFOLD control variates (algo/scaffold.py), all local replicas per call
+# ----------------------------------------------------------------------------
+def scaffold_workspace(n: int, n_local: int, device) -> Tuple[torch.Tensor, Optional[torch.Tensor], Optional[torch.Tensor]]:
+    """``(norm_sq, ws, tickets)`` of :func:`scaffold_corr_`: one squared norm per replica, and on CUDA the per-CTA partials
+    and the replicas' tickets (``None`` on the ATen path)."""
+    norm_sq = torch.zeros(n_local, dtype=torch.float32, device=device)
+    if torch.device(device).type == "cuda" and _cuda(norm_sq):
+        from . import cuda_ops
+
+        return (norm_sq, torch.zeros(n_local * cuda_ops.scaffold_corr_blocks(n), dtype=torch.float32, device=device),
+                torch.zeros(n_local, dtype=torch.int32, device=device))
+    return norm_sq, None, None
+
+
+def scaffold_cv_(cs: List[torch.Tensor], xs: List[torch.Tensor], c: torch.Tensor, z: torch.Tensor,
+                 scales: List[float]) -> None:
+    """SCAFFOLD step 1, in place: ``c_j <- (c_j - c) + s_j (z - x_j)`` for every ``j`` with ``s_j != 0``; the others are
+    not written.  Each operation is rounded to float32, so the CUDA kernel gives the same bits."""
+    if _cuda(c):
+        from . import cuda_ops
+
+        cuda_ops.scaffold_cv(cs, xs, c, z, scales)
+        return
+    for ci, x, s in zip(cs, xs, scales):
+        if s != 0.0:
+            ci.copy_((ci - c) + torch.tensor(s, dtype=torch.float32) * (z - x))
+
+
+def scaffold_corr_(cs: List[torch.Tensor], ds: List[torch.Tensor], c: torch.Tensor, work) -> torch.Tensor:
+    """SCAFFOLD step 3, in place: ``d_j <- c - c_j`` for every ``j``; returns ``norm_sq`` of ``work``
+    (:func:`scaffold_workspace`) holding ``||d_j||^2`` (summed in float64 on the ATen path)."""
+    norm_sq, ws, tickets = work
+    if _cuda(c):
+        from . import cuda_ops
+
+        cuda_ops.scaffold_corr(cs, ds, c, norm_sq, ws, tickets)
+        return norm_sq
+    for j, (ci, d) in enumerate(zip(cs, ds)):
+        torch.sub(c, ci, out=d)
+        norm_sq[j] = d.double().square().sum().float()
+    return norm_sq
+
+
 def multi_dot(pairs) -> torch.Tensor:
     """Several dot products of equal-length vectors in one pass -> 1-D tensor (SURVEY G20)."""
     if pairs and _cuda(pairs[0][0]):

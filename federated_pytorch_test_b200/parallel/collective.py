@@ -338,6 +338,12 @@ class TorchCollective:
         return acc
 
     @torch.no_grad()
+    def average_(self, xs: List[torch.Tensor], z: torch.Tensor) -> None:
+        """In place ``z <- mean_k x_k`` over all K workers, nothing written back and no residual read by the host (the
+        SCAFFOLD server control variate)."""
+        self.fedavg_(xs, z, write_back=False)
+
+    @torch.no_grad()
     def fedavg_(self, xs: List[torch.Tensor], z: torch.Tensor, write_back: bool = True,
                 dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
                 sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> torch.Tensor:

@@ -543,6 +543,13 @@ class FusedCollective(TorchCollective):
 
     # -- operators ----------------------------------------------------------------------
     @torch.no_grad()
+    def average_(self, xs, z) -> None:
+        """``z <- mean_k x_k``: one launch of FedAvg without write-back whose record nobody reads, so it must not set
+        ``_out_pending`` (a following synchronous round would read this launch's pinned copy instead of its own).  A
+        time-out is still raised: ``OUT_STATUS`` is sticky, and the next round's record reports it."""
+        self._launch(1, xs, None, z, 0.0)
+
+    @torch.no_grad()
     def fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
                 compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None,
                 secagg: Optional[SecAggRound] = None):
