@@ -63,8 +63,22 @@ Tensor l1_l2(Tensor g) {
   fb::l1_l2(fptr(g), (int)g.numel(), fptr_mut(out), cur_stream());
   return out;
 }
+// x is read or written element for element alongside ref: the same dtype, device and length, contiguous.  The messages
+// are string literals only: with the torch this extension is built against, a TORCH_CHECK message formatted from
+// run-time values (c10::str) crashes the process instead of raising.
+#define CHECK_LIKE(x, ref)                                                                                     \
+  do {                                                                                                         \
+    CHECK_F32_CUDA(x); CHECK_CONTIG(x);                                                                        \
+    TORCH_CHECK((x).device() == (ref).device(), #x " must be on the device of " #ref);                        \
+    TORCH_CHECK((x).numel() == (ref).numel(), #x " must have the length of " #ref);                           \
+  } while (0)
+#define CHECK_OPT_LIKE(x, ref)                                                                                 \
+  do {                                                                                                         \
+    if ((x).has_value() && (x)->defined()) CHECK_LIKE((*x), ref);                                              \
+  } while (0)
+
 std::vector<Tensor> make_pair(Tensor g, Tensor gprev, Tensor d, double t, double trust) {
-  CHECK_F32_CUDA(g); CHECK_CONTIG(g); CHECK_CONTIG(gprev); CHECK_CONTIG(d);
+  CHECK_F32_CUDA(g); CHECK_CONTIG(g); CHECK_LIKE(gprev, g); CHECK_LIKE(d, g);
   c10::cuda::CUDAGuard guard(g.device());
   auto y = torch::empty_like(g), s = torch::empty_like(g);
   auto out = torch::empty({3}, g.options());
@@ -72,7 +86,8 @@ std::vector<Tensor> make_pair(Tensor g, Tensor gprev, Tensor d, double t, double
   return {y, s, out};
 }
 Tensor welford(Tensor g, Tensor mean, Tensor m2, int64_t n_iter) {
-  CHECK_F32_CUDA(g);
+  CHECK_F32_CUDA(g); CHECK_CONTIG(g); CHECK_LIKE(mean, g); CHECK_LIKE(m2, g);
+  TORCH_CHECK(n_iter >= 1, "welford: n_iter must be >= 1");
   c10::cuda::CUDAGuard guard(g.device());
   auto out = torch::empty({1}, g.options());
   fb::welford(fptr(g), fptr_mut(mean), fptr_mut(m2), (int)g.numel(), 1.0f / (float)n_iter, fptr_mut(out), cur_stream());
@@ -80,13 +95,15 @@ Tensor welford(Tensor g, Tensor mean, Tensor m2, int64_t n_iter) {
 }
 Tensor penalty_value(Tensor x, c10::optional<Tensor> z, c10::optional<Tensor> y, double rho, double l1, double l2) {
   CHECK_F32_CUDA(x); CHECK_CONTIG(x);
+  CHECK_OPT_LIKE(z, x); CHECK_OPT_LIKE(y, x);
   c10::cuda::CUDAGuard guard(x.device());
   auto out = torch::empty({1}, x.options());
   fb::penalty_value(fptr(x), opt_ptr(z), opt_ptr(y), (float)rho, (float)l1, (float)l2, (int)x.numel(), fptr_mut(out), cur_stream());
   return out;
 }
 void penalty_grad(Tensor g, Tensor x, c10::optional<Tensor> z, c10::optional<Tensor> y, double rho, double l1, double l2) {
-  CHECK_F32_CUDA(g); CHECK_CONTIG(g); CHECK_CONTIG(x);
+  CHECK_F32_CUDA(g); CHECK_CONTIG(g); CHECK_LIKE(x, g);
+  CHECK_OPT_LIKE(z, g); CHECK_OPT_LIKE(y, g);
   c10::cuda::CUDAGuard guard(g.device());
   fb::penalty_grad(fptr_mut(g), fptr(x), opt_ptr(z), opt_ptr(y), (float)rho, (float)l1, (float)l2, (int)g.numel(), cur_stream());
 }
@@ -95,7 +112,8 @@ Tensor multi_dot(std::vector<Tensor> a, std::vector<Tensor> b) {
   c10::cuda::CUDAGuard guard(a[0].device());
   std::vector<const float*> pa, pb;
   for (size_t i = 0; i < a.size(); ++i) {
-    CHECK_F32_CUDA(a[i]); CHECK_CONTIG(a[i]); CHECK_CONTIG(b[i]);
+    CHECK_F32_CUDA(a[i]); CHECK_CONTIG(a[i]); CHECK_F32_CUDA(b[i]); CHECK_CONTIG(b[i]);
+    TORCH_CHECK(a[i].device() == a[0].device() && b[i].device() == a[0].device(), "multi_dot: all vectors on one device");
     TORCH_CHECK(a[i].numel() == a[0].numel() && b[i].numel() == a[0].numel(), "multi_dot: equal lengths required");
     pa.push_back(fptr(a[i])); pb.push_back(fptr(b[i]));
   }
@@ -103,14 +121,25 @@ Tensor multi_dot(std::vector<Tensor> a, std::vector<Tensor> b) {
   fb::multi_dot(pa.data(), pb.data(), (int)a.size(), (int)a[0].numel(), fptr_mut(out), cur_stream());
   return out;
 }
-Tensor lbfgs_two_loop(Tensor Y, Tensor S, Tensor order, Tensor g, double hdiag) {
-  CHECK_F32_CUDA(Y); CHECK_CONTIG(Y); CHECK_CONTIG(S); CHECK_CONTIG(g);
-  TORCH_CHECK(order.scalar_type() == torch::kInt32 && order.is_cuda(), "order must be a CUDA int32 tensor");
+// order: the rows of Y and S to use, oldest pair first.  It is checked here and copied to the device with the call.
+Tensor lbfgs_two_loop(Tensor Y, Tensor S, std::vector<int64_t> order, Tensor g, double hdiag) {
+  CHECK_F32_CUDA(g); CHECK_CONTIG(g);
+  CHECK_F32_CUDA(Y); CHECK_CONTIG(Y); CHECK_F32_CUDA(S); CHECK_CONTIG(S);
+  TORCH_CHECK(Y.dim() == 2 && S.sizes() == Y.sizes(), "lbfgs_two_loop: Y and S must be [m, n] of one shape");
+  TORCH_CHECK(Y.device() == g.device() && S.device() == g.device(), "lbfgs_two_loop: Y, S and g on one device");
+  TORCH_CHECK(Y.size(1) == g.numel(), "lbfgs_two_loop: the rows of Y must have the length of g");
+  const int64_t m = Y.size(0);
+  const int k = (int)order.size(), n = (int)g.numel();
+  TORCH_CHECK(k >= 1 && k <= m && k <= fb::kTwoLoopMaxHist,
+              "lbfgs_two_loop: 1 to min(rows of Y, kTwoLoopMaxHist = 32) pairs");
+  for (int64_t r : order) TORCH_CHECK(r >= 0 && r < m, "lbfgs_two_loop: every order entry must be a row of Y");
+  std::vector<int> rows(order.begin(), order.end());
   c10::cuda::CUDAGuard guard(g.device());
-  const int k = (int)order.numel(), n = (int)g.numel();
+  auto dev_order = torch::tensor(rows, torch::kInt32).to(g.device());
   auto d = torch::empty_like(g);
   auto work = torch::empty({(int64_t)fb::lbfgs_two_loop_work_floats(k)}, g.options());
-  fb::lbfgs_two_loop(fptr(Y), fptr(S), order.data_ptr<int>(), k, n, (int)Y.size(1), fptr(g), (float)hdiag, fptr_mut(d), fptr_mut(work), cur_stream());
+  fb::lbfgs_two_loop(fptr(Y), fptr(S), dev_order.data_ptr<int>(), k, n, (int)Y.size(1), fptr(g), (float)hdiag, fptr_mut(d),
+                     fptr_mut(work), cur_stream());
   return d;
 }
 

@@ -107,6 +107,8 @@ void penalty_value(const float* x, const float* z, const float* y, float rho, fl
 void penalty_grad(float* g, const float* x, const float* z, const float* y, float rho, float l1, float l2, int n,
                   cudaStream_t s);
 void multi_dot(const float* const* a, const float* const* b, int npairs, int n, float* out, cudaStream_t s);
+// at most kTwoLoopMaxHist pairs (the kernel keeps the row indices in shared memory); longer histories take the ATen path
+constexpr int kTwoLoopMaxHist = 32;
 void lbfgs_two_loop(const float* Y, const float* S, const int* order, int k, int n, int ld, const float* g, float hdiag,
                     float* d, float* work, cudaStream_t s);
 size_t lbfgs_two_loop_work_floats(int k);

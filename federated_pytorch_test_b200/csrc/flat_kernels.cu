@@ -524,7 +524,7 @@ void multi_dot(const float* const* a, const float* const* b, int npairs, int n, 
 // Each dependent dot product is accumulated during the pass that produces its input vector; passes are
 // separated by a grid barrier.  work layout (floats): ro[k] | al[k] | dots[2k+2]; all zero on entry.
 // ------------------------------------------------------------------------------------------------
-constexpr int TL_MAX_HIST = 32;
+constexpr int TL_MAX_HIST = kTwoLoopMaxHist;
 
 size_t lbfgs_two_loop_work_floats(int k) { return size_t(5 * k + 4); }  // ro[k] | al[k] | dots[3k+1]
 

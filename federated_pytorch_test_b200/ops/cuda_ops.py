@@ -157,9 +157,12 @@ def multi_dot(pairs) -> torch.Tensor:
     return torch.cat(out)
 
 
+TWO_LOOP_MAX_HIST = 32  # kTwoLoopMaxHist: the most curvature pairs lbfgs_two_loop_kernel takes
+
+
 def lbfgs_two_loop(Y, S, order: Sequence[int], g, H_diag: float) -> torch.Tensor:
-    o = torch.tensor(list(order), dtype=torch.int32, device=g.device)
-    return ext().lbfgs_two_loop(Y, S, o, g, float(H_diag))
+    """``d = -H g`` over the pairs ``(Y[r], S[r])`` for ``r`` in ``order`` (oldest first), 1 to TWO_LOOP_MAX_HIST of them."""
+    return ext().lbfgs_two_loop(Y, S, [int(r) for r in order], g, float(H_diag))
 
 
 # ----------------------------------------------------------------------------

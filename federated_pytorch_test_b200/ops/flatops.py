@@ -17,7 +17,8 @@ import torch
 
 
 def _cuda(t: torch.Tensor) -> bool:
-    if not t.is_cuda:
+    """The kernels take float32 CUDA tensors; every other tensor (float64 on a GPU included) takes the ATen path."""
+    if not t.is_cuda or t.dtype != torch.float32:
         return False
     from . import functional
 
@@ -128,12 +129,14 @@ class PairHistory:
         return list(self._al)
 
     def two_loop(self, g: torch.Tensor, H_diag) -> torch.Tensor:
-        """``d = -H g`` by the two-loop recursion (lbfgsnew.py:645-659)."""
+        """``d = -H g`` by the two-loop recursion (lbfgsnew.py:645-659).  One cooperative kernel on CUDA for up to
+        ``cuda_ops.TWO_LOOP_MAX_HIST`` pairs; longer histories run the ATen recursion below."""
         k = len(self.order)
         if _cuda(g) and k > 0:
             from . import cuda_ops
 
-            return cuda_ops.lbfgs_two_loop(self.Y, self.S, self.order, g, float(H_diag))
+            if k <= cuda_ops.TWO_LOOP_MAX_HIST:
+                return cuda_ops.lbfgs_two_loop(self.Y, self.S, self.order, g, float(H_diag))
         ys, ss = self.dirs(), self.steps()
         ro, al = self._ro, self._al
         for i in range(k):

@@ -75,55 +75,6 @@ def test_adam_device_step_counter_and_plain_adam():
     torch.testing.assert_close(x, p.detach(), rtol=1e-5, atol=1e-6)
 
 
-def test_vector_reductions():
-    n = 230144 + 3
-    g, gp, d = (torch.randn(n, device=DEV) for _ in range(3))
-    l1, l2 = cuda_ops.l1_l2(g)
-    assert l1 == pytest.approx(float(g.abs().sum()), rel=1e-4) and l2 == pytest.approx(float(g.norm()), rel=1e-4)
-    y, s, ys, sn, yy = cuda_ops.make_pair(g, gp, d, 0.5, 1e-6)
-    sr = 0.5 * d
-    yr = g - gp + 1e-6 * sr
-    torch.testing.assert_close(y, yr)
-    torch.testing.assert_close(s, sr)
-    assert ys == pytest.approx(float(yr.dot(sr)), rel=1e-3, abs=1e-2) and sn == pytest.approx(float(sr.norm()), rel=1e-4)
-    assert yy == pytest.approx(float(yr.dot(yr)), rel=1e-4)
-    mean, m2 = torch.randn(n, device=DEV), torch.rand(n, device=DEV)
-    mr, m2r = mean.clone(), m2.clone()
-    tot = cuda_ops.welford_update(g, mean, m2, 7)
-    delta = g - mr
-    mr += delta / 7
-    m2r += (g - mr) * delta
-    torch.testing.assert_close(mean, mr)
-    torch.testing.assert_close(m2, m2r, rtol=1e-5, atol=1e-5)
-    assert tot == pytest.approx(float(m2r.sum()), rel=1e-4)
-    x, z = torch.randn(n, device=DEV), torch.randn(n, device=DEV)
-    FX.set_fast_path(False)
-    pv = flatops.penalty_value(x, z, g, 0.2, 1e-3, 2e-3)
-    pg = flatops.penalty_grad(x, gp, z, g, 0.2, 1e-3, 2e-3)
-    FX.set_fast_path(True)
-    assert float(cuda_ops.penalty_value(x, z, g, 0.2, 1e-3, 2e-3)) == pytest.approx(float(pv), rel=1e-4)
-    gq = gp.clone()
-    cuda_ops.penalty_grad_(gq, x, z, g, 0.2, 1e-3, 2e-3)
-    torch.testing.assert_close(gq, pg, rtol=1e-5, atol=1e-6)
-    pairs = [(g, g), (g, gp), (gp, d), (d, d), (x, z), (z, z)]
-    torch.testing.assert_close(cuda_ops.multi_dot(pairs), torch.stack([a.dot(b) for a, b in pairs]), rtol=1e-3, atol=1e-1)
-
-
-@pytest.mark.parametrize("k,n", [(1, 1000), (4, 73984), (10, 295424)])
-def test_lbfgs_two_loop_kernel(k, n):
-    hist = flatops.PairHistory(10, torch.zeros(n, device=DEV))
-    gen = torch.Generator(device=DEV).manual_seed(k)
-    for _ in range(k):
-        s = torch.randn(n, device=DEV, generator=gen)
-        hist.push(s * (1.0 + 0.1 * torch.rand(n, device=DEV, generator=gen)), s)   # y.s > 0
-    g = torch.randn(n, device=DEV, generator=gen)
-    d_fast = hist.two_loop(g, 0.7)
-    FX.set_fast_path(False)
-    d_ref = hist.two_loop(g, 0.7)
-    FX.set_fast_path(True)
-    assert rel_err(d_fast, d_ref) < 2e-4
-
-
 def test_lbfgs_on_cuda_arena_runs_and_descends():
     from federated_pytorch_test_b200.optim import LBFGSNew
     from federated_pytorch_test_b200.utils import FlatArena
