@@ -14,6 +14,9 @@ In a compressed round worker ``k`` uploads its block update ``u_k = x_k - z`` (`
 * with error feedback ``e_k <- u_k - q_k s_k``.
 
 Every step is a correctly rounded float32 operation, so the device codes and scales equal these bit for bit.
+
+Top-k sparsification (:func:`topk_select`) is the other kind of compressed update: worker ``k`` sends the ``k_sel``
+largest-magnitude coordinates of ``u_k`` unchanged, with error feedback ``e_k <- u_k - s_k``.
 """
 from __future__ import annotations
 
@@ -114,3 +117,83 @@ def unpack4(payload: np.ndarray, n: int) -> np.ndarray:
 def relative_error(err_sq: float, norm_sq: float) -> float:
     """``sqrt(sum_k ||u_k - q_k s_k||^2 / sum_k ||u_k||^2)`` (0 for an all-zero update)."""
     return math.sqrt(err_sq / norm_sq) if norm_sq > 0.0 else (0.0 if err_sq == 0.0 else math.inf)
+
+
+# ---- top-k sparsification (Stich et al. 2018; Lin et al. 2018, Deep Gradient Compression) ---------------------------
+# Worker k sends the k_sel coordinates of u = (x_k - z) + e_k with the largest sort key bits(u) & 0x7fffffff (read as
+# uint32: the magnitude order for finite values, then +-inf, then NaN), ties broken by the lower index.  The values are
+# sent unchanged; with error feedback e_k <- u - s_k (0 on the selected coordinates, u elsewhere).  The oracle of
+# csrc/comm_kernels.cu: topk_select_kernel.
+
+TOPK_TILE = 8192                       # coordinates per tile of the sparse payload (csrc: Q_TILE = COMM_THREADS * Q_SEG)
+
+
+def topk_count(n: int, r: float) -> int:
+    """``k_sel = max(1, ceil(r n))``, in float64: the coordinates one worker sends of an ``n``-coordinate block."""
+    return max(1, int(math.ceil(float(r) * float(n))))
+
+
+def topk_keys(u: np.ndarray) -> np.ndarray:
+    """The sort key of every coordinate: ``bits(u) & 0x7fffffff`` as uint32."""
+    return np.ascontiguousarray(u, dtype=np.float32).view(np.uint32) & np.uint32(0x7FFFFFFF)
+
+
+def topk_select(u: np.ndarray, k: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The sparse payload of update ``u`` (float32) with ``k`` coordinates: ``tile_offsets`` (uint32, one per tile of
+    :data:`TOPK_TILE` coordinates counted from the block start, plus the total), then per selected coordinate in ascending
+    index order its offset within its tile (``in_tile_idx``, uint16) and its value (``values``, float32, exactly ``u_i``)."""
+    u = np.ascontiguousarray(u, dtype=np.float32).reshape(-1)
+    n = u.size
+    if not 1 <= k <= n:
+        raise ValueError("top-k needs 1 <= k <= n, got k = %d at n = %d" % (k, n))
+    key = topk_keys(u)
+    thr = np.partition(key, n - k)[n - k]               # the k-th largest key
+    mask = key > thr
+    mask[np.flatnonzero(key == thr)[: k - int(mask.sum())]] = True     # ties: the lowest indices
+    sel = np.flatnonzero(mask)
+    ntiles = -(-n // TOPK_TILE)
+    counts = np.bincount(sel // TOPK_TILE, minlength=ntiles)
+    offsets = np.zeros(ntiles + 1, dtype=np.uint32)
+    offsets[1:] = np.cumsum(counts)
+    return offsets, (sel % TOPK_TILE).astype(np.uint16), u[sel].copy()
+
+
+def topk_indices(tile_offsets: np.ndarray, in_tile_idx: np.ndarray) -> np.ndarray:
+    """The block coordinates of a payload's entries."""
+    tiles = np.repeat(np.arange(tile_offsets.size - 1), np.diff(tile_offsets.astype(np.int64)))
+    return tiles * TOPK_TILE + in_tile_idx.astype(np.int64)
+
+
+def topk_payload_bytes(n: int, k: int) -> int:
+    """Bytes one worker sends for an ``n``-coordinate block with ``k`` entries: ``6 k + 4 (ceil(n / 8192) + 1)``."""
+    return 6 * int(k) + 4 * (-(-int(n) // TOPK_TILE) + 1)
+
+
+def topk_layout(n: int, k: int) -> Tuple[int, int, int, int]:
+    """``(tiles, val, idx, words)`` of the payload buffer (int32 words, ``csrc/fedb200.h: topk_layout``): the ``tiles + 1``
+    offsets from word 0, the ``k`` values from word ``val``, the ``k`` uint16 in-tile offsets (two per word, the lower
+    index in the low half) from word ``idx``; sections start at 16-byte boundaries."""
+    T = -(-int(n) // TOPK_TILE)
+    val = (T + 1 + 3) & ~3
+    idx = val + ((int(k) + 3) & ~3)
+    return T, val, idx, idx + (((int(k) + 1) // 2 + 3) & ~3)
+
+
+def topk_pack(payload: Tuple[np.ndarray, np.ndarray, np.ndarray], n: int) -> np.ndarray:
+    """The buffer words (int32) of a payload ``(tile_offsets, in_tile_idx, values)`` of an ``n``-coordinate block."""
+    offsets, idx, vals = payload
+    k = vals.size
+    T, v0, i0, words = topk_layout(n, k)
+    out = np.zeros(words, dtype=np.int32)
+    out[: T + 1] = offsets.astype(np.uint32).view(np.int32)
+    out[v0: v0 + k] = vals.astype(np.float32).view(np.int32)
+    out[i0: words].view(np.uint16)[:k] = idx
+    return out
+
+
+def topk_unpack(words: np.ndarray, n: int, k: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Inverse of :func:`topk_pack`."""
+    w = np.ascontiguousarray(words, dtype=np.int32)
+    T, v0, i0, n_words = topk_layout(n, k)
+    return (w[: T + 1].view(np.uint32).copy(), w[i0: n_words].view(np.uint16)[:k].copy(),
+            w[v0: v0 + k].view(np.float32).copy())

@@ -47,7 +47,7 @@ from ..optim.schedule import round_lr, schedule_active
 from ..parallel.topology import Topology
 from ..utils.flat import FlatArena
 from ..utils.metrics import MetricsLog, PhaseTimers, nvtx_range
-from .compress import payload_bytes
+from .compress import payload_bytes, topk_payload_bytes
 from .strategies import Penalty, Strategy
 
 BLOCK_OPTIMIZERS = (BlockAdam, BlockSGD)   # fused block update: penalty in the kernel, the step graphed
@@ -597,6 +597,8 @@ class Engine:
             if W > 1:                          # compressed rounds move their payload instead of 4 bytes per coordinate
                 bits = getattr(self.strategy, "q_bits", 0)
                 nbytes = payload_bytes(N, bits) if bits else 4.0 * N
+                if getattr(self.strategy, "topk_r", 0.0):
+                    nbytes = topk_payload_bytes(N, self.strategy.topk_k)
                 out["bus_GBs"] = 2.0 * (W - 1) / W * nbytes / (out["aggregate_us"] * 1e-6) / 1e9
         out["two_shot"] = bool(getattr(self.coll, "last_two_shot", False))
         self._round_mark = {"images": self.images_seen, "t": now, "ms": {k: dict(v) for k, v in summ.items()}}

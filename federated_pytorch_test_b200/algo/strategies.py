@@ -145,6 +145,16 @@ class FedAvg(Strategy):
     ``sa_frac_bits`` (``f``) and ``sa_clipped`` (coordinates clipped, over all K); a non-finite update coordinate codes to
     0 and is reported as ``nonfinite``, so the NaN guard fires.
 
+    ``compress_topk`` ``r`` in (0, 1) sparsifies the workers' uploads (top-k with optional error feedback, Stich et al.
+    2018; ``algo/compress.py: topk_select``): with ``z`` the server model the round started from, worker ``k`` sends the
+    ``k_sel = max(1, ceil(r N))`` coordinates of ``u_k = x_k - z`` (``+ e_k`` with ``compress_ef``) with the largest
+    magnitudes, unchanged, and ``z <- z + (1/K) sum_k s_k``, written back into every replica.  With error feedback
+    ``e_k <- u_k - s_k`` persists per worker and block for the whole run, as for ``compress_bits``.  A round is two launches
+    on the fused collective (select, aggregate), and its sum does not depend on the process layout.  As with DP, ``z``
+    starts each block visit as the replicas' common value instead of 0 (Q6).  The round metrics gain ``topk_k``,
+    ``q_bytes`` (payload bytes per worker: ``6 k_sel + 4 (ceil(N / 8192) + 1)``) and ``q_rel_err``
+    (``sqrt(sum_k ||u_k - s_k||^2 / sum_k ||u_k||^2)``).
+
     ``scaffold`` adds SCAFFOLD control variates (Karimireddy et al. 2020, option II; ``algo/scaffold.py``) to SGD client
     steps: every local step of worker ``i`` adds ``d_i = c - c_i`` to its gradient (``penalty(i).y``), and every round
     first updates the ``c_i`` of the workers that trained from their model change, averages ``c`` over all K and forms the
@@ -160,14 +170,15 @@ class FedAvg(Strategy):
     def __init__(self, collective, topo, aggregator: str = "mean", trim_fraction: float = 0.1, dp_clip: float = 0.0,
                  dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
                  compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None,
-                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None, scaffold: bool = False):
+                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None, scaffold: bool = False,
+                 compress_topk: float = 0.0):
         from ..config import (check_aggregator, check_compress, check_dp, check_sampling, check_scaffold, check_secagg,
                               trim_count)
 
         super().__init__(collective, topo)
         check_aggregator(aggregator, trim_fraction, topo.K)
         check_dp(dp_clip, dp_noise, dp_delta, aggregator)
-        check_compress(compress_bits, compress_ef, dp_clip, aggregator)
+        check_compress(compress_bits, compress_ef, dp_clip, aggregator, compress_topk)
         self.aggregator = aggregator
         self.trim_b = trim_count(trim_fraction, topo.K) if aggregator == "trimmed_mean" else 0
         if aggregator != "mean" and hasattr(collective, "warm_robust"):
@@ -184,23 +195,29 @@ class FedAvg(Strategy):
             if hasattr(collective, "warm_dp"):
                 collective.warm_dp = True
         self.q_bits, self.q_ef_on = int(compress_bits), bool(compress_ef)
+        self.topk_r = float(compress_topk)
         self.q_rounds = 0                      # host mirror of the device round counter q_t
+        self.q_ef: Dict[int, List[torch.Tensor]] = {}      # block index -> error feedback per local replica
+        self._q_restored: Dict[int, torch.Tensor] = {}     # error feedback read from a resume record, installed at the visit
         if self.q_bits:
             from .compress import compress_key
 
             self.q_key = compress_key(seed)
             self.q_t = torch.zeros(1, dtype=torch.int64, device=topo.device)
             self.q_payload: List = []                          # (codes, scales) per local replica, current block
-            self.q_ef: Dict[int, List[torch.Tensor]] = {}      # block index -> error feedback per local replica
-            self._q_restored: Dict[int, torch.Tensor] = {}     # error feedback read from a resume record, installed at the visit
             if hasattr(collective, "warm_compress"):
                 collective.warm_compress = self.q_bits
+        if self.topk_r:
+            self.topk_k = 0                                    # k_sel of the current block
+            self.topk_payload: List[torch.Tensor] = []         # per local replica, current block
+            if hasattr(collective, "warm_topk"):
+                collective.warm_topk = True
         self.sampled = client_n is not None
         self.samp_rounds = 0                   # host mirror of the device round counter samp_t
         if self.sampled:
             from .sampling import sample_key
 
-            check_sampling(clients_per_round, topo.K, "dirichlet", aggregator, dp_clip, compress_bits)
+            check_sampling(clients_per_round, topo.K, "dirichlet", aggregator, dp_clip, compress_bits, compress_topk)
             if len(client_n) != topo.K or min(client_n) < 1:
                 raise ValueError("client_n needs one sample count >= 1 per worker, got %r" % (list(client_n),))
             self.samp_S = int(clients_per_round) or topo.K
@@ -220,7 +237,7 @@ class FedAvg(Strategy):
             from . import secagg as sa
 
             check_secagg(True, secagg_clip, topo.K, aggregator, dp_clip, compress_bits, clients_per_round,
-                         "dirichlet" if client_n is not None else "iid")
+                         "dirichlet" if client_n is not None else "iid", compress_topk)
             self.sa_clip = float(np.float32(secagg_clip))
             self.sa_f = sa.frac_bits(secagg_clip, topo.K)
             keys = sa.pair_keys(seed, topo.K) if secagg_keys is None else np.asarray(secagg_keys, dtype=np.uint32)
@@ -232,7 +249,7 @@ class FedAvg(Strategy):
             self.sa_payload: List[torch.Tensor] = []                 # per local replica, current block
             if hasattr(collective, "warm_secagg"):
                 collective.warm_secagg = True
-        check_scaffold(scaffold, aggregator, dp_clip, compress_bits, secagg)
+        check_scaffold(scaffold, aggregator, dp_clip, compress_bits, secagg, compress_topk=compress_topk)
         self.scaffold = None
         if scaffold:
             from .scaffold import ControlVariates
@@ -242,7 +259,8 @@ class FedAvg(Strategy):
     def begin_block(self, ci: int, N: int, xs: List[torch.Tensor]) -> None:
         super().begin_block(ci, N, xs)
         # the server model: the replicas are equal here, so a local copy suffices
-        if self.dp or self.q_bits or self.sa or (self.scaffold is not None and not self.forms_server_model):
+        if (self.dp or self.q_bits or self.topk_r or self.sa
+                or (self.scaffold is not None and not self.forms_server_model)):
             self.z.copy_(xs[0])
         if self.scaffold is not None:
             self.scaffold.begin_block(ci, xs)
@@ -250,10 +268,15 @@ class FedAvg(Strategy):
             self.sa_payload = [self.coll.payload32_like_block(x) for x in xs]
         if self.q_bits:
             self.q_payload = [self.coll.payload_like_block(x, self.q_bits) for x in xs]
-            if self.q_ef_on and ci not in self.q_ef:
-                self.q_ef[ci] = [torch.zeros_like(x) for x in xs]
-                if ci in self._q_restored:
-                    self._install_ef(ci, self._q_restored.pop(ci))
+        if self.topk_r:
+            from .compress import topk_count
+
+            self.topk_k = topk_count(N, self.topk_r)
+            self.topk_payload = [self.coll.sparse_payload_like_block(x, self.topk_k) for x in xs]
+        if (self.q_bits or self.topk_r) and self.q_ef_on and ci not in self.q_ef:
+            self.q_ef[ci] = [torch.zeros_like(x) for x in xs]
+            if ci in self._q_restored:
+                self._install_ef(ci, self._q_restored.pop(ci))
 
     # -- SCAFFOLD --------------------------------------------------------------------------------------------------------
     def penalty(self, i: int) -> Penalty:
@@ -388,15 +411,25 @@ class FedAvg(Strategy):
         for dst, src in zip(self.q_ef[ci], ef):
             dst.copy_(src.to(dst.device))
 
+    def _ef_state(self) -> Dict[str, object]:
+        """The error feedback of this process' workers; blocks restored but not visited yet keep their record."""
+        if not self.q_ef_on:
+            return {}
+        ef = dict(self._q_restored)
+        ef.update({ci: torch.stack(v) for ci, v in self.q_ef.items()})
+        return {"q_ef": ef}
+
+    def _load_ef(self, st: Dict[str, object]) -> None:
+        for ci, ef in (st.get("q_ef") or {}).items():
+            if ci in self.q_ef:
+                self._install_ef(ci, ef)
+            else:
+                self._q_restored[ci] = ef
+
     def _q_state(self) -> Dict[str, object]:
         if not self.q_bits:
             return {}
-        st: Dict[str, object] = {"compress": (self.q_bits, self.q_ef_on, self.q_key), "q_t": self.q_rounds}
-        if self.q_ef_on:                       # this process' workers; blocks restored but not visited yet keep their record
-            ef = dict(self._q_restored)
-            ef.update({ci: torch.stack(v) for ci, v in self.q_ef.items()})
-            st["q_ef"] = ef
-        return st
+        return {"compress": (self.q_bits, self.q_ef_on, self.q_key), "q_t": self.q_rounds, **self._ef_state()}
 
     def _check_q_state(self, st: Dict[str, object]) -> None:
         got = tuple(st["compress"]) if st.get("compress") is not None else None
@@ -407,11 +440,39 @@ class FedAvg(Strategy):
         if self.q_bits:
             self.q_rounds = int(st["q_t"])
             self.q_t.fill_(self.q_rounds)
-            for ci, ef in (st.get("q_ef") or {}).items():
-                if ci in self.q_ef:
-                    self._install_ef(ci, ef)
-                else:
-                    self._q_restored[ci] = ef
+            self._load_ef(st)
+
+    # -- top-k sparsified updates ------------------------------------------------------------------------------------
+    def _topk_kw(self) -> Dict[str, object]:
+        """The top-k argument of the aggregation."""
+        if not self.topk_r:
+            return {}
+        from ..parallel.collective import TopKRound
+
+        return {"topk": TopKRound(self.topk_k, self.topk_payload, self.q_ef.get(self.ci))}
+
+    def _with_topk(self, metrics: Dict[str, float]) -> Dict[str, float]:
+        if self.topk_r:
+            from .compress import relative_error, topk_payload_bytes
+
+            err, nrm = self.coll.last_q
+            metrics.update(topk_k=float(self.topk_k), q_bytes=float(topk_payload_bytes(self.N, self.topk_k)),
+                           q_rel_err=relative_error(float(err), float(nrm)))
+        return metrics
+
+    def _topk_state(self) -> Dict[str, object]:
+        if not self.topk_r:
+            return {}
+        return {"topk": (self.topk_r, self.q_ef_on), **self._ef_state()}
+
+    def _check_topk_state(self, st: Dict[str, object]) -> None:
+        got = tuple(st["topk"]) if st.get("topk") is not None else None
+        want = self._topk_state().get("topk")
+        if got != want:
+            raise ValueError("resume record holds top-k settings (compress_topk, compress_ef) %r, this run uses %r"
+                             % (got, want))
+        if self.topk_r:
+            self._load_ef(st)
 
     # -- DP -------------------------------------------------------------------------------------------------------
     def set_param_layout(self, ci: int, chunk_counts: List[int]) -> None:
@@ -451,18 +512,18 @@ class FedAvg(Strategy):
         self._scaffold_round()
         if self.aggregator == "mean":
             dual_sq = self.coll.fedavg_(self.xs, self.z, write_back=True, **self._dp_kw(), **self._q_kw(),
-                                        **self._samp_kw(), **self._sa_kw())
+                                        **self._samp_kw(), **self._sa_kw(), **self._topk_kw())
         else:
             dual_sq = self.coll.robust_(self.xs, self.z, self.aggregator, self.trim_b)
-        return self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
-            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))))
+        return self._with_topk(self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))))))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             self._scaffold_round()
             if self.aggregator == "mean":
                 self.coll.launch_fedavg_(self.xs, self.z, True, **self._dp_kw(), **self._q_kw(), **self._samp_kw(),
-                                         **self._sa_kw())
+                                         **self._sa_kw(), **self._topk_kw())
             else:
                 self.coll.launch_robust_(self.xs, self.z, self.aggregator, self.trim_b)
             return ("pending", self.N)
@@ -471,8 +532,8 @@ class FedAvg(Strategy):
     def aggregate_end(self, token) -> Dict[str, float]:
         if token[0] == "done":
             return token[1]
-        return self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
-            {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]})))))
+        return self._with_topk(self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(self.coll.read_record()[0]), 0.0)) / token[1]}))))))
 
     def _robust_state(self) -> Dict[str, object]:
         return {} if self.aggregator == "mean" else {"aggregator": self.aggregator, "trim_b": self.trim_b}
@@ -500,12 +561,13 @@ class FedAvg(Strategy):
 
     def state(self) -> Dict[str, object]:
         return {"z": self.z, **self._robust_state(), **self._dp_state(), **self._q_state(), **self._samp_state(),
-                **self._sa_state(), **self._scaffold_state()}
+                **self._sa_state(), **self._scaffold_state(), **self._topk_state()}
 
     def load_state(self, st: Dict[str, object]) -> None:
         self._check_robust_state(st)
         self._check_dp_state(st)
         self._check_q_state(st)
+        self._check_topk_state(st)
         self._check_samp_state(st)
         self._check_sa_state(st)
         self._check_scaffold_state(st)
@@ -544,12 +606,14 @@ class FedOpt(FedAvg):
                  beta2: float = 0.99, tau: float = 1e-3, aggregator: str = "mean", trim_fraction: float = 0.1,
                  dp_clip: float = 0.0, dp_noise: float = 1.0, dp_delta: float = 1e-5, seed: int = 0, compress_bits: int = 0,
                  compress_ef: bool = False, clients_per_round: int = 0, client_n: Optional[Sequence[int]] = None,
-                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None, scaffold: bool = False):
+                 secagg: bool = False, secagg_clip: float = 1.0, secagg_keys=None, scaffold: bool = False,
+                 compress_topk: float = 0.0):
         from ..config import check_server_opt
         from ..parallel.collective import FEDOPT_KINDS
 
         super().__init__(collective, topo, aggregator, trim_fraction, dp_clip, dp_noise, dp_delta, seed, compress_bits,
-                         compress_ef, clients_per_round, client_n, secagg, secagg_clip, secagg_keys, scaffold)
+                         compress_ef, clients_per_round, client_n, secagg, secagg_clip, secagg_keys, scaffold,
+                         compress_topk)
         if kind not in FEDOPT_KINDS:
             raise ValueError("server optimizer must be one of %s, got %r" % (", ".join(FEDOPT_KINDS), kind))
         check_server_opt(kind, lr, momentum, beta1, beta2, tau)
@@ -575,7 +639,7 @@ class FedOpt(FedAvg):
             if ci in self._restored:
                 self._install(ci, *self._restored.pop(ci))
         self.m, self.v = self.ms[ci], self.vs.get(ci)
-        if not (self.dp or self.q_bits or self.sa):               # (else FedAvg.begin_block copied the replicas' value)
+        if not (self.dp or self.q_bits or self.topk_r or self.sa):   # (else FedAvg.begin_block copied the replicas' value)
             self.coll.fedavg_(xs, self.z, write_back=False)      # the server model: the replicas' mean, no write-back
 
     def _hyper(self):
@@ -587,15 +651,15 @@ class FedOpt(FedAvg):
     def aggregate(self, nadmm: int) -> Dict[str, float]:
         self._scaffold_round()
         dual_sq = self.coll.fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
-                                    **self._q_kw(), **self._samp_kw(), **self._sa_kw())
-        return self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
-            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N})))))
+                                    **self._q_kw(), **self._samp_kw(), **self._sa_kw(), **self._topk_kw())
+        return self._with_topk(self._with_scaffold(self._with_sa(self._with_samp(self._with_q(self._with_dp(
+            {"dual": math.sqrt(max(float(dual_sq), 0.0)) / self.N}))))))
 
     def aggregate_begin(self, nadmm: int):
         if getattr(self.coll, "supports_async", False):
             self._scaffold_round()
             self.coll.launch_fedopt_(self.xs, self.z, self.m, self.v, *self._hyper(), **self._agg_kw(), **self._dp_kw(),
-                                     **self._q_kw(), **self._samp_kw(), **self._sa_kw())
+                                     **self._q_kw(), **self._samp_kw(), **self._sa_kw(), **self._topk_kw())
             return ("pending", self.N)
         return ("done", self.aggregate(nadmm))
 
@@ -607,7 +671,7 @@ class FedOpt(FedAvg):
         ms.update(self.ms)
         vs.update(self.vs)
         return {"z": self.z, "server_opt": self.kind, "m": ms, "v": vs, **self._robust_state(), **self._dp_state(),
-                **self._q_state(), **self._samp_state(), **self._sa_state(), **self._scaffold_state()}
+                **self._q_state(), **self._samp_state(), **self._sa_state(), **self._scaffold_state(), **self._topk_state()}
 
     def _install(self, ci: int, m: torch.Tensor, v: Optional[torch.Tensor]) -> None:
         self.ms[ci].copy_(m.to(self.ms[ci].device))
@@ -620,6 +684,7 @@ class FedOpt(FedAvg):
         self._check_robust_state(st)
         self._check_dp_state(st)
         self._check_q_state(st)
+        self._check_topk_state(st)
         self._check_samp_state(st)
         self._check_sa_state(st)
         self._check_scaffold_state(st)

@@ -21,6 +21,11 @@ optimizer): its block update ``x_k - z`` as stochastically rounded codes with on
 with error feedback (``algo/compress.py``); the new model is still broadcast in fp32.  Round metrics gain ``q_bits``,
 ``q_bytes`` and ``q_rel_err``.
 
+``--compress_topk r [--compress_ef]`` sparsifies what every worker uploads (top-k, with or without a server optimizer and
+error feedback): the ``max(1, ceil(r N))`` largest-magnitude coordinates of its block update ``x_k - z``, unchanged, with
+their indices (``algo/compress.py: topk_select``); the new model is still broadcast in fp32.  Round metrics gain
+``topk_k``, ``q_bytes`` and ``q_rel_err``.
+
 ``--clients_per_round S`` trains and averages a uniform random subset of S of the K workers in every round (FedAvg's
 partial participation, with or without a server optimizer); ``--partition dirichlet --dirichlet_alpha a`` splits the
 training set with Dirichlet label skew into unequal shards.  Either one makes the aggregate the sample-weighted mean
@@ -62,6 +67,8 @@ def make_strategy(cfg: Config, coll, topo, client_n=None):
         robust.update(dp_clip=cfg.dp_clip, dp_noise=cfg.dp_noise, dp_delta=cfg.dp_delta, seed=cfg.seed)
     if cfg.compress_bits:
         robust.update(compress_bits=cfg.compress_bits, compress_ef=cfg.compress_ef, seed=cfg.seed)
+    if cfg.compress_topk:
+        robust.update(compress_topk=cfg.compress_topk, compress_ef=cfg.compress_ef)
     if sampled_rounds(cfg.clients_per_round, cfg.K, cfg.partition):
         robust.update(clients_per_round=cfg.clients_per_round, client_n=client_n or [1] * cfg.K, seed=cfg.seed)
     if cfg.secagg:

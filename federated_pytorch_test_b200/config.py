@@ -265,7 +265,7 @@ def sampled_rounds(clients_per_round: int, K: int, partition: str) -> bool:
 
 
 def check_sampling(clients_per_round: int, K: int, partition: str, aggregator: str, dp_clip: float,
-                   compress_bits: int) -> None:
+                   compress_bits: int, compress_topk: float = 0.0) -> None:
     """Raise ``ValueError`` unless the client-sampling settings of :class:`FederatedConfig` are valid."""
     if not 0 <= clients_per_round <= K:
         raise ValueError("clients_per_round must lie in [0, K] = [0, %d] (0 = all), got %r" % (K, clients_per_round))
@@ -279,14 +279,27 @@ def check_sampling(clients_per_round: int, K: int, partition: str, aggregator: s
                          "subsampling), got dp_clip %r" % (what, dp_clip))
     if compress_bits:
         raise ValueError("%s cannot be combined with compress_bits, got compress_bits %r" % (what, compress_bits))
+    if compress_topk:
+        raise ValueError("%s cannot be combined with compress_topk, got compress_topk %r" % (what, compress_topk))
 
 
-def check_compress(compress_bits: int, compress_ef: bool, dp_clip: float, aggregator: str) -> None:
+def check_compress(compress_bits: int, compress_ef: bool, dp_clip: float, aggregator: str,
+                   compress_topk: float = 0.0) -> None:
     """Raise ``ValueError`` unless the update-compression settings of :class:`FederatedConfig` are valid."""
     if compress_bits not in (0, 8, 4):
         raise ValueError("compress_bits must be 0 (off), 8 or 4, got %r" % (compress_bits,))
-    if compress_ef and not compress_bits:
-        raise ValueError("compress_ef needs compress_bits 8 or 4 (error feedback of uncompressed updates is always 0)")
+    if not (compress_topk == 0.0 or 0.0 < compress_topk < 1.0):
+        raise ValueError("compress_topk must be 0 (off) or lie in (0, 1), got %r" % (compress_topk,))
+    if compress_topk and compress_bits:
+        raise ValueError("compress_topk cannot be combined with compress_bits (the selected values are sent in fp32), got "
+                         "compress_bits %r" % (compress_bits,))
+    if compress_ef and not (compress_bits or compress_topk):
+        raise ValueError("compress_ef needs compress_bits 8 or 4 or compress_topk > 0 (error feedback of uncompressed "
+                         "updates is always 0)")
+    if compress_topk and dp_clip > 0.0:
+        raise ValueError("compress_topk cannot be combined with dp_clip > 0, got dp_clip %r" % (dp_clip,))
+    if compress_topk and aggregator != "mean":
+        raise ValueError("compress_topk needs aggregator 'mean', got aggregator %r" % (aggregator,))
     if compress_bits and dp_clip > 0.0:
         raise ValueError("compress_bits cannot be combined with dp_clip > 0 (quantized updates no longer have the clipped "
                          "sensitivity), got dp_clip %r" % (dp_clip,))
@@ -295,7 +308,7 @@ def check_compress(compress_bits: int, compress_ef: bool, dp_clip: float, aggreg
 
 
 def check_secagg(secagg: bool, secagg_clip: float, K: int, aggregator: str, dp_clip: float, compress_bits: int,
-                 clients_per_round: int, partition: str) -> None:
+                 clients_per_round: int, partition: str, compress_topk: float = 0.0) -> None:
     """Raise ``ValueError`` unless the secure-aggregation settings of :class:`FederatedConfig` are valid."""
     if not secagg:
         return
@@ -310,6 +323,8 @@ def check_secagg(secagg: bool, secagg_clip: float, K: int, aggregator: str, dp_c
         raise ValueError("secagg cannot be combined with dp_clip > 0, got dp_clip %r" % (dp_clip,))
     if compress_bits:
         raise ValueError("secagg cannot be combined with compress_bits, got compress_bits %r" % (compress_bits,))
+    if compress_topk:
+        raise ValueError("secagg cannot be combined with compress_topk, got compress_topk %r" % (compress_topk,))
     if sampled_rounds(clients_per_round, K, partition):
         what = "clients_per_round %d" % clients_per_round if 0 < clients_per_round < K else "partition 'dirichlet'"
         raise ValueError("secagg cannot be combined with sampled rounds (every worker takes part in every round), got %s"
@@ -317,7 +332,7 @@ def check_secagg(secagg: bool, secagg_clip: float, K: int, aggregator: str, dp_c
 
 
 def check_scaffold(scaffold: bool, aggregator: str, dp_clip: float, compress_bits: int, secagg: bool,
-                   optimizer: Optional[str] = None) -> None:
+                   optimizer: Optional[str] = None, compress_topk: float = 0.0) -> None:
     """Raise ``ValueError`` unless the SCAFFOLD settings of :class:`FederatedConfig` are valid.  ``optimizer`` None: not
     checked (the aggregation strategy does not know the client optimizer)."""
     if not scaffold:
@@ -329,7 +344,7 @@ def check_scaffold(scaffold: bool, aggregator: str, dp_clip: float, compress_bit
         raise ValueError("scaffold needs aggregator 'mean' (the control variates are averaged), got aggregator %r"
                          % (aggregator,))
     for name, val, on in (("dp_clip", dp_clip, dp_clip > 0.0), ("compress_bits", compress_bits, bool(compress_bits)),
-                          ("secagg", secagg, bool(secagg))):
+                          ("compress_topk", compress_topk, bool(compress_topk)), ("secagg", secagg, bool(secagg))):
         if on:
             raise ValueError("scaffold cannot be combined with %s (the control-variate update needs the workers' models "
                              "as trained, which %s changes), got %s %r" % (name, name, name, val))
@@ -362,6 +377,9 @@ class FederatedConfig(CommonConfig):
     # one float32 scale per 128 coordinates (algo/compress.py); the new model is still broadcast in fp32
     compress_bits: int = 0          # 0 = off | 8 | 4
     compress_ef: bool = False       # error feedback: each worker carries its quantization error into its next update
+    # top-k sparsified client updates: every worker uploads the max(1, ceil(r N)) largest-magnitude coordinates of its
+    # block update, unchanged (algo/compress.py: topk_select); with compress_ef the rest is carried into its next update
+    compress_topk: float = 0.0      # r: 0 = off, else 0 < r < 1
     # client sampling (FedAvg partial participation): each round trains and averages a uniform random subset of this many
     # workers, weighted by their sample counts (algo/sampling.py); 0 = all K.  --partition dirichlet weights all K by n_k
     clients_per_round: int = 0
@@ -378,12 +396,14 @@ class FederatedConfig(CommonConfig):
         check_aggregator(self.aggregator, self.trim_fraction, self.K)
         check_byzantine(self.byzantine, self.attack, self.attack_scale, self.K)
         check_dp(self.dp_clip, self.dp_noise, self.dp_delta, self.aggregator)
-        check_compress(self.compress_bits, self.compress_ef, self.dp_clip, self.aggregator)
+        check_compress(self.compress_bits, self.compress_ef, self.dp_clip, self.aggregator, self.compress_topk)
         check_partition(self.partition, self.dirichlet_alpha)
-        check_sampling(self.clients_per_round, self.K, self.partition, self.aggregator, self.dp_clip, self.compress_bits)
+        check_sampling(self.clients_per_round, self.K, self.partition, self.aggregator, self.dp_clip, self.compress_bits,
+                       self.compress_topk)
         check_secagg(self.secagg, self.secagg_clip, self.K, self.aggregator, self.dp_clip, self.compress_bits,
-                     self.clients_per_round, self.partition)
-        check_scaffold(self.scaffold, self.aggregator, self.dp_clip, self.compress_bits, self.secagg, self.optimizer)
+                     self.clients_per_round, self.partition, self.compress_topk)
+        check_scaffold(self.scaffold, self.aggregator, self.dp_clip, self.compress_bits, self.secagg, self.optimizer,
+                       self.compress_topk)
 
 
 @dataclass

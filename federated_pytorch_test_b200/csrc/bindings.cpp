@@ -839,6 +839,23 @@ static void set_sa(fb::CommArgs& a, const std::vector<int64_t>& local_idx, int64
   }
   for (int j = 0; j < a.n_local; ++j) a.q_worker[j] = (int)local_idx[j];
 }
+// Top-k rounds (topk_k > 0): k_sel, the payload pointers of ALL K workers (TopKLayout words, local or peer-mapped) and the
+// statistics buffer that topk_select filled.
+static void set_topk(fb::CommArgs& a, int64_t topk_k, const std::vector<int64_t>& topk_pay_ptrs,
+                     const c10::optional<Tensor>& topk_part) {
+  if (topk_k == 0) return;
+  TORCH_CHECK(topk_k >= 1 && topk_k <= a.n, "top-k rounds need 1 <= k <= n");
+  TORCH_CHECK(topk_part.has_value() && topk_part->defined() && topk_part->numel() >= fb::TOPK_STATS_FLOATS,
+              "top-k rounds need the selection statistics buffer");
+  CHECK_F32_CUDA((*topk_part));
+  TORCH_CHECK((int)topk_pay_ptrs.size() == a.K, "top-k rounds need K payload pointers");
+  a.topk_k = (int)topk_k;
+  a.q_part = topk_part->data_ptr<float>();
+  for (int k = 0; k < a.K; ++k) {
+    TORCH_CHECK(topk_pay_ptrs[k] % 16 == 0, "payload slices must be 16-byte aligned");
+    a.q_codes[k] = reinterpret_cast<unsigned char*>(topk_pay_ptrs[k]);
+  }
+}
 static void fill_ctrl(uint32_t** dst, const std::vector<int64_t>& ctrl_ptrs, int world) {
   for (int p = 0; p < world && p < (int)ctrl_ptrs.size(); ++p) dst[p] = reinterpret_cast<uint32_t*>(ctrl_ptrs[p]);
 }
@@ -853,7 +870,8 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
                   std::vector<Tensor> q_ef, c10::optional<Tensor> q_part, int64_t samp_S, int64_t samp_key,
                   c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n, int64_t sa_frac_bits, double sa_clip,
                   c10::optional<Tensor> sa_keys, c10::optional<Tensor> sa_t, std::vector<int64_t> sa_pay_ptrs,
-                  c10::optional<Tensor> sa_part) {
+                  c10::optional<Tensor> sa_part, int64_t topk_k, std::vector<int64_t> topk_pay_ptrs,
+                  c10::optional<Tensor> topk_part) {
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch);
   TORCH_CHECK(out.numel() >= fb::COMM_OUT_FLOATS && scratch.numel() >= fb::COMM_SCRATCH_FLOATS, "out / scratch too small");
   c10::cuda::CUDAGuard guard(z.device());
@@ -895,6 +913,7 @@ void block_reduce(int64_t mode, std::vector<int64_t> x_ptrs, std::vector<int64_t
   set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
   set_samp(a, samp_S, samp_key, samp_t, client_n);
   set_sa(a, local_idx, sa_frac_bits, sa_clip, sa_keys, sa_t, sa_pay_ptrs, sa_part);
+  set_topk(a, topk_k, topk_pay_ptrs, topk_part);
   fb::block_reduce_launch(a, cur_stream());
 }
 
@@ -912,7 +931,8 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
                          std::vector<Tensor> q_ef, c10::optional<Tensor> q_part, int64_t samp_S, int64_t samp_key,
                          c10::optional<Tensor> samp_t, c10::optional<Tensor> client_n, int64_t sa_frac_bits,
                          double sa_clip, c10::optional<Tensor> sa_keys, c10::optional<Tensor> sa_t,
-                         std::vector<int64_t> sa_pay_ptrs, c10::optional<Tensor> sa_part) {
+                         std::vector<int64_t> sa_pay_ptrs, c10::optional<Tensor> sa_part, int64_t topk_k,
+                         std::vector<int64_t> topk_pay_ptrs, c10::optional<Tensor> topk_part) {
   TORCH_CHECK(opt >= fb::FEDOPT_AVGM && opt <= fb::FEDOPT_YOGI, "block_reduce_fedopt: unknown server optimizer ", opt);
   const bool adaptive = opt != fb::FEDOPT_AVGM;
   CHECK_F32_CUDA(z); CHECK_F32_CUDA(out); CHECK_F32_CUDA(scratch); CHECK_F32_CUDA(m); CHECK_CONTIG(m);
@@ -959,6 +979,7 @@ void block_reduce_fedopt(int64_t opt, double lr, double beta1, double beta2, dou
   set_q(a, local_idx, q_bits, q_group, q_key, q_t, q_code_ptrs, q_scale_ptrs, q_ef, q_part);
   set_samp(a, samp_S, samp_key, samp_t, client_n);
   set_sa(a, local_idx, sa_frac_bits, sa_clip, sa_keys, sa_t, sa_pay_ptrs, sa_part);
+  set_topk(a, topk_k, topk_pay_ptrs, topk_part);
   fb::block_reduce_launch(a, cur_stream());
 }
 
@@ -978,6 +999,55 @@ void dp_clip(std::vector<Tensor> xs, Tensor z, double bound, Tensor stats, int64
   a.z = fptr(z);
   a.stats = fptr_mut(stats);
   fb::dp_clip_launch(a, cur_stream());
+}
+
+// Top-k selection of the local replicas xs against the server model z, k_sel entries each; see TopKArgs.  pay: the
+// replicas' payload slices (int32, at least topk_payload_words(n, k) words, 16-byte aligned); ef: their error-feedback
+// slices (empty: off); u: [n_local, >= n] float32 scratch when error feedback is off; ws: int32 workspace of
+// topk_ws_ints(n, n_local) words, zero at first use; stats: the aggregation's statistics buffer.
+static void check_vec4(const std::vector<Tensor>& ts, const char* name);
+int64_t topk_payload_words(int64_t n, int64_t k) { return fb::topk_layout((int)n, (int)k).words; }
+int64_t topk_ws_ints(int64_t n, int64_t n_local) { return fb::topk_ws_ints((int)n, (int)n_local); }
+void topk_select(std::vector<Tensor> xs, Tensor z, int64_t k, std::vector<Tensor> pay, std::vector<Tensor> ef,
+                 c10::optional<Tensor> u, Tensor ws, Tensor stats, int64_t max_blocks) {
+  TORCH_CHECK(!xs.empty() && xs.size() <= (size_t)fb::COMM_MAX_LOCAL, "topk_select: 1 to 16 replicas");
+  TORCH_CHECK(pay.size() == xs.size() && (ef.empty() || ef.size() == xs.size()),
+              "topk_select: one payload (and error-feedback slice) per replica");
+  CHECK_F32_CUDA(z); CHECK_CONTIG(z); CHECK_F32_CUDA(stats);
+  fb::TopKArgs a{};
+  a.n = (int)z.numel(); a.n_local = (int)xs.size(); a.k = (int)k; a.max_blocks = (int)max_blocks;
+  TORCH_CHECK(a.n >= 1 && k >= 1 && k <= a.n, "topk_select: needs 1 <= k <= n");
+  TORCH_CHECK(stats.numel() >= fb::TOPK_STATS_FLOATS, "topk_select: statistics buffer too small");
+  TORCH_CHECK(ws.is_cuda() && ws.scalar_type() == at::kInt && ws.is_contiguous() && ws.numel() >= fb::topk_ws_ints(a.n, a.n_local),
+              "topk_select: workspace must be an int32 CUDA tensor of topk_ws_ints(n, n_local) words");
+  const int words = fb::topk_layout(a.n, a.k).words;
+  if (ef.empty()) {
+    TORCH_CHECK(u.has_value() && u->defined(), "topk_select: without error feedback it needs the u scratch");
+    CHECK_F32_CUDA((*u)); CHECK_CONTIG((*u));
+    TORCH_CHECK(u->dim() == 2 && u->size(0) == a.n_local && u->size(1) >= a.n && u->size(1) % 4 == 0,
+                "topk_select: u scratch [n_local, >= n] with rows of a multiple of 4 floats");
+  }
+  for (int j = 0; j < a.n_local; ++j) {
+    CHECK_F32_CUDA(xs[j]); CHECK_CONTIG(xs[j]);
+    TORCH_CHECK(xs[j].numel() == a.n, "topk_select: block slices must have z's length");
+    TORCH_CHECK(pay[j].is_cuda() && pay[j].scalar_type() == at::kInt && pay[j].is_contiguous() && pay[j].numel() >= words,
+                "topk_select: payload slices must be int32 CUDA tensors of topk_payload_words(n, k) words");
+    a.x[j] = fptr(xs[j]);
+    a.pay[j] = reinterpret_cast<uint32_t*>(pay[j].data_ptr<int>());
+    if (!ef.empty()) {
+      CHECK_F32_CUDA(ef[j]); CHECK_CONTIG(ef[j]);
+      TORCH_CHECK(ef[j].numel() == a.n, "topk_select: error feedback slices must have the block's length");
+      a.ef[j] = fptr_mut(ef[j]);
+    } else {
+      a.u[j] = fptr_mut(*u) + (int64_t)j * u->size(1);
+    }
+  }
+  a.z = fptr(z);
+  a.ws = ws.data_ptr<int>();
+  a.stats = fptr_mut(stats);
+  check_vec4(xs, "topk_select"); check_vec4(pay, "topk_select"); check_vec4(ef, "topk_select"); check_vec4({z}, "topk_select");
+  c10::cuda::CUDAGuard guard(z.device());
+  fb::topk_select_launch(a, cur_stream());
 }
 
 // SCAFFOLD control variates of the local replicas; see ScaffoldArgs.
@@ -1177,6 +1247,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("block_reduce", &block_reduce);
   m.def("block_reduce_fedopt", &block_reduce_fedopt);
   m.def("dp_clip", &dp_clip);
+  m.def("topk_select", &topk_select);
+  m.def("topk_payload_words", &topk_payload_words);
+  m.def("topk_ws_ints", &topk_ws_ints);
   m.def("bb_update", &bb_update);
   m.def("ipc_get_handle", &ipc_get_handle);
   m.def("ipc_open_handle", &ipc_open_handle);

@@ -405,14 +405,14 @@ __device__ __forceinline__ void q_bcast4(float* mc, float* const* w, int world, 
 __device__ __forceinline__ float4 q_f4(const float* v, int q) { return make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]); }
 __device__ __forceinline__ void q_unf4(float* v, int q, float4 t) { v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w; }
 
-// Slice s of a compressed round: whole groups, coordinates [lo, hi).
+// Slice s of a compressed round: whole groups (top-k rounds: whole tiles, unit = Q_TILE), coordinates [lo, hi).
 struct QSlice {
   int lo, hi;
 };
-__device__ __forceinline__ QSlice q_slice(const CommArgs& a, int s) {
-  const int ng = (a.n + Q_GROUP - 1) / Q_GROUP;
+__device__ __forceinline__ QSlice q_slice(const CommArgs& a, int s, int unit = Q_GROUP) {
+  const int ng = (a.n + unit - 1) / unit;
   const int per = a.two_shot ? (ng + a.world - 1) / a.world : ng;
-  return {min(a.n, s * per * Q_GROUP), min(a.n, (s + 1) * per * Q_GROUP)};
+  return {min(a.n, s * per * unit), min(a.n, (s + 1) * per * unit)};
 }
 
 // Phase 0: encode the local replicas' updates on this CTA's tiles of every slice, update e_j, and accumulate this
@@ -629,6 +629,46 @@ __device__ __forceinline__ void q_gather(const CommArgs& a, int c0, float (&acc)
   }
 }
 
+// ---- top-k sparsified updates: the K workers' sparse payloads (TopKLayout) of one tile, summed in shared memory -------
+__device__ __forceinline__ uint32_t ld_sys_u32(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint32_t ld_sys_u16(const uint16_t* p) {
+  unsigned short v;
+  asm volatile("ld.relaxed.sys.global.u16 %0, [%1];" : "=h"(v) : "l"(p) : "memory");
+  return v;
+}
+// acc = sum over the K workers, in worker order, of their sparse updates s_k at this thread's Q_SEG coordinates of the
+// tile starting at tb.  Run by the whole CTA (barriers inside): the entries of tile tb / Q_TILE of worker k are
+// scatter-added into a shared-memory accumulator, one worker after the other; a worker's indices are distinct, so no two
+// threads add to one coordinate at once.  Adding 0 is exact and the accumulator never holds -0, so skipping the
+// unselected coordinates gives the dense sum in worker order bit for bit.
+__device__ __forceinline__ void topk_gather(const CommArgs& a, int tb, float (&acc)[Q_SEG]) {
+  __shared__ __align__(16) float s_acc[Q_TILE];
+  const TopKLayout L = topk_layout(a.n, a.topk_k);
+  const int t = tb / Q_TILE;
+  float4* s4 = reinterpret_cast<float4*>(s_acc) + threadIdx.x * (Q_SEG / 4);
+#pragma unroll
+  for (int q = 0; q < Q_SEG / 4; ++q) s4[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+  __syncthreads();
+  for (int k = 0; k < a.K; ++k) {
+    const uint32_t* p = reinterpret_cast<const uint32_t*>(a.q_codes[k]);
+    const uint32_t o0 = ld_sys_u32(p + t), o1 = min(ld_sys_u32(p + t + 1), uint32_t(a.topk_k));
+    const float* val = reinterpret_cast<const float*>(p + L.val);
+    const uint16_t* idx = reinterpret_cast<const uint16_t*>(p + L.idx);
+    for (uint32_t e = o0 + threadIdx.x; e < o1; e += blockDim.x) {
+      const uint32_t i = ld_sys_u16(idx + e) & (Q_TILE - 1);
+      s_acc[i] = __fadd_rn(s_acc[i], ld_sys_f32(val + e));
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int q = 0; q < Q_SEG / 4; ++q) q_unf4(acc, q, s4[q]);
+  __syncthreads();                                 // the next tile clears s_acc
+}
+
 // Server optimizer step from the pseudo-gradient d itself (compressed rounds: d is the dequantized mean update, not
 // formed as (z + d) - z).  FedAvgM: z + lr m, which is z + d when beta = 0 and lr = 1.
 __device__ __forceinline__ float fedopt_step_d(const CommArgs& a, float z, float d, float& m, float& v) {
@@ -651,16 +691,18 @@ __device__ __forceinline__ float fedopt_step_d(const CommArgs& a, float z, float
 
 // Pass 1 of a compressed round on this CTA's tiles of slice my_slice: z' = z + (1/K) sum_k q_k s_k (or the server step
 // along that d); one-shot stores z' (and m, v) locally, two-shot broadcasts them into every rank.
-template <bool FEDOPT, int QBITS>
+// TOPK: the top-k rounds' sum of sparse payloads on whole-tile slices.
+template <bool FEDOPT, int QBITS, bool TOPK = false>
 __device__ __forceinline__ void q_reduce(const CommArgs& a, int my_slice, float inv_k, float& dual, float& bad) {
-  const QSlice sl = q_slice(a, my_slice);
+  const QSlice sl = q_slice(a, my_slice, TOPK ? Q_TILE : Q_GROUP);
   const bool adaptive = FEDOPT && a.opt != FEDOPT_AVGM;
   for (int tb = sl.lo + blockIdx.x * Q_TILE; tb < sl.hi; tb += gridDim.x * Q_TILE) {
     const int c0 = tb + Q_SEG * threadIdx.x;
-    if (c0 >= sl.hi) continue;
     float acc[Q_SEG];
+    if constexpr (TOPK) topk_gather(a, tb, acc);   // the whole CTA, before the partial tile's idle threads leave
+    if (c0 >= sl.hi) continue;
     if constexpr (QBITS == SA_QBITS) sa_gather(a, c0, acc);
-    else q_gather<QBITS>(a, c0, acc);
+    else if constexpr (!TOPK) q_gather<QBITS>(a, c0, acc);
 #pragma unroll
     for (int q = 0; q < Q_SEG / 4; ++q) {
       const int c = c0 + 4 * q;
@@ -697,9 +739,9 @@ __device__ __forceinline__ void q_reduce(const CommArgs& a, int my_slice, float 
 
 // Pass 2 of a compressed round (FedAvg's, on the compressed tiling): one-shot writes z into every local replica,
 // two-shot copies the broadcast weights of every slice into z and takes the dual residual and NaN count from them.
-__device__ __forceinline__ void q_write_back(const CommArgs& a, int nslices, float& dual, float& bad) {
+__device__ __forceinline__ void q_write_back(const CommArgs& a, int nslices, float& dual, float& bad, int unit) {
   for (int s = 0; s < nslices; ++s) {
-    const QSlice sl = q_slice(a, s);
+    const QSlice sl = q_slice(a, s, unit);
     for (int tb = sl.lo + blockIdx.x * Q_TILE; tb < sl.hi; tb += gridDim.x * Q_TILE) {
       const int c0 = tb + Q_SEG * threadIdx.x;
       if (c0 >= sl.hi) continue;
@@ -841,8 +883,12 @@ __device__ __forceinline__ void exchange_sum(const CommArgs& a, uint32_t epoch, 
 // peer memory with P2P loads only (multimem.ld_reduce would add every bound device with weight 1; the two-shot broadcast
 // may still use multimem.st); pass 2 is FedAvg's, so every replica, participant or not, receives z; the last CTA advances
 // samp_t.
-template <bool FEDOPT, int AGG_PAD, bool DP = false, int QBITS = 0, bool SAMP = false>
+// TOPK: the top-k instantiations (mode 0, the mean), on the compressed skeleton with whole-tile slices: topk_select_kernel
+// has written the payloads before this launch; pass 1 scatter-adds the K workers' entries of each tile into shared memory
+// in worker order (P2P loads only) and applies the compressed rounds' epilogue; phase C exchanges the selection statistics.
+template <bool FEDOPT, int AGG_PAD, bool DP = false, int QBITS = 0, bool SAMP = false, bool TOPK = false>
 __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const CommArgs a) {
+  constexpr bool TILED = QBITS != 0 || TOPK;     // both passes walk the compressed tiling
   __shared__ float sm[32];
   __shared__ int s_abort;
   __shared__ int s_last;
@@ -889,9 +935,9 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
 
   // ---- 1: reduce, scale, new z, dual residual ---------------------------------------------------------------------
   float dual = 0.f, bad = 0.f;
-  if constexpr (QBITS != 0) {
-    // SecAgg: 1/K correctly rounded (the extension is built with --use_fast_math), as the oracle's float32(1) / K
-    q_reduce<FEDOPT, QBITS>(a, my_slice, QBITS == SA_QBITS ? __frcp_rn(float(a.K)) : inv_scale, dual, bad);
+  if constexpr (TILED) {
+    // SecAgg, top-k: 1/K correctly rounded (the extension is built with --use_fast_math), as the oracle's float32(1) / K
+    q_reduce<FEDOPT, QBITS, TOPK>(a, my_slice, (QBITS == SA_QBITS || TOPK) ? __frcp_rn(float(a.K)) : inv_scale, dual, bad);
   } else {
     const int lo = my_slice * chunk4;
     const int hi = min(n4, lo + chunk4);
@@ -943,7 +989,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   }
   // scalar tail (n % 4 elements): every rank reduces it for itself, one-shot style
   const int tail0 = n4 << 2;
-  if (QBITS == 0 && blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
+  if (!TILED && blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
     const int i = tail0 + threadIdx.x;
     float acc = 0.f;
     if constexpr (AGG_PAD > 0) {
@@ -980,8 +1026,8 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
   float pr[COMM_MAX_LOCAL];
 #pragma unroll
   for (int j = 0; j < COMM_MAX_LOCAL; ++j) pr[j] = 0.f;
-  if constexpr (QBITS != 0) q_write_back(a, nslices, dual, bad);
-  for (int s = 0; s < (QBITS == 0 ? nslices : 0); ++s) {
+  if constexpr (TILED) q_write_back(a, nslices, dual, bad, TOPK ? Q_TILE : Q_GROUP);
+  for (int s = 0; s < (TILED ? 0 : nslices); ++s) {
     const int lo = s * chunk4;
     const int hi = min(n4, lo + chunk4);
     for (int i = lo + t0; i < hi; i += stride) {
@@ -1013,7 +1059,7 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       }
     }
   }
-  if (QBITS == 0 && blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
+  if (!TILED && blockIdx.x == 0 && tail0 + int(threadIdx.x) < a.n) {
     const int i = tail0 + threadIdx.x;
     const float zv = a.z[i];
 #pragma unroll
@@ -1082,6 +1128,9 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       }
       s_c[0] = __uint_as_float(c);
       s_c[1] = __uint_as_float(b);
+    } else if constexpr (TOPK) {                   // topk_select_kernel summed them over the CTAs in CTA order
+      s_c[0] = __ldcg(a.q_part + 0);
+      s_c[1] = __ldcg(a.q_part + 1);
     } else if constexpr (QBITS != 0) {
       float e = 0.f, u = 0.f;
       for (int b = 0; b < int(gridDim.x); ++b) {
@@ -1097,8 +1146,8 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
     }
   }
   using Word = typename std::conditional<QBITS == SA_QBITS, uint32_t, float>::type;
-  constexpr int NW = (DP || QBITS != 0) ? 2 : 3;
-  if (a.world > 1 && (DP || QBITS != 0 || a.mode != 0)) exchange_sum<Word, NW>(a, epoch, s_c, &s_abort);
+  constexpr int NW = (DP || TILED) ? 2 : 3;
+  if (a.world > 1 && (DP || TILED || a.mode != 0)) exchange_sum<Word, NW>(a, epoch, s_c, &s_abort);
   if (threadIdx.x == 0) {
     if constexpr (DP) {
       a.out[OUT_DP_CLIPPED] = s_c[0];
@@ -1113,6 +1162,9 @@ __global__ void __launch_bounds__(COMM_THREADS, 1) block_reduce_kernel(const Com
       a.out[OUT_Q_ERR_SQ] = s_c[0];
       a.out[OUT_Q_NORM_SQ] = s_c[1];
       *a.q_t += 1;                                 // every CTA has read t: the next round (or graph replay) draws t + 1
+    } else if constexpr (TOPK) {
+      a.out[OUT_Q_ERR_SQ] = s_c[0];
+      a.out[OUT_Q_NORM_SQ] = s_c[1];
     } else if (a.world > 1 && a.mode != 0) {
       if (a.two_shot) {                            // one-shot: every rank already holds the full dual residual and NaN count
         dual_sq = s_c[0];
@@ -1144,12 +1196,13 @@ static int comm_max_blocks() {
 }
 
 // block_reduce_kernel's instantiation for a round, as an index into the launcher's table: the mean, the robust rules on
-// <= 4, <= 8 and <= 16 workers, the DP mean, 8-bit codes, 4-bit codes, the sampled weighted mean and secure aggregation,
-// plus REDUCE_VARIANTS with a server optimizer
-constexpr int REDUCE_VARIANTS = 9;
+// <= 4, <= 8 and <= 16 workers, the DP mean, 8-bit codes, 4-bit codes, the sampled weighted mean, secure aggregation and
+// top-k payloads, plus REDUCE_VARIANTS with a server optimizer
+constexpr int REDUCE_VARIANTS = 10;
 static int reduce_variant(const CommArgs& a) {
   int v;
-  if (a.sa) v = 8;
+  if (a.topk_k != 0) v = 9;
+  else if (a.sa) v = 8;
   else if (a.samp_S != 0 || a.samp_t != nullptr) v = 7;
   else if (a.qbits != 0) v = a.qbits == 8 ? 5 : 6;
   else if (a.dp) v = 4;
@@ -1210,17 +1263,30 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
     if (args.two_shot && (args.xw[args.world - 1] == nullptr || (args.opt != FEDOPT_NONE && args.mw[args.world - 1] == nullptr)))
       throw std::runtime_error("fedb200: block_reduce: two-shot secure aggregation needs P2P broadcast targets");
   }
+  if (args.topk_k != 0) {
+    if (args.mode != 0 || args.agg != AGG_MEAN || args.dp || args.qbits != 0 || samp || args.sa)
+      throw std::runtime_error("fedb200: block_reduce: top-k rounds need mode 0 and the mean, without DP, compression, "
+                               "sampling or secure aggregation");
+    if (args.topk_k < 1 || args.topk_k > args.n || args.q_part == nullptr)
+      throw std::runtime_error("fedb200: block_reduce: top-k rounds need 1 <= k <= n and the selection statistics");
+    for (int k = 0; k < args.K; ++k)
+      if (args.q_codes[k] == nullptr) throw std::runtime_error("fedb200: block_reduce: top-k rounds need K payloads");
+    if (args.two_shot && (args.xw[args.world - 1] == nullptr || (args.opt != FEDOPT_NONE && args.mw[args.world - 1] == nullptr)))
+      throw std::runtime_error("fedb200: block_reduce: two-shot top-k rounds need P2P broadcast targets");
+  }
   static const void* const kernels[2 * REDUCE_VARIANTS] = {
       (const void*)block_reduce_kernel<false, 0>, (const void*)block_reduce_kernel<false, 4>,
       (const void*)block_reduce_kernel<false, 8>, (const void*)block_reduce_kernel<false, 16>,
       (const void*)block_reduce_kernel<false, 0, true>, (const void*)block_reduce_kernel<false, 0, false, 8>,
       (const void*)block_reduce_kernel<false, 0, false, 4>, (const void*)block_reduce_kernel<false, 0, false, 0, true>,
       (const void*)block_reduce_kernel<false, 0, false, SA_QBITS>,
+      (const void*)block_reduce_kernel<false, 0, false, 0, false, true>,
       (const void*)block_reduce_kernel<true, 0>, (const void*)block_reduce_kernel<true, 4>,
       (const void*)block_reduce_kernel<true, 8>, (const void*)block_reduce_kernel<true, 16>,
       (const void*)block_reduce_kernel<true, 0, true>, (const void*)block_reduce_kernel<true, 0, false, 8>,
       (const void*)block_reduce_kernel<true, 0, false, 4>, (const void*)block_reduce_kernel<true, 0, false, 0, true>,
-      (const void*)block_reduce_kernel<true, 0, false, SA_QBITS>};
+      (const void*)block_reduce_kernel<true, 0, false, SA_QBITS>,
+      (const void*)block_reduce_kernel<true, 0, false, 0, false, true>};
   const void* kernel = kernels[reduce_variant(args)];
   int cap = comm_max_blocks();
   if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;
@@ -1231,6 +1297,10 @@ void block_reduce_launch(const CommArgs& args_in, cudaStream_t s) {
     const int ng = (args.n + Q_GROUP - 1) / Q_GROUP;
     const int per = args.two_shot ? (ng + args.world - 1) / args.world : ng;
     want = (per * Q_GROUP + Q_TILE - 1) / Q_TILE;
+  }
+  if (args.topk_k != 0) {                              // whole tiles per slice
+    const int nt = (args.n + Q_TILE - 1) / Q_TILE;
+    want = args.two_shot ? (nt + args.world - 1) / args.world : nt;
   }
   int grid = want < 1 ? 1 : (want > cap ? cap : want);
   if (args.timeout_cycles <= 0) args.timeout_cycles = 240000000000LL;   // ~2 min at 2 GHz
@@ -1349,6 +1419,282 @@ void dp_clip_launch(const DPClipArgs& args, cudaStream_t s) {
   void* kargs[] = {(void*)&args};
   cudaError_t e = cudaLaunchCooperativeKernel((void*)dp_clip_kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
   if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: dp_clip launch: ") + cudaGetErrorString(e));
+  count_launch();
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Top-k selection of the local replicas' updates (Stich et al. 2018; Lin et al. 2018) — see TopKArgs in fedb200.h
+// ------------------------------------------------------------------------------------------------------------------
+static_assert(TOPK_TILE == Q_TILE, "a top-k tile is a tile of the compressed tiling");
+
+__device__ __forceinline__ uint32_t topk_key(float u) { return __float_as_uint(u) & 0x7fffffffu; }
+
+// float4 at coordinate c (a multiple of 4) of a length-n vector, from L2 (written by other CTAs of this grid); coordinates
+// >= n read as 0
+__device__ __forceinline__ float4 ldcg4(const float* p, int c, int n) {
+  if (c + 4 <= n) return __ldcg(reinterpret_cast<const float4*>(p + c));
+  float v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) v[i] = c + i < n ? __ldcg(p + c + i) : 0.f;
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+
+// exclusive prefix sum over the CTA of one uint32 per thread; *total gets the CTA's sum.  s holds COMM_THREADS / 32 + 1
+// words.
+__device__ __forceinline__ uint32_t block_exscan_u32(uint32_t v, uint32_t* s, uint32_t* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) s[w] = incl;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t run = 0u;
+    for (int i = 0; i < int(blockDim.x >> 5); ++i) {
+      const uint32_t t = s[i];
+      s[i] = run;
+      run += t;
+    }
+    s[COMM_THREADS / 32] = run;
+  }
+  __syncthreads();
+  const uint32_t r = s[w] + incl - v;
+  *total = s[COMM_THREADS / 32];
+  __syncthreads();
+  return r;
+}
+
+// histogram update of one warp-wide batch of bins (bin TOPK_RADIX = no count): lanes with the same bin add once
+__device__ __forceinline__ void topk_hist_add(uint32_t* h, uint32_t bin) {
+  const unsigned peers = __match_any_sync(0xffffffffu, bin);
+  if (bin < TOPK_RADIX && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(h + bin, uint32_t(__popc(peers)));
+}
+
+__global__ void __launch_bounds__(COMM_THREADS, 1) topk_select_kernel(const TopKArgs a) {
+  cg::grid_group grid = cg::this_grid();
+  __shared__ uint32_t s_hist[COMM_MAX_LOCAL * TOPK_RADIX];
+  __shared__ uint32_t s_thr[COMM_MAX_LOCAL];     // replica j's threshold key, digit by digit
+  __shared__ uint32_t s_need[COMM_MAX_LOCAL];    // keys still to select at or below the digits fixed so far
+  __shared__ uint32_t s_scan[COMM_THREADS / 32 + 1];
+  __shared__ float sm[32];
+  const TopKLayout L = topk_layout(a.n, a.k);
+  const int T = L.tiles;
+  uint32_t* hist = reinterpret_cast<uint32_t*>(a.ws);                    // [4][COMM_MAX_LOCAL][TOPK_RADIX]
+  uint32_t* cnt_gt = hist + 4 * COMM_MAX_LOCAL * TOPK_RADIX;             // [n_local][T] keys above the threshold
+  uint32_t* cnt_eq = cnt_gt + a.n_local * T;                            // [n_local][T] keys equal to it
+  uint32_t* take_eq = cnt_eq + a.n_local * T;                           // [n_local][T] of those, selected
+  const int lane = threadIdx.x & 31;
+  const int wtid = blockIdx.x * blockDim.x + threadIdx.x - lane;        // warp-uniform loops: every lane takes part
+  const int nth = gridDim.x * blockDim.x;
+  const int n4 = a.n >> 2;
+  if (threadIdx.x < COMM_MAX_LOCAL) {
+    s_thr[threadIdx.x] = 0u;
+    s_need[threadIdx.x] = uint32_t(a.k);
+  }
+
+  // ---- radix select of the k-th largest key, 8 bits per pass from bit 24 (keys have 31 bits) -------------------
+  for (int pass = 0; pass < 4; ++pass) {
+    const int shift = 24 - 8 * pass;
+    const uint32_t hmask = pass == 0 ? 0u : 0xffffffffu << (shift + 8);
+    for (int i = threadIdx.x; i < a.n_local * TOPK_RADIX; i += blockDim.x) s_hist[i] = 0u;
+    __syncthreads();
+    for (int j = 0; j < a.n_local; ++j) {
+      const uint32_t pre = s_thr[j];
+      uint32_t* h = s_hist + j * TOPK_RADIX;
+      float* u = a.ef[j] != nullptr ? a.ef[j] : a.u[j];
+      for (int b = wtid; b < n4; b += nth) {
+        const int i = b + lane;
+        float4 uv = make_float4(0.f, 0.f, 0.f, 0.f);
+        const bool on = i < n4;
+        if (on && pass == 0) {                     // materialise u = (x - z) + e once
+          const float4 xv = reinterpret_cast<const float4*>(a.x[j])[i];
+          const float4 zv = reinterpret_cast<const float4*>(a.z)[i];
+          const float4 ev = a.ef[j] != nullptr ? reinterpret_cast<const float4*>(a.ef[j])[i] : uv;
+          uv = make_float4(__fadd_rn(__fsub_rn(xv.x, zv.x), ev.x), __fadd_rn(__fsub_rn(xv.y, zv.y), ev.y),
+                           __fadd_rn(__fsub_rn(xv.z, zv.z), ev.z), __fadd_rn(__fsub_rn(xv.w, zv.w), ev.w));
+          reinterpret_cast<float4*>(u)[i] = uv;
+        } else if (on) {
+          uv = __ldcg(reinterpret_cast<const float4*>(u) + i);
+        }
+        const float w4[4] = {uv.x, uv.y, uv.z, uv.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const uint32_t key = topk_key(w4[q]);
+          topk_hist_add(h, on && (key & hmask) == pre ? (key >> shift) & (TOPK_RADIX - 1) : TOPK_RADIX);
+        }
+      }
+      for (int b = (n4 << 2) + wtid; b < a.n; b += nth) {   // scalar tail (n % 4 coordinates)
+        const int i = b + lane;
+        const bool on = i < a.n;
+        float uv = 0.f;
+        if (on && pass == 0) {
+          uv = __fadd_rn(__fsub_rn(a.x[j][i], a.z[i]), a.ef[j] != nullptr ? a.ef[j][i] : 0.f);
+          u[i] = uv;
+        } else if (on) {
+          uv = __ldcg(u + i);
+        }
+        const uint32_t key = topk_key(uv);
+        topk_hist_add(h, on && (key & hmask) == pre ? (key >> shift) & (TOPK_RADIX - 1) : TOPK_RADIX);
+      }
+    }
+    __syncthreads();
+    uint32_t* gh = hist + pass * COMM_MAX_LOCAL * TOPK_RADIX;
+    for (int i = threadIdx.x; i < a.n_local * TOPK_RADIX; i += blockDim.x)
+      if (s_hist[i] != 0u) atomicAdd(gh + i, s_hist[i]);
+    grid.sync();
+    for (int i = threadIdx.x; i < a.n_local * TOPK_RADIX; i += blockDim.x) s_hist[i] = __ldcg(gh + i);
+    __syncthreads();                             // (the walk below then costs shared-memory latency, not L2 round trips)
+    if (threadIdx.x < a.n_local) {               // every CTA fixes the same digit: the largest d with count(>= d) >= need
+      const int j = threadIdx.x;
+      const uint32_t need = s_need[j];
+      uint32_t above = 0u;
+      int d = TOPK_RADIX - 1;
+      for (; d > 0; --d) {
+        const uint32_t c = s_hist[j * TOPK_RADIX + d];
+        if (above + c >= need) break;
+        above += c;
+      }
+      s_need[j] = need - above;
+      s_thr[j] |= uint32_t(d) << shift;
+    }
+    __syncthreads();
+  }
+
+  // ---- per tile: keys above and equal to the threshold ------------------------------------------------------------
+  for (int t = blockIdx.x; t < T; t += gridDim.x) {
+    const int c0 = t * TOPK_TILE + Q_SEG * threadIdx.x;
+    for (int j = 0; j < a.n_local; ++j) {
+      const float* u = a.ef[j] != nullptr ? a.ef[j] : a.u[j];
+      const uint32_t thr = s_thr[j];
+      uint32_t gt = 0u, eq = 0u;
+#pragma unroll
+      for (int q = 0; q < Q_SEG / 4; ++q) {
+        const int c = c0 + 4 * q;
+        const float4 uv = ldcg4(u, c, a.n);
+        const float w4[4] = {uv.x, uv.y, uv.z, uv.w};
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const uint32_t key = topk_key(w4[r]);
+          if (c + r < a.n) {
+            gt += key > thr ? 1u : 0u;
+            eq += key == thr ? 1u : 0u;
+          }
+        }
+      }
+      uint32_t tot;
+      block_exscan_u32((eq << 16) | gt, s_scan, &tot);   // <= 8192 each: the halves do not carry into each other
+      if (threadIdx.x == 0) {
+        cnt_gt[j * T + t] = tot & 0xffffu;
+        cnt_eq[j * T + t] = tot >> 16;
+      }
+    }
+  }
+  grid.sync();
+
+  // ---- CTA j scans replica j's tiles: tile offsets, and the equal keys each tile takes in index order ------------
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 4 * COMM_MAX_LOCAL * TOPK_RADIX; i += nth)
+    hist[i] = 0u;                                // every CTA has read the histograms: clean for the next launch
+  if (blockIdx.x < a.n_local) {
+    const int j = blockIdx.x;
+    const uint32_t need = s_need[j];
+    uint32_t* off = a.pay[j];
+    uint32_t run_sel = 0u, run_eq = 0u;
+    for (int base = 0; base < T; base += blockDim.x) {
+      const int t = base + threadIdx.x;
+      const uint32_t gt = t < T ? __ldcg(cnt_gt + j * T + t) : 0u;
+      const uint32_t eq = t < T ? __ldcg(cnt_eq + j * T + t) : 0u;
+      uint32_t tot_eq, tot_sel;
+      const uint32_t eq_before = run_eq + block_exscan_u32(eq, s_scan, &tot_eq);
+      const uint32_t take = eq_before >= need ? 0u : min(eq, need - eq_before);
+      const uint32_t sel_before = run_sel + block_exscan_u32(gt + take, s_scan, &tot_sel);
+      if (t < T) {
+        off[t] = sel_before;
+        take_eq[j * T + t] = take;
+      }
+      run_eq += tot_eq;
+      run_sel += tot_sel;
+    }
+    if (threadIdx.x == 0) off[T] = run_sel;      // = k
+  }
+  grid.sync();
+
+  // ---- per tile: entries in index order, error feedback, statistics --------------------------------------------------
+  float err = 0.f, nrm = 0.f;
+  for (int t = blockIdx.x; t < T; t += gridDim.x) {
+    const int c0 = t * TOPK_TILE + Q_SEG * threadIdx.x;
+    for (int j = 0; j < a.n_local; ++j) {
+      float* u = a.ef[j] != nullptr ? a.ef[j] : a.u[j];
+      const uint32_t thr = s_thr[j];
+      const uint32_t take = __ldcg(take_eq + j * T + t);
+      float v[Q_SEG];
+      uint32_t gt = 0u, eq = 0u;
+#pragma unroll
+      for (int q = 0; q < Q_SEG / 4; ++q) q_unf4(v, q, ldcg4(u, c0 + 4 * q, a.n));
+#pragma unroll
+      for (int i = 0; i < Q_SEG; ++i) {
+        const uint32_t key = topk_key(v[i]);
+        if (c0 + i < a.n) {
+          gt += key > thr ? 1u : 0u;
+          eq += key == thr ? 1u : 0u;
+        }
+      }
+      uint32_t tot;
+      const uint32_t ex = block_exscan_u32((eq << 16) | gt, s_scan, &tot);
+      uint32_t eq_seen = ex >> 16;
+      uint32_t pos = __ldcg(a.pay[j] + t) + (ex & 0xffffu) + min(eq_seen, take);
+      float* val = reinterpret_cast<float*>(a.pay[j] + L.val);
+      uint16_t* idx = reinterpret_cast<uint16_t*>(a.pay[j] + L.idx);
+#pragma unroll
+      for (int i = 0; i < Q_SEG; ++i) {
+        const int c = c0 + i;
+        if (c >= a.n) break;
+        const uint32_t key = topk_key(v[i]);
+        bool sel = key > thr;
+        if (key == thr) sel = eq_seen++ < take;
+        nrm = fmaf(v[i], v[i], nrm);
+        if (sel) {
+          val[pos] = v[i];
+          idx[pos] = uint16_t(c - t * TOPK_TILE);
+          ++pos;
+          if (a.ef[j] != nullptr) u[c] = 0.f;     // e <- u - s: 0 where selected, u (already stored) elsewhere
+        } else {
+          err = fmaf(v[i], v[i], err);
+        }
+      }
+    }
+  }
+  err = block_add(err, sm);
+  nrm = block_add(nrm, sm);
+  if (threadIdx.x == 0) {
+    a.stats[2 + 2 * blockIdx.x] = err;
+    a.stats[3 + 2 * blockIdx.x] = nrm;
+  }
+  grid.sync();
+  if (blockIdx.x == 0 && threadIdx.x == 0) {     // in CTA order: the same bits on every run
+    float e = 0.f, s = 0.f;
+    for (int b = 0; b < int(gridDim.x); ++b) {
+      e += __ldcg(a.stats + 2 + 2 * b);
+      s += __ldcg(a.stats + 3 + 2 * b);
+    }
+    a.stats[0] = e;
+    a.stats[1] = s;
+  }
+}
+
+void topk_select_launch(const TopKArgs& args, cudaStream_t s) {
+  if (args.n_local < 1 || args.n_local > COMM_MAX_LOCAL || args.n < 1 || args.k < 1 || args.k > args.n)
+    throw std::runtime_error("fedb200: topk_select: needs 1 to 16 replicas and 1 <= k <= n");
+  int cap = comm_max_blocks();
+  if (args.max_blocks > 0 && args.max_blocks < cap) cap = args.max_blocks;
+  if (cap < args.n_local) throw std::runtime_error("fedb200: topk_select: needs at least one CTA per replica");
+  const int want = ((args.n >> 2) + COMM_THREADS - 1) / COMM_THREADS;
+  const int grid = want < args.n_local ? args.n_local : (want > cap ? cap : want);
+  void* kargs[] = {(void*)&args};
+  cudaError_t e = cudaLaunchCooperativeKernel((void*)topk_select_kernel, dim3(grid), dim3(COMM_THREADS), kargs, 0, s);
+  if (e != cudaSuccess) throw std::runtime_error(std::string("fedb200: topk_select launch: ") + cudaGetErrorString(e));
   count_launch();
 }
 

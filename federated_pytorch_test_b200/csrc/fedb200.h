@@ -317,6 +317,11 @@ struct CommArgs {
   int sa_frac_bits;                  // f: K rint(R 2^f) <= 2^31 - 1, 0 <= f <= 126
   float sa_clip;                     // R
   const uint32_t* sa_keys;           // device: [K (K - 1) / 2][8] pair keys, pairs (i < j) in lexicographic order
+  // ---- top-k sparsified updates (mode 0 with the mean, with or without a server optimizer, without DP, compression,
+  // sampling or SecAgg): topk_select_kernel has written every local worker's sparse payload (layout: TopKLayout) and its
+  // statistics (q_part[0], q_part[1]); pass 1 scatter-adds the K workers' entries tile by tile into shared memory, in
+  // worker order.  The payload pointers of ALL K workers go in q_codes.
+  int topk_k;                        // 0 selects the instantiations above; else k_sel entries per worker
 };
 constexpr int Q_GROUP = 128;                             // coordinates per scale
 constexpr int Q_SEG = 16;                                // coordinates per thread and tile in the compressed instantiations
@@ -327,8 +332,46 @@ constexpr int AGG_MEAN = 0, AGG_MEDIAN = 1, AGG_TRIMMED = 2;
 constexpr int COMM_MAX_K_ROBUST = 16;
 constexpr int SA_MAX_FRAC_BITS = 126;                   // 2^f and 2^-f stay normal floats
 // block_reduce_launch picks the instantiation: the mean, a robust rule, DP, compressed codes (qbits), client sampling
-// (samp_S) or secure aggregation (sa); it rejects combinations the kernel does not implement.
+// (samp_S), secure aggregation (sa) or top-k payloads (topk_k); it rejects combinations the kernel does not implement.
 void block_reduce_launch(const CommArgs& args, cudaStream_t s);
+
+// ---- top-k sparse payload of one worker and block (int32 words; algo/compress.py: topk_select is the oracle) ----------
+// words [0, T]: uint32 tile offsets (T = ceil(n / TOPK_TILE) tiles from the block start; offset T = k), then from word
+// val the k float32 values, then from word idx the k uint16 in-tile offsets, two per word (the lower index in the low
+// half).  Entries are in ascending coordinate order.  Sections start at 16-byte boundaries.
+constexpr int TOPK_TILE = COMM_THREADS * Q_SEG;          // 8192 coordinates: one tile of the compressed tiling
+struct TopKLayout {
+  int tiles, val, idx, words;
+};
+__host__ __device__ inline TopKLayout topk_layout(int n, int k) {
+  const int T = (n + TOPK_TILE - 1) / TOPK_TILE;
+  const int val = (T + 1 + 3) & ~3;
+  const int idx = val + ((k + 3) & ~3);
+  return {T, val, idx, idx + (((k + 1) / 2 + 3) & ~3)};
+}
+
+// Top-k selection of the local replicas' updates as ONE cooperative kernel touching no peer memory.  Per replica j:
+// u = (x_j - z) + e_j is materialised into e_j (error feedback) or u[j]; the k-th largest key bits(u) & 0x7fffffff is
+// found by a 4-digit radix select (global integer histograms, grid.sync() between digits); each tile counts its keys above
+// and equal to it, replica j's tile offsets are scanned by CTA j, and every tile writes its entries in index order by an
+// in-CTA prefix scan (ties go to the lower index).  With error feedback e_j <- u - s_j.  q_part[0] / q_part[1] receive
+// sum_j ||u_j - s_j||^2 and sum_j ||u_j||^2, summed in a fixed order: the same bits on every run.
+struct TopKArgs {
+  int n, n_local, k, max_blocks;
+  const float* x[COMM_MAX_LOCAL];    // this process' replicas
+  const float* z;                    // the server model the round started from
+  float* ef[COMM_MAX_LOCAL];         // error feedback e_j (in / out), or nullptr (off: u goes to u[j])
+  float* u[COMM_MAX_LOCAL];          // scratch for u_j when error feedback is off
+  uint32_t* pay[COMM_MAX_LOCAL];     // the replicas' payloads (TopKLayout)
+  int* ws;                           // [topk_ws_ints(n, n_local)] workspace; its histograms are zero between launches
+  float* stats;                      // [TOPK_STATS_FLOATS] (the aggregation's q_part): [0] err, [1] norm, per-CTA partials
+};
+constexpr int TOPK_RADIX = 256;
+constexpr int TOPK_STATS_FLOATS = 2 + 2 * COMM_MAX_BLOCKS;
+inline int topk_ws_ints(int n, int n_local) {
+  return 4 * COMM_MAX_LOCAL * TOPK_RADIX + 3 * n_local * ((n + TOPK_TILE - 1) / TOPK_TILE);
+}
+void topk_select_launch(const TopKArgs& args, cudaStream_t s);
 
 // DP-FedAvg update clipping on the local replicas, as ONE cooperative kernel touching no peer memory: ||x_j - z|| per
 // replica, grid.sync(), then x_j <- z + (C / ||x_j - z||) (x_j - z) for the replicas over the bound C only (the others are

@@ -13,7 +13,9 @@ one device):
   ``fedavg_`` / ``fedopt_`` only the round's ``S`` sampled workers are averaged, weighted by their sample counts
   (``z' = sum_{k in P} n_k x_k / sum_{k in P} n_k``, ``algo/sampling.py``), and every replica receives ``z'``; with
   ``secagg=`` on ``fedavg_`` / ``fedopt_`` every worker uploads its update ``x_k - z`` as int32 fixed-point codes masked
-  with pairwise ChaCha20 keystreams that cancel in the sum (``algo/secagg.py``), and ``z' = z + decode(sum_k y_k)``
+  with pairwise ChaCha20 keystreams that cancel in the sum (``algo/secagg.py``), and ``z' = z + decode(sum_k y_k)``; with
+  ``topk=`` on ``fedavg_`` / ``fedopt_`` every worker uploads the ``k_sel`` largest-magnitude coordinates of its update
+  (``algo/compress.py: topk_select``), and ``z' = z + mean_k s_k``
 * X2 FedProx ``z' = mean``; ``dual``; ``primal = sum_k ||rho (x_k - z')||``; no write-back
   (fedprox_multi.py:211-232)
 * X3 ADMM    ``z' = sum_k (y_k + rho x_k) / (K rho)``; ``dual``; ``y_k += rho (x_k - z')``;
@@ -115,6 +117,18 @@ class SecAggRound:
     payload: List[torch.Tensor]
 
 
+@dataclass
+class TopKRound:
+    """Top-k sparsification of one round (``algo/compress.py: topk_select``): every worker sends the ``k`` coordinates of
+    its update ``(x_k - z) + e_k`` with the largest magnitudes.  ``payload`` holds the local replicas' payload slices
+    (:meth:`TorchCollective.sparse_payload_like_block`; on the fused collective peers read them), ``ef`` the local
+    replicas' error-feedback vectors (in / out; None = off)."""
+
+    k: int
+    payload: List[torch.Tensor]
+    ef: Optional[List[torch.Tensor]] = None
+
+
 class TorchCollective:
     """ATen + torch.distributed implementation (baseline / oracle / CPU)."""
 
@@ -125,7 +139,7 @@ class TorchCollective:
         self.topo = topo
         self.launches = 0  # number of framework-owned kernels launched (0 here: library path)
         self.last_dp = (0.0, 0.0)   # DP rounds: (#clipped workers, sum of their pre-clip update norms) over all K
-        self.last_q = (0.0, 0.0)    # compressed rounds: (sum_k ||u_k - q_k s_k||^2, sum_k ||u_k||^2) over all K
+        self.last_q = (0.0, 0.0)    # compressed / top-k rounds: (sum_k ||u_k - q_k s_k||^2, sum_k ||u_k||^2) over all K
         self.last_sa = (0, 0)       # secure-aggregation rounds: (#clipped, #non-finite coordinates) over all K
 
     # -- arena hooks ------------------------------------------------------
@@ -155,6 +169,13 @@ class TorchCollective:
         """Zeroed secure-aggregation payload of block slice ``x``: int32, one word per coordinate, whole segments of 16
         coordinates (one ChaCha20 block each).  The fused backend hands out slices of symmetric arenas."""
         return torch.zeros(-(-x.numel() // 16) * 16, dtype=torch.int32, device=x.device)
+
+    def sparse_payload_like_block(self, x: torch.Tensor, k_sel: int) -> torch.Tensor:
+        """Zeroed top-k payload of block slice ``x`` with ``k_sel`` entries: int32 words, layout
+        ``algo/compress.py: topk_layout``.  The fused backend hands out slices of symmetric arenas."""
+        from ..algo.compress import topk_layout
+
+        return torch.zeros(topk_layout(x.numel(), k_sel)[3], dtype=torch.int32, device=x.device)
 
     # -- primitives -------------------------------------------------------
     def _allreduce(self, t: torch.Tensor) -> torch.Tensor:
@@ -298,6 +319,38 @@ class TorchCollective:
         return acc.mul_(1.0 / self.topo.K)
 
     @torch.no_grad()
+    def _topk_update(self, xs: List[torch.Tensor], z: torch.Tensor, tk: TopKRound) -> torch.Tensor:
+        """``d = (1/K) sum_k s_k`` of a top-k round, summed in float32 in worker order ``k = 0 .. K-1``: every local
+        replica's update is selected with the oracle (updating its error feedback and its payload slice), then the K
+        sparse updates are gathered densely.  The statistics go to :attr:`last_q`."""
+        from ..algo.compress import topk_indices, topk_pack, topk_select
+
+        sparse, stats = [], torch.zeros(2, dtype=torch.float64, device=z.device)
+        for j, x in enumerate(xs):
+            u = x - z
+            if tk.ef is not None:
+                u = u + tk.ef[j]
+            pay = topk_select(u.detach().cpu().numpy(), tk.k)
+            sel = torch.from_numpy(topk_indices(pay[0], pay[1])).to(z.device)
+            s = torch.zeros_like(u)
+            s[sel] = u[sel]
+            e = u.clone()
+            e[sel] = 0.0
+            if tk.ef is not None:
+                tk.ef[j].copy_(e)
+            stats[0] += e.double().square().sum()
+            stats[1] += u.double().square().sum()
+            words = torch.from_numpy(topk_pack(pay, u.numel()))
+            tk.payload[j][: words.numel()].copy_(words)
+            sparse.append(s)
+        full = self.gather_blocks(sparse)
+        acc = full[0].clone()
+        for k in range(1, self.topo.K):
+            acc.add_(full[k])
+        self.last_q = tuple(self.sum_scalars(stats).tolist())
+        return acc.mul_(1.0 / self.topo.K)
+
+    @torch.no_grad()
     def _secagg_update(self, xs: List[torch.Tensor], z: torch.Tensor, sa: SecAggRound) -> torch.Tensor:
         """``d = decode(sum_k y_k)`` of a secure-aggregation round: every local replica's update is encoded and masked with
         the oracle (into its payload slice), the K payloads are gathered and summed as integers mod 2^32, then decoded.
@@ -346,13 +399,17 @@ class TorchCollective:
     @torch.no_grad()
     def fedavg_(self, xs: List[torch.Tensor], z: torch.Tensor, write_back: bool = True,
                 dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> torch.Tensor:
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None,
+                topk: Optional[TopKRound] = None) -> torch.Tensor:
         """In place: ``z <- mean_k x_k``, optionally ``x_k <- z``; returns ``||z_old - z_new||^2`` (0-dim).  With ``dp``
         the mean is noised (:class:`DPRound`; clip the replicas with :meth:`dp_clip_` first).  With ``compress``
         (:class:`QuantRound`) ``z <- z + (1/K) sum_k q_k s_k``, the workers' updates as uploaded.  With ``sample``
         (:class:`SampleRound`) ``z <-`` the sample-weighted mean of the round's participants; every replica receives it.
-        With ``secagg`` (:class:`SecAggRound`) ``z <- z + d``, ``d`` decoded from the sum of the masked payloads."""
-        if secagg is not None:
+        With ``secagg`` (:class:`SecAggRound`) ``z <- z + d``, ``d`` decoded from the sum of the masked payloads.  With
+        ``topk`` (:class:`TopKRound`) ``z <- z + (1/K) sum_k s_k``, the workers' sparse updates as uploaded."""
+        if topk is not None:
+            znew = z + self._topk_update(xs, z, topk)
+        elif secagg is not None:
             znew = z + self._secagg_update(xs, z, secagg)
         elif sample is not None:
             znew = self._sampled_mean(xs, sample)
@@ -388,16 +445,19 @@ class TorchCollective:
     def fedopt_(self, xs: List[torch.Tensor], z: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], kind: str,
                 lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean", trim_b: int = 0,
                 dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> torch.Tensor:
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None,
+                topk: Optional[TopKRound] = None) -> torch.Tensor:
         """FedAvg with a server optimizer, in place: ``d = mean_k x_k - z`` is the pseudo-gradient of server optimizer
         ``kind`` (one of :data:`FEDOPT_KINDS`; ``beta1`` is the momentum of 'avgm'), whose state ``m`` (and ``v``, unused
         by 'avgm') it updates; ``z`` and every replica receive the new server model.  Returns ``||z_old - z_new||^2``.
         With a robust rule ``agg`` (one of :data:`ROBUST_AGGS`) its aggregate replaces the mean in ``d``; with ``dp`` the
         noised mean does (DP-FedOpt: post-processing); with ``compress`` ``d`` is the dequantized mean update itself
         (FedPAQ with a server optimizer); with ``sample`` the sample-weighted mean of the round's participants does; with
-        ``secagg`` ``d`` is the decoded sum of the masked payloads."""
+        ``secagg`` ``d`` is the decoded sum of the masked payloads; with ``topk`` ``d`` is the mean sparse update itself."""
         mean = None
-        if secagg is not None:
+        if topk is not None:
+            d = self._topk_update(xs, z, topk)
+        elif secagg is not None:
             d = self._secagg_update(xs, z, secagg)
         elif sample is not None:
             mean = self._sampled_mean(xs, sample)

@@ -53,6 +53,12 @@ subtracts the K - 1 ChaCha20 keystreams of its pairs, computed in registers, int
 (:meth:`FusedCollective.payload32_like_block`); pass 1 sums the K payloads over P2P as integers mod 2^32, where the masks
 cancel, and decodes.  The sum is exact, so the new model does not depend on the process layout or on one-shot versus
 two-shot.  The nonce counter lives in device memory as the DP one.
+
+Top-k rounds (sparsified updates, optional error feedback) are two launches: a cooperative selection kernel on each rank's
+own replicas (no peer memory) writes every replica's sparse payload (tile offsets, then its entries in index order) into
+symmetric payload arenas (:meth:`FusedCollective.sparse_payload_like_block`), then the top-k instantiations of the
+aggregation kernel scatter-add the K workers' entries of each tile into shared memory in worker order, over P2P.  Adding
+zeros is exact, so the new model does not depend on the process layout or on one-shot versus two-shot.
 """
 from __future__ import annotations
 
@@ -64,8 +70,8 @@ import torch
 import torch.distributed as dist
 
 from ..ops import cuda_ops
-from .collective import (FEDOPT_KINDS, ROBUST_AGGS, DPRound, QuantRound, SampleRound, SecAggRound, TorchCollective,
-                         check_robust)
+from .collective import (FEDOPT_KINDS, ROBUST_AGGS, DPRound, QuantRound, SampleRound, SecAggRound, TopKRound,
+                         TorchCollective, check_robust)
 from .topology import Topology
 
 _MAX_LOCAL = 16
@@ -74,7 +80,7 @@ _SCRATCH_FLOATS = 4 + _MAX_LOCAL
 _MAX_BLOCKS = 160                                         # csrc/fedb200.h: COMM_MAX_BLOCKS
 _DP_STATS_FLOATS = 2 * _MAX_LOCAL * _MAX_BLOCKS + 2 * _MAX_LOCAL      # DP_STATS_FLOATS: double partials, norms, flags
 _BB_SCRATCH_FLOATS = 8 * _MAX_LOCAL + 8 + _MAX_LOCAL
-_Q_PART_FLOATS = 2 * _MAX_BLOCKS                          # Q_PART_FLOATS: per-CTA partial statistics
+_Q_PART_FLOATS = 2 * _MAX_BLOCKS + 2                      # TOPK_STATS_FLOATS (>= Q_PART_FLOATS): per-CTA partials
 _Q_GROUP = 128                                            # Q_GROUP (algo/compress.py: GROUP)
 _PAD_WORDS = 8192
 OUT_DUAL_SQ, OUT_PRIMAL, OUT_NONFINITE, OUT_STATUS, OUT_RHO, OUT_EPOCH, OUT_TWO_SHOT = range(7)
@@ -194,6 +200,8 @@ class FusedCollective(TorchCollective):
         self.ctrl_ptrs = list(self.heap.locate(self.ctrl)[0]["peer_ptrs"])
         self._aux: Dict[Tuple[int, str], torch.Tensor] = {}
         self._payload: Dict[Tuple[int, int], Tuple[torch.Tensor, torch.Tensor]] = {}   # (arena base, bits) -> code / scale arenas
+        self._sparse: Dict[int, torch.Tensor] = {}      # arena base -> top-k payload arena
+        self._topk_ws: Dict[Tuple[int, int, bool], Tuple[torch.Tensor, Optional[torch.Tensor]]] = {}
         # in-switch reduction pays from 4 peers on; between 2 GPUs there is nothing to reduce in the switch and the P2P variant of
         # the same kernel is used.  FEDB200_MULTIMEM=0|1 forces either.
         mm = os.environ.get("FEDB200_MULTIMEM", "auto")
@@ -211,6 +219,7 @@ class FusedCollective(TorchCollective):
         self.warm_compress = 0            # set by compressing strategies to their bit width: warm those instantiations too
         self.warm_sample = False          # set by sampling strategies: warm the sampled instantiation(s) too
         self.warm_secagg = False          # set by secure-aggregation strategies: warm the SecAgg instantiation(s) too
+        self.warm_topk = False            # set by top-k strategies: warm the selection kernel and top-k instantiation(s) too
 
     def warmup(self) -> None:
         """One tiny aggregation of every kind on scratch buffers: CUDA module loading, occupancy queries and the first
@@ -219,7 +228,7 @@ class FusedCollective(TorchCollective):
         robust kernels (of this K; with the server optimizer if both are set) only when ``warm_robust`` is set, the DP
         kernels (likewise) only when ``warm_dp`` is set, the compressed ones of ``warm_compress`` bits (likewise) only when
         that is set, the sampled ones (likewise) only when ``warm_sample`` is set, the SecAgg ones (likewise) only when
-        ``warm_secagg`` is set; their round counters are throwaway tensors, so warm-up advances no counter of the run.
+        ``warm_secagg`` is set, the top-k ones (likewise) only when ``warm_topk`` is set; their round counters are throwaway tensors, so warm-up advances no counter of the run.
         Collective: every rank calls it at the same point."""
         if getattr(self, "_warm", False):
             return
@@ -243,6 +252,8 @@ class FusedCollective(TorchCollective):
             sa = SecAggRound(1.0, 0, torch.zeros(K * (K - 1) // 2, 8, dtype=torch.int32, device=self.topo.device),
                              torch.zeros(1, dtype=torch.int64, device=self.topo.device),
                              [self.payload32_like_block(x) for x in xs])
+        if self.warm_topk:
+            tk = TopKRound(8, [self.sparse_payload_like_block(x, 8) for x in xs])
         keep = self.two_shot_mode
         for mode_2shot in ("0", "1"):
             self.two_shot_mode = mode_2shot
@@ -273,6 +284,10 @@ class FusedCollective(TorchCollective):
                 self._launch(0, xs, None, z, 0.0, secagg=sa)
                 if self.warm_fedopt:
                     self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, secagg=sa)
+            if self.warm_topk:
+                self._launch(0, xs, None, z, 0.0, topk=tk)
+                if self.warm_fedopt:
+                    self._launch_fedopt(xs, z, m, v, "adam", 1e-2, 0.9, 0.99, 1e-3, topk=tk)
         self.two_shot_mode = keep
         x0 = [torch.zeros_like(x) for x in xs]
         yh = [torch.zeros_like(x) for x in xs]
@@ -328,6 +343,52 @@ class FusedCollective(TorchCollective):
         the codes arena of :meth:`payload_like_block` for 32-bit codes, viewed as int32, so the arena's float ``i`` has its
         word at word ``i`` and every block slice its own payload at the same offset in every rank."""
         return self.payload_like_block(x, 32)[0].view(torch.int32)
+
+    def sparse_payload_like_block(self, x: torch.Tensor, k_sel: int) -> torch.Tensor:
+        """The top-k payload slice of block slice ``x`` with ``k_sel`` entries (layout:
+        :meth:`TorchCollective.sparse_payload_like_block`) in a symmetric arena that mirrors ``x``'s arena: two words per
+        float of the arena, the block starting at float ``i`` at word ``2 i``.  A payload takes at most
+        ``1.5 n + n / 8192 + 9`` words and blocks start at multiples of 32 floats, so every block slice has its own payload
+        at the same offset in every rank."""
+        from ..algo.compress import topk_layout
+
+        a, off = self.heap.locate(x)
+        i0 = off // 4
+        if i0 % 32:
+            raise ValueError("top-k rounds need block slices that start at a multiple of 32 floats, got %d" % i0)
+        buf = self._sparse.get(a["base"])
+        if buf is None:
+            buf = self.heap.alloc(2 * (a["nbytes"] // 4) + 64, dtype=torch.int32)
+            self._sparse[a["base"]] = buf
+        pay = buf[2 * i0: 2 * i0 + topk_layout(x.numel(), k_sel)[3]]
+        pay.zero_()
+        return pay
+
+    def _topk_scratch(self, n: int, n_local: int, ef: bool):
+        """The selection kernel's workspace (its histograms are zero between launches) and, without error feedback, its
+        ``u`` scratch: one pair per block length, kept for the collective's lifetime (graphs capture their addresses)."""
+        key = (n, n_local, ef)
+        got = self._topk_ws.get(key)
+        if got is None:
+            dev = self.topo.device
+            ws = torch.zeros(self.ext.topk_ws_ints(n, n_local), dtype=torch.int32, device=dev)
+            u = None if ef else torch.empty(n_local, -(-n // 4) * 4, dtype=torch.float32, device=dev)
+            got = self._topk_ws[key] = (ws, u)
+        return got
+
+    def _select_topk(self, xs, z, tk: TopKRound) -> None:
+        """The first launch of a top-k round: every local replica's payload, error feedback and statistics."""
+        ef = list(tk.ef) if tk.ef is not None else []
+        ws, u = self._topk_scratch(z.numel(), len(xs), bool(ef))
+        self.ext.topk_select(list(xs), z, int(tk.k), list(tk.payload), ef, u, ws, self.q_part, self.max_blocks)
+        self.launches += 1
+
+    def _topk_args(self, tk: Optional[TopKRound]):
+        """The top-k arguments of the aggregation bindings: k_sel, the K workers' payload pointers, the statistics buffer."""
+        if tk is None:
+            return 0, [], None
+        pp, _, _ = self._tables(tk.payload)
+        return int(tk.k), pp, self.q_part
 
     # -- pointer tables -------------------------------------------------------------
     def _tables(self, slices: List[torch.Tensor]):
@@ -398,10 +459,12 @@ class FusedCollective(TorchCollective):
 
     def _launch(self, mode: int, xs, ys, z, rho: float, rho_dev=None, agg: str = "mean", trim_b: int = 0,
                 dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> None:
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None,
+                topk: Optional[TopKRound] = None) -> None:
         """Modes 0 / 1 take a robust rule ``agg`` (:data:`ROBUST_AGGS`) in place of the mean; mode 0 with the mean takes
         the noise of a DP round (``dp``; after :meth:`dp_clip_`), compresses the workers' updates (``compress``),
-        averages the sampled participants of the round (``sample``) or sums their masked updates (``secagg``)."""
+        averages the sampled participants of the round (``sample``), sums their masked updates (``secagg``) or sums
+        their top-k updates (``topk``; the selection is a launch of its own)."""
         if dp is not None and (mode != 0 or agg != "mean"):
             raise ValueError("DP aggregation needs FedAvg with the mean")
         if compress is not None and (mode != 0 or agg != "mean" or dp is not None):
@@ -410,10 +473,16 @@ class FusedCollective(TorchCollective):
             raise ValueError("sampled aggregation needs FedAvg with the mean, without DP or compression")
         if secagg is not None and (mode != 0 or agg != "mean" or dp is not None or compress is not None or sample is not None):
             raise ValueError("secure aggregation needs FedAvg with the mean, without DP, compression or sampling")
+        if topk is not None and (mode != 0 or agg != "mean" or dp is not None or compress is not None or sample is not None
+                                 or secagg is not None):
+            raise ValueError("top-k aggregation needs FedAvg with the mean, without DP, compression, sampling or secure "
+                             "aggregation")
         code = self._agg_code(agg, trim_b)
         n = xs[0].numel()
         if any(t.numel() != n for t in xs) or z.numel() != n:
             raise ValueError("block slices must have equal length")
+        if topk is not None:
+            self._select_topk(xs, z, topk)
         W = self.topo.world_size
         xp, local_idx, mcx = self._tables(xs)
         yp, mcy = [], 0
@@ -433,19 +502,21 @@ class FusedCollective(TorchCollective):
         self.ext.block_reduce(mode, xp, yp, local_idx, z, n, float(rho), rho_dev, self.out, self.scratch, self.ctrl_ptrs,
                               self.sync, W, self.topo.rank, mcx, mcy, mcz, xw, zw, bool(two), self.max_blocks,
                               self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress),
-                              *self._samp_args(sample), *self._sa_args(secagg))
+                              *self._samp_args(sample), *self._sa_args(secagg), *self._topk_args(topk))
         self.launches += 1
         self.last_two_shot = bool(two)
 
     def _launch_fedopt(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
                        trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                       sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> None:
+                       sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None,
+                       topk: Optional[TopKRound] = None) -> None:
         """FedAvg with a server optimizer: mode 0 of the kernel's FedOpt instantiation.  Two-shot, rank r broadcasts slice r
         of the new weights, of ``m`` and of ``v`` into every rank, so ``m`` / ``v`` must be symmetric slices then
         (:meth:`zeros_like_block`).  A robust rule ``agg`` replaces the mean as the aggregate the step is taken towards; a
         DP round (``dp``, mean only) noises the mean first; a compressed round (``compress``, mean only) steps along the
         dequantized mean update; a sampled round (``sample``, mean only) steps towards the participants' weighted mean; a
-        SecAgg round (``secagg``, mean only) steps along the decoded sum of the masked updates."""
+        SecAgg round (``secagg``, mean only) steps along the decoded sum of the masked updates; a top-k round (``topk``,
+        mean only) steps along the mean sparse update."""
         code = self._agg_code(agg, trim_b)
         if dp is not None and agg != "mean":
             raise ValueError("DP aggregation needs the mean")
@@ -455,10 +526,15 @@ class FusedCollective(TorchCollective):
             raise ValueError("sampled aggregation needs the mean, without DP or compression")
         if secagg is not None and (agg != "mean" or dp is not None or compress is not None or sample is not None):
             raise ValueError("secure aggregation needs the mean, without DP, compression or sampling")
+        if topk is not None and (agg != "mean" or dp is not None or compress is not None or sample is not None
+                                 or secagg is not None):
+            raise ValueError("top-k aggregation needs the mean, without DP, compression, sampling or secure aggregation")
         n = xs[0].numel()
         adaptive = kind != "avgm"
         if any(t.numel() != n for t in xs) or z.numel() != n or m.numel() != n or (adaptive and v.numel() != n):
             raise ValueError("block slices must have equal length")
+        if topk is not None:
+            self._select_topk(xs, z, topk)
         W = self.topo.world_size
         xp, local_idx, mcx = self._tables(xs)
         two = self._want_two_shot(0, xs, z, n) and self.heap.contains(m) and (not adaptive or self.heap.contains(v))
@@ -473,7 +549,7 @@ class FusedCollective(TorchCollective):
                                      v if adaptive else None, xp, local_idx, z, n, self.out, self.scratch, self.ctrl_ptrs,
                                      self.sync, W, self.topo.rank, mcx, mcm, mcv, xw, mw, vw, bool(two), self.max_blocks,
                                      self.timeout_s, code, int(trim_b), *self._dp_args(dp), *self._q_args(compress),
-                                     *self._samp_args(sample), *self._sa_args(secagg))
+                                     *self._samp_args(sample), *self._sa_args(secagg), *self._topk_args(topk))
         self.launches += 1
         self.last_two_shot = bool(two)
 
@@ -490,14 +566,16 @@ class FusedCollective(TorchCollective):
 
     def launch_fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
                        compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None,
-                       secagg: Optional[SecAggRound] = None) -> None:
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample, secagg=secagg)
+                       secagg: Optional[SecAggRound] = None, topk: Optional[TopKRound] = None) -> None:
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample, secagg=secagg,
+                     topk=topk)
         self._record_async()
 
     def launch_fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
                        trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                       sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None) -> None:
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample, secagg)
+                       sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None,
+                       topk: Optional[TopKRound] = None) -> None:
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample, secagg, topk)
         self._record_async()
 
     @torch.no_grad()
@@ -552,8 +630,9 @@ class FusedCollective(TorchCollective):
     @torch.no_grad()
     def fedavg_(self, xs, z, write_back: bool = True, dp: Optional[DPRound] = None,
                 compress: Optional[QuantRound] = None, sample: Optional[SampleRound] = None,
-                secagg: Optional[SecAggRound] = None):
-        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample, secagg=secagg)
+                secagg: Optional[SecAggRound] = None, topk: Optional[TopKRound] = None):
+        self._launch(0 if write_back else 1, xs, None, z, 0.0, dp=dp, compress=compress, sample=sample, secagg=secagg,
+                     topk=topk)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
@@ -564,8 +643,9 @@ class FusedCollective(TorchCollective):
     @torch.no_grad()
     def fedopt_(self, xs, z, m, v, kind: str, lr: float, beta1: float, beta2: float, tau: float, agg: str = "mean",
                 trim_b: int = 0, dp: Optional[DPRound] = None, compress: Optional[QuantRound] = None,
-                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None):
-        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample, secagg)
+                sample: Optional[SampleRound] = None, secagg: Optional[SecAggRound] = None,
+                topk: Optional[TopKRound] = None):
+        self._launch_fedopt(xs, z, m, v, kind, lr, beta1, beta2, tau, agg, trim_b, dp, compress, sample, secagg, topk)
         return self.read_record()[OUT_DUAL_SQ]
 
     @torch.no_grad()
