@@ -35,7 +35,7 @@ _SPECS: Dict[str, Dict] = {
     "fedb200_runtime": {"sources": ["batch_loader.cpp"], "cuda": False},
     "fedb200_cuda": {
         "sources": ["bindings.cpp", "flat_kernels.cu", "elementwise_kernels.cu", "norm_kernels.cu", "loss_kernels.cu",
-                    "comm_kernels.cu", "gemm_wgmma.cu", "aux_kernels.cu"],
+                    "comm_kernels.cu", "gemm_wgmma.cu", "aux_kernels.cu", "stem_kernels.cu"],
         "cuda": True,
     },
 }

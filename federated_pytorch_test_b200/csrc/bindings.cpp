@@ -244,6 +244,44 @@ std::vector<Tensor> bn_elu_fwd(Tensor y, c10::optional<Tensor> stats, Tensor gam
                  fptr_mut(si), M, C, (float)eps, (float)momentum, act ? 1 : 0, self_clean ? 1 : 0, cur_stream());
   return {out, sm, si};
 }
+// ResNet stem (stem_kernels.cu).  x: [N,H,32,3] contiguous, w: [64,3,3,3] contiguous (KRSC), stats: [sum | sumsq | counter].
+// mode STORE_Y returns (y); STATS_ONLY returns (); APPLY returns (out, save_mean, save_invstd).
+bool stem_conv_supported(int64_t H, int64_t W, int64_t C_in, int64_t C_out) {
+  return fb::stem_conv_supported((int)H, (int)W, (int)C_in, (int)C_out);
+}
+std::vector<Tensor> stem_conv_bn(Tensor x, Tensor w, Tensor stats, int64_t mode, c10::optional<Tensor> gamma,
+                                 c10::optional<Tensor> beta, c10::optional<Tensor> running_mean, c10::optional<Tensor> running_var,
+                                 double eps, double momentum, bool act, bool self_clean) {
+  CHECK_F32_CUDA(x); CHECK_CONTIG(x); CHECK_F32_CUDA(w); CHECK_CONTIG(w); CHECK_F32_CUDA(stats);
+  TORCH_CHECK(x.dim() == 4 && w.dim() == 4 && x.size(3) == 3 && w.size(0) == 64 && w.size(1) == 3 && w.size(2) == 3 &&
+                  w.size(3) == 3 && fb::stem_conv_supported((int)x.size(1), (int)x.size(2), 3, 64),
+              "stem_conv_bn: x [N,H,32,3] with H % 4 == 0, w [64,3,3,3]");
+  TORCH_CHECK(stats.numel() >= 2 * 64 + 1 && stats.is_contiguous(), "stem_conv_bn: stats buffer too small");
+  TORCH_CHECK(x.size(0) * x.size(1) * x.size(2) * 64 < (int64_t(1) << 31), "stem_conv_bn: batch too large");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int NB = (int)x.size(0), H = (int)x.size(1);
+  if (mode == fb::STEM_STATS_ONLY) {
+    fb::stem_conv_bn(fb::STEM_STATS_ONLY, fptr(x), fptr(w), nullptr, fptr_mut(stats), nullptr, nullptr, nullptr, nullptr, nullptr,
+                     nullptr, NB, H, 0.f, 0.f, 0, 0, cur_stream());
+    return {};
+  }
+  auto out = torch::empty({NB, H, x.size(2), 64}, x.options());
+  if (mode == fb::STEM_STORE_Y) {
+    fb::stem_conv_bn(fb::STEM_STORE_Y, fptr(x), fptr(w), fptr_mut(out), fptr_mut(stats), nullptr, nullptr, nullptr, nullptr,
+                     nullptr, nullptr, NB, H, 0.f, 0.f, 0, 0, cur_stream());
+    return {out};
+  }
+  TORCH_CHECK(mode == fb::STEM_APPLY, "stem_conv_bn: mode must be 0 (STORE_Y), 1 (STATS_ONLY) or 2 (APPLY)");
+  TORCH_CHECK(gamma.has_value() && gamma->defined() && beta.has_value() && beta->defined(), "stem_conv_bn: APPLY needs gamma and beta");
+  CHECK_F32_CUDA((*gamma)); CHECK_F32_CUDA((*beta));
+  float* rm = (running_mean.has_value() && running_mean->defined()) ? running_mean->data_ptr<float>() : nullptr;
+  float* rv = (running_var.has_value() && running_var->defined()) ? running_var->data_ptr<float>() : nullptr;
+  TORCH_CHECK((rm == nullptr) == (rv == nullptr), "stem_conv_bn: running_mean and running_var go together");
+  auto sm = torch::empty({64}, x.options()), si = torch::empty({64}, x.options());
+  fb::stem_conv_bn(fb::STEM_APPLY, fptr(x), fptr(w), fptr_mut(out), fptr_mut(stats), fptr(*gamma), fptr(*beta), rm, rv,
+                   fptr_mut(sm), fptr_mut(si), NB, H, (float)eps, (float)momentum, act ? 1 : 0, self_clean ? 1 : 0, cur_stream());
+  return {out, sm, si};
+}
 // Returns (dy, dres or undefined); accumulates into dgamma / dbeta when given.
 std::vector<Tensor> bn_elu_bwd(Tensor dout, c10::optional<Tensor> out, Tensor y, Tensor mean, Tensor invstd, Tensor gamma,
                                c10::optional<Tensor> beta, c10::optional<Tensor> dgamma, c10::optional<Tensor> dbeta,
@@ -1196,6 +1234,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("running_mean"), py::arg("running_var"), py::arg("eps"), py::arg("momentum"), py::arg("act"),
         py::arg("self_clean"), py::arg("use_running") = false);
   m.def("bn_elu_bwd", &bn_elu_bwd);
+  m.def("stem_conv_supported", &stem_conv_supported);
+  m.def("stem_conv_bn", &stem_conv_bn, py::arg("x"), py::arg("w"), py::arg("stats"), py::arg("mode"), py::arg("gamma") = py::none(),
+        py::arg("beta") = py::none(), py::arg("running_mean") = py::none(), py::arg("running_var") = py::none(),
+        py::arg("eps") = 1e-5, py::arg("momentum") = 0.1, py::arg("act") = true, py::arg("self_clean") = false);
   m.def("gn_elu_fwd", &gn_elu_fwd, py::arg("y"), py::arg("gamma"), py::arg("beta"), py::arg("residual"), py::arg("groups"),
         py::arg("eps"), py::arg("act"));
   m.def("gn_elu_bwd", &gn_elu_bwd, py::arg("dout"), py::arg("out"), py::arg("y"), py::arg("mean"), py::arg("rstd"),

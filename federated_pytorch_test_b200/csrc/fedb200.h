@@ -83,6 +83,16 @@ bool conv_wgrad_supported(int C_x, int C_out, int stride, int W_out, int H_out);
 void conv_wgrad_tf32(const float* x, const float* dy, float* dw, int NB, int H, int W, int C_x, int C_w, int C_out, int kh,
                      int kw, int stride, int pad, int dil, int H_out, int W_out, cudaStream_t stream);
 
+// ---- ResNet stem: 3 -> 64 channels, 3 x 3, stride 1, padding 1, + training-mode BatchNorm + ELU (stem_kernels.cu) ----------
+// STORE_Y: y [N,H,32,64] and its batch statistics added into stats [sum 64 | sumsq 64 | counter]; STATS_ONLY: the statistics
+// alone; APPLY: out = act(BN(conv(x))) from the complete statistics, save_mean / save_invstd, the running-statistics update
+// (running_mean may be nullptr) and, with self_clean, the reset of stats and its counter, as bn_elu_fwd does.
+enum { STEM_STORE_Y = 0, STEM_STATS_ONLY = 1, STEM_APPLY = 2 };
+bool stem_conv_supported(int H, int W, int C_in, int C_out);
+void stem_conv_bn(int mode, const float* x, const float* w, float* out, float* stats, const float* gamma, const float* beta,
+                  float* running_mean, float* running_var, float* save_mean, float* save_invstd, int NB, int H, float eps,
+                  float momentum, int act, int self_clean, cudaStream_t stream);
+
 
 // ---- flat-vector kernels (flat_kernels.cu) ---------------------------------------------------------
 void adam_prox(float* x, const float* g, float* m, float* v, const int* step_dev, int n, float lr, float b1, float b2,

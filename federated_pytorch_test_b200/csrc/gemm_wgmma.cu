@@ -503,10 +503,10 @@ bool conv_wgrad_supported(int C_x, int C_out, int stride, int W_out, int H_out) 
   return W_out > 0 && H_out > 0;
 }
 
-template <int BN>
+template <int BN, int BM = WG_BM>
 static void launch_wgrad(const float* x, const float* dy, const WgradParams& p, int grid, cudaStream_t stream) {
-  constexpr int smem = 2 * (WG_A_BYTES + BN * WG_BK * 4);
-  auto kernel = wgrad_wgmma_kernel<BN>;
+  constexpr int smem = 2 * (BM * WG_BK * 4 + BN * WG_BK * 4);
+  auto kernel = wgrad_wgmma_kernel<BN, BM>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -531,7 +531,9 @@ void conv_wgrad_tf32(const float* x, const float* dy, float* dw, int NB, int H, 
   p.P = NB * H_out * W_out;
   p.dw = dw;
   const int bn = C_out <= 32 ? 32 : (C_out <= 64 ? 64 : 128);   // all output channels in one tile when they fit
-  p.j_tiles = (p.J + WG_BM - 1) / WG_BM;
+  // one 64-row tile over every stored channel (16-byte gathers) when the taps x C_x rows fit in it
+  const bool small_j = kh * kw * C_x <= WG_BM_SMALL && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  p.j_tiles = small_j ? 1 : (p.J + WG_BM - 1) / WG_BM;
   p.co_tiles = (C_out + bn - 1) / bn;
   // Split the pixel range until ~two CTAs per SM exist (every split adds a full |dW| of red.add traffic in the
   // epilogue), keeping >= 8 k-blocks per CTA.
@@ -543,6 +545,14 @@ void conv_wgrad_tf32(const float* x, const float* dy, float* dw, int NB, int H, 
   p.kb_per_split = (kb_total + splits - 1) / splits;
   splits = (kb_total + p.kb_per_split - 1) / p.kb_per_split;       // no empty slices
   const int grid = base * splits;
+  if (small_j) {
+    switch (bn) {
+      case 32: launch_wgrad<32, WG_BM_SMALL>(x, dy, p, grid, stream); break;
+      case 64: launch_wgrad<64, WG_BM_SMALL>(x, dy, p, grid, stream); break;
+      default: launch_wgrad<128, WG_BM_SMALL>(x, dy, p, grid, stream); break;
+    }
+    return;
+  }
   switch (bn) {
     case 32: launch_wgrad<32>(x, dy, p, grid, stream); break;
     case 64: launch_wgrad<64>(x, dy, p, grid, stream); break;

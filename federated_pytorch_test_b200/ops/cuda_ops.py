@@ -10,6 +10,8 @@ Kernel inventory (SURVEY §2.10 ids):
   G1  conv2d_nhwc          wgmma implicit GEMM (TMA 4-D boxes -> smem -> wgmma tf32 -> registers), BN stats in epilogue
   G2/3 bn_elu_fwd/bwd      BatchNorm(train) + residual + ELU fused, two-pass backward
        conv2d_nhwc_bn_eval  conv + BatchNorm(eval, running statistics) + residual + ELU in the conv epilogue (inference)
+       stem_conv_bn        the ResNet stem (3 -> 64 channels, 3x3): y + BN statistics, or, without a gradient to take,
+                           statistics then BN + ELU on the recomputed convolution, y never stored (stem_kernels.cu)
        gn_elu_fwd/bwd      GroupNorm + residual + ELU, three kernels each way, no floating-point atomics (norm_kernels.cu)
   G4  avgpool / pool_linear
   G5  linear_tf32          wgmma GEMM with bias+ELU epilogue
@@ -484,12 +486,20 @@ class _ConvBnAct(torch.autograd.Function):
         e = ext()
         xn = _nhwc(x)
         wk = _krsc(weight)
-        if xn.shape[3] == 3:  # stem: pad 3 -> 4 channels so that the pixel pitch is 16 B (TMA requirement)
-            xn = F.pad(xn, (0, 1))
-            wk = F.pad(wk, (0, 1))
         Co = weight.shape[0]
         stats, self_clean = _stats_buffer(weight, Co)
-        y = e.conv2d_nhwc(xn, wk, stats, stride, pad, 1)
+        if _stem_supported(x, weight, stride, pad, residual):
+            y = e.stem_conv_bn(xn, wk, stats, STEM_STORE_Y)[0]
+            # the backward's wgmma kernels read 4-channel pixels (16-byte pitch): pad what each gradient needs
+            if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+                xn = F.pad(xn, (0, 1))
+            if ctx.needs_input_grad[0]:
+                wk = F.pad(wk, (0, 1))
+        else:
+            if xn.shape[3] == 3:  # stem: pad 3 -> 4 channels so that the pixel pitch is 16 B (TMA requirement)
+                xn = F.pad(xn, (0, 1))
+                wk = F.pad(wk, (0, 1))
+            y = e.conv2d_nhwc(xn, wk, stats, stride, pad, 1)
         res = _nhwc(residual) if residual is not None else None
         out, mean, invstd = e.bn_elu_fwd(y, stats, gamma, beta, res, running_mean, running_var, eps, momentum, act, self_clean)
         ctx.save_for_backward(xn, wk, y, out, mean, invstd, gamma, beta)
@@ -893,7 +903,32 @@ def conv_act(x: torch.Tensor, conv: nn.Module, act: bool = True) -> torch.Tensor
     return _ConvAct.apply(x, conv.weight, conv.bias, conv.stride[0], conv.padding[0], conv.dilation[0], bool(act))
 
 
+STEM_STORE_Y, STEM_STATS_ONLY, STEM_APPLY = 0, 1, 2     # stem_conv_bn modes (csrc/fedb200.h)
+
+
+def _stem_supported(x: torch.Tensor, weight: torch.Tensor, stride: int, pad: int, residual) -> bool:
+    """The ResNet stem of stem_kernels.cu: 3 -> 64 channels, 3 x 3, stride 1, padding 1, no residual, 32-pixel rows."""
+    return (residual is None and x.dim() == 4 and tuple(weight.shape) == (64, 3, 3, 3) and stride == 1 and pad == 1
+            and bool(ext().stem_conv_supported(x.shape[2], x.shape[3], 3, 64)))
+
+
+def _stem_bn_act(x: torch.Tensor, conv: nn.Conv2d, bn: nn.BatchNorm2d, act: bool) -> torch.Tensor:
+    """The stem's conv + training-mode BatchNorm + ELU without a gradient to take: the statistics pass, then one pass that
+    recomputes the convolution and writes the normalised output (and updates the running statistics once); y is never stored."""
+    e = ext()
+    xn = _nhwc(x)
+    wk = _krsc(conv.weight)
+    stats, self_clean = _stats_buffer(conv.weight, 64)
+    e.stem_conv_bn(xn, wk, stats, STEM_STATS_ONLY)
+    out = e.stem_conv_bn(xn, wk, stats, STEM_APPLY, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, bn.momentum,
+                         bool(act), self_clean)[0]
+    return out.permute(0, 3, 1, 2)
+
+
 def conv_bn_act(x, conv: nn.Conv2d, bn: nn.BatchNorm2d, residual=None, act: bool = True) -> torch.Tensor:
+    if _stem_supported(x, conv.weight, conv.stride[0], conv.padding[0], residual) and not (
+            torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, conv.weight, bn.weight, bn.bias))):
+        return _stem_bn_act(x, conv, bn, act)
     return _ConvBnAct.apply(x, conv.weight, bn.weight, bn.bias, residual, bn.running_mean, bn.running_var,
                             conv.stride[0], conv.padding[0], bn.eps, bn.momentum, bool(act))
 
